@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- end-to-end frames/s of the depth -> stereo hot path on B200.
+"""bench.py -- end-to-end frames/s of the depth -> stereo hot path on an H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload 1080p|4k] [--impl ours|reference]
-                    [--no-4k] [--no-cpu-baseline] [--dof S] [--exact]
+                    [--no-4k] [--no-cpu-baseline] [--dof S] [--exact] [--dump-outputs DIR]
 
 A step = one batch of `frames_per_step` synthetic frames through the hot path (DPT processor + Depth-Anything-V2
 forward + u8 depth handoff in HBM + the DIBR frame loop of render_sbs_3d + pack).  With the defaults (20 steps of
@@ -10,14 +10,19 @@ forward + u8 depth handoff in HBM + the DIBR frame loop of render_sbs_3d + pack)
 `value`   : frames/s, inputs resident in HBM, CUDA events on the engine's stream, max over ranks.
 `e2e`     : the same through the public host-buffer API (vd3d_render_clip_depth on pinned host frames, H2D and D2H
             inside the timed region).
-`roofline`: the dominant kernel of the step -- the persistent tcgen05 GEMM (its fc1 launches timed live with CUDA
-            events) against the measured bf16 peak; `roofline_depth_stage`, `roofline_dibr_stage` (whole DIBR frame,
+`roofline`: the dominant kernel of the step -- the persistent wgmma GEMM (its fc1 launches timed live with CUDA
+            events) against the bf16 peak; `roofline_depth_stage`, `roofline_dibr_stage` (whole DIBR frame,
             SURVEY 8(d) algorithmic bytes) and `roofline_dibr_render` (the fused warp/feather/compose/pack kernel)
-            against the measured HBM peak explain the rest.  `dibr_only` is the DIBR stage run back to back on
+            against the HBM peak explain the rest.  Peaks come from MEASURED_PEAKS.json when present, else from the
+            H100 SXM data sheet (dense bf16 989 TFLOP/s, HBM3 3.35 TB/s, at 700 W).  `dibr_only` is the DIBR stage run back to back on
             device-resident depth (its throughput form: bytes_per_frame x stage_fps).
 `arm_4k`  : the same measurement on configs[2]'s per-GPU share (4K, DA-V2-Large, Full-SBS), emitted in the same run.
 `cpu_baseline`: the oracle port of the reference path timed on a bounded sample on the host cores (rank 0, N=1).
 `--impl reference`: that CPU port as the timed arm, same JSON line and the same `config`.
+`--dump-outputs DIR`: after the timed steps, the SBS frames the last timed step of the workload's arm produced (what
+            vd3d_render_clip_depth hands its caller) go to DIR/sbs_frames.npy as float32 [frames, samples], with the
+            flat byte positions sampled in DIR/sbs_sample_index.npy: a fixed seeded sample, both files within 48 MB.  Inputs and
+            weights are seeded, so two builds run with the same arguments can be compared output for output.
 Multi-GPU: one process per GPU (torchrun), contiguous chunks of frames per rank, one NCCL broadcast of the weights,
 no per-frame collective; max-over-ranks device time.  `--sharding exact` hands the temporal state from rank to
 rank (bit-identical to one GPU); the default `replicas` keeps independent state per chunk.
@@ -50,16 +55,12 @@ WORKLOADS = {
                w=3840, h=2160, fmt="Full-SBS", preserve=True, model="vitl", pool=12, frames_per_step=12,
                dibr_bytes=18 * 3840 * 2160),
 }
-# dram__bytes_read.sum + dram__bytes_write.sum of one launch of the fused render kernel from `ncu --set full`
-# (profiles/r02_ncu_dibr.md); None until captured for that configuration
-NCU_RENDER_TRAFFIC = {"4k": 115_862_272, "1080p": 49_949_440}
-# smsp__issue_active.avg.pct_of_peak_sustained_active of the same launches: the DIBR kernels are issue bound, not HBM
-# bound (DESIGN.md section 3.1), so this is the roofline fraction that describes them
-NCU_RENDER_ISSUE_ACTIVE = {"4k": 70.6, "1080p": 62.9}
-# same for one fc1 launch of k_umma_gemm<128,3> of a 4-frame forward (DA-V2-Base: M=10123, N=3072, K=768): 20.4 MB read +
-# 11.7 MB written, cold L2 (profiles/r02_ncu_depth_final.md; algorithmic: 15.5 MB A + 4.7 MB W + 62.2 MB out, the output
-# mostly stays in the 126 MB L2 for fc2)
-NCU_GEMM_FC1_TRAFFIC = {"vitb": 32_100_000, "vitl": None, "vits": None}
+# DRAM traffic (dram__bytes_read.sum + dram__bytes_write.sum) and issue activity
+# (smsp__issue_active.avg.pct_of_peak_sustained_active) of one launch of the fused render kernel and of one fc1 GEMM
+# launch, from an `ncu --set full` capture on the GPU the numbers describe; keyed by workload / model, none captured
+NCU_RENDER_TRAFFIC = {}
+NCU_RENDER_ISSUE_ACTIVE = {}
+NCU_GEMM_FC1_TRAFFIC = {}
 COMMON = dict(fg=4.5, mg=-1.5, bg=-6.0, sharp=0.2, feather=10.0, ksize=9, tracking=True, floating=True,
               zps=0.01, dof=0.0)
 
@@ -68,15 +69,15 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 def peaks_burst():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return json.load(open(p)).get("bf16_tflops", 1590.0)
-    return 1590.0
+        return json.load(open(p)).get("bf16_tflops", 989.0)
+    return 989.0
 
 
 def common_config(wl, world, sharding="replicas"):
@@ -360,12 +361,25 @@ class GpuArm:
 
     def step(self, mem):
         idx, wl, _lib = self._idx(), self.wl, self._lib
+        self.last_idx = idx
         if mem == _lib.MEM_DEVICE:
             a, c = self.ptr_array(self.f_dev, idx), self.ptr_array(self.o_dev, idx)
         else:
             a, c = self.ptr_array(self.f_host, idx), self.ptr_array(self.o_host, idx)
         self.ctx.check(self.lib.vd3d_render_clip_depth(self.ctx.h, self.deng.h, self.B, a, wl["h"], wl["w"],
                                                        C.byref(self.rp), c, mem))
+
+    def dump_outputs(self, out_dir, budget_bytes=48 << 20):
+        """Write the output frames of the last step (device arm) as float32, sampled at fixed seeded byte positions;
+        the samples and their positions together stay within budget_bytes."""
+        os.makedirs(out_dir, exist_ok=True)
+        self.torch.cuda.synchronize()
+        frames = np.stack([self.o_dev[i].cpu().numpy().reshape(-1) for i in self.last_idx])
+        n = frames.shape[1]
+        k = min(n, budget_bytes // (4 * len(frames) + 8))  # float32 samples + their float64 positions
+        pos = np.arange(n) if k == n else np.sort(np.random.default_rng(0).choice(n, k, replace=False))
+        np.save(os.path.join(out_dir, "sbs_frames.npy"), frames[:, pos].astype(np.float32))
+        np.save(os.path.join(out_dir, "sbs_sample_index.npy"), pos.astype(np.float64))
 
     def step_dibr(self):
         idx, wl, _lib = self._idx(), self.wl, self._lib
@@ -489,7 +503,7 @@ class GpuArm:
         wall = self.reduce_max(time.perf_counter() - t0)
         return self.reduce_max(e0.elapsed_time(e1)), wall
 
-    def measure(self, local_rank, full=True):
+    def measure(self, local_rank, dump_dir=None):
         args, wl, _lib, lib, ctx, deng = self.args, self.wl, self._lib, self.lib, self.ctx, self.deng
         B, world = self.B, self.world
         frames = args.steps * B
@@ -499,6 +513,8 @@ class GpuArm:
         l0 = ctx.launches + deng.launches
         ms, _ = self.timed(lambda: self.step(_lib.MEM_DEVICE), args.steps, args.warmup)
         launches = ctx.launches + deng.launches - l0 - 0
+        if dump_dir and self.rank == 0:
+            self.dump_outputs(dump_dir)
         value = world * frames / (ms / 1000.0)
         # ---------------- end-to-end arm (pinned host buffers through the public API) ----------------
         _, e2e_s = self.timed(lambda: self.step(_lib.MEM_HOST), args.steps, args.warmup)
@@ -576,13 +592,13 @@ class GpuArm:
             "clocks": clk,
             "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
             "gpu_launches": int(launches),
-            "roofline": {"bound": "tensor", "kernel": "k_umma_gemm<128,3> (fc1 launches)",
+            "roofline": {"bound": "tensor", "kernel": "k_umma_gemm<128,4> (fc1 launches)",
                          "achieved": gemm_tf, "peak": tf_burst, "unit": "TFLOP/s", "frac": gemm_tf / tf_burst,
                          "traffic": NCU_GEMM_FC1_TRAFFIC.get(wl["model"]),
-                         "peak_source": which + " (cuBLAS bf16 burst: kernel timed alone)",
+                         "peak_source": which,
                          "algorithmic_gflop_per_launch": g_gf.value, "avg_launch_ms": gemm_ms, "launches_timed": g_n.value},
             "roofline_depth_stage": {"bound": "tensor", "achieved": depth_tf, "peak": tf_peak, "unit": "TFLOP/s",
-                                     "frac": depth_tf / tf_peak, "peak_source": which + " (cuBLAS bf16 sustained)",
+                                     "frac": depth_tf / tf_peak, "peak_source": which,
                                      "algorithmic_gflop_per_frame": DEPTH_GFLOP[wl["model"]], "avg_frame_ms": depth_ms,
                                      "share_of_step": depth_ms / max(depth_ms + stage_ms, 1e-9),
                                      "achieved_in_timed_region": DEPTH_GFLOP[wl["model"]] * (value / world) / 1000.0},
@@ -590,8 +606,6 @@ class GpuArm:
                                      "achieved": rend_gbs, "peak": hbm_peak, "unit": "GB/s", "frac": rend_gbs / hbm_peak,
                                      "traffic": NCU_RENDER_TRAFFIC.get(self.key),
                                      "issue_active_pct": NCU_RENDER_ISSUE_ACTIVE.get(self.key),
-                                     "note": "instruction-issue bound (~1000 thread-instructions per eye pixel against a machine "
-                                             "balance of 5.5 instructions per byte): frac vs HBM is not the binding roofline",
                                      "peak_source": which, "algorithmic_bytes_per_launch": rend_bytes, "avg_launch_ms": rend_ms},
             "roofline_dibr_stage": {"bound": "hbm", "what": "whole DIBR frame (ingest..pack), serial eager launches",
                                     "achieved": stage_gbs, "peak": hbm_peak, "unit": "GB/s", "frac": stage_gbs / hbm_peak,
@@ -620,6 +634,8 @@ def main():
     ap.add_argument("--no-4k", action="store_true", help="skip the 4K / DA-V2-Large / Full-SBS arm of the default run")
     ap.add_argument("--exact", action="store_true", help="DIBR in the bit-exact one-kernel-per-op mode")
     ap.add_argument("--sharding", default="replicas", choices=["replicas", "exact"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the SBS frames of the last timed step (sampled, float32) to DIR/*.npy")
     ap.add_argument("--dof", type=float, default=None,
                     help="dof_strength (default 0 = the warp/fill/compose variant; 2.0 = the reference GUI default)")
     args = ap.parse_args()
@@ -648,7 +664,7 @@ def main():
             dist.destroy_process_group()
         return
     arm = GpuArm(args, args.workload, rank, local_rank, world, dist)
-    line = arm.measure(local_rank)
+    line = arm.measure(local_rank, dump_dir=args.dump_outputs)
     del arm
     torch.cuda.empty_cache()
     if args.workload == "1080p" and not args.no_4k:

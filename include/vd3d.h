@@ -1,4 +1,4 @@
-/* vd3d.h -- C ABI of libvd3d.so, the B200 (sm_100a) depth->stereo engine.
+/* vd3d.h -- C ABI of libvd3d.so, the H100 (sm_90a) depth->stereo engine.
  *
  * The reference (VisionDepth3D) has no FFI: its boundary is the Python function
  * surface of core/render_3d.py and the `pipe` callable of core/render_depth.py
@@ -246,8 +246,8 @@ int vd3d_dof_grade(vd3d_ctx* ctx, const uint8_t* eye_bgr, int h, int w, const fl
 
 /* ---- depth forward (Depth-Anything-V2: DINOv2 ViT + DPT neck/head) ----------
  * Replaces model.forward inside transformers' depth-estimation pipeline as called by
- * hf_batch_safe_pipe (core/render_depth.py:1106-1119).  GEMMs / 3x3 convs run on tcgen05
- * tensor cores (f16 operands, fp32 accumulation in TMEM) fed by TMA. */
+ * hf_batch_safe_pipe (core/render_depth.py:1106-1119).  GEMMs / 3x3 convs run on wgmma
+ * tensor cores (f16 operands, fp32 accumulation) fed by TMA. */
 typedef struct {
   int32_t hidden, layers, heads; /* 384/12/6, 768/12/12, 1024/24/16 */
   int32_t taps[4];               /* out_indices of the backbone (1-based layer numbers) */
@@ -295,7 +295,7 @@ int vd3d_get_depth_batch(vd3d_ctx* ctx);
  * The reference runs an ONNX export of xinntao/Real-ESRGAN's SRVGGNetCompact (realesr-general-x4v3: 32 body convs;
  * realesr-animevideov3: 16) through ONNXRuntime.  vd3d_sr_create returns an engine container (weights by name through
  * vd3d_depth_set_tensor: "sr.c{i}.w" f16 [Cout, 9*64], "sr.c{i}.b" f32, "sr.a{i}" f32 PReLU slopes; destroy with
- * vd3d_depth_destroy).  vd3d_sr_forward: BGR u8 [h,w,3] -> BGR u8 [4h,4w,3] = preprocess_esr -> network (tcgen05
+ * vd3d_depth_destroy).  vd3d_sr_forward: BGR u8 [h,w,3] -> BGR u8 [4h,4w,3] = preprocess_esr -> network (wgmma
  * implicit-GEMM convs, f16 activations, fp32 accumulate, fp32 last layer) -> PixelShuffle + input -> postprocess_esr. */
 int vd3d_sr_create(void* cuda_stream, vd3d_depth** out);
 int vd3d_sr_forward(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, int num_conv, uint8_t* out_bgr, int mem);
@@ -303,9 +303,11 @@ int vd3d_sr_forward(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, int n
 int vd3d_depth_get_buffer(vd3d_depth* e, const char* name, void* host_out, size_t bytes);
 /* unit-test hooks for the tensor-core kernels */
 int vd3d_gemm_f16(vd3d_depth* e, const void* A_f16, const void* B_f16, int M, int N, int K, float* C_host, int bn);
-/* tuning hook: average launch time (ms) of one M x N x K GEMM on device-resident operands. variant: 0 <128,3> two
-   CTAs/SM, 1 <128,6>, 2 <128,3> one CTA/SM, 10-12 CTA pair 256x256 (6/4/2 stages), 20-22 CTA pair 256x128;
-   dbg: 0 normal, 1 no MMAs (operand-feed rate), 2 no TMA loads (MMA rate); act: 0 none, 1 GELU */
+/* tuning hook: average launch time (ms) of one M x N x K GEMM on device-resident operands, on the 128 x 128 tile
+   kernel with an operand ring of 4 (variant 0, the default), 3 (variant 1) or 2 (variant 2) stages; other variants
+   return VD3D_ERR_ARG.  dbg (low 3 bits): 0 normal, 2 no TMA loads (MMA rate), 3 prologue + teardown only, 4 no
+   epilogue, other values VD3D_ERR_ARG; bit 3: poll barriers with test_wait.  act: 0 none, 1 GELU; 0x100 selects the
+   residual (proj / fc2) epilogue */
 int vd3d_gemm_bench(vd3d_depth* e, int M, int N, int K, int variant, int dbg, int act, int iters, float* ms_out);
 int vd3d_conv_f16(vd3d_depth* e, const void* in_nhwc_f16, int H, int W, int cin, const void* w_f16, int cout,
                   int k3, const float* bias, int relu, float* out_host);

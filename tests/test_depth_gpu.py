@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 GEMM / implicit-GEMM conv kernels and the Depth-Anything-V2 forward
+"""GPU: the wgmma GEMM / implicit-GEMM conv kernels and the Depth-Anything-V2 forward
 against fp32 references (numpy matmul, torch conv2d, oracle/depth.py).
 
 Tolerances: GEMM/conv operands are f16 (10-bit mantissa) with fp32 accumulation, so unit
@@ -20,7 +20,8 @@ def eng():
 
 
 @pytest.mark.parametrize("shape", [(128, 128, 64), (128, 128, 128), (256, 384, 768), (2443, 1152, 384),
-                                   (100, 200, 72), (2442, 48 + 16, 384), (300, 32, 576), (129, 130, 8)])
+                                   (100, 200, 72), (2442, 48 + 16, 384), (300, 32, 576), (129, 130, 8),
+                                   (2443, 768, 3072), (2443, 2304, 768)])
 def test_gemm_matches_numpy(eng, shape):
     M, N, K = shape
     rng = np.random.default_rng(M * 7 + N)
@@ -30,20 +31,6 @@ def test_gemm_matches_numpy(eng, shape):
     for bn in ((0,) if N < 64 else (0, 64, 32)):
         out = eng.gemm(A, B, bn)
         assert np.abs(out - ref).max() <= 2e-3 * max(1.0, np.abs(ref).max()), (shape, bn)
-
-
-@pytest.mark.parametrize("bn", [256, -128])
-@pytest.mark.parametrize("shape", [(256, 256, 64), (256, 512, 768), (300, 640, 256), (2443, 2304, 768),
-                                   (2443, 768, 3072), (129, 130, 8), (1000, 96, 128)])
-def test_gemm_cta_pair_matches_numpy(eng, shape, bn):
-    """cta_group::2 kernel (256-row tiles over two SMs): odd 128-row tile counts, ragged N and K, many k-blocks."""
-    M, N, K = shape
-    rng = np.random.default_rng(M * 11 + N + (bn & 255))
-    A = (rng.standard_normal((M, K)) * 0.5).astype(np.float16)
-    B = (rng.standard_normal((N, K)) * 0.5).astype(np.float16)
-    ref = A.astype(np.float32) @ B.astype(np.float32).T
-    out = eng.gemm(A, B, bn)
-    assert np.abs(out - ref).max() <= 2e-3 * max(1.0, np.abs(ref).max()), (shape, bn)
 
 
 @pytest.mark.parametrize("case", [(37, 66, 64, 64, True), (74, 132, 128, 64, True), (19, 33, 64, 128, True),

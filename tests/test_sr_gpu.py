@@ -1,4 +1,4 @@
-"""GPU: the Real-ESRGAN stage (SURVEY 8(f) rank 3) -- SRVGGNetCompact on the tcgen05 implicit-GEMM convs against the
+"""GPU: the Real-ESRGAN stage (SURVEY 8(f) rank 3) -- SRVGGNetCompact on the wgmma implicit-GEMM convs against the
 fp32 torch restatement (oracle/sr.py; the reference's ONNX model runs in fp16), and run_esrgan's resize / blend chain
 against the cv2-pinned oracle."""
 import numpy as np
@@ -17,9 +17,8 @@ def _np_sd(sd):
 
 @pytest.mark.parametrize("num_conv,w,h", [(4, 96, 54), (16, 160, 90), (32, 320, 180), (32, 157, 93)])
 def test_sr_forward_matches_oracle(num_conv, w, h):
-    """u8 output <= 1 LSB against the fp32 oracle; f16 activations through up to 34 layers put 0.8 % (4 body convs),
-    1.2 % (16), 2.7 % (32) of the bytes on the other side of the x255 truncation (measured on B200; the reference's own
-    ONNX model runs in fp16 end to end)."""
+    """u8 output <= 1 LSB against the fp32 oracle; f16 activations through up to 34 layers put a few per cent of the
+    bytes on the other side of the x255 truncation (the reference's own ONNX model runs in fp16 end to end)."""
     import torch
     from visiondepth3d_b200 import merged_pipeline as MP
     sd = S.srvgg_state_dict(num_conv=num_conv, seed=3)

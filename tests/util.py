@@ -10,7 +10,8 @@ def u8_diff(a, b):
 # Parameter sets used by tools/gen_golden.py (kept in one place so the oracle and the
 # CUDA path are driven exactly like the reference was).
 PS_CASES = {
-    "ps_smooth_320x180.npz": dict(w=320, h=180, iw=320, ih=180, n=3, kind="smooth",
+    # rows=k: every k-th row of the stored eyes (keeps the three-frame fixture under 1 MB)
+    "ps_smooth_320x180.npz": dict(w=320, h=180, iw=320, ih=180, n=3, kind="smooth", rows=2,
                                   kw=dict(blur_ksize=9, feather_strength=10.0, zero_parallax_strength=0.01)),
     "ps_up2_320x180.npz": dict(w=320, h=180, iw=160, ih=90, n=2, kind="smooth",
                                kw=dict(blur_ksize=5, feather_strength=4.0, enable_floating_window=False,
@@ -20,7 +21,7 @@ PS_CASES = {
                                          use_subject_tracking=False)),
 }
 
-# oracle-vs-reference only for now (CPU); add to the GPU golden test once run on a B200
+# oracle-vs-reference only for now (CPU)
 PS_CASES_EXTRA = {
     # tools/gen_golden.py extra: every shaping / balance control of pixel_shift_cuda off its default
     "ps_controls_256x144.npz": dict(w=256, h=144, iw=256, ih=144, n=2, kind="smooth",
@@ -75,7 +76,7 @@ LOOP_CASES_EXTRA = {
 # < 0.1 % one-LSB flips (torch's Sleef powf/expf differ from IEEE by <= 1 ulp), and full frames -- sharpening ON, which
 # amplifies an isolated flip up to 7.7 LSB -- have < 0.1 % of bytes off by more than one (2-3 % on the smooth set).
 PS_NATURAL = {
-    "ps_natural_320x180.npz": dict(w=320, h=180, iw=320, ih=180, n=3, kind="natural",
+    "ps_natural_320x180.npz": dict(w=320, h=180, iw=320, ih=180, n=3, kind="natural", rows=4,
                                    kw=dict(blur_ksize=9, feather_strength=10.0, zero_parallax_strength=0.01)),
 }
 LOOP_NATURAL = {

@@ -1,4 +1,4 @@
-"""Depth stage only: batched DA-V2 forward on synthetic frames (the command the ncu captures of the tcgen05 kernels run).
+"""Depth stage only: batched DA-V2 forward on synthetic frames (a profiler target for the wgmma kernels).
    python tools/depth_only.py [vitb|vitl|vits] [batch] [reps]"""
 import os
 import sys

@@ -1,5 +1,5 @@
-"""DIBR stage only (no depth engine) on device-resident synthetic frames: the command the ncu captures of the DIBR
-kernels run (profiles/r02_*).   python tools/dibr_only.py [1080p|4k] [frames] [--eager] [--exact]"""
+"""DIBR stage only (no depth engine) on device-resident synthetic frames: a profiler target for the DIBR
+kernels.   python tools/dibr_only.py [1080p|4k] [frames] [--eager] [--exact]"""
 import ctypes as C
 import os
 import sys

@@ -43,6 +43,11 @@ def run_pixel_shift(r3d, torch, w, h, iw, ih, n_frames, kind, **kw):
     return out
 
 
+def every_row(g, step):
+    """Every step-th row of the stored eyes (tests/util.py `rows`): keeps a fixture under 1 MB."""
+    return {k: (v[::step] if k.startswith(("left", "right")) else v) for k, v in g.items()}
+
+
 def run_loop(r3d, torch, cv2, src_w, src_h, n_frames, kind, rp):
     """Drive the body of render_sbs_3d in memory by writing lossless-ish input is not
     possible (codecs are lossy) -> we run the real render_sbs_3d with cv2 capture
@@ -138,7 +143,7 @@ def main():
     # A. pixel_shift_cuda, identity resize, GUI-style params, 3 consecutive frames
     g = run_pixel_shift(r3d, torch, 320, 180, 320, 180, 3, "smooth",
                         blur_ksize=9, feather_strength=10.0, zero_parallax_strength=0.01)
-    np.savez_compressed(os.path.join(OUT, "ps_smooth_320x180.npz"), **g, **meta)
+    np.savez_compressed(os.path.join(OUT, "ps_smooth_320x180.npz"), **every_row(g, 2), **meta)
     # B. 2x upsample inside pixel_shift (Half-SBS style), no floating window
     g = run_pixel_shift(r3d, torch, 320, 180, 160, 90, 2, "smooth",
                         blur_ksize=5, feather_strength=4.0, enable_floating_window=False,
@@ -289,7 +294,7 @@ def gen_natural():
                 use_floating_window=True, preserve_original_aspect=False, zero_parallax_strength=0.01)
     g = run_pixel_shift(r3d, torch, 320, 180, 320, 180, 3, "natural",
                         blur_ksize=9, feather_strength=10.0, zero_parallax_strength=0.01)
-    np.savez_compressed(os.path.join(OUT, "ps_natural_320x180.npz"), **g, **meta)
+    np.savez_compressed(os.path.join(OUT, "ps_natural_320x180.npz"), **every_row(g, 4), **meta)
     g = run_loop(r3d, torch, cv2, 320, 180, 5, "natural", base)
     np.savez_compressed(os.path.join(OUT, "loop_natural_halfsbs_320x180.npz"), **g, **meta)
     g = run_loop(r3d, torch, cv2, 320, 180, 4, "natural", dict(base, output_format="Full-SBS", preserve_original_aspect=True))

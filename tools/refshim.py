@@ -1,17 +1,18 @@
-"""Import shim for the UNMODIFIED reference (read-only at /root/reference).
+"""Import shim for the UNMODIFIED reference (a VisionDepth3D checkout named by $VD3D_REFERENCE).
 
 Test infrastructure only: used in the build container by tools/gen_golden.py to
 produce tests/golden/*.npz and to pin oracle/ against the real reference.
-Nothing here (and nothing under /root/reference) is needed at run time on the
-GPU box.  Recipe follows SURVEY.md section 8(c): stub GUI / ORT modules with a
+Nothing here (and nothing in the reference checkout) is needed at run time on
+the GPU.  Recipe follows SURVEY.md section 8(c): stub GUI / ORT modules with a
 real __spec__, register a bare `core` package so core/__init__.py never runs.
 """
 import importlib
 import importlib.machinery
+import os
 import sys
 import types
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("VD3D_REFERENCE", "")
 
 
 class _Anything(types.ModuleType):
@@ -41,6 +42,9 @@ def _stub(name, is_pkg=False):
 
 def load_reference(modules=("render_3d",)):
     """Return {name: module} for core.<name>, reference files untouched."""
+    if not REF_ROOT or not os.path.isdir(os.path.join(REF_ROOT, "core")):
+        raise SystemExit("set VD3D_REFERENCE to a VisionDepth3D checkout (the directory holding core/render_3d.py); "
+                         f"got {REF_ROOT!r}")
     import PIL  # real
 
     for n in ("tkinter", "tkinter.filedialog", "tkinter.messagebox",

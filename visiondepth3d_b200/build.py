@@ -1,4 +1,4 @@
-"""Build libvd3d.so in-tree with nvcc for sm_100a (no torch extension machinery:
+"""Build libvd3d.so in-tree with nvcc for sm_90a (no torch extension machinery:
 the boundary is a plain C ABI).  Used by __graft_entry__.build()."""
 import os
 import subprocess
@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libvd3d.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-I", os.path.join(HERE, "..", "include")]
 
 # (source, extra flags).  The DIBR kernels reproduce the reference's fp32 rounding one

@@ -1,5 +1,5 @@
 // depth_engine.cu -- Depth-Anything-V2 (DINOv2 ViT + DPT neck/head) forward as a fixed
-// launch sequence of tcgen05 GEMMs and small fused kernels.  Host side: named device
+// launch sequence of wgmma GEMMs and small fused kernels.  Host side: named device
 // tensors (pushed by the Python loader in HF state_dict terms), TMA tensor maps, buffers.
 //
 // Reference call path: core/render_depth.py:1106-1119 -> transformers pipeline
@@ -160,71 +160,18 @@ GemmArgs base_args(int M, int N, int K, int epi) {
   return g;
 }
 
+// Tile width of a GEMM / conv: one 128 x bn kernel for every shape.  The choice depends on N only, never on the
+// batch size, so a frame's depth is the same inferred alone or in a batch
+// (tests/test_depth_gpu.py::test_infer_batch_equals_single_frames; exact sharding == one GPU).
 int pick_bn(int N) { return N >= 128 ? 128 : (N >= 64 ? 64 : 32); }
-
-// B tensor-map box rows for a tile code (see launch_gemm): the CTA-pair kernels stage half the tile's N per CTA
-int box_rows(int bn) { return bn == 256 ? 128 : (bn == -128 ? 64 : (bn == 1128 ? 128 : bn)); }
-
-// VD3D_GEMM_2CTA=1: route large plain GEMMs through the cta_group::2 kernel (256-row tiles)
-int pair_mode() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* v = getenv("VD3D_GEMM_2CTA");
-    mode = v ? atoi(v) : 0;
-  }
-  return mode;
-}
-// Kernel choice of the token GEMMs (VD3D_GEMM_POLICY=0: everything on the 128x128 single-CTA kernel).
-//  * fc2 (fp32 residual epilogue, K = 4D) and the QKV GEMM of the Large model (K = 1024) run on the CTA-pair kernel, 256x256
-//    tiles: the 128x128 kernel is bound by the L2->smem operand feed (~20 TB/s device-wide at 64 FLOP/B), the pair tile
-//    halves the bytes per FLOP.  In situ, 4 frames per forward: fc2 63 -> 54 us (Base), 95 -> 82 (Large); QKV-Large 60 -> 57.
-//    fc1 stays: its bias + GELU epilogue is ALU bound and the pair kernel has half the epilogue warps per SM (54 -> 72 us).
-//    The pair kernel's fp32 accumulation is not bit-identical to the single-CTA kernel's, so this choice depends on the
-//    model and the per-image token count only, never on the batch size: a frame's depth is the same inferred alone or in
-//    a batch (tests/test_depth_gpu.py::test_infer_batch_equals_single_frames; exact sharding == one GPU).
-//  * proj (K = D: two tiles per CTA, 1.6 us of MMAs per tile) of a batched forward runs one CTA per SM with 16 epilogue
-//    warps, each prefetching its slice of the residual stream while the MMAs run (41 -> 38.6 us; same MMA shape as the
-//    default kernel: bit-identical).
-int gemm_policy() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* v = getenv("VD3D_GEMM_POLICY");
-    mode = v ? atoi(v) : 1;
-  }
-  return mode;
-}
-int pick_bn_gemm(const vd3d_depth* e, int M, int N, int K, int epi) {
-  const int pm = pair_mode();
-  if (pm == 3) {  // tuning: every large batched GEMM on the pair kernel
-    if (M >= 4096 && N >= 768 && (long)N * K >= 1536L * 768) return 256;
-    return pick_bn(N);
-  }
-  if (pm && M >= 512) {
-    if (N >= 1536) return 256;
-    if (N >= 512) return -128;
-  }
-  if (gemm_policy() && e->ntok >= 1024 && (N % 256) == 0) {
-    if (epi == EPI_RESID_LS && K >= 1536) return 256;
-    if (epi == EPI_QKV && K >= 1024) return 256;
-  }
-  if (gemm_policy() && epi == EPI_RESID_LS && M >= 4096 && N >= 128) return 1128;
-  return pick_bn(N);
-}
-int pick_bn_conv(int M, int N) {  // VD3D_GEMM_2CTA=2: implicit-GEMM convs too (two pixel tiles per pair)
-  if (pair_mode() >= 2 && M >= 2048) {
-    if (N >= 256) return 256;
-    if (N >= 128) return -128;
-  }
-  return pick_bn(N);
-}
 
 // plain GEMM: A [M, K] (lda), B [N, K] (ldb)
 int gemm(vd3d_depth* e, const __half* A, int lda, const __half* B, int ldb, GemmArgs g, int bn = 0) {
-  if (!bn) bn = pick_bn_gemm(e, g.M, g.N, g.K, g.epi);  // (64-wide tiles for sub-wave grids were measured slower: L2->smem fill bound)
+  if (!bn) bn = pick_bn(g.N);
   CUtensorMap ma, mb;
   int r;
   if ((r = make_map(e, &ma, A, g.K, g.M, 1, lda, (uint64_t)lda * g.M, 128, 1))) return r;
-  if ((r = make_map(e, &mb, B, g.K, g.N, 1, ldb, (uint64_t)ldb * g.N, box_rows(bn), 1))) return r;
+  if ((r = make_map(e, &mb, B, g.K, g.N, 1, ldb, (uint64_t)ldb * g.N, bn, 1))) return r;
   cudaError_t ce = launch_gemm(bn, ma, mb, g, (g.M + 127) / 128, 1, e->cur ? e->cur : e->stream);
   if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("gemm launch: ") + cudaGetErrorString(ce));
   e->launches++;
@@ -237,7 +184,7 @@ int gemm_batched(vd3d_depth* e, const __half* A, int lda, uint64_t sa, const __h
   CUtensorMap ma, mb;
   int r;
   if ((r = make_map(e, &ma, A, g.K, g.M, batch, lda, sa, 128, 1))) return r;
-  if ((r = make_map(e, &mb, B, g.K, g.N, batch, ldb, sb, box_rows(bn), 1))) return r;
+  if ((r = make_map(e, &mb, B, g.K, g.N, batch, ldb, sb, bn, 1))) return r;
   cudaError_t ce = launch_gemm(bn, ma, mb, g, (g.M + 127) / 128, batch, e->cur ? e->cur : e->stream);
   if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("gemm launch: ") + cudaGetErrorString(ce));
   e->launches++;
@@ -260,7 +207,7 @@ void pick_tile(int W, int H, int& tw, int& th) {
 // conv over an NHWC f16 map [H, W, cin] (3x3 pad 1 when k3, else 1x1); weights [N, taps*cin]
 int conv(vd3d_depth* e, const __half* in, int H, int W, int cin, const __half* wt, bool k3, GemmArgs g, int bn = 0) {
   if (cin % 64) return dfail(e, VD3D_ERR_ARG, "conv: cin must be a multiple of 64");
-  if (!bn) bn = pick_bn_conv(H * W, g.N);
+  if (!bn) bn = pick_bn(g.N);
   int tw, th;
   pick_tile(W, H, tw, th);
   g.conv = k3 ? 1 : 2;
@@ -274,7 +221,7 @@ int conv(vd3d_depth* e, const __half* in, int H, int W, int cin, const __half* w
   CUtensorMap ma, mb;
   int r;
   if ((r = make_map(e, &ma, in, cin, W, H, cin, (uint64_t)cin * W, tw, th))) return r;
-  if ((r = make_map(e, &mb, wt, g.K, g.N, 1, g.K, (uint64_t)g.K * g.N, box_rows(bn), 1))) return r;
+  if ((r = make_map(e, &mb, wt, g.K, g.N, 1, g.K, (uint64_t)g.K * g.N, bn, 1))) return r;
   int m_tiles = ((W + tw - 1) / tw) * ((H + th - 1) / th);
   cudaError_t ce = launch_gemm(bn, ma, mb, g, m_tiles, 1, e->cur ? e->cur : e->stream);
   if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("conv launch: ") + cudaGetErrorString(ce));
@@ -445,7 +392,7 @@ int vd3d_depth_get_buffer(vd3d_depth* e, const char* name, void* host_out, size_
   return VD3D_OK;
 }
 
-// unit-test hook: C[M,N] f32 = A[M,K] f16 x B[N,K]^T f16 through the tcgen05 kernel
+// unit-test hook: C[M,N] f32 = A[M,K] f16 x B[N,K]^T f16 through the wgmma kernel
 int vd3d_gemm_f16(vd3d_depth* e, const void* A, const void* B, int M, int N, int K, float* C_host, int bn) {
   if (!e || !A || !B || !C_host || (K % 8)) return VD3D_ERR_ARG;
   void *da, *db, *dc;
@@ -467,6 +414,7 @@ int vd3d_gemm_f16(vd3d_depth* e, const void* A, const void* B, int M, int N, int
 // kernel variant (launch_gemm_variant) and debug mode (GemmArgs::dbg); returns the average launch time in ms
 int vd3d_gemm_bench(vd3d_depth* e, int M, int N, int K, int variant, int dbg, int act, int iters, float* ms_out) {
   if (!e || !ms_out || (K % 8) || iters < 1) return VD3D_ERR_ARG;
+  if (variant < 0 || variant > 2 || (dbg & 7) == 1 || (dbg & 7) > 4) return VD3D_ERR_ARG;
   void *da, *db, *dc;
   int r;
   if ((r = get_buf(e, "t.ba", (size_t)M * K * 2, &da))) return r;
@@ -491,7 +439,7 @@ int vd3d_gemm_bench(vd3d_depth* e, int M, int N, int K, int variant, int dbg, in
   }
   CUtensorMap ma, mb;
   if ((r = make_map(e, &ma, da, K, M, 1, K, (uint64_t)K * M, 128, 1))) return r;
-  if ((r = make_map(e, &mb, db, K, N, 1, K, (uint64_t)K * N, variant >= 20 ? 64 : 128, 1))) return r;
+  if ((r = make_map(e, &mb, db, K, N, 1, K, (uint64_t)K * N, 128, 1))) return r;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   auto done = [&](int rc) {
     if (e0) cudaEventDestroy(e0);
@@ -643,7 +591,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     e->span_end(sp_, s);
     sp_ = e->span_begin("attn", s);
     if (e->flash) {
-      // fused tcgen05 attention: scores stay in TMEM, probabilities in shared memory
+      // fused wgmma attention: scores and probabilities stay in registers
       CUtensorMap mq, mk, mv;
       if ((r = make_map(e, &mq, q, 64, NT, B * Hh, 64, (uint64_t)NP * 64, 128, 1))) return r;
       if ((r = make_map(e, &mk, k, 64, NT, B * Hh, 64, (uint64_t)NP * 64, 128, 1))) return r;
@@ -1056,7 +1004,7 @@ int vd3d_depth_infer_batch(vd3d_depth* e, int B, const uint8_t* const* frames_bg
 // ---------------------------------------------------------------------------
 // Real-ESRGAN upscale stage (core/merged_pipeline.py:240-267; the network is the ONNX export of xinntao/Real-ESRGAN's
 // SRVGGNetCompact: conv3x3(3->64)+PReLU, num_conv x [conv3x3(64->64)+PReLU], conv3x3(64->48), PixelShuffle(4), + nearest
-// x4 of the input).  Every conv is the tcgen05 implicit GEMM of the depth neck (f16 NHWC activations, fp32 accumulate);
+// x4 of the input).  Every conv is the wgmma implicit GEMM of the depth neck (f16 NHWC activations, fp32 accumulate);
 // the last one keeps fp32.  The engine object is the depth engine's container (named weights + buffers).
 int vd3d_sr_create(void* stream, vd3d_depth** out) {
   if (!out) return VD3D_ERR_ARG;

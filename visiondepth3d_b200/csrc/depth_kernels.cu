@@ -1,5 +1,5 @@
 // depth_kernels.cu -- non-GEMM kernels of the Depth-Anything-V2 forward and the
-// instantiations / launchers of the tcgen05 GEMM (umma_gemm.cuh).
+// instantiations / launchers of the wgmma GEMM and attention kernels (umma_gemm.cuh, umma_attention.cuh).
 // Reference: transformers 5.5.0 models/dinov2/modeling_dinov2.py and
 // models/depth_anything/modeling_depth_anything.py as called by
 // core/render_depth.py:1106-1119 (hf_batch_safe_pipe).
@@ -7,7 +7,6 @@
 
 #include "depth_launch.h"
 #include "umma_gemm.cuh"
-#include "umma_gemm2.cuh"
 #include "umma_attention.cuh"
 
 namespace vd3d {
@@ -448,43 +447,26 @@ void launch_relu_f16(const __half* in, __half* out, size_t n, cudaStream_t s) {
   k_relu_f16<<<(unsigned)((n8 + 255) / 256), 256, 0, s>>>(in, out, n8);
 }
 
-template <int BN, int STAGES, int EW = 8>
+template <int BN, int STAGES>
 static cudaError_t launch_gemm_t(const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, dim3 grid,
                                  cudaStream_t s) {
   static bool attr_set = false;
   constexpr int smem = GemmSmem<BN, STAGES>::kTotal;
   if (!attr_set) {
-    cudaError_t e =
-        cudaFuncSetAttribute(k_umma_gemm<BN, STAGES, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(k_umma_gemm<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  k_umma_gemm<BN, STAGES, EW><<<grid, 64 + 32 * EW, smem, s>>>(a, b, g);
+  k_umma_gemm<BN, STAGES><<<grid, kGemmThreads, smem, s>>>(a, b, g);
   return cudaGetLastError();
 }
 
 cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, int ntok, int dmodel,
                              __half* out, int heads, int images, int npad, cudaStream_t s) {
   static bool attr_set = false;
-  static int mode = 2;  // VD3D_ATTN_MODE: -2 two-pass, -1 k_umma_attention_1p, 0 / 1 / 2 k_umma_attention_v3<MODE>, 3 / 4 v3<2> + polynomial exp2
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(k_umma_attention, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_umma_attention_1p, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_umma_attention_v3<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_umma_attention_v3<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_umma_attention_v3<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_umma_attention_v3<2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(k_umma_attention_v3<2, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
-    if (e != cudaSuccess) return e;
-    if (const char* v = getenv("VD3D_ATTN_2PASS"))
-      if (atoi(v)) mode = -2;
-    if (const char* v = getenv("VD3D_ATTN_MODE")) mode = atoi(v);
     attr_set = true;
   }
   AttnArgs a;
@@ -494,122 +476,52 @@ cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const C
   a.heads = heads;
   a.npad = npad;
   dim3 grid((ntok + 127) / 128, heads * images);
-  switch (mode) {
-    case -2: k_umma_attention<<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a); break;
-    case -1: k_umma_attention_1p<<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a); break;
-    case 0: k_umma_attention_v3<0><<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a); break;
-    case 1: k_umma_attention_v3<1><<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a); break;
-    case 3: k_umma_attention_v3<2, 2><<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a); break;  // 25 % of the exps on the FMA pipe
-    case 4: k_umma_attention_v3<2, 4><<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a); break;  // 50 %
-    default: k_umma_attention_v3<2><<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a); break;
-  }
+  k_umma_attention<<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a);
   return cudaGetLastError();
 }
 
-// CTA-pair kernel: cluster of 2, one CTA per SM, persistent over pair tiles (256 x BN)
-template <int BN, int STAGES>
-static cudaError_t launch_gemm2_t(const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, int npairs,
-                                  cudaStream_t s) {
-  static bool attr_set = false;
-  constexpr int smem = Gemm2Smem<BN, STAGES>::kTotal;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(k_umma_gemm2<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
+static int sm_count() {
+  static int sms = 0;
+  if (!sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof cfg);
-  cfg.gridDim = dim3(2 * npairs, 1, 1);
-  cfg.blockDim = dim3(kGemm2Threads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, k_umma_gemm2<BN, STAGES>, a, b, g);
+  return sms;
 }
 
-// tuning hook (vd3d_gemm_bench): pick the kernel instantiation / grid shape explicitly.
-//   0: <128,3> two CTAs per SM   1: <128,6> one CTA per SM   2: <128,3> one CTA per SM
-//  10..12: CTA pair 256x256, 6 / 4 / 2 stages     20..22: CTA pair 256x128, 8 / 4 stages / 4 stages two pairs per TPC
+// tuning hook (vd3d_gemm_bench): pick the ring depth of the 128 x 128 kernel explicitly.
+//   0: 4 stages (the default)   1: 3 stages   2: 2 stages
 cudaError_t launch_gemm_variant(int variant, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g_in,
                                 int m_tiles, int batch, cudaStream_t s) {
   GemmArgs g = g_in;
-  const int tile_n = variant >= 20 ? 128 : (variant >= 10 ? 256 : 128);
-  g.nt = (g.N + tile_n - 1) / tile_n;
+  g.nt = (g.N + 127) / 128;
   g.mt = m_tiles;
   g.nz = batch;
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (variant >= 10) {
-    int total = g.nt * ((g.mt + 1) / 2) * g.nz;
-    int cap = variant == 22 ? sms : sms / 2;
-    int npairs = total < cap ? total : cap;
-    switch (variant) {
-      case 10: return launch_gemm2_t<256, 6>(a, b, g, npairs, s);
-      case 11: return launch_gemm2_t<256, 4>(a, b, g, npairs, s);
-      case 12: return launch_gemm2_t<256, 2>(a, b, g, npairs, s);
-      case 20: return launch_gemm2_t<128, 8>(a, b, g, npairs, s);
-      case 21:
-      case 22: return launch_gemm2_t<128, 4>(a, b, g, npairs, s);
-      default: return cudaErrorInvalidValue;
-    }
-  }
-  int total = g.nt * g.mt * g.nz;
-  int cap = variant == 0 ? 2 * sms : sms;
-  dim3 grid(total < cap ? total : cap, 1, 1);
+  const int total = g.nt * g.mt * g.nz, sms = sm_count();
+  dim3 grid(total < sms ? total : sms, 1, 1);
   switch (variant) {
-    case 0:
-    case 2: return launch_gemm_t<128, 3>(a, b, g, grid, s);
-    case 1: return launch_gemm_t<128, 6>(a, b, g, grid, s);
-    case 3: return launch_gemm_t<128, 6, 16>(a, b, g, grid, s);  // one CTA per SM, 16 epilogue warps
+    case 0: return launch_gemm_t<128, 4>(a, b, g, grid, s);
+    case 1: return launch_gemm_t<128, 3>(a, b, g, grid, s);
+    case 2: return launch_gemm_t<128, 2>(a, b, g, grid, s);
     default: return cudaErrorInvalidValue;
   }
 }
 
-// bn: 32 / 64 / 128 = single-CTA 128 x bn tiles; 256 = CTA-pair 256 x 256 tiles (B box 128 rows);
-//     -128 = CTA-pair 256 x 128 tiles (B box 64 rows)
+// bn: 32 / 64 / 128 = 128 x bn tiles; the B tensor map's box has bn rows
 cudaError_t launch_gemm(int bn, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g_in, int m_tiles,
                         int batch, cudaStream_t s) {
   GemmArgs g = g_in;
-  const int tile_n = bn < 0 ? -bn : bn;
-  g.nt = (g.N + tile_n - 1) / tile_n;
+  g.nt = (g.N + bn - 1) / bn;
   g.mt = m_tiles;
   g.nz = batch;
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  if (bn == 256 || bn == -128) {
-    int total = g.nt * ((g.mt + 1) / 2) * g.nz;
-    int npairs = total < sms / 2 ? total : sms / 2;
-    if (bn == 256) return launch_gemm2_t<256, 6>(a, b, g, npairs, s);
-    return launch_gemm2_t<128, 8>(a, b, g, npairs, s);
-  }
-  if (bn == 1128) {  // residual GEMMs of a batched forward: one CTA per SM, 6-stage ring, 16 epilogue warps (one chunk each)
-    g.nt = (g.N + 127) / 128;
-    int total = g.nt * g.mt * g.nz;
-    return launch_gemm_t<128, 6, 16>(a, b, g, dim3(total < sms ? total : sms, 1, 1), s);
-  }
-  // persistent grid: two CTAs per SM (97 KB smem, 2 x BN TMEM columns each), each walks its tiles
-  const int resident = 2 * sms;
-  int total = g.nt * g.mt * g.nz;
-  dim3 grid(total < resident ? total : resident, 1, 1);
+  // persistent grid: one CTA per SM (two consumer warpgroups, up to 144 KB of operand ring), each walks its tiles
+  const int total = g.nt * g.mt * g.nz, sms = sm_count();
+  dim3 grid(total < sms ? total : sms, 1, 1);
   switch (bn) {
-    case 128:
-      // <= one CTA per SM: a deeper operand ring (6 x 32 KB) keeps twice the TMA bytes in flight
-      if (total <= resident / 2) return launch_gemm_t<128, 6>(a, b, g, grid, s);
-      return launch_gemm_t<128, 3>(a, b, g, grid, s);
-    case 64: return launch_gemm_t<64, 4>(a, b, g, grid, s);
-    case 32: return launch_gemm_t<32, 4>(a, b, g, grid, s);
+    case 128: return launch_gemm_t<128, 4>(a, b, g, grid, s);
+    case 64: return launch_gemm_t<64, 6>(a, b, g, grid, s);
+    case 32: return launch_gemm_t<32, 6>(a, b, g, grid, s);
     default: return cudaErrorInvalidValue;
   }
 }

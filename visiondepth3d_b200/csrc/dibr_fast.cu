@@ -702,8 +702,8 @@ __global__ void __launch_bounds__(NT, 1) k_stats(StatsArgs a) {
 // ---------------------------------------------------------------------------------------------------------------
 // k_shift_fast: shift map + suppress_artifacts_with_edge_mask (core/render_3d.py:198-216, 620-680), fast arithmetic.
 // 64 x 16 pixels per CTA (4 per thread), sigmoid through ex2 / rcp approximations, the 5 x 5 pool as row sums then
-// column sums.  ~1/3 of the instructions of the one-pixel-per-thread exact kernel (which it replaced after ncu showed
-// that kernel 86-90 % issue-bound at 385 thread-instructions per pixel, profiles/r02_ncu_dibr.md).
+// column sums.  ~1/3 of the instructions of the one-pixel-per-thread exact kernel (385 thread-instructions per
+// pixel, issue bound).
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int SHX = 64, SHY = 16;
 __device__ __forceinline__ float sqrt_approx(float x) {

@@ -1,11 +1,11 @@
-// dibr_kernels.cuh -- sm_100a kernels of the DIBR (depth-image-based rendering) stage.
+// dibr_kernels.cuh -- sm_90a kernels of the DIBR (depth-image-based rendering) stage.
 //
 // Reference behaviour restated from core/render_3d.py (file:line cited per kernel);
 // arithmetic follows oracle/dibr.py one rounding at a time: this TU is compiled with
 // -fmad=false and uses __fmaf_rn exactly where torch / cv2 fuse (grid_sample and
 // bilinear accumulation, Gaussian conv and filter2D chains, linspace).
 //
-// Memory-bound design (B200: 148 SMs, ~6.5 TB/s HBM, 126 MB L2):
+// Memory-bound design (H100: 132 SMs, 3.35 TB/s HBM3, 50 MB L2):
 //   * u8 frames are consumed as they arrive (BGR interleaved) -- no f32 RGB planes
 //     are materialised on the identity-resize path (4K Full-SBS);
 //   * every intermediate (depth planes, shift map, edge masks, eyes) is written once

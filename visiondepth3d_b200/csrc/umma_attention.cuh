@@ -1,17 +1,17 @@
-// umma_attention.cuh -- fused multi-head attention for the ViT blocks on tcgen05.
+// umma_attention.cuh -- fused multi-head attention for the ViT blocks on Hopper wgmma.
 //
 //   O[m, :] = softmax_n(q[m] . k[n]) v[n]      head_dim 64, q pre-scaled by 1/sqrt(64)
 //
-// One CTA per (128-query block, head).  Scores never leave the SM: S = Q K^T is accumulated in
-// tensor memory (two 128-column buffers), the softmax warps read it with tcgen05.ld, and the
-// probabilities are written (f16, 128B-swizzled K-major) into shared memory where they are the
-// A operand of the second MMA, O += P V, whose accumulator also lives in TMEM.
-// Two passes over the keys (N <= 3072 here): pass A finds the exact row maximum, pass B
-// recomputes S, exponentiates against the final maximum and accumulates P V -- no online
-// rescaling of O, at the price of issuing the (cheap, K = 64) QK^T MMAs twice.
+// One CTA per (128-query block, head): two consumer warpgroups own 64 query rows each.  Scores never leave
+// the registers: S = Q K^T (wgmma m64n128k16, Q and K from shared memory) is accumulated in registers, the
+// online softmax runs on that fragment, and the probabilities are converted in place into f16 A fragments
+// of the second wgmma, O += P V (m64n64k16, A from registers, V^T from shared memory).
+// Online softmax in log2 units with an exact running maximum per row; each row lives in the four threads of
+// a quad, so row reductions are two shuffles.  Probabilities are expressed against (maximum - 8), so they lie in
+// (0, 256]: small weights stay out of the f16 subnormal range, and the row sum adds the same f16-rounded values that
+// enter P V, so numerator and denominator agree.
 //
-// warp 0: TMA producer (Q once; K tiles twice; V^T tiles once)   warp 1: MMA issuer + TMEM alloc
-// warps 2-9: softmax / epilogue (two threads per query row, 64 keys of every 128-key tile each)
+// warp 0: TMA producer (Q once; K and V^T tiles through a two-deep ring)   warps 4-11: two consumer warpgroups
 //
 // Replaces Dinov2SelfAttention (transformers 5.5 models/dinov2/modeling_dinov2.py) inside the depth
 // forward called from core/render_depth.py:1106-1119.
@@ -28,598 +28,34 @@ struct AttnArgs {
   int npad;     // rows per image in `out`
 };
 
-constexpr bool kAttnPolyExp = false;  // true: a third of the softmax exponentials on the FMA pipe (umma::ex2_poly) -- measured 2 % SLOWER (profiles/r01_ncu_full_final.md)
-constexpr int kAttnThreads = 320;  // warp 0 TMA, warp 1 MMA, warps 2-9 softmax (2 per TMEM lane quarter)
-// Two CTAs per SM (96 KB smem, 256 TMEM columns each) so one CTA's softmax overlaps the other's MMAs
-// and 240 CTAs (20 query blocks x 12 heads) fit in a single wave of 296 slots.
-constexpr int kAttnKS = 2, kAttnVS = 1, kAttnSB = 1, kAttnPB = 1;
-constexpr int kAttnTmemCols = 256;  // S: kAttnSB x 128, O: 64
-constexpr int kAttnSmem = 16384 /*Q*/ + kAttnKS * 16384 + kAttnVS * 16384 + kAttnPB * 32768 /*P*/ + 1024 + 512 + 2560;
+constexpr int kAttnThreads = 384;
+constexpr int kAttnKS = 2;  // K / V^T ring depth (128 keys per stage)
+constexpr int kAttnSmem = 16384 /*Q*/ + kAttnKS * (16384 /*K*/ + 16384 /*V^T*/) + 1024 /*align*/ + 256 /*barriers*/;
 
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-
-__global__ void __launch_bounds__(kAttnThreads, 2)
-k_umma_attention(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                 const __grid_constant__ CUtensorMap tmV, const AttnArgs g) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* sQ = smem;
-  uint8_t* sK = smem + 16384;
-  uint8_t* sV = sK + kAttnKS * 16384;
-  uint8_t* sP = sV + kAttnVS * 16384;
-  uint64_t* bars = (uint64_t*)(sP + kAttnPB * 32768);
-  uint64_t* q_full = bars;               // 1
-  uint64_t* k_full = bars + 1;           // KS
-  uint64_t* k_empty = k_full + kAttnKS;  // KS
-  uint64_t* v_full = k_empty + kAttnKS;  // VS
-  uint64_t* v_empty = v_full + kAttnVS;  // VS
-  uint64_t* s_full = v_empty + kAttnVS;  // 2
-  uint64_t* s_empty = s_full + 2;        // 2 (4 arrivals: one per softmax warp)
-  uint64_t* p_full = s_empty + 2;        // 2 (4 arrivals)
-  uint64_t* p_empty = p_full + 2;        // 2
-  uint64_t* o_full = p_empty + 2;        // 1
-  uint32_t* tmem_slot = (uint32_t*)(o_full + 1);
-  float* xch = (float*)(bars + 64);  // [2][128] row max / row sum exchange between the two half-row threads
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qblk = blockIdx.x, zq = blockIdx.y, h = zq % g.heads, img = zq / g.heads;
-  const int T = (g.ntok + 127) / 128;  // key tiles
-
-  if (warp == 0 && lane == 0) {
-    umma::prefetch_tmap(&tmQ);
-    umma::prefetch_tmap(&tmK);
-    umma::prefetch_tmap(&tmV);
-    umma::mbar_init(umma::smem_u32(q_full), 1);
-    for (int i = 0; i < kAttnKS; ++i) {
-      umma::mbar_init(umma::smem_u32(&k_full[i]), 1);
-      umma::mbar_init(umma::smem_u32(&k_empty[i]), 1);
-    }
-    for (int i = 0; i < kAttnVS; ++i) {
-      umma::mbar_init(umma::smem_u32(&v_full[i]), 1);
-      umma::mbar_init(umma::smem_u32(&v_empty[i]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {  // (slots beyond kAttnSB / kAttnPB are simply unused)
-      umma::mbar_init(umma::smem_u32(&s_full[i]), 1);
-      umma::mbar_init(umma::smem_u32(&s_empty[i]), 8);
-      umma::mbar_init(umma::smem_u32(&p_full[i]), 8);
-      umma::mbar_init(umma::smem_u32(&p_empty[i]), 1);
-    }
-    umma::mbar_init(umma::smem_u32(o_full), 1);
-    umma::fence_barrier_init();
-  }
-  if (warp == 1) umma::tmem_alloc(umma::smem_u32(tmem_slot), kAttnTmemCols);
-  umma::tc_fence_before();
-  __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S[2] = {tmem_base, tmem_base + 128};  // [1] only used when kAttnSB == 2
-  const uint32_t tmem_O = tmem_base + kAttnSB * 128;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      umma::mbar_expect_tx(umma::smem_u32(q_full), 16384);
-      umma::tma_load_3d(umma::smem_u32(sQ), &tmQ, umma::smem_u32(q_full), 0, qblk * 128, zq);
-      int kiter = 0;
-      for (int pass = 0; pass < 2; ++pass) {
-        for (int t = 0; t < T; ++t, ++kiter) {
-          const int ks = kiter % kAttnKS;
-          umma::mbar_wait(umma::smem_u32(&k_empty[ks]), ((kiter / kAttnKS) & 1) ^ 1);
-          umma::mbar_expect_tx(umma::smem_u32(&k_full[ks]), 16384);
-          umma::tma_load_3d(umma::smem_u32(sK + ks * 16384), &tmK, umma::smem_u32(&k_full[ks]), 0, t * 128, zq);
-          if (pass == 1) {
-            const int vs = t % kAttnVS;
-            umma::mbar_wait(umma::smem_u32(&v_empty[vs]), ((t / kAttnVS) & 1) ^ 1);
-            umma::mbar_expect_tx(umma::smem_u32(&v_full[vs]), 16384);
-            const uint32_t dst = umma::smem_u32(sV + vs * 16384);
-            umma::tma_load_3d(dst, &tmV, umma::smem_u32(&v_full[vs]), t * 128, 0, zq);
-            umma::tma_load_3d(dst + 8192, &tmV, umma::smem_u32(&v_full[vs]), t * 128 + 64, 0, zq);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma::make_idesc(128);
-      constexpr uint32_t idesc_o = umma::make_idesc(64);
-      umma::mbar_wait(umma::smem_u32(q_full), 0);
-      umma::tc_fence_after();
-      const uint64_t dq = umma::make_desc(umma::smem_u32(sQ));
-      int kiter = 0;
-      auto issue_S = [&](int gi) {  // gi: global S iteration 0 .. 2T-1
-        const int ks = kiter % kAttnKS;
-        umma::mbar_wait(umma::smem_u32(&k_full[ks]), (kiter / kAttnKS) & 1);
-        const int sb = gi % kAttnSB;
-        umma::mbar_wait(umma::smem_u32(&s_empty[sb]), ((gi / kAttnSB) & 1) ^ 1);
-        umma::tc_fence_after();
-        const uint64_t dk = umma::make_desc(umma::smem_u32(sK + ks * 16384));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma::mma_f16(tmem_S[sb], dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), idesc_s, k ? 1u : 0u);
-        umma::umma_commit(umma::smem_u32(&k_empty[ks]));
-        umma::umma_commit(umma::smem_u32(&s_full[sb]));
-        ++kiter;
-      };
-      // pass A: scores only (row maxima)
-      for (int t = 0; t < T; ++t) issue_S(t);
-      // pass B: scores again, then O += P V (S of tile t+1 is issued before waiting for P of tile t)
-      issue_S(T);
-      for (int t = 0; t < T; ++t) {
-        if (t + 1 < T) issue_S(T + t + 1);
-        const int pb = t % kAttnPB, vs = t % kAttnVS;
-        umma::mbar_wait(umma::smem_u32(&p_full[pb]), (t / kAttnPB) & 1);
-        umma::mbar_wait(umma::smem_u32(&v_full[vs]), (t / kAttnVS) & 1);
-        umma::tc_fence_after();
-        const uint32_t pa = umma::smem_u32(sP + pb * 32768);
-        const uint32_t va = umma::smem_u32(sV + vs * 16384);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint64_t da = umma::make_desc(pa + (kk >> 2) * 16384) + (uint64_t)(2 * (kk & 3));
-          const uint64_t db = umma::make_desc(va + (kk >> 2) * 8192) + (uint64_t)(2 * (kk & 3));
-          umma::mma_f16(tmem_O, da, db, idesc_o, (t | kk) ? 1u : 0u);
-        }
-        umma::umma_commit(umma::smem_u32(&v_empty[vs]));
-        umma::umma_commit(umma::smem_u32(&p_empty[pb]));
-      }
-      umma::umma_commit(umma::smem_u32(o_full));
-    }
-  } else {
-    // ===================== softmax / epilogue warps =====================
-    const int q = warp & 3;             // TMEM lane quarter (hardware: warp id % 4)
-    const int half = (warp - 2) >> 2;   // which 64 keys of every 128-key tile
-    const int r = q * 32 + lane;        // query row inside the block == TMEM lane
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const uint32_t col_off = (uint32_t)(half * 64);
-    float mx = -INFINITY;
-    // ---- pass A: exact row maximum ----
-    for (int gi = 0; gi < T; ++gi) {
-      const int sb = gi % kAttnSB;
-      umma::mbar_wait(umma::smem_u32(&s_full[sb]), (gi / kAttnSB) & 1);
-      umma::tc_fence_after();
-      const int nvalid = min(128, g.ntok - gi * 128) - half * 64;
-      {
-        uint32_t v[64];
-        umma::tmem_ld_32x64(tmem_S[sb] + lane_off + col_off, v);
-        if (nvalid >= 64) {  // full tile: no masking
-          float m0 = mx, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll
-          for (int j = 0; j < 64; j += 4) {
-            m0 = fmaxf(m0, __uint_as_float(v[j]));
-            m1 = fmaxf(m1, __uint_as_float(v[j + 1]));
-            m2 = fmaxf(m2, __uint_as_float(v[j + 2]));
-            m3 = fmaxf(m3, __uint_as_float(v[j + 3]));
-          }
-          mx = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-        } else {
-#pragma unroll
-          for (int j = 0; j < 64; ++j)
-            if (j < nvalid) mx = fmaxf(mx, __uint_as_float(v[j]));
-        }
-      }
-      umma::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(umma::smem_u32(&s_empty[sb]));
-    }
-    xch[half * 128 + r] = mx;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    mx = fmaxf(xch[r], xch[128 + r]);
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    // ---- pass B: p = exp(s - max), P -> smem (swizzled, A operand of the PV MMA) ----
-    float sum = 0.f;
-    const float mxl = mx * 1.4426950408889634f;
-    for (int t = 0; t < T; ++t) {
-      const int gi = T + t, sb = gi % kAttnSB, pb = t % kAttnPB;
-      umma::mbar_wait(umma::smem_u32(&s_full[sb]), (gi / kAttnSB) & 1);
-      umma::mbar_wait(umma::smem_u32(&p_empty[pb]), ((t / kAttnPB) & 1) ^ 1);
-      umma::tc_fence_after();
-      const int nvalid = min(128, g.ntok - t * 128) - half * 64;
-      uint8_t* pblk = sP + pb * 32768 + half * 16384 + (r >> 3) * 1024 + (r & 7) * 128;  // this row, this 64-key block
-      {
-        uint32_t v[64];
-        umma::tmem_ld_32x64(tmem_S[sb] + lane_off + col_off, v);
-        uint32_t pk[32];
-        const float L2E = 1.4426950408889634f;
-        if (nvalid >= 64) {  // full tile: one FFMA + MUFU.EX2 + FADD per score
-          float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-          for (int j = 0; j < 64; j += 2) {
-            float p0 = umma::ex2_fast(fmaf(__uint_as_float(v[j]), L2E, -mxl));
-            float p1 = umma::ex2_fast(fmaf(__uint_as_float(v[j + 1]), L2E, -mxl));
-            s0 += p0;
-            s1 += p1;
-            __half2 hp = __floats2half2_rn(p0, p1);
-            pk[j >> 1] = *(uint32_t*)&hp;
-          }
-          sum += s0 + s1;
-        } else {
-#pragma unroll
-          for (int j = 0; j < 64; j += 2) {
-            float p0 = (j < nvalid) ? umma::ex2_fast(fmaf(__uint_as_float(v[j]), L2E, -mxl)) : 0.f;
-            float p1 = (j + 1 < nvalid) ? umma::ex2_fast(fmaf(__uint_as_float(v[j + 1]), L2E, -mxl)) : 0.f;
-            sum += p0 + p1;
-            __half2 hp = __floats2half2_rn(p0, p1);
-            pk[j >> 1] = *(uint32_t*)&hp;
-          }
-        }
-#pragma unroll
-        for (int idx = 0; idx < 8; ++idx) {    // logical 16-byte chunk inside the 128-byte row
-          const int phys = idx ^ (r & 7);      // 128B swizzle
-          *(uint4*)(pblk + phys * 16) = make_uint4(pk[4 * idx], pk[4 * idx + 1], pk[4 * idx + 2], pk[4 * idx + 3]);
-        }
-      }
-      umma::fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      umma::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(umma::smem_u32(&s_empty[sb]));
-        mbar_arrive(umma::smem_u32(&p_full[pb]));
-      }
-    }
-    xch[half * 128 + r] = sum;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    sum = xch[r] + xch[128 + r];
-    // ---- epilogue: O / sum -> out[m, 64h + 32*half .. +31] ----
-    umma::mbar_wait(umma::smem_u32(o_full), 0);
-    umma::tc_fence_after();
-    const int m = qblk * 128 + r;
-    const float inv = 1.0f / sum;
-    {
-      uint32_t v[32];
-      umma::tmem_ld_32x32(tmem_O + lane_off + (uint32_t)(half * 32), v);
-      if (m < g.ntok) {
-        uint4* dst = (uint4*)(g.out + ((size_t)img * g.npad + m) * g.dmodel + h * 64 + half * 32);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          __half2 h0 = __floats2half2_rn(__uint_as_float(v[8 * i + 0]) * inv, __uint_as_float(v[8 * i + 1]) * inv);
-          __half2 h1 = __floats2half2_rn(__uint_as_float(v[8 * i + 2]) * inv, __uint_as_float(v[8 * i + 3]) * inv);
-          __half2 h2 = __floats2half2_rn(__uint_as_float(v[8 * i + 4]) * inv, __uint_as_float(v[8 * i + 5]) * inv);
-          __half2 h3 = __floats2half2_rn(__uint_as_float(v[8 * i + 6]) * inv, __uint_as_float(v[8 * i + 7]) * inv);
-          uint4 u;
-          u.x = *(uint32_t*)&h0;
-          u.y = *(uint32_t*)&h1;
-          u.z = *(uint32_t*)&h2;
-          u.w = *(uint32_t*)&h3;
-          dst[i] = u;
-        }
-      }
-    }
-  }
-  umma::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) umma::tmem_dealloc(tmem_base, kAttnTmemCols);
-}
-
-// ---------------------------------------------------------------------------
-// Single-pass variant (default): online softmax with LAZY rescaling.  The two-pass kernel above is
-// bound by tensor-memory read bandwidth (every score is read from TMEM twice, ~64 B/clk/SM); here S is
-// computed and read once.  Each row keeps a reference maximum m_ref; probabilities are 2^(s - m_ref) and
-// m_ref is only raised (and O, sum rescaled by 2^(m_ref_old - m_ref_new)) when the running maximum
-// exceeds it by more than 8 (log2 units), so p <= 256 stays comfortably inside f16 and rescales of the
-// TMEM accumulator (tcgen05.ld -> multiply -> tcgen05.st) are rare after the first tiles.
-// Two threads share a query row (64 keys of each tile each); their tile maxima are exchanged through
-// shared memory so both take the same rescale decision.
-// ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(kAttnThreads, 2)
-k_umma_attention_1p(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                    const __grid_constant__ CUtensorMap tmV, const AttnArgs g) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* sQ = smem;
-  uint8_t* sK = smem + 16384;
-  uint8_t* sV = sK + kAttnKS * 16384;
-  uint8_t* sP = sV + kAttnVS * 16384;
-  uint64_t* bars = (uint64_t*)(sP + kAttnPB * 32768);
-  uint64_t* q_full = bars;
-  uint64_t* k_full = bars + 1;
-  uint64_t* k_empty = k_full + kAttnKS;
-  uint64_t* v_full = k_empty + kAttnKS;
-  uint64_t* v_empty = v_full + kAttnVS;
-  uint64_t* s_full = v_empty + kAttnVS;
-  uint64_t* s_empty = s_full + 2;
-  uint64_t* p_full = s_empty + 2;
-  uint64_t* p_empty = p_full + 2;
-  uint64_t* o_full = p_empty + 2;
-  uint32_t* tmem_slot = (uint32_t*)(o_full + 1);
-  float* xch = (float*)(bars + 64);  // [2 buffers][2 halves][128 rows]
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qblk = blockIdx.x, zq = blockIdx.y, h = zq % g.heads, img = zq / g.heads;
-  const int T = (g.ntok + 127) / 128;
-
-  if (warp == 0 && lane == 0) {
-    umma::prefetch_tmap(&tmQ);
-    umma::prefetch_tmap(&tmK);
-    umma::prefetch_tmap(&tmV);
-    umma::mbar_init(umma::smem_u32(q_full), 1);
-    for (int i = 0; i < kAttnKS; ++i) {
-      umma::mbar_init(umma::smem_u32(&k_full[i]), 1);
-      umma::mbar_init(umma::smem_u32(&k_empty[i]), 1);
-    }
-    for (int i = 0; i < kAttnVS; ++i) {
-      umma::mbar_init(umma::smem_u32(&v_full[i]), 1);
-      umma::mbar_init(umma::smem_u32(&v_empty[i]), 1);
-    }
-    umma::mbar_init(umma::smem_u32(&s_full[0]), 1);
-    umma::mbar_init(umma::smem_u32(&s_empty[0]), 8);
-    umma::mbar_init(umma::smem_u32(&p_full[0]), 8);
-    umma::mbar_init(umma::smem_u32(&p_empty[0]), 1);
-    umma::mbar_init(umma::smem_u32(o_full), 1);
-    umma::fence_barrier_init();
-  }
-  if (warp == 1) umma::tmem_alloc(umma::smem_u32(tmem_slot), kAttnTmemCols);
-  umma::tc_fence_before();
-  __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base, tmem_O = tmem_base + 128;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      umma::mbar_expect_tx(umma::smem_u32(q_full), 16384);
-      umma::tma_load_3d(umma::smem_u32(sQ), &tmQ, umma::smem_u32(q_full), 0, qblk * 128, zq);
-      for (int t = 0; t < T; ++t) {
-        const int ks = t % kAttnKS, vs = t % kAttnVS;
-        umma::mbar_wait(umma::smem_u32(&k_empty[ks]), ((t / kAttnKS) & 1) ^ 1);
-        umma::mbar_expect_tx(umma::smem_u32(&k_full[ks]), 16384);
-        umma::tma_load_3d(umma::smem_u32(sK + ks * 16384), &tmK, umma::smem_u32(&k_full[ks]), 0, t * 128, zq);
-        umma::mbar_wait(umma::smem_u32(&v_empty[vs]), ((t / kAttnVS) & 1) ^ 1);
-        umma::mbar_expect_tx(umma::smem_u32(&v_full[vs]), 16384);
-        const uint32_t dst = umma::smem_u32(sV + vs * 16384);
-        umma::tma_load_3d(dst, &tmV, umma::smem_u32(&v_full[vs]), t * 128, 0, zq);
-        umma::tma_load_3d(dst + 8192, &tmV, umma::smem_u32(&v_full[vs]), t * 128 + 64, 0, zq);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma::make_idesc(128);
-      constexpr uint32_t idesc_o = umma::make_idesc(64);
-      umma::mbar_wait(umma::smem_u32(q_full), 0);
-      umma::tc_fence_after();
-      const uint64_t dq = umma::make_desc(umma::smem_u32(sQ));
-      auto issue_S = [&](int t) {
-        const int ks = t % kAttnKS;
-        umma::mbar_wait(umma::smem_u32(&k_full[ks]), (t / kAttnKS) & 1);
-        umma::mbar_wait(umma::smem_u32(&s_empty[0]), (t & 1) ^ 1);
-        umma::tc_fence_after();
-        const uint64_t dk = umma::make_desc(umma::smem_u32(sK + ks * 16384));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma::mma_f16(tmem_S, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), idesc_s, k ? 1u : 0u);
-        umma::umma_commit(umma::smem_u32(&k_empty[ks]));
-        umma::umma_commit(umma::smem_u32(&s_full[0]));
-      };
-      issue_S(0);
-      for (int t = 0; t < T; ++t) {
-        if (t + 1 < T) issue_S(t + 1);  // S of the next tile while the softmax warps work on this one
-        const int vs = t % kAttnVS;
-        umma::mbar_wait(umma::smem_u32(&p_full[0]), t & 1);
-        umma::mbar_wait(umma::smem_u32(&v_full[vs]), (t / kAttnVS) & 1);
-        umma::tc_fence_after();
-        const uint32_t pa = umma::smem_u32(sP);
-        const uint32_t va = umma::smem_u32(sV + vs * 16384);
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint64_t da = umma::make_desc(pa + (kk >> 2) * 16384) + (uint64_t)(2 * (kk & 3));
-          const uint64_t db = umma::make_desc(va + (kk >> 2) * 8192) + (uint64_t)(2 * (kk & 3));
-          umma::mma_f16(tmem_O, da, db, idesc_o, (t | kk) ? 1u : 0u);
-        }
-        umma::umma_commit(umma::smem_u32(&v_empty[vs]));
-        umma::umma_commit(umma::smem_u32(&p_empty[0]));
-      }
-      umma::umma_commit(umma::smem_u32(o_full));
-    }
-  } else {
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int r = q * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const uint32_t col_off = (uint32_t)(half * 64);
-    const float L2E = 1.4426950408889634f;
-    float m_ref = -INFINITY;  // reference maximum (log2 units) the probabilities are expressed against
-    float sum = 0.f;
-    for (int t = 0; t < T; ++t) {
-      umma::mbar_wait(umma::smem_u32(&s_full[0]), t & 1);
-      umma::tc_fence_after();
-      const int nvalid = min(128, g.ntok - t * 128) - half * 64;
-      uint32_t v[64];
-      umma::tmem_ld_32x64(tmem_S + lane_off + col_off, v);
-      // S is in registers: the MMA warp may overwrite the buffer with the next tile's scores
-      umma::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(umma::smem_u32(&s_empty[0]));
-      float mx = -INFINITY;
-      if (nvalid >= 64) {
-        float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < 64; j += 4) {
-          m0 = fmaxf(m0, __uint_as_float(v[j]));
-          m1 = fmaxf(m1, __uint_as_float(v[j + 1]));
-          m2 = fmaxf(m2, __uint_as_float(v[j + 2]));
-          m3 = fmaxf(m3, __uint_as_float(v[j + 3]));
-        }
-        mx = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-      } else {
-#pragma unroll
-        for (int j = 0; j < 64; ++j)
-          if (j < nvalid) mx = fmaxf(mx, __uint_as_float(v[j]));
-      }
-      float* xb = xch + (t & 1) * 256;
-      xb[half * 128 + r] = mx;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      const float m_tile = fmaxf(xb[r], xb[128 + r]) * L2E;  // both threads of the row see the same value
-      // lazy rescale: raise the reference only when it is exceeded by more than 2^8
-      float scale = 1.0f;
-      bool resc = false;
-      if (t == 0) {
-        m_ref = m_tile;
-      } else if (m_tile > m_ref + 8.0f) {
-        scale = umma::ex2_fast(m_ref - m_tile);
-        m_ref = m_tile;
-        resc = true;
-      }
-      // P buffer and the O accumulator are quiescent once the previous PV MMA has retired
-      umma::mbar_wait(umma::smem_u32(&p_empty[0]), (t & 1) ^ 1);
-      umma::tc_fence_after();
-      if (__any_sync(0xffffffffu, resc)) {
-#pragma unroll 1
-        for (int cc = 0; cc < 2; ++cc) {  // 16 columns at a time: 64 scores are live in registers
-          uint32_t o[16];
-          const uint32_t ta = tmem_O + lane_off + (uint32_t)(half * 32 + cc * 16);
-          umma::tmem_ld_32x16(ta, o);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) o[j] = __float_as_uint(__uint_as_float(o[j]) * scale);
-          umma::tmem_st_32x16(ta, o);
-        }
-        sum *= scale;
-      }
-      uint8_t* pblk = sP + half * 16384 + (r >> 3) * 1024 + (r & 7) * 128;
-      uint32_t pk[32];
-      if (nvalid >= 64) {
-        float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-        for (int j = 0; j < 64; j += 2) {
-          // one exponential in three on the FMA pipe (ex2_poly), the rest on the MUFU: the loop is MUFU bound otherwise
-          const float x0 = fmaf(__uint_as_float(v[j]), L2E, -m_ref);
-          const float x1 = fmaf(__uint_as_float(v[j + 1]), L2E, -m_ref);
-          const int sel = (j >> 1) % 3;
-          float p0 = (kAttnPolyExp && sel == 0) ? umma::ex2_poly(x0) : umma::ex2_fast(x0);
-          float p1 = (kAttnPolyExp && sel == 1) ? umma::ex2_poly(x1) : umma::ex2_fast(x1);
-          s0 += p0;
-          s1 += p1;
-          __half2 hp = __floats2half2_rn(p0, p1);
-          pk[j >> 1] = *(uint32_t*)&hp;
-        }
-        sum += s0 + s1;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 64; j += 2) {
-          float p0 = (j < nvalid) ? umma::ex2_fast(fmaf(__uint_as_float(v[j]), L2E, -m_ref)) : 0.f;
-          float p1 = (j + 1 < nvalid) ? umma::ex2_fast(fmaf(__uint_as_float(v[j + 1]), L2E, -m_ref)) : 0.f;
-          sum += p0 + p1;
-          __half2 hp = __floats2half2_rn(p0, p1);
-          pk[j >> 1] = *(uint32_t*)&hp;
-        }
-      }
-#pragma unroll
-      for (int idx = 0; idx < 8; ++idx) {
-        const int phys = idx ^ (r & 7);
-        *(uint4*)(pblk + phys * 16) = make_uint4(pk[4 * idx], pk[4 * idx + 1], pk[4 * idx + 2], pk[4 * idx + 3]);
-      }
-      umma::fence_proxy_async();
-      umma::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(umma::smem_u32(&p_full[0]));
-    }
-    float* xb = xch + (T & 1) * 256;
-    xb[half * 128 + r] = sum;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    sum = xb[r] + xb[128 + r];
-    umma::mbar_wait(umma::smem_u32(o_full), 0);
-    umma::tc_fence_after();
-    const int m = qblk * 128 + r;
-    const float inv = 1.0f / sum;
-    {
-      uint32_t v[32];
-      umma::tmem_ld_32x32(tmem_O + lane_off + (uint32_t)(half * 32), v);
-      if (m < g.ntok) {
-        uint4* dst = (uint4*)(g.out + ((size_t)img * g.npad + m) * g.dmodel + h * 64 + half * 32);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          __half2 h0 = __floats2half2_rn(__uint_as_float(v[8 * i + 0]) * inv, __uint_as_float(v[8 * i + 1]) * inv);
-          __half2 h1 = __floats2half2_rn(__uint_as_float(v[8 * i + 2]) * inv, __uint_as_float(v[8 * i + 3]) * inv);
-          __half2 h2 = __floats2half2_rn(__uint_as_float(v[8 * i + 4]) * inv, __uint_as_float(v[8 * i + 5]) * inv);
-          __half2 h3 = __floats2half2_rn(__uint_as_float(v[8 * i + 6]) * inv, __uint_as_float(v[8 * i + 7]) * inv);
-          uint4 u;
-          u.x = *(uint32_t*)&h0;
-          u.y = *(uint32_t*)&h1;
-          u.z = *(uint32_t*)&h2;
-          u.w = *(uint32_t*)&h3;
-          dst[i] = u;
-        }
-      }
-    }
-  }
-  umma::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) umma::tmem_dealloc(tmem_base, kAttnTmemCols);
-}
-
-
-// ---------------------------------------------------------------------------
-// Third generation of the single-pass kernel.  What the sampled profile of k_umma_attention_1p showed (profiles/
-// r02_ncu_depth.md): the 123 per-tile bookkeeping instructions of a softmax warp collect more stall samples (42 %) than
-// the max / exp loops (31 %): shared memory was addressed through GENERIC pointers (ST.E.128 / LD.E + MEMBAR.ALL.CTA
-// before the proxy fence), the two threads of a row exchanged their tile maximum through a named barrier every tile,
-// and the probabilities went through 8 stores + a proxy fence before the MMA warp could be signalled.
-//   MODE 0: same algorithm, shared memory addressed in the shared state space (STS / LDS)
-//   MODE 1: + one O accumulator per key half (O0 <- keys 0..63 of every tile, O1 <- keys 64..127): the two threads of a
-//           row keep INDEPENDENT running maxima / sums and are only combined in the epilogue -- no per-tile exchange
-//           (TMEM: S 128 + O0 64 + O1 64 columns)
-//   MODE 2: MODE 0 + probabilities written to TENSOR memory (tcgen05.st, f16 pairs, 64 columns) and consumed as the A
-//           operand of the PV MMA from there: no shared-memory stores, no proxy fence; the freed 32 KB hold a second
-//           V stage (TMEM: S 128 + O 64 + P 64 columns)
-// ---------------------------------------------------------------------------
 namespace umma {
-__device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+// reductions over the four threads of a quad: one fragment row
+__device__ __forceinline__ float quad_max(float x) {
+  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
+  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
 }
-__device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
-  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+__device__ __forceinline__ float quad_sum(float x) {
+  x += __shfl_xor_sync(0xffffffffu, x, 1);
+  return x + __shfl_xor_sync(0xffffffffu, x, 2);
 }
-__device__ __forceinline__ float lds_f32(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
-  return v;
-}
-// 2^x for x <= 16 on the FMA / ALU pipes, degree-3 minimax of 2^f on [-0.5, 0.5] (relative error 7.7e-5: below the f16
-// rounding of the probabilities it produces); see ex2_poly
-__device__ __forceinline__ float ex2_poly3(float x) {
-  x = fmaxf(x, -125.0f);
-  const float t = x + 12582912.0f;
-  const float f = x - (t - 12582912.0f);
-  float p = fmaf(f, 0.05511401f, 0.24260628f);
-  p = fmaf(f, p, 0.69327159f);
-  p = fmaf(f, p, 0.99992867f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-__device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
-  return v;
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: A is read from tensor memory (lane = row, two f16 of consecutive K per column)
-__device__ __forceinline__ void mma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *(uint32_t*)&h;
 }
 }  // namespace umma
 
-// POLY: of every 8 exponentials of a full tile, this many are evaluated on the FMA pipe (umma::ex2_poly3) instead of the
-// MUFU: the probabilities are rounded to f16 anyway, and the XU pipe is the kernel's first bound (16 results per clock
-// and SM: 1024 clocks per 128 x 128 tile against 512 for the two MMAs).
-template <int MODE, int POLY = 0>
-__global__ void __launch_bounds__(kAttnThreads, 2)
-k_umma_attention_v3(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                    const __grid_constant__ CUtensorMap tmV, const AttnArgs g) {
-  constexpr bool kSplitO = MODE == 1, kPTmem = MODE == 2;
-  constexpr int KS = 2, VS = kPTmem ? 2 : 1;
+__global__ void __launch_bounds__(kAttnThreads, 1)
+k_umma_attention(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                 const __grid_constant__ CUtensorMap tmV, const AttnArgs g) {
   extern __shared__ uint8_t smem_raw[];
-  // every shared-memory access below goes through 32-bit shared-space addresses (TMA / MMA descriptors, STS, LDS)
   const uint32_t sm = (umma::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sQ = sm, sK = sm + 16384, sV = sK + KS * 16384, sP = sV + VS * 16384;
-  const uint32_t bars = sP + (kPTmem ? 0 : 32768);
-  const uint32_t q_full = bars, k_full = bars + 8, k_empty = k_full + 8 * KS, v_full = k_empty + 8 * KS,
-                 v_empty = v_full + 8 * VS, s_full = v_empty + 8 * VS, s_empty = s_full + 8, p_full = s_empty + 8,
-                 p_empty = p_full + 8, o_full = p_empty + 8, tmem_slot = o_full + 8;
-  const uint32_t xch = bars + 512;  // [2 buffers][2 halves][128 rows] floats
+  const uint32_t sQ = sm, sK = sm + 16384, sV = sK + kAttnKS * 16384;
+  const uint32_t bars = sV + kAttnKS * 16384;
+  const uint32_t q_full = bars, kv_full = bars + 8, kv_empty = kv_full + 8 * kAttnKS;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int qblk = blockIdx.x, zq = blockIdx.y, h = zq % g.heads, img = zq / g.heads;
@@ -630,249 +66,127 @@ k_umma_attention_v3(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     umma::prefetch_tmap(&tmK);
     umma::prefetch_tmap(&tmV);
     umma::mbar_init(q_full, 1);
-    for (int i = 0; i < KS; ++i) {
-      umma::mbar_init(k_full + 8 * i, 1);
-      umma::mbar_init(k_empty + 8 * i, 1);
+    for (int i = 0; i < kAttnKS; ++i) {
+      umma::mbar_init(kv_full + 8 * i, 1);
+      umma::mbar_init(kv_empty + 8 * i, 2);  // one arrive per consumer warpgroup
     }
-    for (int i = 0; i < VS; ++i) {
-      umma::mbar_init(v_full + 8 * i, 1);
-      umma::mbar_init(v_empty + 8 * i, 1);
-    }
-    umma::mbar_init(s_full, 1);
-    umma::mbar_init(s_empty, 8);
-    umma::mbar_init(p_full, 8);
-    umma::mbar_init(p_empty, 1);
-    umma::mbar_init(o_full, 1);
     umma::fence_barrier_init();
   }
-  if (warp == 1) umma::tmem_alloc(tmem_slot, kAttnTmemCols);
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = umma::lds_u32(tmem_slot);
-  const uint32_t tmem_S = tmem_base, tmem_O = tmem_base + 128, tmem_O1 = tmem_base + 192, tmem_P = tmem_base + 192;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
       umma::mbar_expect_tx(q_full, 16384);
       umma::tma_load_3d(sQ, &tmQ, q_full, 0, qblk * 128, zq);
       for (int t = 0; t < T; ++t) {
-        const int ks = t % KS, vs = t % VS;
-        umma::mbar_wait(k_empty + 8 * ks, ((t / KS) & 1) ^ 1);
-        umma::mbar_expect_tx(k_full + 8 * ks, 16384);
-        umma::tma_load_3d(sK + ks * 16384, &tmK, k_full + 8 * ks, 0, t * 128, zq);
-        umma::mbar_wait(v_empty + 8 * vs, ((t / VS) & 1) ^ 1);
-        umma::mbar_expect_tx(v_full + 8 * vs, 16384);
-        const uint32_t dst = sV + vs * 16384;
-        umma::tma_load_3d(dst, &tmV, v_full + 8 * vs, t * 128, 0, zq);
-        umma::tma_load_3d(dst + 8192, &tmV, v_full + 8 * vs, t * 128 + 64, 0, zq);
+        const int ks = t % kAttnKS;
+        umma::mbar_wait(kv_empty + 8 * ks, ((t / kAttnKS) & 1) ^ 1);
+        const uint32_t fb = kv_full + 8 * ks;
+        umma::mbar_expect_tx(fb, 32768);
+        umma::tma_load_3d(sK + ks * 16384, &tmK, fb, 0, t * 128, zq);
+        const uint32_t dst = sV + ks * 16384;  // V^T: [64 dims][64 keys] twice (keys 0..63, 64..127 of the tile)
+        umma::tma_load_3d(dst, &tmV, fb, t * 128, 0, zq);
+        umma::tma_load_3d(dst + 8192, &tmV, fb, t * 128 + 64, 0, zq);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma::make_idesc(128);
-      constexpr uint32_t idesc_o = umma::make_idesc(64);
-      umma::mbar_wait(q_full, 0);
-      umma::tc_fence_after();
-      const uint64_t dq = umma::make_desc(sQ);
-      auto issue_S = [&](int t) {
-        const int ks = t % KS;
-        umma::mbar_wait(k_full + 8 * ks, (t / KS) & 1);
-        umma::mbar_wait(s_empty, (t & 1) ^ 1);
-        umma::tc_fence_after();
-        const uint64_t dk = umma::make_desc(sK + ks * 16384);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma::mma_f16(tmem_S, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), idesc_s, k ? 1u : 0u);
-        umma::umma_commit(k_empty + 8 * ks);
-        umma::umma_commit(s_full);
-      };
-      issue_S(0);
-      for (int t = 0; t < T; ++t) {
-        if (t + 1 < T) issue_S(t + 1);  // S of the next tile while the softmax warps work on this one
-        const int vs = t % VS;
-        umma::mbar_wait(p_full, t & 1);
-        umma::mbar_wait(v_full + 8 * vs, (t / VS) & 1);
-        umma::tc_fence_after();
-        const uint32_t va = sV + vs * 16384;
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint64_t db = umma::make_desc(va + (kk >> 2) * 8192) + (uint64_t)(2 * (kk & 3));
-          if (kPTmem) {
-            umma::mma_f16_ts(tmem_O, tmem_P + (uint32_t)(kk * 8), db, idesc_o, (t | kk) ? 1u : 0u);
-          } else {
-            const uint64_t da = umma::make_desc(sP + (kk >> 2) * 16384) + (uint64_t)(2 * (kk & 3));
-            if (kSplitO)
-              umma::mma_f16((kk < 4) ? tmem_O : tmem_O1, da, db, idesc_o, (t | (kk & 3)) ? 1u : 0u);
-            else
-              umma::mma_f16(tmem_O, da, db, idesc_o, (t | kk) ? 1u : 0u);
-          }
-        }
-        umma::umma_commit(v_empty + 8 * vs);
-        umma::umma_commit(p_empty);
-      }
-      umma::umma_commit(o_full);
-    }
-  } else {
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int r = q * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const uint32_t col_off = (uint32_t)(half * 64);
-    const float L2E = 1.4426950408889634f;
-    const uint32_t tmem_Oown = kSplitO ? (half ? tmem_O1 : tmem_O) : tmem_O;
-    float m_ref = -INFINITY;  // reference maximum (log2 units) the probabilities are expressed against
-    float sum = 0.f;
-    for (int t = 0; t < T; ++t) {
-      umma::mbar_wait(s_full, t & 1);
-      umma::tc_fence_after();
-      const int nvalid = min(128, g.ntok - t * 128) - half * 64;
-      uint32_t v[64];
-      umma::tmem_ld_32x64(tmem_S + lane_off + col_off, v);
-      // S is in registers: the MMA warp may overwrite the buffer with the next tile's scores
-      umma::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_empty);
-      float mx = -INFINITY;
-      if (nvalid >= 64) {
-        float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < 64; j += 4) {
-          m0 = fmaxf(m0, __uint_as_float(v[j]));
-          m1 = fmaxf(m1, __uint_as_float(v[j + 1]));
-          m2 = fmaxf(m2, __uint_as_float(v[j + 2]));
-          m3 = fmaxf(m3, __uint_as_float(v[j + 3]));
-        }
-        mx = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
-      } else {
-#pragma unroll
-        for (int j = 0; j < 64; ++j)
-          if (j < nvalid) mx = fmaxf(mx, __uint_as_float(v[j]));
-      }
-      float m_tile;
-      if (kSplitO) {
-        m_tile = mx * L2E;  // this thread's 64 keys only: its own accumulator, its own reference
-      } else {
-        const uint32_t xb = xch + (uint32_t)(t & 1) * 1024u;
-        umma::sts_f32(xb + (uint32_t)(half * 128 + r) * 4u, mx);
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        m_tile = fmaxf(umma::lds_f32(xb + (uint32_t)r * 4u), umma::lds_f32(xb + (uint32_t)(128 + r) * 4u)) * L2E;
-      }
-      // lazy rescale: raise the reference only when it is exceeded by more than 2^8
-      float scale = 1.0f;
-      bool resc = false;
-      if (t == 0) {
-        m_ref = m_tile;
-      } else if (m_tile > m_ref + 8.0f) {
-        scale = umma::ex2_fast(m_ref - m_tile);  // m_ref == -inf (no valid key so far): 0, the accumulator holds zeros
-        m_ref = m_tile;
-        resc = true;
-      }
-      // P buffer and the O accumulator(s) are quiescent once the previous PV MMA has retired
-      umma::mbar_wait(p_empty, (t & 1) ^ 1);
-      umma::tc_fence_after();
-      if (__any_sync(0xffffffffu, resc)) {
-        constexpr int kCols = kSplitO ? 64 : 32;  // columns of the accumulator this thread rescales
-#pragma unroll 1
-        for (int cc = 0; cc < kCols / 16; ++cc) {  // 16 columns at a time: 64 scores are live in registers
-          uint32_t o[16];
-          const uint32_t ta = tmem_Oown + lane_off + (uint32_t)((kSplitO ? 0 : half * 32) + cc * 16);
-          umma::tmem_ld_32x16(ta, o);
-#pragma unroll
-          for (int j = 0; j < 16; ++j) o[j] = __float_as_uint(__uint_as_float(o[j]) * scale);
-          umma::tmem_st_32x16(ta, o);
-        }
-        sum *= scale;
-      }
-      uint32_t pk[32];
-      if (nvalid >= 64) {
-        float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-        for (int j = 0; j < 64; j += 2) {
-          const float x0 = fmaf(__uint_as_float(v[j]), L2E, -m_ref), x1 = fmaf(__uint_as_float(v[j + 1]), L2E, -m_ref);
-          const float p0 = ((j & 7) < POLY) ? umma::ex2_poly3(x0) : umma::ex2_fast(x0);
-          const float p1 = ((j & 7) < POLY) ? umma::ex2_poly3(x1) : umma::ex2_fast(x1);
-          s0 += p0;
-          s1 += p1;
-          __half2 hp = __floats2half2_rn(p0, p1);
-          pk[j >> 1] = *(uint32_t*)&hp;
-        }
-        sum += s0 + s1;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 64; j += 2) {
-          float p0 = (j < nvalid) ? umma::ex2_fast(fmaf(__uint_as_float(v[j]), L2E, -m_ref)) : 0.f;
-          float p1 = (j + 1 < nvalid) ? umma::ex2_fast(fmaf(__uint_as_float(v[j + 1]), L2E, -m_ref)) : 0.f;
-          sum += p0 + p1;
-          __half2 hp = __floats2half2_rn(p0, p1);
-          pk[j >> 1] = *(uint32_t*)&hp;
-        }
-      }
-      if (kPTmem) {
-        // P[r, 64 half .. +63] as f16 pairs: 32 columns of the A operand of the PV MMA
-        umma::tmem_st_32x32(tmem_P + lane_off + (uint32_t)(half * 32), pk);
-      } else {
-        const uint32_t pblk = sP + (uint32_t)(half * 16384 + (r >> 3) * 1024 + (r & 7) * 128);
-#pragma unroll
-        for (int idx = 0; idx < 8; ++idx)  // logical 16-byte chunk idx of the 128-byte row, 128B swizzle
-          umma::sts_v4(pblk + (uint32_t)((idx ^ (r & 7)) * 16), pk[4 * idx], pk[4 * idx + 1], pk[4 * idx + 2], pk[4 * idx + 3]);
-        umma::fence_proxy_async();
-      }
-      umma::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-    }
-    // ---- epilogue: combine the two threads of a row, O / sum -> out[m, 64h + 32*half .. +31] ----
-    const uint32_t xb = kSplitO ? xch : xch + (uint32_t)(T & 1) * 1024u;  // (split mode never used xch before)
-    umma::sts_f32(xb + (uint32_t)(half * 128 + r) * 4u, sum);
-    if (kSplitO) umma::sts_f32(xb + 1024u + (uint32_t)(half * 128 + r) * 4u, m_ref);
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    float w0 = 1.f, w1 = 1.f;
-    const float s_a = umma::lds_f32(xb + (uint32_t)r * 4u), s_b = umma::lds_f32(xb + (uint32_t)(128 + r) * 4u);
-    if (kSplitO) {
-      const float ma = umma::lds_f32(xb + 1024u + (uint32_t)r * 4u), mb = umma::lds_f32(xb + 1024u + (uint32_t)(128 + r) * 4u);
-      const float mm = fmaxf(ma, mb);  // half 0 always holds a valid key: finite
-      w0 = umma::ex2_fast(ma - mm);
-      w1 = umma::ex2_fast(mb - mm);    // -inf (no valid key in this half at all) -> 0
-    }
-    const float inv = 1.0f / (w0 * s_a + w1 * s_b);
-    umma::mbar_wait(o_full, 0);
-    umma::tc_fence_after();
-    const int m = qblk * 128 + r;
-    {
-      uint32_t va[32];
-      umma::tmem_ld_32x32(tmem_O + lane_off + (uint32_t)(half * 32), va);
-      float o[32];
-      if (kSplitO) {
-        uint32_t vb[32];
-        umma::tmem_ld_32x32(tmem_O1 + lane_off + (uint32_t)(half * 32), vb);
-        const float wa = w0 * inv, wb = w1 * inv;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = fmaf(__uint_as_float(va[i]), wa, __uint_as_float(vb[i]) * wb);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = __uint_as_float(va[i]) * inv;
-      }
-      if (m < g.ntok) {
-        uint4* dst = (uint4*)(g.out + ((size_t)img * g.npad + m) * g.dmodel + h * 64 + half * 32);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          __half2 h0 = __floats2half2_rn(o[8 * i + 0], o[8 * i + 1]);
-          __half2 h1 = __floats2half2_rn(o[8 * i + 2], o[8 * i + 3]);
-          __half2 h2 = __floats2half2_rn(o[8 * i + 4], o[8 * i + 5]);
-          __half2 h3 = __floats2half2_rn(o[8 * i + 6], o[8 * i + 7]);
-          uint4 u;
-          u.x = *(uint32_t*)&h0;
-          u.y = *(uint32_t*)&h1;
-          u.z = *(uint32_t*)&h2;
-          u.w = *(uint32_t*)&h3;
-          dst[i] = u;
-        }
-      }
-    }
+    return;
   }
-  umma::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) umma::tmem_dealloc(tmem_base, kAttnTmemCols);
+
+  const int wg = (warp >> 2) - 1;
+  const int wq = warp & 3;
+  const float L2E = 1.4426950408889634f;
+  // this thread's rows of the fragments: 64 wg + 16 wq + lane/4 (+8); its key / dim columns: 8 j + 2 (lane & 3) (+1)
+  const int cq = 2 * (lane & 3);
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+  umma::mbar_wait(q_full, 0);
+  const uint64_t dq = umma::make_desc(sQ + (uint32_t)(wg * 64 * 128));
+  for (int t = 0; t < T; ++t) {
+    const int ks = t % kAttnKS;
+    umma::mbar_wait(kv_full + 8 * ks, (t / kAttnKS) & 1);
+    float s[64];
+    {
+      const uint64_t dk = umma::make_desc(sK + ks * 16384);
+      umma::wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) umma::wgmma_m64n128_ss(s, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k), k ? 1u : 0u);
+      umma::wgmma_commit();
+      umma::wgmma_wait<0>();
+      umma::fence_regs(s);
+    }
+    const int nvalid = g.ntok - t * 128;  // keys of this tile that exist
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if (nvalid < 128 && 8 * j + cq + (i & 1) >= nvalid) s[4 * j + i] = -INFINITY;
+        mx[i >> 1] = fmaxf(mx[i >> 1], s[4 * j + i]);
+      }
+    float scale[2], mref[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const float m_new = fmaxf(m_run[rr], umma::quad_max(mx[rr]) * L2E);  // tile 0 always holds a valid key: finite
+      scale[rr] = umma::ex2_fast(m_run[rr] - m_new);                      // -inf - finite -> 0
+      m_run[rr] = m_new;
+      mref[rr] = m_new - 8.0f;
+    }
+    float ls[2] = {0.f, 0.f};
+    uint32_t p[32];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const float p0 = umma::ex2_fast(fmaf(s[4 * j + 0], L2E, -mref[0]));
+      const float p1 = umma::ex2_fast(fmaf(s[4 * j + 1], L2E, -mref[0]));
+      const float p2 = umma::ex2_fast(fmaf(s[4 * j + 2], L2E, -mref[1]));
+      const float p3 = umma::ex2_fast(fmaf(s[4 * j + 3], L2E, -mref[1]));
+      p[2 * j] = umma::pack_h2(p0, p1);      // row r
+      p[2 * j + 1] = umma::pack_h2(p2, p3);  // row r + 8
+      const float2 h0 = __half22float2(*(const __half2*)&p[2 * j]), h1 = __half22float2(*(const __half2*)&p[2 * j + 1]);
+      ls[0] += h0.x + h0.y;
+      ls[1] += h1.x + h1.y;
+    }
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) l_run[rr] = l_run[rr] * scale[rr] + ls[rr];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      o[4 * j + 0] *= scale[0];
+      o[4 * j + 1] *= scale[0];
+      o[4 * j + 2] *= scale[1];
+      o[4 * j + 3] *= scale[1];
+    }
+    // O += P V: k-slice kk covers keys 16 kk .. 16 kk + 15 of the tile; its A fragment is S columns 16 kk + cq (+1)
+    // and 16 kk + 8 + cq (+1) of rows r and r + 8 -- the accumulator fragments j = 2 kk and 2 kk + 1
+    umma::fence_regs(o);
+    umma::wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      const uint32_t a[4] = {p[4 * kk], p[4 * kk + 1], p[4 * kk + 2], p[4 * kk + 3]};
+      const uint64_t db = umma::make_desc(sV + ks * 16384 + (kk >> 2) * 8192) + (uint64_t)(2 * (kk & 3));
+      umma::wgmma_m64n64_rs(o, a, db, 1u);
+    }
+    umma::wgmma_commit();
+    umma::wgmma_wait<0>();
+    umma::fence_regs(o);
+    if ((threadIdx.x & 127) == 0) umma::mbar_arrive(kv_empty + 8 * ks);
+  }
+
+  // ---- epilogue: O / sum -> out[m, 64h .. 64h + 63] ----
+  float inv[2];
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) inv[rr] = 1.0f / umma::quad_sum(l_run[rr]);
+  const int r0 = qblk * 128 + wg * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int m = r0 + 8 * rr;
+    if (m >= g.ntok) continue;
+    __half* dst = g.out + ((size_t)img * g.npad + m) * g.dmodel + h * 64 + cq;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      *(uint32_t*)(dst + 8 * j) = umma::pack_h2(o[4 * j + 2 * rr] * inv[rr], o[4 * j + 2 * rr + 1] * inv[rr]);
+  }
 }
 
 }  // namespace vd3d

@@ -1,14 +1,16 @@
-// umma_gemm.cuh -- hand-written sm_100a GEMM on the 5th-gen tensor cores.
+// umma_gemm.cuh -- hand-written sm_90a GEMM on the Hopper tensor cores (wgmma).
 //
-//   D[M,N] (fp32 in TMEM) = A[M,K] (f16, K-major) x B[N,K]^T (f16, K-major)
+//   D[M,N] (fp32 in registers) = A[M,K] (f16, K-major) x B[N,K]^T (f16, K-major)
 //
 // * operands staged by TMA (cp.async.bulk.tensor, 128B swizzle) into a STAGES-deep
-//   shared-memory ring guarded by mbarriers;
-// * one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN, K=16),
-//   accumulating in tensor memory; tcgen05.commit releases ring slots / signals the epilogue;
-// * four epilogue warps read the accumulator with tcgen05.ld (32 lanes x 32 columns per
-//   warp) and apply the fused epilogue (bias, GELU, LayerScale+residual, QKV head split with
-//   V transposed, pixel-shuffle for ConvTranspose, ReLU / residual for convs, DPT head).
+//   shared-memory ring guarded by mbarriers; one producer warp issues the loads;
+// * two consumer warpgroups each own 64 rows of the 128 x BN tile and issue
+//   wgmma.mma_async m64nBNk16 (A and B read from shared memory through matrix descriptors),
+//   accumulating in registers; a ring slot is released once the wgmmas reading it retired;
+// * the accumulator is staged through shared memory so that one thread owns 32 consecutive
+//   columns of one row, and the fused epilogue (bias, GELU, LayerScale+residual, QKV head
+//   split with V transposed, pixel-shuffle for ConvTranspose, ReLU / residual for convs,
+//   DPT head) runs on that chunk.
 // * A can also be an NHWC activation read through a 3-D tensor map (C, W, H): the K loop
 //   then walks the 3x3 taps and channel blocks (implicit GEMM); out-of-image taps are
 //   zero-filled by TMA, so no im2col buffer and no padding copies exist.
@@ -64,9 +66,8 @@ struct GemmArgs {
   // EPI_HEAD
   const float* w3;
   const float* b3p;
-  // tuning hook (vd3d_gemm_bench), low 3 bits: 0 = normal, 1 = skip the MMAs (operand-feed rate), 2 = skip the TMA
-  // loads (MMA rate), 3 = prologue + teardown only, 4 = epilogue only hands the accumulator back, 5 = epilogue
-  // reads TMEM but stores nothing; bit 3 (8): poll barriers with test_wait instead of try_wait
+  // tuning hook (vd3d_gemm_bench), low 3 bits: 0 = normal, 2 = skip the TMA loads (MMA rate), 3 = prologue +
+  // teardown only, 4 = no epilogue; bit 3 (8): poll barriers with test_wait instead of try_wait
   int dbg;
 };
 
@@ -79,6 +80,9 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   asm volatile(
@@ -116,14 +120,7 @@ __device__ __forceinline__ void mbar_wait_dbg(uint32_t bar, uint32_t parity, int
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"((uint64_t)tm), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1,
                                             int c2) {
   asm volatile(
@@ -135,140 +132,105 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)tm) : "memory");
 }
 
-// K-major, 128B-swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
-// start>>4 | LBO(=1, unused for swizzled K-major)<<16 | SBO(1024B>>4)<<32 | version 1<<46 | SWIZZLE_128B(2)<<61
+// K-major, 128B-swizzle wgmma matrix descriptor: start>>4 | LBO(=1, unused for swizzled K-major)<<16 |
+// SBO(1024 B = 8 rows of 128 B)>>4 <<32 | layout SWIZZLE_128B (1) <<62.  Advancing 16 f16 along K inside the
+// swizzle atom adds 32 B (+2 in 16-byte units) to the start address.
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// cute::UMMA::InstrDescriptor for kind::f16: D=f32, A=B=f16, both K-major, M=128, N=BN
-__host__ __device__ constexpr uint32_t make_idesc(int n) {
-  return (1u << 4) /*c_format f32*/ | (0u << 7) /*a f16*/ | (0u << 10) /*b f16*/ | (0u << 15) | (0u << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
+// keeps the compiler from moving accumulator reads / writes across a wgmma_wait
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// eight consecutive accumulator registers as read-write asm operands
+#define VD3D_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                     "+f"(d[i + 6]), "+f"(d[i + 7])
+// D[64 x 32] (+)= A[64 x 16] (smem desc) * B[32 x 16]^T (smem desc); both operands K-major
+__device__ __forceinline__ void wgmma_m64n32_ss(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : VD3D_ACC8(0), VD3D_ACC8(8)
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// D[64 x 64] (+)= A[64 x 16] (smem desc) * B[64 x 16]^T (smem desc); both operands K-major
+__device__ __forceinline__ void wgmma_m64n64_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : VD3D_ACC8(0), VD3D_ACC8(8), VD3D_ACC8(16), VD3D_ACC8(24)
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// D[64 x 128] (+)= A[64 x 16] (smem desc) * B[128 x 16]^T (smem desc); both operands K-major
+__device__ __forceinline__ void wgmma_m64n128_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : VD3D_ACC8(0), VD3D_ACC8(8), VD3D_ACC8(16), VD3D_ACC8(24), VD3D_ACC8(32), VD3D_ACC8(40), VD3D_ACC8(48), VD3D_ACC8(56)
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// D[64 x 64] (+)= A[64 x 16] (f16 registers, accumulator fragment layout) * B[64 x 16]^T (smem desc, K-major)
+__device__ __forceinline__ void wgmma_m64n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n"
+      "}\n"
+      : VD3D_ACC8(0), VD3D_ACC8(8), VD3D_ACC8(16), VD3D_ACC8(24)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// 32 lanes x 32 fp32 columns -> 32 registers per thread (thread = lane = accumulator row)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// accumulator tile (64 x N) of one warpgroup, K = 16 per instruction, both operands in shared memory
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (N == 32) wgmma_m64n32_ss(d, da, db, accumulate);
+  else if constexpr (N == 64) wgmma_m64n64_ss(d, da, db, accumulate);
+  else wgmma_m64n128_ss(d, da, db, accumulate);
 }
 
-// 32 lanes x 64 fp32 columns -> 64 registers per thread
-__device__ __forceinline__ void tmem_ld_32x64(uint32_t taddr, uint32_t (&v)[64]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x64.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31]),
-        "=r"(v[32]), "=r"(v[33]), "=r"(v[34]), "=r"(v[35]), "=r"(v[36]), "=r"(v[37]), "=r"(v[38]), "=r"(v[39]),
-        "=r"(v[40]), "=r"(v[41]), "=r"(v[42]), "=r"(v[43]), "=r"(v[44]), "=r"(v[45]), "=r"(v[46]), "=r"(v[47]),
-        "=r"(v[48]), "=r"(v[49]), "=r"(v[50]), "=r"(v[51]), "=r"(v[52]), "=r"(v[53]), "=r"(v[54]), "=r"(v[55]),
-        "=r"(v[56]), "=r"(v[57]), "=r"(v[58]), "=r"(v[59]), "=r"(v[60]), "=r"(v[61]), "=r"(v[62]), "=r"(v[63])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// registers -> TMEM, 32 lanes x 32 fp32 columns (used to rescale the attention output accumulator)
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-        "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-        "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-        "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-// 16-column variants (keep register pressure low where a whole 32/64-column chunk is already live)
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-        "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ float ex2_fast(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
 
-// 2^x on the FMA / ALU pipes (no MUFU): x = n + f with n = round(x) taken from the low mantissa bits of x + 1.5 * 2^23,
-// degree-4 minimax of 2^f on [-0.5, 0.5] (relative error 2.7e-6 in fp32), n added to the exponent field.  Valid for
-// -125 <= x < 2^21 (clamped below).  The attention softmax runs a third of its exponentials here: ex2.approx issues at
-// a quarter of a warp per SM sub-partition clock on B200 and was the kernel's bound (ncu: XU pipe 71 % of elapsed).
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -125.0f);
-  const float t = x + 12582912.0f;
-  const float f = x - (t - 12582912.0f);
-  float p = fmaf(f, 0.009570102207362652f, 0.05591785907745361f);
-  p = fmaf(f, p, 0.240247443318367f);
-  p = fmaf(f, p, 0.6931217908859253f);
-  p = fmaf(f, p, 0.9999992847442627f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-
 // GELU(x) = 0.5 x (1 + erf(x / sqrt 2)), exact-erf form as in HF's "gelu".  erfc(z) for z >= 0 from Abramowitz-Stegun
 // 7.1.26 (|error| <= 1.5e-7): erfc(z) = t (a1 + t (a2 + t (a3 + t (a4 + t a5)))) exp(-z^2), t = 1 / (1 + p z), and
 // GELU(x) = max(x, 0) - 0.5 |x| erfc(|x| / sqrt 2)  (no cancellation for x < 0).  ~14 FP32 ops + 2 MUFU instead of
-// the ~45 of erff(): the fc1 epilogue was ALU bound on erff (tools/gemm_sweep.py).  Output is stored as f16.
+// the ~45 of erff(): the fc1 epilogue is ALU bound on erff.  Output is stored as f16.
 __device__ __forceinline__ float gelu_erf(float x) {
   const float ax = fabsf(x);
   const float z = ax * 0.70710678118654752440f;
@@ -283,19 +245,22 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaf(-0.5f * ax * p, e, fmaxf(x, 0.f));
 }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.256): one full 32-byte sector per thread and instruction
+// 32-byte global accesses as two 128-bit instructions (the widest Hopper has)
 __device__ __forceinline__ void ldg_v8(const void* p, uint32_t (&r)[8]) {
-  asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
+  asm volatile("ld.global.v4.b32 {%0, %1, %2, %3}, [%8];\n\t"
+               "ld.global.v4.b32 {%4, %5, %6, %7}, [%8+16];"
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
                : "l"(p));
 }
 __device__ __forceinline__ void ldg_nc_v8(const void* p, uint32_t (&r)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
+  asm volatile("ld.global.nc.v4.b32 {%0, %1, %2, %3}, [%8];\n\t"
+               "ld.global.nc.v4.b32 {%4, %5, %6, %7}, [%8+16];"
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
                : "l"(p));
 }
 __device__ __forceinline__ void stg_v8(void* p, const uint32_t (&r)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]),
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};\n\t"
+               "st.global.v4.b32 [%0+16], {%5, %6, %7, %8};" ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]),
                "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
                : "memory");
 }
@@ -315,44 +280,8 @@ __device__ __forceinline__ void pack16(const float (&a)[32], int base, bool relu
 
 }  // namespace umma
 
-// proj / fc2 epilogue (EPI_RESID_LS) split in two so that the read of the fp32 residual stream -- which does not depend on
-// the MMAs -- can be issued BEFORE the accumulator is complete: issued after tmem_full, its ~1.5 us of L2 latency per
-// chunk was exposed twice per tile (proj, K = 768, spends 1.6 us per tile in the MMAs).
-__device__ __forceinline__ bool resid_split_ok(const GemmArgs& g) {
-  return g.epi == EPI_RESID_LS && (g.N & 31) == 0 && (g.ldc & 7) == 0 && g.bias != nullptr && g.conv == 0;
-}
-__device__ __forceinline__ void resid_load(const GemmArgs& g, const int m, const int n0, uint32_t (&x)[32]) {
-  const float* src = g.out_f32 + (size_t)m * g.ldc + n0;
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(x[8 * j]), "=r"(x[8 * j + 1]), "=r"(x[8 * j + 2]), "=r"(x[8 * j + 3]), "=r"(x[8 * j + 4]),
-                   "=r"(x[8 * j + 5]), "=r"(x[8 * j + 6]), "=r"(x[8 * j + 7])
-                 : "l"(src + 8 * j));
-}
-// x[m, n0 .. n0+31] = x + ls * (acc + bias), x already in registers
-__device__ __forceinline__ void resid_apply_store(const GemmArgs& g, const uint32_t (&v)[32], const int m, const int n0,
-                                                  uint32_t (&x)[32]) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const float4 b4 = __ldg((const float4*)(g.bias + n0) + j);
-    const float4 l4 = __ldg((const float4*)(g.ls + n0) + j);
-    x[4 * j + 0] = __float_as_uint(fmaf(l4.x, __uint_as_float(v[4 * j + 0]) + b4.x, __uint_as_float(x[4 * j + 0])));
-    x[4 * j + 1] = __float_as_uint(fmaf(l4.y, __uint_as_float(v[4 * j + 1]) + b4.y, __uint_as_float(x[4 * j + 1])));
-    x[4 * j + 2] = __float_as_uint(fmaf(l4.z, __uint_as_float(v[4 * j + 2]) + b4.z, __uint_as_float(x[4 * j + 2])));
-    x[4 * j + 3] = __float_as_uint(fmaf(l4.w, __uint_as_float(v[4 * j + 3]) + b4.w, __uint_as_float(x[4 * j + 3])));
-  }
-  float* dst = g.out_f32 + (size_t)m * g.ldc + n0;
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst + 8 * j), "r"(x[8 * j]),
-                 "r"(x[8 * j + 1]), "r"(x[8 * j + 2]), "r"(x[8 * j + 3]), "r"(x[8 * j + 4]), "r"(x[8 * j + 5]),
-                 "r"(x[8 * j + 6]), "r"(x[8 * j + 7])
-                 : "memory");
-}
-
 // Fused epilogue of one 32-column chunk of one accumulator row (thread == row): v = raw fp32 accumulator bits,
-// m = logical output row, n0 = first output column.  Shared by the 1-CTA and the CTA-pair kernels; every
+// m = logical output row, n0 = first output column.  Every
 // register array is indexed with compile-time constants only so the chunk stays in registers.
 __device__ __forceinline__ void gemm_epilogue_chunk(const GemmArgs& g, const uint32_t (&v)[32], const int m, const int z,
                                                     const int n0, const bool row_ok, float& head_acc) {
@@ -538,32 +467,33 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmArgs& g, const uin
   }
 }
 
-constexpr int kGemmThreads = 320;  // warp 0: TMA, warp 1: MMA + TMEM alloc, warps 2-9: epilogue (2 per lane quarter)
-constexpr int kBK = 64;            // 64 f16 = 128 B = one swizzle row
+// warp 0: TMA producer; warps 4-11: two consumer warpgroups (64 accumulator rows each).  Warps 1-3 only fill the
+// producer's warpgroup so that the consumers are whole, aligned warpgroups.
+constexpr int kGemmThreads = 384;
+constexpr int kBK = 64;  // 64 f16 = 128 B = one swizzle row
+constexpr int kPromote = 4;  // k-blocks (K = 256) per tensor-core accumulation group
 
 template <int BN, int STAGES>
 struct GemmSmem {
   static constexpr int kABytes = 128 * kBK * 2;
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStage = kABytes + kBBytes;
-  static constexpr int kTotal = STAGES * kStage + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kPitch = BN + 4;  // floats per staged row (+4: no bank conflicts on the row reads)
+  static constexpr int kEpi = 2 * 64 * kPitch * 4;  // one 64 x BN fp32 staging tile per consumer warpgroup
+  static constexpr int kTotal = STAGES * kStage + kEpi + 1024 /*align*/ + 256 /*barriers*/;
 };
 
-// EW: epilogue warps (8: two per TMEM lane quarter, two CTAs per SM; 16: four per quarter for the one-CTA-per-SM launches
-// of the residual GEMMs, where every warp owns ONE chunk of a tile and prefetches its slice of the residual stream)
-template <int BN, int STAGES, int EW = 8>
-__global__ void __launch_bounds__(64 + 32 * EW, EW == 8 ? 0 : 1)
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(kGemmThreads, 1)
 k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs g) {
   using S = GemmSmem<BN, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for SWIZZLE_128B
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = (uint64_t*)(smem + STAGES * S::kStage);
+  float* epi_buf = (float*)(smem + STAGES * S::kStage);
+  uint64_t* bars = (uint64_t*)(smem + STAGES * S::kStage + S::kEpi);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES;   // [2] accumulator stage complete (MMA -> epilogue)
-  uint64_t* tmem_empty = bars + 2 * STAGES + 2;  // [2] accumulator stage drained (epilogue -> MMA)
-  uint32_t* tmem_slot = (uint32_t*)(bars + 2 * STAGES + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -577,19 +507,11 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     umma::prefetch_tmap(&tmB);
     for (int s = 0; s < STAGES; ++s) {
       umma::mbar_init(umma::smem_u32(&full[s]), 1);
-      umma::mbar_init(umma::smem_u32(&empty[s]), 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      umma::mbar_init(umma::smem_u32(&tmem_full[i]), 1);
-      umma::mbar_init(umma::smem_u32(&tmem_empty[i]), EW);
+      umma::mbar_init(umma::smem_u32(&empty[s]), 2);  // one arrive per consumer warpgroup
     }
     umma::fence_barrier_init();
   }
-  if (warp == 1) umma::tmem_alloc(umma::smem_u32(tmem_slot), 2 * BN);  // two accumulator stages
-  umma::tc_fence_before();
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   auto decode = [&](int tile, int& n_blk, int& m_blk, int& z, int& px0, int& py0) {
     n_blk = tile % g.nt;
@@ -606,137 +528,133 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
   if (dmode == 3) {
     // tuning: prologue + teardown only
-  } else if (warp == 0) {
+  } else if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");  // hand registers to the consumer warpgroups
+    if (warp == 0 && lane == 0) {
       int kit = 0;  // k-block counter across tiles (ring position)
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      int n_blk, m_blk, z, px0, py0;
-      decode(tile, n_blk, m_blk, z, px0, py0);
-      for (int kb = 0; kb < nkb; ++kb, ++kit) {
-        const int s = kit % STAGES;
-        const uint32_t ph = (kit / STAGES) & 1;
-        umma::mbar_wait_dbg(umma::smem_u32(&empty[s]), ph ^ 1, spin);
-        const uint32_t fb = umma::smem_u32(&full[s]);
-        if (dmode == 2) {
-          asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(fb) : "memory");
-          continue;
-        }
-        umma::mbar_expect_tx(fb, S::kStage);
-        const uint32_t sa = umma::smem_u32(smem + s * S::kStage);
-        const uint32_t sb = sa + S::kABytes;
-        if (g.conv == 0) {
-          umma::tma_load_3d(sa, &tmA, fb, kb * kBK, m_blk * 128, z);
-        } else {
-          const int cblocks = g.cin / kBK;
-          const int tap = kb / cblocks, cb = kb % cblocks;
-          int dx = 0, dy = 0;
-          if (g.conv == 1) {
-            dy = tap / 3 - 1;
-            dx = tap % 3 - 1;
+        int n_blk, m_blk, z, px0, py0;
+        decode(tile, n_blk, m_blk, z, px0, py0);
+        for (int kb = 0; kb < nkb; ++kb, ++kit) {
+          const int s = kit % STAGES;
+          const uint32_t ph = (kit / STAGES) & 1;
+          umma::mbar_wait_dbg(umma::smem_u32(&empty[s]), ph ^ 1, spin);
+          const uint32_t fb = umma::smem_u32(&full[s]);
+          if (dmode == 2) {
+            umma::mbar_arrive(fb);
+            continue;
           }
-          umma::tma_load_3d(sa, &tmA, fb, cb * kBK, px0 + dx, py0 + dy);
-        }
-        umma::tma_load_3d(sb, &tmB, fb, kb * kBK, n_blk * BN, z);
-      }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma::make_idesc(BN);
-      int kit = 0, it = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;  // accumulator stage
-      umma::mbar_wait_dbg(umma::smem_u32(&tmem_empty[as]), ((it >> 1) & 1) ^ 1, spin);
-      umma::tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + (uint32_t)(as * BN);
-      for (int kb = 0; kb < nkb; ++kb, ++kit) {
-        const int s = kit % STAGES;
-        const uint32_t ph = (kit / STAGES) & 1;
-        umma::mbar_wait_dbg(umma::smem_u32(&full[s]), ph, spin);
-        umma::tc_fence_after();
-        const uint32_t sa = umma::smem_u32(smem + s * S::kStage);
-        const uint32_t sb = sa + S::kABytes;
-        const uint64_t da = umma::make_desc(sa);
-        const uint64_t db = umma::make_desc(sb);
-        if (dmode != 1) {
-#pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            // advance 16 elements (32 B) along K inside the swizzle atom: +2 in 16-byte units
-            umma::mma_f16(tmem_acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) ? 1u : 0u);
+          umma::mbar_expect_tx(fb, S::kStage);
+          const uint32_t sa = umma::smem_u32(smem + s * S::kStage);
+          const uint32_t sb = sa + S::kABytes;
+          if (g.conv == 0) {
+            umma::tma_load_3d(sa, &tmA, fb, kb * kBK, m_blk * 128, z);
+          } else {
+            const int cblocks = g.cin / kBK;
+            const int tap = kb / cblocks, cb = kb % cblocks;
+            int dx = 0, dy = 0;
+            if (g.conv == 1) {
+              dy = tap / 3 - 1;
+              dx = tap % 3 - 1;
+            }
+            umma::tma_load_3d(sa, &tmA, fb, cb * kBK, px0 + dx, py0 + dy);
           }
+          umma::tma_load_3d(sb, &tmB, fb, kb * kBK, n_blk * BN, z);
         }
-        umma::umma_commit(umma::smem_u32(&empty[s]));  // frees this ring slot when the MMAs retire
-      }
-      umma::umma_commit(umma::smem_u32(&tmem_full[as]));  // accumulator complete
       }
     }
   } else {
-    // ===================== epilogue (warps 2..9) =====================
-    // Two warps per TMEM lane quarter, each taking half of the tile's 32-column chunks.  Every register
-    // array below is indexed with compile-time constants only (fully unrolled, predicated) so the 32
-    // accumulator values of a chunk stay in registers.
-    const int q = warp & 3;            // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;  // which share of the chunks (0 .. EW/4 - 1)
-    constexpr int kChunks = BN / 32;
-    constexpr int kStride = EW / 4;
-    const bool split = EW == 16 && resid_split_ok(g) && dmode == 0;  // (8-warp kernels: 76 registers, two CTAs per SM)
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-    int n_blk, m_blk, z, px0, py0;
-    decode(tile, n_blk, m_blk, z, px0, py0);
-    const int as = it & 1;
-    const int r = q * 32 + lane;  // accumulator row inside the tile
-    int m;                        // logical output row
-    bool row_ok;
-    if (g.conv) {
-      int ly = r / g.tw, lx = r % g.tw;
-      int y = py0 + ly, x = px0 + lx;
-      row_ok = (y < g.imgH) && (x < g.imgW);
-      m = y * g.imgW + x;
-    } else {
-      m = m_blk * 128 + r;
-      row_ok = m < g.M;
-    }
-    uint32_t xr[32];  // residual-stream slice of this thread's next chunk, in flight while the MMAs run
-    if (split && row_ok && half < kChunks) resid_load(g, m, n_blk * BN + half * 32, xr);
-    umma::mbar_wait_dbg(umma::smem_u32(&tmem_full[as]), (it >> 1) & 1, spin);
-    umma::tc_fence_after();
-    const uint32_t tmem_acc = tmem_base + (uint32_t)(as * BN);
-    float head_acc = 0.f;
-#pragma unroll 1
-    for (int ci = half; ci < kChunks; ci += kStride) {
-      if (dmode == 4) break;
-      const int c0 = ci * 32;
-      uint32_t v[32];
-      umma::tmem_ld_32x32(tmem_acc + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-      const int n0 = n_blk * BN + c0;
-      if (dmode == 5) {
-        if (v[0] == 0x7fc12345u && v[17] == 0x12345u) g.out_f32[0] = 1.f;  // keep the load alive
-        continue;
-      }
-      if (split) {
-        if (row_ok) {
-          resid_apply_store(g, v, m, n0, xr);
-          if (ci + kStride < kChunks) resid_load(g, m, n0 + kStride * 32, xr);
+    // ===================== consumers: MMA + epilogue =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");  // 128 x 40 + 256 x 232 <= 64 K registers
+    const int wg = (warp >> 2) - 1;      // consumer warpgroup: accumulator rows 64 wg .. 64 wg + 63
+    const int t = threadIdx.x & 127;     // thread in the warpgroup
+    const int wq = t >> 5;               // warp in the warpgroup: fragment rows 16 wq .. 16 wq + 15
+    float* ebuf = epi_buf + wg * 64 * S::kPitch;
+    int kit = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      int n_blk, m_blk, z, px0, py0;
+      decode(tile, n_blk, m_blk, z, px0, py0);
+      // The tensor core adds each k16 product sum into its accumulator with truncation, so over long reductions (fc2:
+      // K = 4D) the error grows with K.  Each group of kPromote k-blocks is therefore accumulated from zero in `acc`
+      // and then added into the fp32 total `tot` in the FP32 pipe.
+      float acc[BN / 2];  // the first k-block of a group overwrites it (scale-d = 0)
+      float tot[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) tot[i] = 0.f;
+      int prev = -1;  // ring slot still read by the wgmmas in flight
+      // groups of kPromote k-blocks: the loop structure, not a data-dependent branch, decides where a group ends, and the
+      // accumulator is only read after the group's wgmma.wait_group 0
+      for (int kb0 = 0; kb0 < nkb; kb0 += kPromote) {
+        const int kend = min(nkb, kb0 + kPromote);
+        for (int kb = kb0; kb < kend; ++kb, ++kit) {
+          const int s = kit % STAGES;
+          const uint32_t ph = (kit / STAGES) & 1;
+          umma::mbar_wait_dbg(umma::smem_u32(&full[s]), ph, spin);
+          const uint32_t sa = umma::smem_u32(smem + s * S::kStage) + (uint32_t)(wg * 64 * 128);
+          const uint32_t sb = umma::smem_u32(smem + s * S::kStage) + S::kABytes;
+          const uint64_t da = umma::make_desc(sa), db = umma::make_desc(sb);
+          umma::wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kBK / 16; ++k)
+            umma::wgmma_ss<BN>(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), ((kb - kb0) | k) ? 1u : 0u);
+          umma::wgmma_commit();
+          umma::wgmma_wait<1>();  // the previous k-block's wgmmas have retired: its slot may be refilled
+          if (prev >= 0 && t == 0) umma::mbar_arrive(umma::smem_u32(&empty[prev]));
+          prev = s;
         }
-        continue;
+        umma::wgmma_wait<0>();
+        umma::fence_regs(acc);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) tot[i] += acc[i];
       }
-      gemm_epilogue_chunk(g, v, m, z, n0, row_ok, head_acc);
-    }
-    // DPT head: N == 32 is a single chunk, owned by the half-0 warps
-    if (g.epi == EPI_HEAD && half == 0 && row_ok && n_blk == 0) g.out_f32[m] = fmaxf(head_acc + g.b3p[0], 0.f);
-    // this accumulator stage may be overwritten by the MMA warp
-    umma::tc_fence_before();
-    __syncwarp();
-    if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(umma::smem_u32(&tmem_empty[as])) : "memory");
+      if (prev >= 0 && t == 0) umma::mbar_arrive(umma::smem_u32(&empty[prev]));
+      if (dmode == 4) continue;
+
+      // ---- epilogue: the warpgroup's 64 x BN accumulator goes through shared memory, then thread
+      // (row t & 63, chunks t >> 6, +2, ...) runs the fused epilogue on 32 consecutive columns of its row ----
+      const int er = t & 63, ec = t >> 6;
+      const int r = wg * 64 + er;  // accumulator row inside the tile
+      int m;                       // logical output row
+      bool row_ok;
+      if (g.conv) {
+        int ly = r / g.tw, lx = r % g.tw;
+        int y = py0 + ly, x = px0 + lx;
+        row_ok = (y < g.imgH) && (x < g.imgW);
+        m = y * g.imgW + x;
+      } else {
+        m = m_blk * 128 + r;
+        row_ok = m < g.M;
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // staging buffer free (previous tile read)
+      // fragment of m64nN: tot[4 j + i] is row 16 wq + lane/4 + 8 (i >> 1), column 8 j + 2 (lane & 3) + (i & 1)
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + 2 * (lane & 3);
+        const int r0 = 16 * wq + (lane >> 2);
+        *(float2*)(ebuf + r0 * S::kPitch + c) = make_float2(tot[4 * j], tot[4 * j + 1]);
+        *(float2*)(ebuf + (r0 + 8) * S::kPitch + c) = make_float2(tot[4 * j + 2], tot[4 * j + 3]);
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+      float head_acc = 0.f;
+#pragma unroll 1
+      for (int ci = ec; ci < BN / 32; ci += 2) {
+        uint32_t v[32];
+        const float4* src = (const float4*)(ebuf + er * S::kPitch + ci * 32);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const float4 f = src[i];
+          v[4 * i] = __float_as_uint(f.x);
+          v[4 * i + 1] = __float_as_uint(f.y);
+          v[4 * i + 2] = __float_as_uint(f.z);
+          v[4 * i + 3] = __float_as_uint(f.w);
+        }
+        gemm_epilogue_chunk(g, v, m, z, n_blk * BN + ci * 32, row_ok, head_acc);
+      }
+      // DPT head: N == 32 is a single chunk, owned by the chunk-0 threads
+      if (g.epi == EPI_HEAD && ec == 0 && row_ok && n_blk == 0) g.out_f32[m] = fmaxf(head_acc + g.b3p[0], 0.f);
     }
   }
-
-  umma::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) umma::tmem_dealloc(tmem_base, 2 * BN);
 }
 
 }  // namespace vd3d

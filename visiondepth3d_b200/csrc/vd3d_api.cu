@@ -239,7 +239,7 @@ SelJob make_job(const JobMem& m, const float* data, int W, int x0, int x1, int y
 }
 
 int sel_blocks(int rows) {
-  int b = 148 * 4;
+  int b = 132 * 4;  // four CTAs per SM of an H100
   return rows < b ? rows : b;
 }
 

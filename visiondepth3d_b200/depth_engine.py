@@ -66,7 +66,7 @@ def _bind(lib):
 
 
 class DepthEngine:
-    """Depth-Anything-V2 forward on tcgen05 tensor cores.  `cfg` is a key of CONFIGS or a dict."""
+    """Depth-Anything-V2 forward on wgmma tensor cores.  `cfg` is a key of CONFIGS or a dict."""
 
     def __init__(self, cfg="vits", image_h=518, image_w=924, ctx=None, device=0):
         self.lib = _lib.load()

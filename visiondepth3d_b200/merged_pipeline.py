@@ -1,5 +1,5 @@
 """Drop-in for the Real-ESRGAN upscale stage of the reference's core/merged_pipeline.py (run_esrgan and its helpers,
-lines 221-284), backed by libvd3d.so: the SRVGGNetCompact network on tcgen05 implicit-GEMM convolutions, cv2's INTER_AREA
+lines 221-284), backed by libvd3d.so: the SRVGGNetCompact network on wgmma implicit-GEMM convolutions, cv2's INTER_AREA
 / INTER_CUBIC resizes and addWeighted as CUDA kernels.  RIFE interpolation, the image-folder driver and the ffmpeg
 writer of that module are outside the hot path.
 

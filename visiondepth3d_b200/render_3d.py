@@ -1,5 +1,5 @@
 """Drop-in for the hot-path surface of the reference's core/render_3d.py, backed by
-libvd3d.so (hand-written sm_100a CUDA).  Same names, argument meaning, return types and
+libvd3d.so (hand-written sm_90a CUDA).  Same names, argument meaning, return types and
 error behaviour as the reference (file:line cited per function); no Tk, no ONNXRuntime,
 no CPU fallback.
 
@@ -449,7 +449,7 @@ def render_sbs_3d(
     import shutil
     import cv2
     if auto_crop_black_bars or skip_blank_frames:
-        print("⚠️ auto_crop_black_bars / skip_blank_frames are outside the B200 hot path")
+        print("⚠️ auto_crop_black_bars / skip_blank_frames are outside the GPU hot path")
         return
     if use_ffmpeg and shutil.which("ffmpeg") is None:
         print("⚠️ ffmpeg binary not found: writing through cv2.VideoWriter instead")
@@ -764,7 +764,7 @@ def _dialog(kind, **kw):
     try:
         from tkinter import filedialog
     except Exception as e:  # headless box: the dialogs are GUI-only
-        raise RuntimeError("file dialogs need tkinter (GUI helper, outside the B200 hot path)") from e
+        raise RuntimeError("file dialogs need tkinter (GUI helper, outside the GPU hot path)") from e
     return getattr(filedialog, kind)(**kw)
 
 

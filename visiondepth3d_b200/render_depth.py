@@ -1,7 +1,7 @@
 """Drop-in for the hot-path surface of the reference's core/render_depth.py: the `pipe`
 callable protocol and the depth -> uint8 normalisation, backed by the libvd3d depth engine
-(Depth-Anything-V2 on tcgen05 tensor cores).  GUI, ONNX, Marigold, DepthCrafter and the
-letterbox tracker are outside the B200 hot path (SURVEY.md section 2).
+(Depth-Anything-V2 on wgmma tensor cores).  GUI, ONNX, Marigold, DepthCrafter and the
+letterbox tracker are outside the GPU hot path (SURVEY.md section 2).
 
 Protocol kept (core/render_depth.py:1113-1119, consumers 201-268 and 1894-1917):
     pipe(images: list[PIL.Image], inference_size: (W, H) | None) -> list[{"predicted_depth": Tensor[h, w]}]
@@ -234,7 +234,7 @@ def _find_checkpoint_file(folder):
 
 def ensure_model_downloaded(checkpoint):
     """Resolve a checkpoint id to (model, metadata) like core/render_depth.py:728-829 does for HF ids and local
-    folders.  There is no network on the B200 box: an HF id is looked up in the reference's cache layout
+    folders.  No network is assumed: an HF id is looked up in the reference's cache layout
     (weights/<org>_<name>/...), a directory is searched for model.safetensors / pytorch_model.bin.  Returns
     (state_dict, {"arch", "is_b200": True}) or (None, None) with a message, as the reference does on failure."""
     if not isinstance(checkpoint, str):
@@ -284,11 +284,11 @@ def update_pipeline(selected_model_var, status_label_widget, inference_res_var, 
             if sd is None:
                 _notify(status_label_widget, f"❌ Failed to load model: {name}")
                 return
-            _notify(status_label_widget, "🔄 Warming up B200 depth engine...")
+            _notify(status_label_widget, "🔄 Warming up H100 depth engine...")
             load_depth_model(meta["arch"], sd, 384, 384)
             from PIL import Image
             pipe([Image.new("RGB", (384, 384), (127, 127, 127))])
-            _notify(status_label_widget, f"✅ Depth model loaded: {name} (libvd3d, sm_100a)")
+            _notify(status_label_widget, f"✅ Depth model loaded: {name} (libvd3d, sm_90a)")
         except Exception as e:
             _notify(status_label_widget, f"💥 Init error: {e}")
 
@@ -394,7 +394,7 @@ def depth_video_from_video(input_path, output_path, invert=False, inference_size
 
 def _gui_only(name):
     def f(*_a, **_k):
-        raise RuntimeError(f"{name} is a Tk GUI driver of the reference (core/render_depth.py); on the B200 path use "
+        raise RuntimeError(f"{name} is a Tk GUI driver of the reference (core/render_depth.py); on the GPU path use "
                            "depth_video_from_video() / hf_batch_safe_pipe() instead")
     f.__name__ = name
     return f
