@@ -54,7 +54,6 @@ struct vd3d_depth {
   uint64_t launches = 0;
   int ph = 0, pw = 0, ntok = 0, npad = 0;
   bool planned = false;
-  bool flash = true;  // fused attention kernel (VD3D_FLASH=0 selects the 3-kernel path)
   // the per-image neck / head tails of a batch run on side streams (forked after the transformer, joined at the end)
   cudaStream_t cur = nullptr;          // stream the helpers launch on (null: `stream`)
   cudaStream_t aux[8] = {};
@@ -178,19 +177,6 @@ int gemm(vd3d_depth* e, const __half* A, int lda, const __half* B, int ldb, Gemm
   return VD3D_OK;
 }
 
-// batched GEMM over blockIdx.z: A [batch][M, K] (lda, sa), B [batch][N, K] (ldb, sb)
-int gemm_batched(vd3d_depth* e, const __half* A, int lda, uint64_t sa, const __half* B, int ldb, uint64_t sb,
-                 int batch, GemmArgs g, int bn) {
-  CUtensorMap ma, mb;
-  int r;
-  if ((r = make_map(e, &ma, A, g.K, g.M, batch, lda, sa, 128, 1))) return r;
-  if ((r = make_map(e, &mb, B, g.K, g.N, batch, ldb, sb, bn, 1))) return r;
-  cudaError_t ce = launch_gemm(bn, ma, mb, g, (g.M + 127) / 128, batch, e->cur ? e->cur : e->stream);
-  if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("gemm launch: ") + cudaGetErrorString(ce));
-  e->launches++;
-  return VD3D_OK;
-}
-
 void pick_tile(int W, int H, int& tw, int& th) {
   const int cand[4][2] = {{128, 1}, {64, 2}, {32, 4}, {16, 8}};
   long best = -1;
@@ -249,7 +235,6 @@ int vd3d_depth_create(const vd3d_depth_config* cfg, void* stream, vd3d_depth** o
   e->pw = cfg->image_w / 14;
   e->ntok = e->ph * e->pw + 1;
   e->npad = round_up(e->ntok, 128);
-  if (const char* f = getenv("VD3D_FLASH")) e->flash = atoi(f) != 0;
   if (e->ntok > 3072) {
     delete e;
     return VD3D_ERR_UNSUPPORTED;
@@ -327,7 +312,6 @@ int vd3d_depth_clone(vd3d_depth* src, void* stream, vd3d_depth** out) {
   e->pw = src->pw;
   e->ntok = src->ntok;
   e->npad = src->npad;
-  e->flash = src->flash;
   *out = e;
   return VD3D_OK;
 }
@@ -514,19 +498,13 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
   int r;
   char nm[96];
   // ---- buffers ----
-  void *x, *xn, *q, *k, *vt, *S, *P, *attn, *hb, *ape;
+  void *x, *xn, *q, *k, *vt, *attn, *hb, *ape;
   const int MT = (B - 1) * NP + NT;  // rows of the stacked token matrix
-  if (B > 1 && !e->flash) return dfail(e, VD3D_ERR_UNSUPPORTED, "batched forward needs the fused attention kernel");
   if ((r = get_buf(e, "x", (size_t)B * NP * D * 4, &x))) return r;
   if ((r = get_buf(e, "xn", (size_t)B * NP * D * 2, &xn))) return r;
   if ((r = get_buf(e, "q", (size_t)B * Hh * NP * 64 * 2, &q))) return r;
   if ((r = get_buf(e, "k", (size_t)B * Hh * NP * 64 * 2, &k))) return r;
   if ((r = get_buf(e, "vt", (size_t)B * Hh * 64 * NP * 2, &vt))) return r;
-  S = P = nullptr;
-  if (!e->flash) {
-    if ((r = get_buf(e, "S", (size_t)Hh * NP * NP * 4, &S))) return r;
-    if ((r = get_buf(e, "P", (size_t)Hh * NP * NP * 2, &P))) return r;
-  }
   if ((r = get_buf(e, "attn", (size_t)B * NP * D * 2, &attn))) return r;
   if ((r = get_buf(e, "h", (size_t)B * NP * 4 * D * 2, &hb))) return r;
   if ((r = get_buf(e, "ape", (size_t)NPATCH * KPE * 2, &ape))) return r;
@@ -590,8 +568,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     }
     e->span_end(sp_, s);
     sp_ = e->span_begin("attn", s);
-    if (e->flash) {
-      // fused wgmma attention: scores and probabilities stay in registers
+    {  // fused wgmma attention: scores and probabilities stay in registers
       CUtensorMap mq, mk, mv;
       if ((r = make_map(e, &mq, q, 64, NT, B * Hh, 64, (uint64_t)NP * 64, 128, 1))) return r;
       if ((r = make_map(e, &mk, k, 64, NT, B * Hh, 64, (uint64_t)NP * 64, 128, 1))) return r;
@@ -599,27 +576,6 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
       cudaError_t ce = launch_attention(mq, mk, mv, NT, D, (__half*)attn, Hh, B, NP, s);
       if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("attention launch: ") + cudaGetErrorString(ce));
       e->launches++;
-    } else {
-      {  // scores = (q / sqrt(d)) k^T, per head
-        GemmArgs g = base_args(NT, NT, 64, EPI_F32);
-        g.out_f32 = (float*)S;
-        g.ldc = NP;
-        g.out_batch_stride = (long long)NP * NP;
-        if ((r = gemm_batched(e, (const __half*)q, 64, (uint64_t)NP * 64, (const __half*)k, 64, (uint64_t)NP * 64, Hh,
-                              g, 128)))
-          return r;
-      }
-      launch_softmax((const float*)S, (__half*)P, NT, Hh, NT, NP, s);
-      e->launches++;
-      {  // context = P v, written head-interleaved into attn [NT, D]
-        GemmArgs g = base_args(NT, 64, NT, EPI_F16);
-        g.out_f16 = (__half*)attn;
-        g.ldc = D;
-        g.out_batch_stride = 64;
-        if ((r = gemm_batched(e, (const __half*)P, NP, (uint64_t)NP * NP, (const __half*)vt, NP, (uint64_t)64 * NP, Hh,
-                              g, 64)))
-          return r;
-      }
     }
     e->span_end(sp_, s);
     sp_ = e->span_begin("proj", s);

@@ -57,41 +57,6 @@ __global__ void __launch_bounds__(256) k_layernorm(const float* __restrict__ x, 
     }
 }
 
-// softmax over keys (scores already scaled: q was multiplied by 1/sqrt(d)); one warp per row,
-// the row lives in registers (fully unrolled, predicated) so S is read once and P written once
-template <int MAXI>
-__global__ void __launch_bounds__(256) k_softmax(const float* __restrict__ S, __half* __restrict__ P, int rows_per_head,
-                                                 int heads, int ncols, int ld) {
-  int gr = blockIdx.x * 8 + (threadIdx.x >> 5);
-  int lane = threadIdx.x & 31;
-  if (gr >= rows_per_head * heads) return;
-  int h = gr / rows_per_head, r = gr % rows_per_head;
-  const float* s = S + ((size_t)h * ld + r) * ld;
-  __half* p = P + ((size_t)h * ld + r) * ld;
-  float v[MAXI];
-  float mx = -INFINITY;
-#pragma unroll
-  for (int i = 0; i < MAXI; ++i) {
-    int c = lane + 32 * i;
-    v[i] = (c < ncols) ? __ldcs(s + c) : -INFINITY;
-    mx = fmaxf(mx, v[i]);
-  }
-  for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  float sum = 0.f;
-#pragma unroll
-  for (int i = 0; i < MAXI; ++i) {
-    v[i] = (lane + 32 * i < ncols) ? expf(v[i] - mx) : 0.f;
-    sum += v[i];
-  }
-  for (int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  float inv = 1.0f / sum;
-#pragma unroll
-  for (int i = 0; i < MAXI; ++i) {
-    int c = lane + 32 * i;
-    if (c < ncols) p[c] = __float2half_rn(v[i] * inv);
-  }
-}
-
 // patch embedding im2col: pixel_values f32 [3, IH, IW] -> A f16 [ph*pw, kpad], k = c*196 + dy*14 + dx
 __global__ void __launch_bounds__(256) k_patch_im2col(const float* __restrict__ px, int IH, int IW, int ph, int pw,
                                                       __half* __restrict__ A, int kpad) {
@@ -373,14 +338,6 @@ void launch_add_relu_f16(const __half* a, const __half* b, __half* sum, __half* 
 void launch_layernorm(const float* x, int rows, int D, const float* g, const float* b, __half* out, int row_off,
                       cudaStream_t s) {
   k_layernorm<<<(rows + 7) / 8, 256, 0, s>>>(x, rows, D, g, b, out, row_off, 1e-6f);
-}
-void launch_softmax(const float* S, __half* P, int rows, int heads, int ncols, int ld, cudaStream_t s) {
-  if (ncols <= 32 * 8)
-    k_softmax<8><<<(rows * heads + 7) / 8, 256, 0, s>>>(S, P, rows, heads, ncols, ld);
-  else if (ncols <= 32 * 80)
-    k_softmax<80><<<(rows * heads + 7) / 8, 256, 0, s>>>(S, P, rows, heads, ncols, ld);
-  else
-    k_softmax<96><<<(rows * heads + 7) / 8, 256, 0, s>>>(S, P, rows, heads, ncols, ld);
 }
 void launch_patch_im2col(const float* px, int IH, int IW, int ph, int pw, __half* A, int kpad, cudaStream_t s) {
   int total = ph * pw * 588;

@@ -9,7 +9,6 @@ namespace vd3d {
 struct GemmArgs;
 void launch_layernorm(const float* x, int rows, int D, const float* g, const float* b, __half* out, int row_off,
                       cudaStream_t s);
-void launch_softmax(const float* S, __half* P, int rows, int heads, int ncols, int ld, cudaStream_t s);
 void launch_patch_im2col(const float* px, int IH, int IW, int ph, int pw, __half* A, int kpad, cudaStream_t s);
 void launch_set_cls(float* x, const float* cls, const float* pos, int D, cudaStream_t s);
 void launch_im2col_s2(const __half* in, int H, int W, int C, int ldc, __half* out, int OH, int OW, cudaStream_t s);

@@ -103,6 +103,7 @@ void launch_ingest(const IngestArgs& a, cudaStream_t s);
 void launch_resize_planar(const float* src, int C, int sh, int sw, float* dst, int oh, int ow, cudaStream_t s);
 // 3 histogram passes + 3 bin searches; b may be null.  b's region must lie inside a's
 // and share a.data.  nblocks = grid of the pass kernels.
+constexpr int kSelectLaunches = 6;
 void launch_select(const SelJob& a, const SelJob* b, int nblocks, cudaStream_t s);
 void launch_fin_pct(const SelJob& j, float w_lo, float w_hi, float alpha, float oma, DevState* st, FrameScalars* fs,
                     cudaStream_t s);

@@ -81,11 +81,10 @@ struct vd3d_ctx {
   // CUDA graphs of the per-frame kernel sequence, keyed by (staging slot, depth ping-pong parity)
   struct FrameGraph {
     cudaGraphExec_t exec = nullptr;
-    uint64_t n_ctx = 0, n_depth = 0;
+    uint64_t n_ctx = 0;
   } fg[kSlots][2];
   vd3d_render_params fg_rp;
   int fg_h = 0, fg_w = 0, fg_dch = 0, fg_warm = 0;
-  void* fg_depth = nullptr;
   // depth stage of the depth+stereo clip: two engine clones (shared weights) on two streams so the
   // depth forwards of consecutive frames overlap each other and the DIBR kernels of the previous frame
   vd3d_depth* dclone[kClones] = {};
@@ -261,6 +260,58 @@ struct CoreIn {
   uint8_t* right;
 };
 
+// the feathering box sizes the compose kernels support
+int check_blur_ksize(vd3d_ctx* ctx, int feather, int k) {
+  if (feather && (k < 1 || k > 63)) return fail(ctx, VD3D_ERR_UNSUPPORTED, "blur_ksize must be in [1,63]");
+  return VD3D_OK;
+}
+
+// compose inputs of a core whose shift map is in ctx->shift (e2: left to the caller)
+ComposeArgs compose_args(vd3d_ctx* ctx, const CoreIn& in) {
+  ComposeArgs ca;
+  memset(&ca, 0, sizeof ca);
+  ca.src_u8 = in.src_u8;
+  ca.src_pitch = in.src_pitch;
+  ca.cx0 = in.cx0;
+  ca.cy0 = in.cy0;
+  ca.src_f32 = in.src_f32;
+  ca.shift = (const float*)ctx->shift.p;
+  ca.xs = (const float*)ctx->xs.p;
+  ca.ys = (const float*)ctx->ys.p;
+  ca.H = in.H;
+  ca.W = in.W;
+  ca.k = in.p.blur_ksize;
+  ca.feather = in.p.enable_feathering ? 1 : 0;
+  ca.grade = in.grade;
+  ca.sat = in.sat;
+  ca.con = in.con;
+  ca.bri = in.bri;
+  ca.left = in.left;
+  ca.right = in.right;
+  return ca;
+}
+
+// generic tail of both cores, any box size: [k_warp_edges ->] k_compose into in.left / in.right
+int compose_generic(vd3d_ctx* ctx, const CoreIn& in) {
+  cudaStream_t s = ctx->stream;
+  ComposeArgs ca = compose_args(ctx, in);
+  if (ca.feather) {
+    int r;
+    if ((r = ensure(ctx, ctx->e2, sizeof(float2) * (size_t)ca.W * ca.H))) return r;
+    launch_warp_edges((const float*)ctx->d.p, ca.shift, (float2*)ctx->e2.p, ca.H, ca.W, ca.xs, ca.ys,
+                      (float)in.p.feather_strength, s);
+    ctx->launches += 1;
+  }
+  ca.e2 = (const float2*)ctx->e2.p;
+  {
+    ProfScope ps(ctx, 1);
+    launch_compose(ca, s);
+  }
+  ctx->launches += 1;
+  CK(cudaGetLastError());
+  return VD3D_OK;
+}
+
 int run_core(vd3d_ctx* ctx, const CoreIn& in) {
   cudaStream_t s = ctx->stream;
   const int W = in.W, H = in.H;
@@ -281,59 +332,32 @@ int run_core(vd3d_ctx* ctx, const CoreIn& in) {
   quantile_rank(in.p.depth_stretch_lo, (long long)W * H, l0, l1, wlo);
   quantile_rank(in.p.depth_stretch_hi, (long long)W * H, h0, h1, whi);
   launch_set_ranks(ctx->jm[2].tg, l0, l1, h0, h1, s);
+  ctx->launches += 1;
   SelJob qj = make_job(ctx->jm[2], d, W, 0, W, 0, H, 0, 4, 0, false);
   SelJob s0 = make_job(ctx->jm[3], d, W, W / 5, W * 4 / 5, H / 5, H * 4 / 5, 1, 1, 1, true);
   launch_select(qj, &s0, sel_blocks(H), s);
+  ctx->launches += kSelectLaunches;
   launch_fin_d0(qj, s0, wlo, whi, ctx->fs, s);
+  ctx->launches += 1;
   launch_shape(d, W * H, ctx->fs, (float)in.p.depth_pop_mid, (float)in.p.depth_pop_gamma, s);
+  ctx->launches += 1;
   SelJob s1 = make_job(ctx->jm[4], d, W, W / 5, W * 4 / 5, H / 5, H * 4 / 5, 1, 1, 1, true);
   launch_select(s1, nullptr, sel_blocks(H * 4 / 5 - H / 5), s);
+  ctx->launches += kSelectLaunches;
   ShiftArgs sa;
   sa.p = in.p;
   sa.W = W;
   sa.H = H;
   launch_fin_shape(s1, sa, ctx->st, ctx->fs, s);
+  ctx->launches += 1;
   if (ctx->stats_only) {  // every temporal state update of the frame has happened by now
-    ctx->launches += 1 + 6 + 1 + 1 + 6 + 1;
     CK(cudaGetLastError());
     return VD3D_OK;
   }
   launch_shift(d, shift, H, W, ctx->fs, in.p.enable_edge_masking ? 1 : 0, (float)in.p.feather_strength, s);
-  ctx->launches += 1 + 6 + 1 + 1 + 6 + 1 + 1;
-  int feather = in.p.enable_feathering ? 1 : 0;
-  if (feather) {
-    if (in.p.blur_ksize < 1 || in.p.blur_ksize > 63) return fail(ctx, VD3D_ERR_UNSUPPORTED, "blur_ksize must be in [1,63]");
-    if ((r = ensure(ctx, ctx->e2, sizeof(float2) * (size_t)W * H))) return r;
-    launch_warp_edges(d, shift, (float2*)ctx->e2.p, H, W, xs, ys, (float)in.p.feather_strength, s);
-    ctx->launches += 1;
-  }
-  ComposeArgs ca;
-  ca.src_u8 = in.src_u8;
-  ca.src_pitch = in.src_pitch;
-  ca.cx0 = in.cx0;
-  ca.cy0 = in.cy0;
-  ca.src_f32 = in.src_f32;
-  ca.shift = shift;
-  ca.e2 = (const float2*)ctx->e2.p;
-  ca.xs = xs;
-  ca.ys = ys;
-  ca.H = H;
-  ca.W = W;
-  ca.k = in.p.blur_ksize;
-  ca.feather = feather;
-  ca.grade = in.grade;
-  ca.sat = in.sat;
-  ca.con = in.con;
-  ca.bri = in.bri;
-  ca.left = in.left;
-  ca.right = in.right;
-  {
-    ProfScope ps(ctx, 1);
-    launch_compose(ca, s);
-  }
   ctx->launches += 1;
-  CK(cudaGetLastError());
-  return VD3D_OK;
+  if ((r = check_blur_ksize(ctx, in.p.enable_feathering, in.p.blur_ksize))) return r;
+  return compose_generic(ctx, in);
 }
 
 // ---------------------------------------------------------------------------
@@ -356,6 +380,7 @@ struct FastPost {  // fused bars + sharpen + fit + pack (fuse == 0: write the ey
   const float4* src_rgbx = nullptr;
 };
 
+// Box sizes k_render does not support (render_supports) take run_core instead.
 int run_core_fast(vd3d_ctx* ctx, const CoreIn& in, const FastLoop* lp, const FastPost& post) {
   cudaStream_t s = ctx->stream;
   const int W = in.W, H = in.H;
@@ -367,9 +392,6 @@ int run_core_fast(vd3d_ctx* ctx, const CoreIn& in, const FastLoop* lp, const Fas
   const float* ys = (const float*)ctx->ys.p;
   float* d = (float*)ctx->d.p;
   float* shift = (float*)ctx->shift.p;
-  int feather = in.p.enable_feathering ? 1 : 0;
-  if (feather && (in.p.blur_ksize < 1 || in.p.blur_ksize > 63))
-    return fail(ctx, VD3D_ERR_UNSUPPORTED, "blur_ksize must be in [1,63]");
 
   StatsArgs sa;
   memset(&sa, 0, sizeof sa);
@@ -411,61 +433,25 @@ int run_core_fast(vd3d_ctx* ctx, const CoreIn& in, const FastLoop* lp, const Fas
     launch_shift_fast(d, shift, H, W, ctx->fs, in.p.enable_edge_masking ? 1 : 0, (float)in.p.feather_strength, s);
   ctx->launches += 1;
 
-  ComposeArgs ca;
-  memset(&ca, 0, sizeof ca);
-  ca.src_u8 = in.src_u8;
-  ca.src_pitch = in.src_pitch;
-  ca.cx0 = in.cx0;
-  ca.cy0 = in.cy0;
-  ca.src_f32 = in.src_f32;
-  ca.shift = shift;
-  ca.xs = xs;
-  ca.ys = ys;
-  ca.H = H;
-  ca.W = W;
-  ca.k = in.p.blur_ksize;
-  ca.feather = feather;
-  ca.grade = in.grade;
-  ca.sat = in.sat;
-  ca.con = in.con;
-  ca.bri = in.bri;
-  ca.left = in.left;
-  ca.right = in.right;
-  if (render_supports(feather, in.p.blur_ksize)) {
-    RenderArgs ra;
-    memset(&ra, 0, sizeof ra);
-    ra.c = ca;
-    ra.src_rgbx = post.src_rgbx;
-    ra.d = d;
-    ra.feather_strength = (float)in.p.feather_strength;
-    ra.fuse = post.fuse;
-    ra.fs = ctx->fs;
-    ra.sharpen = post.sharpen;
-    ra.kc = post.kc;
-    ra.ke = post.ke;
-    ra.out = post.out;
-    ra.out_w = post.out_w;
-    ra.per_eye_w = post.per_eye_w;
-    {
-      ProfScope ps(ctx, 1);
-      CK(launch_render(ra, s));
-    }
-    ctx->launches += 1;
-  } else {
-    // even / large box sizes: the generic kernels of the exact path (callers never request fuse for these)
-    if (post.src_rgbx) return fail(ctx, VD3D_ERR_STATE, "generic compose needs planar RGB");
-    if (feather) {
-      if ((r = ensure(ctx, ctx->e2, sizeof(float2) * (size_t)W * H))) return r;
-      launch_warp_edges(d, shift, (float2*)ctx->e2.p, H, W, xs, ys, (float)in.p.feather_strength, s);
-      ctx->launches += 1;
-    }
-    ca.e2 = (const float2*)ctx->e2.p;
-    {
-      ProfScope ps(ctx, 1);
-      launch_compose(ca, s);
-    }
-    ctx->launches += 1;
+  RenderArgs ra;
+  memset(&ra, 0, sizeof ra);
+  ra.c = compose_args(ctx, in);
+  ra.src_rgbx = post.src_rgbx;
+  ra.d = d;
+  ra.feather_strength = (float)in.p.feather_strength;
+  ra.fuse = post.fuse;
+  ra.fs = ctx->fs;
+  ra.sharpen = post.sharpen;
+  ra.kc = post.kc;
+  ra.ke = post.ke;
+  ra.out = post.out;
+  ra.out_w = post.out_w;
+  ra.per_eye_w = post.per_eye_w;
+  {
+    ProfScope ps(ctx, 1);
+    CK(launch_render(ra, s));
   }
+  ctx->launches += 1;
   CK(cudaGetLastError());
   return VD3D_OK;
 }
@@ -473,6 +459,7 @@ int run_core_fast(vd3d_ctx* ctx, const CoreIn& in, const FastLoop* lp, const Fas
 int begin_frame(vd3d_ctx* ctx) {
   CK(cudaMemsetAsync(ctx->jobwords, 0, sizeof(uint32_t) * (kJobs * kJobWords + kBarWords), ctx->stream));
   CK(cudaMemsetAsync(ctx->fs, 0, sizeof(FrameScalars), ctx->stream));
+  ctx->launches += 2;
   return VD3D_OK;
 }
 
@@ -758,6 +745,99 @@ int copy_in(vd3d_ctx* ctx, Buf& b, const void* src, size_t bytes, int mem, cudaS
   return VD3D_OK;
 }
 
+// where a stage entry point writes its output: dst itself, or the staging buffer b when dst is host memory
+int stage_out(vd3d_ctx* ctx, Buf& b, void* dst, size_t bytes, int mem, void** dev) {
+  *dev = dst;
+  if (mem != VD3D_MEM_HOST) return VD3D_OK;
+  int r = ensure(ctx, b, bytes);
+  if (r) return r;
+  *dev = b.p;
+  return VD3D_OK;
+}
+
+// after the launch: check it, copy a staged output back to dst and wait for the result
+int stage_finish(vd3d_ctx* ctx, void* dst, const void* dev, size_t bytes, int mem) {
+  CK(cudaGetLastError());
+  if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(dst, dev, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return VD3D_OK;
+}
+
+// DOF blur + colour grade of an eye pair [H, W] from a depth map [dh, dw] with the cached five-level Gaussian bank
+// (levels == 1: grade only); sources, destinations and the focal depth are the caller's
+DofArgs dof_args(const vd3d_ctx* ctx, int levels, int H, int W, const float* depth, int dh, int dw, double sat,
+                 double con, double bri) {
+  DofArgs da;
+  memset(&da, 0, sizeof da);
+  da.H = H;
+  da.W = W;
+  da.depth = depth;
+  da.dh = dh;
+  da.dw = dw;
+  da.focus_w = (float)(0.35 + 1e-6);
+  da.idx_max = (float)(5 - 1 - 1e-6);
+  da.nlevels = levels;
+  if (levels > 1) {
+    for (int i = 0; i < 8; ++i) {
+      da.ksize[i] = ctx->dof_ksize[i];
+      da.koff[i] = ctx->dof_koff[i];
+    }
+    da.kern = (const float*)ctx->dof_kern.p;
+    da.halo = ctx->dof_halo;
+  }
+  da.sat = (float)sat;
+  da.con = (float)con;
+  da.bri = (float)bri;
+  return da;
+}
+
+// k_post on one image [h, w] in the single-eye pass-through layout: identity fit onto an ow x oh output, no bars
+PostArgs single_eye_post(const void* src, int h, int w, uint8_t* out, int ow, int oh) {
+  PostArgs pa;
+  memset(&pa, 0, sizeof pa);
+  pa.left = (const uint8_t*)src;
+  pa.right = (const uint8_t*)src;
+  pa.H = h;
+  pa.W = w;
+  pa.fmt = VD3D_FMT_INTERLACED;
+  pa.per_eye_w = ow;
+  pa.per_eye_h = oh;
+  pa.fit_w = ow;
+  pa.fit_h = oh;
+  pa.sx = pa.sy = 1;
+  pa.inv_area = 1.f;
+  pa.out = out;
+  pa.out_w = ow;
+  pa.out_h = oh;
+  return pa;
+}
+
+// Capture what enqueue() launches on stream s into *exec.  When capture is unavailable or fails, this context
+// switches to eager launches for good (with a message on stderr) and false is returned: the caller then undoes its
+// bookkeeping of the captured enqueue and launches eagerly.
+template <class Enqueue>
+bool capture(vd3d_ctx* ctx, cudaStream_t s, cudaGraphExec_t* exec, Enqueue enqueue) {
+  if (cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal) != cudaSuccess) {
+    fprintf(stderr, "vd3d: CUDA graph capture unavailable (%s); continuing with eager launches\n",
+            cudaGetErrorString(cudaGetLastError()));
+    ctx->use_graphs = 0;
+    return false;
+  }
+  const int r = enqueue();
+  cudaGraph_t graph = nullptr;
+  const cudaError_t ce = cudaStreamEndCapture(s, &graph);
+  if (r != VD3D_OK || ce != cudaSuccess || !graph || cudaGraphInstantiate(exec, graph, 0) != cudaSuccess) {
+    fprintf(stderr, "vd3d: CUDA graph capture failed (r=%d, %s); continuing with eager launches\n", r,
+            cudaGetErrorString(cudaGetLastError()));
+    if (graph) cudaGraphDestroy(graph);
+    *exec = nullptr;
+    ctx->use_graphs = 0;
+    return false;
+  }
+  cudaGraphDestroy(graph);
+  return true;
+}
+
 }  // namespace
 
 // ===========================================================================
@@ -990,8 +1070,10 @@ int vd3d_pixel_shift(vd3d_ctx* ctx, const float* rgb, const float* depth, int in
   int r;
   const bool fastp = !ctx->exact && render_supports(p->enable_feathering ? 1 : 0, p->blur_ksize);
   if ((r = begin_frame(ctx))) return r;
-  if (!fastp) launch_set_shifts(ctx->fs, p->fg_shift, p->mg_shift, p->bg_shift, s);  // k_stats does it itself
-  ctx->launches += 2;
+  if (!fastp) {  // k_stats does it itself
+    launch_set_shifts(ctx->fs, p->fg_shift, p->mg_shift, p->bg_shift, s);
+    ctx->launches += 1;
+  }
   const void *rgb_d, *depth_d;
   if ((r = copy_in(ctx, ctx->in_rgbf, rgb, sizeof(float) * 3 * (size_t)in_h * in_w, mem, s, &rgb_d))) return r;
   if ((r = copy_in(ctx, ctx->in_depthf, depth, sizeof(float) * (size_t)in_h * in_w, mem, s, &depth_d))) return r;
@@ -1002,14 +1084,10 @@ int vd3d_pixel_shift(vd3d_ctx* ctx, const float* rgb, const float* depth, int in
     ctx->launches += 1;
     src_f32 = (const float*)ctx->frameB.p;
   }
-  uint8_t *l_d = left_bgr, *r_d = right_bgr;
+  void *l_d, *r_d;
   size_t eye_bytes = (size_t)W * H * 3;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->eyeL, eye_bytes))) return r;
-    if ((r = ensure(ctx, ctx->eyeR, eye_bytes))) return r;
-    l_d = (uint8_t*)ctx->eyeL.p;
-    r_d = (uint8_t*)ctx->eyeR.p;
-  }
+  if ((r = stage_out(ctx, ctx->eyeL, left_bgr, eye_bytes, mem, &l_d))) return r;
+  if ((r = stage_out(ctx, ctx->eyeR, right_bgr, eye_bytes, mem, &r_d))) return r;
   CoreIn ci;
   ci.depth = (const float*)depth_d;
   ci.sh = in_h;
@@ -1025,8 +1103,8 @@ int vd3d_pixel_shift(vd3d_ctx* ctx, const float* rgb, const float* depth, int in
   ci.sat = 1.f;
   ci.con = 1.f;
   ci.bri = 0.f;
-  ci.left = l_d;
-  ci.right = r_d;
+  ci.left = (uint8_t*)l_d;
+  ci.right = (uint8_t*)r_d;
   if (fastp) {
     FastPost post;
     if ((r = run_core_fast(ctx, ci, nullptr, post))) return r;
@@ -1144,36 +1222,20 @@ static vd3d_shift_params loop_shift_params(const vd3d_render_params* rp) {
 
 // fast-path core of one loop iteration: k_stats (ingest .. scalar trackers) -> k_shift -> k_render.  *fused tells the
 // caller that bars + sharpen + eye fit + pack already happened inside k_render (out_d is complete).
-static int enqueue_core_fast(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_t* depth_d, int depth_channels,
-                             int src_h, int src_w, const vd3d_render_params* rp, const vd3d_size_plan& pl,
-                             uint8_t* out_d, bool ident, bool* fused) {
+static int enqueue_core_fast(vd3d_ctx* ctx, const IngestArgs& ia, const LoopArgs& la, float* dn, const float* dn_prev,
+                             CoreIn ci, const vd3d_render_params* rp, const vd3d_size_plan& pl, uint8_t* out_d,
+                             bool ident, bool* fused) {
   int r;
-  const int tw = pl.target_eye_w, th = pl.target_eye_h;
-  const int W = pl.resized_width, H = pl.resized_height;
-  const size_t tpx = (size_t)tw * th;
-  IngestArgs ia;
-  memset(&ia, 0, sizeof ia);
-  ia.frame = frame_d;
-  ia.depth = depth_d;
-  ia.depth_ch = depth_channels;
-  ia.src_w = src_w;
-  ia.src_h = src_h;
-  ia.cx0 = pl.crop_x0;
-  ia.cy0 = pl.crop_y0;
-  ia.cw = pl.crop_w;
-  ia.ch = pl.crop_h;
-  ia.tw = tw;
-  ia.th = th;
-  ia.tdf = (float*)ctx->tdf.p;
-  ia.alpha = 0.5f;
-  ia.one_minus_alpha = (float)(1 - 0.5);
-  ia.st = ctx->st;
+  const int tw = ia.tw, th = ia.th, W = ci.W, H = ci.H;
   FastLoop lp;
   memset(&lp, 0, sizeof lp);
   lp.ia = &ia;
+  lp.dn = dn;
+  lp.dn_prev = dn_prev;
+  lp.la = &la;
   FastPost post;
   if (!ident) {
-    if ((r = ensure(ctx, ctx->rgb_s, sizeof(float4) * tpx))) return r;
+    if ((r = ensure(ctx, ctx->rgb_s, sizeof(float4) * (size_t)tw * th))) return r;
     lp.rgbx_s = (float4*)ctx->rgb_s.p;
     post.src_rgbx = lp.rgbx_s;
     if (W != tw || H != th) {
@@ -1182,43 +1244,10 @@ static int enqueue_core_fast(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_
       post.src_rgbx = lp.rgbx;
     }
   }
-  lp.dn = (float*)(ctx->frame_parity ? ctx->dn1.p : ctx->dn0.p);
-  lp.dn_prev = (const float*)(ctx->frame_parity ? ctx->dn0.p : ctx->dn1.p);
-  LoopArgs la;
-  la.fg = rp->fg_shift;
-  la.mg = rp->mg_shift;
-  la.bg = rp->bg_shift;
-  la.ipd = rp->ipd_factor;
-  la.resized_width = W;
-  la.use_floating_window = rp->use_floating_window;
-  la.use_subject_tracking = rp->use_subject_tracking;
-  la.crop_count = (long long)(th * 3 / 4 - th / 4) * (long long)(tw * 3 / 4 - tw / 4);
-  la.npix = (long long)tpx;
-  la.dyn_min = (float)0.90;
-  la.dyn_span = (float)(1.15 - 0.90);
-  lp.la = &la;
-
-  const size_t eye_bytes = (size_t)W * H * 3;
-  CoreIn ci;
-  memset(&ci, 0, sizeof ci);
-  ci.depth = lp.dn;
-  ci.sh = th;
-  ci.sw = tw;
-  ci.src_u8 = ident ? frame_d : nullptr;
-  ci.src_pitch = src_w;
-  ci.cx0 = pl.crop_x0;
-  ci.cy0 = pl.crop_y0;
-  ci.W = W;
-  ci.H = H;
-  ci.p = loop_shift_params(rp);
-  const bool dof = rp->dof_strength > 0.0;
-  ci.grade = dof ? 0 : 1;
-  ci.sat = (float)rp->color_saturation;
-  ci.con = (float)rp->color_contrast;
-  ci.bri = (float)rp->color_brightness;
 
   // can k_render finish the frame?  SBS formats whose eye fit is the identity or cv2's integer 2:1 horizontal INTER_AREA
   *fused = false;
+  const bool dof = rp->dof_strength > 0.0;
   if (!ctx->stats_only && !dof && (rp->output_format == VD3D_FMT_HALF_SBS || rp->output_format == VD3D_FMT_FULL_SBS)) {
     FitPlan fp;
     if ((r = plan_fit(ctx, rp->output_format, W, H, pl.per_eye_w, pl.per_eye_h, fp))) return r;
@@ -1235,6 +1264,7 @@ static int enqueue_core_fast(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_
     post.per_eye_w = pl.per_eye_w;
     *fused = true;
   } else if (!ctx->stats_only) {
+    const size_t eye_bytes = (size_t)W * H * 3;
     if ((r = ensure(ctx, ctx->eyeL, eye_bytes))) return r;
     if ((r = ensure(ctx, ctx->eyeR, eye_bytes))) return r;
     ci.left = (uint8_t*)ctx->eyeL.p;
@@ -1243,174 +1273,83 @@ static int enqueue_core_fast(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_
   return run_core_fast(ctx, ci, &lp, post);
 }
 
-// enqueue one loop iteration on ctx->stream; inputs/outputs are DEVICE pointers
-static int enqueue_frame(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_t* depth_d, int depth_channels,
-                         int src_h, int src_w, const vd3d_render_params* rp, const vd3d_size_plan& pl,
-                         uint8_t* out_d) {
+// exact-path core of one loop iteration, one kernel per reference op: ingest + TemporalDepthFilter,
+// DepthPercentileEMA, normalisation + subject estimate, then pixel_shift_cuda into eyeL / eyeR
+static int enqueue_core_exact(vd3d_ctx* ctx, IngestArgs ia, const LoopArgs& la, float* dn, const float* dn_prev,
+                              CoreIn ci, bool ident) {
   cudaStream_t s = ctx->stream;
   int r;
-  ProfScope frame_scope(ctx, 0);
-  const int tw = pl.target_eye_w, th = pl.target_eye_h;
-  const int W = pl.resized_width, H = pl.resized_height;
-  if (tw < 8 || th < 8 || W < 8 || H < 8) return fail(ctx, VD3D_ERR_ARG, "frame too small");
-  size_t tpx = (size_t)tw * th;
-  if (ctx->tdf_w != tw || ctx->tdf_h != th) {
-    if ((r = ensure(ctx, ctx->tdf, sizeof(float) * tpx))) return r;
-    if ((r = ensure(ctx, ctx->dn0, sizeof(float) * tpx))) return r;
-    if ((r = ensure(ctx, ctx->dn1, sizeof(float) * tpx))) return r;
-    ctx->tdf_w = tw;
-    ctx->tdf_h = th;
-    if ((r = vd3d_reset_state(ctx, VD3D_STATE_CLIP))) return r;
-  }
-  bool ident = (tw == pl.crop_w && th == pl.crop_h && W == tw && H == th);
-  bool need_rgb_s = !ident;
-  if ((r = begin_frame(ctx))) return r;
-  ctx->launches += 2;
-
-  const bool fastp = !ctx->exact && render_supports(rp->enable_feathering ? 1 : 0, rp->blur_ksize);
-  bool fused = false;
-  if (fastp) {
-    if ((r = enqueue_core_fast(ctx, frame_d, depth_d, depth_channels, src_h, src_w, rp, pl, out_d, ident, &fused)))
-      return r;
-    if (ctx->stats_only || fused) {
-      ctx->frame_parity ^= 1;
-      return VD3D_OK;
-    }
-  } else {
-  // ---- ingest + TemporalDepthFilter
-  IngestArgs ia;
-  ia.frame = frame_d;
-  ia.depth = depth_d;
-  ia.depth_ch = depth_channels;
-  ia.src_w = src_w;
-  ia.src_h = src_h;
-  ia.cx0 = pl.crop_x0;
-  ia.cy0 = pl.crop_y0;
-  ia.cw = pl.crop_w;
-  ia.ch = pl.crop_h;
-  ia.tw = tw;
-  ia.th = th;
-  ia.tdf = (float*)ctx->tdf.p;
-  ia.rgb_s = nullptr;
-  if (need_rgb_s) {
+  const int tw = ia.tw, th = ia.th, W = ci.W, H = ci.H;
+  const size_t tpx = (size_t)tw * th;
+  if (!ident) {
     if ((r = ensure(ctx, ctx->rgb_s, sizeof(float) * 3 * tpx))) return r;
     ia.rgb_s = (float*)ctx->rgb_s.p;
   }
-  ia.alpha = 0.5f;
-  ia.one_minus_alpha = (float)(1 - 0.5);
-  ia.st = ctx->st;
   launch_ingest(ia, s);
+  ctx->launches += 1;
   // ---- DepthPercentileEMA(p_lo=.02, p_hi=.98, alpha=.92)
   uint32_t l0, l1, h0, h1;
   float wlo, whi;
   quantile_rank(0.02, (long long)tpx, l0, l1, wlo);
   quantile_rank(0.98, (long long)tpx, h0, h1, whi);
   launch_set_ranks(ctx->jm[0].tg, l0, l1, h0, h1, s);
-  SelJob pj = make_job(ctx->jm[0], (const float*)ctx->tdf.p, tw, 0, tw, 0, th, 0, 4, 0, false);
+  ctx->launches += 1;
+  SelJob pj = make_job(ctx->jm[0], ia.tdf, tw, 0, tw, 0, th, 0, 4, 0, false);
   launch_select(pj, nullptr, sel_blocks(th), s);
+  ctx->launches += kSelectLaunches;
   launch_fin_pct(pj, wlo, whi, 0.92f, (float)(1 - 0.92), ctx->st, ctx->fs, s);
-  float* dn = (float*)(ctx->frame_parity ? ctx->dn1.p : ctx->dn0.p);
-  const float* dn_prev = (const float*)(ctx->frame_parity ? ctx->dn0.p : ctx->dn1.p);
-  launch_normalize((const float*)ctx->tdf.p, dn, dn_prev, th, tw, ctx->st, ctx->fs, s);
+  ctx->launches += 1;
+  launch_normalize(ia.tdf, dn, dn_prev, th, tw, ctx->st, ctx->fs, s);
+  ctx->launches += 1;
   SelJob sn = make_job(ctx->jm[1], dn, tw, tw / 5, tw * 4 / 5, th / 5, th * 4 / 5, 1, 1, 1, true);
   launch_select(sn, nullptr, sel_blocks(th * 4 / 5 - th / 5), s);
-  LoopArgs la;
-  la.fg = rp->fg_shift;
-  la.mg = rp->mg_shift;
-  la.bg = rp->bg_shift;
-  la.ipd = rp->ipd_factor;
-  la.resized_width = W;
-  la.use_floating_window = rp->use_floating_window;
-  la.use_subject_tracking = rp->use_subject_tracking;
-  la.crop_count = (long long)(th * 3 / 4 - th / 4) * (long long)(tw * 3 / 4 - tw / 4);
-  la.npix = (long long)tpx;
-  la.dyn_min = (float)0.90;
-  la.dyn_span = (float)(1.15 - 0.90);
+  ctx->launches += kSelectLaunches;
   launch_fin_norm(sn, la, ctx->st, ctx->fs, s);
-  ctx->launches += 1 + 1 + 6 + 1 + 1 + 6 + 1;
+  ctx->launches += 1;
 
   // ---- pixel_shift_cuda
-  size_t eye_bytes = (size_t)W * H * 3;
+  const size_t eye_bytes = (size_t)W * H * 3;
   if ((r = ensure(ctx, ctx->eyeL, eye_bytes))) return r;
   if ((r = ensure(ctx, ctx->eyeR, eye_bytes))) return r;
-  CoreIn ci;
-  ci.depth = dn;
-  ci.sh = th;
-  ci.sw = tw;
-  ci.src_u8 = nullptr;
-  ci.src_pitch = src_w;
-  ci.cx0 = pl.crop_x0;
-  ci.cy0 = pl.crop_y0;
-  ci.src_f32 = nullptr;
-  if (ident) {
-    ci.src_u8 = frame_d;
-  } else {
-    const float* base = (const float*)ctx->rgb_s.p;
-    if (W == tw && H == th) {
-      ci.src_f32 = base;
-    } else {
+  if (!ident) {
+    ci.src_f32 = ia.rgb_s;
+    if (W != tw || H != th) {
       if ((r = ensure(ctx, ctx->frameB, sizeof(float) * 3 * (size_t)W * H))) return r;
-      launch_resize_planar(base, 3, th, tw, (float*)ctx->frameB.p, H, W, s);
+      launch_resize_planar(ia.rgb_s, 3, th, tw, (float*)ctx->frameB.p, H, W, s);
       ctx->launches += 1;
       ci.src_f32 = (const float*)ctx->frameB.p;
     }
   }
-  ci.W = W;
-  ci.H = H;
-  ci.p = loop_shift_params(rp);
-  bool dof = rp->dof_strength > 0.0;
-  ci.grade = dof ? 0 : 1;
-  ci.sat = (float)rp->color_saturation;
-  ci.con = (float)rp->color_contrast;
-  ci.bri = (float)rp->color_brightness;
   ci.left = (uint8_t*)ctx->eyeL.p;
   ci.right = (uint8_t*)ctx->eyeR.p;
-  if ((r = run_core(ctx, ci))) return r;
+  return run_core(ctx, ci);
+}
 
-  if (ctx->stats_only) {
-    ctx->frame_parity ^= 1;
-    return VD3D_OK;
-  }
-  }  // exact path
-  const size_t eye_bytes = (size_t)W * H * 3;
-  const bool dof = rp->dof_strength > 0.0;
-  float* dn = (float*)(ctx->frame_parity ? ctx->dn1.p : ctx->dn0.p);
+// DOF (when on), then bars + sharpen + eye fit + pack of the eyes in eyeL / eyeR into out_d
+static int enqueue_dof_post(vd3d_ctx* ctx, const vd3d_render_params* rp, const vd3d_size_plan& pl, const float* dn,
+                            uint8_t* out_d) {
+  cudaStream_t s = ctx->stream;
+  int r;
+  const int W = pl.resized_width, H = pl.resized_height;
   const uint8_t* eye_l = (const uint8_t*)ctx->eyeL.p;
   const uint8_t* eye_r = (const uint8_t*)ctx->eyeR.p;
-  if (dof) {
+  if (rp->dof_strength > 0.0) {
+    const size_t eye_bytes = (size_t)W * H * 3;
     if ((r = ensure_dof_kernels(ctx, rp->dof_strength, 5))) return r;
     if ((r = ensure(ctx, ctx->eyeL2, eye_bytes))) return r;
     if ((r = ensure(ctx, ctx->eyeR2, eye_bytes))) return r;
-    DofArgs da;
+    DofArgs da = dof_args(ctx, 5, H, W, dn, pl.target_eye_h, pl.target_eye_w, rp->color_saturation,
+                          rp->color_contrast, rp->color_brightness);
     da.src_l = eye_l;
     da.src_r = eye_r;
     da.dst_l = (uint8_t*)ctx->eyeL2.p;
     da.dst_r = (uint8_t*)ctx->eyeR2.p;
-    da.H = H;
-    da.W = W;
-    da.depth = dn;
-    da.dh = th;
-    da.dw = tw;
-    da.focal = 0.f;
     da.fs = ctx->fs;  // focal comes from the FocalDepthTracker state on the device
-    da.focus_w = (float)(0.35 + 1e-6);
-    da.idx_max = (float)(5 - 1 - 1e-6);
-    da.nlevels = 5;
-    for (int i = 0; i < 8; ++i) {
-      da.ksize[i] = ctx->dof_ksize[i];
-      da.koff[i] = ctx->dof_koff[i];
-    }
-    da.kern = (const float*)ctx->dof_kern.p;
-    da.halo = ctx->dof_halo;
-    da.sat = (float)rp->color_saturation;
-    da.con = (float)rp->color_contrast;
-    da.bri = (float)rp->color_brightness;
     launch_dof(da, 2, s);
     ctx->launches += 1;
     eye_l = da.dst_l;
     eye_r = da.dst_r;
   }
-  // ---- bars + sharpen + fit + pack
   FitPlan fp;
   if ((r = plan_fit(ctx, rp->output_format, W, H, pl.per_eye_w, pl.per_eye_h, fp))) return r;
   PostArgs pa;
@@ -1436,6 +1375,86 @@ static int enqueue_frame(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_t* d
   launch_post(pa, s);
   ctx->launches += 1;
   CK(cudaGetLastError());
+  return VD3D_OK;
+}
+
+// enqueue one loop iteration on ctx->stream; inputs/outputs are DEVICE pointers
+static int enqueue_frame(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_t* depth_d, int depth_channels,
+                         int src_h, int src_w, const vd3d_render_params* rp, const vd3d_size_plan& pl,
+                         uint8_t* out_d) {
+  int r;
+  ProfScope frame_scope(ctx, 0);
+  const int tw = pl.target_eye_w, th = pl.target_eye_h;
+  const int W = pl.resized_width, H = pl.resized_height;
+  if (tw < 8 || th < 8 || W < 8 || H < 8) return fail(ctx, VD3D_ERR_ARG, "frame too small");
+  const size_t tpx = (size_t)tw * th;
+  if (ctx->tdf_w != tw || ctx->tdf_h != th) {
+    if ((r = ensure(ctx, ctx->tdf, sizeof(float) * tpx))) return r;
+    if ((r = ensure(ctx, ctx->dn0, sizeof(float) * tpx))) return r;
+    if ((r = ensure(ctx, ctx->dn1, sizeof(float) * tpx))) return r;
+    ctx->tdf_w = tw;
+    ctx->tdf_h = th;
+    if ((r = vd3d_reset_state(ctx, VD3D_STATE_CLIP))) return r;
+  }
+  if ((r = begin_frame(ctx))) return r;
+
+  // ---- loop-level inputs: ingest + TemporalDepthFilter, trackers, normalised-depth ping-pong, pixel_shift_cuda
+  IngestArgs ia;
+  memset(&ia, 0, sizeof ia);
+  ia.frame = frame_d;
+  ia.depth = depth_d;
+  ia.depth_ch = depth_channels;
+  ia.src_w = src_w;
+  ia.src_h = src_h;
+  ia.cx0 = pl.crop_x0;
+  ia.cy0 = pl.crop_y0;
+  ia.cw = pl.crop_w;
+  ia.ch = pl.crop_h;
+  ia.tw = tw;
+  ia.th = th;
+  ia.tdf = (float*)ctx->tdf.p;
+  ia.alpha = 0.5f;
+  ia.one_minus_alpha = (float)(1 - 0.5);
+  ia.st = ctx->st;
+  LoopArgs la;
+  la.fg = rp->fg_shift;
+  la.mg = rp->mg_shift;
+  la.bg = rp->bg_shift;
+  la.ipd = rp->ipd_factor;
+  la.resized_width = W;
+  la.use_floating_window = rp->use_floating_window;
+  la.use_subject_tracking = rp->use_subject_tracking;
+  la.crop_count = (long long)(th * 3 / 4 - th / 4) * (long long)(tw * 3 / 4 - tw / 4);
+  la.npix = (long long)tpx;
+  la.dyn_min = (float)0.90;
+  la.dyn_span = (float)(1.15 - 0.90);
+  float* dn = (float*)(ctx->frame_parity ? ctx->dn1.p : ctx->dn0.p);
+  const float* dn_prev = (const float*)(ctx->frame_parity ? ctx->dn0.p : ctx->dn1.p);
+  const bool ident = (tw == pl.crop_w && th == pl.crop_h && W == tw && H == th);
+  CoreIn ci;
+  memset(&ci, 0, sizeof ci);
+  ci.depth = dn;
+  ci.sh = th;
+  ci.sw = tw;
+  ci.src_u8 = ident ? frame_d : nullptr;
+  ci.src_pitch = src_w;
+  ci.cx0 = pl.crop_x0;
+  ci.cy0 = pl.crop_y0;
+  ci.W = W;
+  ci.H = H;
+  ci.p = loop_shift_params(rp);
+  ci.grade = rp->dof_strength > 0.0 ? 0 : 1;
+  ci.sat = (float)rp->color_saturation;
+  ci.con = (float)rp->color_contrast;
+  ci.bri = (float)rp->color_brightness;
+
+  bool fused = false;
+  if (!ctx->exact && render_supports(rp->enable_feathering ? 1 : 0, rp->blur_ksize))
+    r = enqueue_core_fast(ctx, ia, la, dn, dn_prev, ci, rp, pl, out_d, ident, &fused);
+  else
+    r = enqueue_core_exact(ctx, ia, la, dn, dn_prev, ci, ident);
+  if (r) return r;
+  if (!ctx->stats_only && !fused && (r = enqueue_dof_post(ctx, rp, pl, dn, out_d))) return r;
   ctx->frame_parity ^= 1;
   return VD3D_OK;
 }
@@ -1503,27 +1522,11 @@ static int run_depth_group(vd3d_ctx* ctx, vd3d_depth* parent, int c, int slot0, 
   }
   vd3d_ctx::DepthGraph& g = ctx->dg[c][nb];
   if (!g.exec) {
-    uint64_t l0 = vd3d_depth_launch_count(e);
-    if (cudaStreamBeginCapture(ctx->s_depth[c], cudaStreamCaptureModeThreadLocal) != cudaSuccess) {
-      fprintf(stderr, "vd3d: CUDA graph capture unavailable (%s); continuing with eager launches\n",
-              cudaGetErrorString(cudaGetLastError()));
-      ctx->use_graphs = 0;
+    const uint64_t l0 = vd3d_depth_launch_count(e);
+    if (!capture(ctx, ctx->s_depth[c], &g.exec,
+                 [&] { return vd3d_depth_infer_batch_device(e, nb, f_d, src_h, src_w, d_d, nullptr, 0); }))
       return eager();
-    }
-    int r = vd3d_depth_infer_batch_device(e, nb, f_d, src_h, src_w, d_d, nullptr, 0);
-    cudaGraph_t graph = nullptr;
-    cudaError_t ce = cudaStreamEndCapture(ctx->s_depth[c], &graph);
-    uint64_t n = vd3d_depth_launch_count(e) - l0;
-    if (r != VD3D_OK || ce != cudaSuccess || !graph || cudaGraphInstantiate(&g.exec, graph, 0) != cudaSuccess) {
-      fprintf(stderr, "vd3d: CUDA graph capture failed (r=%d, %s); continuing with eager launches\n", r,
-              cudaGetErrorString(cudaGetLastError()));
-      if (graph) cudaGraphDestroy(graph);
-      g.exec = nullptr;
-      ctx->use_graphs = 0;
-      return eager();
-    }
-    cudaGraphDestroy(graph);
-    g.n = n;
+    g.n = vd3d_depth_launch_count(e) - l0;
   }
   CK(cudaGraphLaunch(g.exec, ctx->s_depth[c]));
   vd3d_depth_add_launches(parent, g.n);
@@ -1540,26 +1543,16 @@ static void drop_graphs(vd3d_ctx* ctx) {
   ctx->fg_warm = 0;
 }
 
-// One frame on the staging buffers of slot b: [depth inference ->] render_sbs_3d loop body.
+// One frame on the staging buffers of slot b: the render_sbs_3d loop body.
 // After two eager frames of an unchanged configuration the launch sequence (~200 kernels) is captured
 // once per (slot, parity) into a CUDA graph and replayed; all scalars it depends on live on the device.
-static int run_frame_slot(vd3d_ctx* ctx, vd3d_depth* depth, int b, int depth_channels, int src_h, int src_w,
+static int run_frame_slot(vd3d_ctx* ctx, int b, int depth_channels, int src_h, int src_w,
                           const vd3d_render_params* rp, const vd3d_size_plan& pl) {
   const uint8_t* f_d = (const uint8_t*)ctx->in_frame[b].p;
   uint8_t* d_d = (uint8_t*)ctx->in_depth[b].p;
   uint8_t* o_d = (uint8_t*)ctx->out_dev[b].p;
-  auto eager = [&]() -> int {
-    int r;
-    if (depth) {
-      ProfScope ps(ctx, 2);
-      if ((r = vd3d_depth_infer_device(depth, f_d, src_h, src_w, d_d, nullptr, 0))) {
-        ctx->err = std::string("depth engine: ") + vd3d_depth_last_error(depth);
-        return r;
-      }
-    }
-    return enqueue_frame(ctx, f_d, d_d, depth ? 1 : depth_channels, src_h, src_w, rp, pl, o_d);
-  };
-  bool same = ctx->fg_h == src_h && ctx->fg_w == src_w && ctx->fg_dch == depth_channels && ctx->fg_depth == depth &&
+  auto eager = [&]() { return enqueue_frame(ctx, f_d, d_d, depth_channels, src_h, src_w, rp, pl, o_d); };
+  bool same = ctx->fg_h == src_h && ctx->fg_w == src_w && ctx->fg_dch == depth_channels &&
               memcmp(&ctx->fg_rp, rp, sizeof *rp) == 0;
   if (ctx->fg_epoch != ctx->res_epoch) {  // another entry point moved / rewrote something the graphs bake in
     drop_graphs(ctx);
@@ -1570,7 +1563,6 @@ static int run_frame_slot(vd3d_ctx* ctx, vd3d_depth* depth, int b, int depth_cha
     ctx->fg_h = src_h;
     ctx->fg_w = src_w;
     ctx->fg_dch = depth_channels;
-    ctx->fg_depth = depth;
     ctx->fg_rp = *rp;
   }
   if (!ctx->use_graphs || ctx->prof || ctx->fg_warm < 3) {
@@ -1580,36 +1572,15 @@ static int run_frame_slot(vd3d_ctx* ctx, vd3d_depth* depth, int b, int depth_cha
   const int par = ctx->frame_parity;
   vd3d_ctx::FrameGraph& g = ctx->fg[b][par];
   if (!g.exec) {
-    uint64_t l0 = ctx->launches, d0 = depth ? vd3d_depth_launch_count(depth) : 0;
-    if (cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) {
-      fprintf(stderr, "vd3d: CUDA graph capture unavailable (%s); continuing with eager launches\n",
-              cudaGetErrorString(cudaGetLastError()));
-      ctx->use_graphs = 0;
-      return eager();
-    }
-    int r = eager();
-    cudaGraph_t graph = nullptr;
-    cudaError_t ce = cudaStreamEndCapture(ctx->stream, &graph);
+    const uint64_t l0 = ctx->launches;
+    const bool ok = capture(ctx, ctx->stream, &g.exec, eager);
     ctx->frame_parity = par;  // capture does not execute
-    uint64_t nl = ctx->launches - l0, nd = depth ? vd3d_depth_launch_count(depth) - d0 : 0;
+    g.n_ctx = ctx->launches - l0;
     ctx->launches = l0;
-    if (depth) vd3d_depth_add_launches(depth, (uint64_t)0 - nd);
-    if (r != VD3D_OK || ce != cudaSuccess || !graph ||
-        cudaGraphInstantiate(&g.exec, graph, 0) != cudaSuccess) {
-      fprintf(stderr, "vd3d: CUDA graph capture failed (r=%d, %s); continuing with eager launches\n", r,
-              cudaGetErrorString(cudaGetLastError()));
-      if (graph) cudaGraphDestroy(graph);
-      g.exec = nullptr;
-      ctx->use_graphs = 0;  // fall back to eager launches for the rest of this ctx
-      return eager();
-    }
-    cudaGraphDestroy(graph);
-    g.n_ctx = nl;
-    g.n_depth = nd;
+    if (!ok) return eager();
   }
   CK(cudaGraphLaunch(g.exec, ctx->stream));
   ctx->launches += g.n_ctx;
-  if (depth) vd3d_depth_add_launches(depth, g.n_depth);
   ctx->frame_parity ^= 1;
   return VD3D_OK;
 }
@@ -1640,12 +1611,10 @@ int vd3d_render_frame(vd3d_ctx* ctx, const uint8_t* frame_bgr, const uint8_t* de
   if ((r = copy_in(ctx, ctx->in_frame[0], frame_bgr, fb, mem, s, &f_d))) return r;
   if ((r = copy_in(ctx, ctx->in_depth[0], depth, db, mem, s, &d_d))) return r;
   size_t ob = out_bytes(rp, pl);
-  uint8_t* o_d = out_bgr;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->out_dev[0], ob))) return r;
-    o_d = (uint8_t*)ctx->out_dev[0].p;
-  }
-  if ((r = enqueue_frame(ctx, (const uint8_t*)f_d, (const uint8_t*)d_d, depth_channels, src_h, src_w, rp, pl, o_d)))
+  void* o_d;
+  if ((r = stage_out(ctx, ctx->out_dev[0], out_bgr, ob, mem, &o_d))) return r;
+  if ((r = enqueue_frame(ctx, (const uint8_t*)f_d, (const uint8_t*)d_d, depth_channels, src_h, src_w, rp, pl,
+                         (uint8_t*)o_d)))
     return r;
   if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(out_bgr, o_d, ob, cudaMemcpyDeviceToHost, s));
   if (info) return fetch_info(ctx, info);
@@ -1685,7 +1654,7 @@ int vd3d_render_clip(vd3d_ctx* ctx, int n, const uint8_t* const* frames, const u
       CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[b], 0));
       if (i >= kSlots) CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_d2h[b], 0));
     }
-    if ((r = run_frame_slot(ctx, nullptr, b, depth_channels, src_h, src_w, rp, pl))) return r;
+    if ((r = run_frame_slot(ctx, b, depth_channels, src_h, src_w, rp, pl))) return r;
     if (infos && (r = fetch_info(ctx, &infos[i]))) return r;
     CK(cudaEventRecord(ctx->ev_done[b], ctx->stream));
     CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[b], 0));
@@ -1763,7 +1732,7 @@ int vd3d_render_clip_depth(vd3d_ctx* ctx, vd3d_depth* depth, int n, const uint8_
     for (int j = 0; j < nb; ++j) {
       const int sl = slot0 + j;
       if (reuse) CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_d2h[sl], 0));  // out_dev[slot] drained
-      if ((r = run_frame_slot(ctx, nullptr, sl, 1, src_h, src_w, rp, pl))) return r;
+      if ((r = run_frame_slot(ctx, sl, 1, src_h, src_w, rp, pl))) return r;
       CK(cudaEventRecord(ctx->ev_done[sl], ctx->stream));
       CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[sl], 0));
       CK(cudaMemcpyAsync(outs[i0 + j], ctx->out_dev[sl].p, ob, kout, ctx->s_d2h));
@@ -1891,7 +1860,6 @@ int vd3d_release_depth(vd3d_ctx* ctx, vd3d_depth* depth) {
       ctx->dclone[i] = nullptr;
     }
     ctx->dclone_parent = nullptr;
-    ctx->fg_depth = nullptr;
   }
   return VD3D_OK;
 }
@@ -1907,8 +1875,7 @@ int vd3d_check_config(vd3d_ctx* ctx, int src_h, int src_w, const vd3d_render_par
   if (r) return fail(ctx, r, "unsupported output format / sizes");
   if (pl.target_eye_w < 8 || pl.target_eye_h < 8 || pl.resized_width < 8 || pl.resized_height < 8)
     return fail(ctx, VD3D_ERR_ARG, "frame too small");
-  if (rp->enable_feathering && (rp->blur_ksize < 1 || rp->blur_ksize > 63))
-    return fail(ctx, VD3D_ERR_UNSUPPORTED, "blur_ksize must be in [1,63]");
+  if ((r = check_blur_ksize(ctx, rp->enable_feathering, rp->blur_ksize))) return r;
   FitPlan fp;
   if ((r = plan_fit(ctx, rp->output_format, pl.resized_width, pl.resized_height, pl.per_eye_w, pl.per_eye_h, fp)))
     return r;
@@ -1925,20 +1892,14 @@ int vd3d_resize_cubic(vd3d_ctx* ctx, const uint8_t* src, int h, int w, int ch, u
   const void* s_d;
   int r;
   if ((r = copy_in(ctx, ctx->eyeL, src, (size_t)h * w * ch, mem, s, &s_d))) return r;
-  uint8_t* o_d = dst;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->out_dev[0], (size_t)oh * ow * ch))) return r;
-    o_d = (uint8_t*)ctx->out_dev[0].p;
-  }
+  void* o_d;
+  if ((r = stage_out(ctx, ctx->out_dev[0], dst, (size_t)oh * ow * ch, mem, &o_d))) return r;
   if (h == oh && w == ow)
     CK(cudaMemcpyAsync(o_d, s_d, (size_t)h * w * ch, cudaMemcpyDeviceToDevice, s));  // cv2.resize copies on equal sizes
   else
-    launch_resize_cubic_u8((const uint8_t*)s_d, h, w, ch, o_d, oh, ow, s);
+    launch_resize_cubic_u8((const uint8_t*)s_d, h, w, ch, (uint8_t*)o_d, oh, ow, s);
   ctx->launches += 1;
-  CK(cudaGetLastError());
-  if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(dst, o_d, (size_t)oh * ow * ch, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return VD3D_OK;
+  return stage_finish(ctx, dst, o_d, (size_t)oh * ow * ch, mem);
 }
 int vd3d_resize_cubic_u8(vd3d_ctx* ctx, const uint8_t* src, int h, int w, uint8_t* dst, int oh, int ow, int mem) {
   return vd3d_resize_cubic(ctx, src, h, w, 1, dst, oh, ow, mem);
@@ -1953,17 +1914,11 @@ int vd3d_add_weighted(vd3d_ctx* ctx, const uint8_t* a, double alpha, const uint8
   const void *a_d, *b_d;
   int r;
   if ((r = copy_in(ctx, ctx->eyeL, a, n, mem, s, &a_d)) || (r = copy_in(ctx, ctx->eyeR, b, n, mem, s, &b_d))) return r;
-  uint8_t* o_d = dst;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->out_dev[0], n))) return r;
-    o_d = (uint8_t*)ctx->out_dev[0].p;
-  }
-  launch_add_weighted((const uint8_t*)a_d, (float)alpha, (const uint8_t*)b_d, (float)beta, o_d, n, s);
+  void* o_d;
+  if ((r = stage_out(ctx, ctx->out_dev[0], dst, n, mem, &o_d))) return r;
+  launch_add_weighted((const uint8_t*)a_d, (float)alpha, (const uint8_t*)b_d, (float)beta, (uint8_t*)o_d, n, s);
   ctx->launches += 1;
-  CK(cudaGetLastError());
-  if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(dst, o_d, n, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return VD3D_OK;
+  return stage_finish(ctx, dst, o_d, n, mem);
 }
 
 // apply_color_grade (core/render_3d.py:734-767) on f32 RGB planes [3,h,w] in 0..1
@@ -1976,17 +1931,11 @@ int vd3d_color_grade(vd3d_ctx* ctx, const float* rgb, int h, int w, double sat, 
   const void* r_d;
   int r;
   if ((r = copy_in(ctx, ctx->in_rgbf, rgb, bytes, mem, s, &r_d))) return r;
-  float* o_d = out;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->frameB, bytes))) return r;
-    o_d = (float*)ctx->frameB.p;
-  }
-  launch_grade_f32((const float*)r_d, o_d, h * w, (float)sat, (float)con, (float)bri, s);
+  void* o_d;
+  if ((r = stage_out(ctx, ctx->frameB, out, bytes, mem, &o_d))) return r;
+  launch_grade_f32((const float*)r_d, (float*)o_d, h * w, (float)sat, (float)con, (float)bri, s);
   ctx->launches += 1;
-  CK(cudaGetLastError());
-  if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(out, o_d, bytes, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return VD3D_OK;
+  return stage_finish(ctx, out, o_d, bytes, mem);
 }
 
 int vd3d_sharpen(vd3d_ctx* ctx, const uint8_t* src, int h, int w, double factor, uint8_t* dst, int mem) {
@@ -1997,36 +1946,14 @@ int vd3d_sharpen(vd3d_ctx* ctx, const uint8_t* src, int h, int w, double factor,
   const void* s_d;
   int r;
   if ((r = copy_in(ctx, ctx->eyeL, src, bytes, mem, s, &s_d))) return r;
-  uint8_t* o_d = dst;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->out_dev[0], bytes))) return r;
-    o_d = (uint8_t*)ctx->out_dev[0].p;
-  }
-  PostArgs pa;
-  memset(&pa, 0, sizeof pa);
-  pa.left = (const uint8_t*)s_d;
-  pa.right = (const uint8_t*)s_d;
-  pa.H = h;
-  pa.W = w;
-  pa.fs = nullptr;
+  void* o_d;
+  if ((r = stage_out(ctx, ctx->out_dev[0], dst, bytes, mem, &o_d))) return r;
+  PostArgs pa = single_eye_post(s_d, h, w, (uint8_t*)o_d, w, h);
   pa.sharpen = 1;
   sharpen_coeffs(factor, pa.kc, pa.ke);
-  pa.fmt = VD3D_FMT_INTERLACED;  // single-eye pass-through layout
-  pa.per_eye_w = w;
-  pa.per_eye_h = h;
-  pa.fit_w = w;
-  pa.fit_h = h;
-  pa.sx = pa.sy = 1;
-  pa.inv_area = 1.f;
-  pa.out = o_d;
-  pa.out_w = w;
-  pa.out_h = h;
   launch_post(pa, s);
   ctx->launches += 1;
-  CK(cudaGetLastError());
-  if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(dst, o_d, bytes, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return VD3D_OK;
+  return stage_finish(ctx, dst, o_d, bytes, mem);
 }
 
 // heal_missing_pixels (core/render_3d.py:431-459) on f32 RGB planes [3,h,w]; edge_mask [h,w] or null
@@ -2041,17 +1968,11 @@ int vd3d_heal(vd3d_ctx* ctx, const float* warped, const float* original, const f
   if ((r = copy_in(ctx, ctx->in_rgbf, warped, bytes, mem, s, &w_d))) return r;
   if ((r = copy_in(ctx, ctx->frameB, original, bytes, mem, s, &o_d))) return r;
   if (edge_mask && (r = copy_in(ctx, ctx->in_depthf, edge_mask, bytes / 3, mem, s, &e_d))) return r;
-  float* out_d = out;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->rgb_s, bytes))) return r;
-    out_d = (float*)ctx->rgb_s.p;
-  }
-  launch_heal((const float*)w_d, (const float*)o_d, (const float*)e_d, out_d, h, w, (float)heal_strength, s);
+  void* out_d;
+  if ((r = stage_out(ctx, ctx->rgb_s, out, bytes, mem, &out_d))) return r;
+  launch_heal((const float*)w_d, (const float*)o_d, (const float*)e_d, (float*)out_d, h, w, (float)heal_strength, s);
   ctx->launches += 1;
-  CK(cudaGetLastError());
-  if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(out, out_d, bytes, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return VD3D_OK;
+  return stage_finish(ctx, out, out_d, bytes, mem);
 }
 
 // format_3d_output / generate_anaglyph_3d (core/render_3d.py:837-883) on two same-size u8 BGR eyes
@@ -2071,11 +1992,8 @@ int vd3d_pack(vd3d_ctx* ctx, const uint8_t* left, const uint8_t* right, int h, i
   int r;
   if ((r = copy_in(ctx, ctx->eyeL, left, bytes, mem, s, &l_d))) return r;
   if ((r = copy_in(ctx, ctx->eyeR, right, bytes, mem, s, &r_d))) return r;
-  uint8_t* o_d = dst;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->out_dev[0], obytes))) return r;
-    o_d = (uint8_t*)ctx->out_dev[0].p;
-  }
+  void* o_d;
+  if ((r = stage_out(ctx, ctx->out_dev[0], dst, obytes, mem, &o_d))) return r;
   PostArgs pa;
   memset(&pa, 0, sizeof pa);
   pa.left = (const uint8_t*)l_d;
@@ -2089,15 +2007,12 @@ int vd3d_pack(vd3d_ctx* ctx, const uint8_t* left, const uint8_t* right, int h, i
   pa.fit_h = h;
   pa.sx = pa.sy = 1;
   pa.inv_area = 1.f;
-  pa.out = o_d;
+  pa.out = (uint8_t*)o_d;
   pa.out_w = sbs ? 2 * w : w;
   pa.out_h = h;
   launch_post(pa, s);
   ctx->launches += 1;
-  CK(cudaGetLastError());
-  if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(dst, o_d, obytes, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return VD3D_OK;
+  return stage_finish(ctx, dst, o_d, obytes, mem);
 }
 
 // eye fit on one u8 BGR image: keep_aspect != 0 -> pad_to_aspect_ratio(image, target_w, target_h) with a black canvas
@@ -2112,32 +2027,15 @@ int vd3d_fit_eye(vd3d_ctx* ctx, const uint8_t* src, int h, int w, int target_w, 
   const void* s_d;
   int r;
   if ((r = copy_in(ctx, ctx->eyeL, src, bytes, mem, s, &s_d))) return r;
-  uint8_t* o_d = dst;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->out_dev[0], obytes))) return r;
-    o_d = (uint8_t*)ctx->out_dev[0].p;
-  }
+  void* o_d;
+  if ((r = stage_out(ctx, ctx->out_dev[0], dst, obytes, mem, &o_d))) return r;
   FitPlan fp;
   if ((r = plan_fit(ctx, keep_aspect ? VD3D_FMT_FULL_SBS : VD3D_FMT_HALF_SBS, w, h, target_w, target_h, fp, 1))) return r;
-  PostArgs pa;
-  memset(&pa, 0, sizeof pa);
-  pa.left = (const uint8_t*)s_d;
-  pa.right = (const uint8_t*)s_d;
-  pa.H = h;
-  pa.W = w;
-  pa.fmt = VD3D_FMT_INTERLACED;  // single-eye pass-through layout
-  pa.per_eye_w = target_w;
-  pa.per_eye_h = target_h;
+  PostArgs pa = single_eye_post(s_d, h, w, (uint8_t*)o_d, target_w, target_h);
   set_fit(pa, fp);
-  pa.out = o_d;
-  pa.out_w = target_w;
-  pa.out_h = target_h;
   launch_post(pa, s);
   ctx->launches += 1;
-  CK(cudaGetLastError());
-  if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(dst, o_d, obytes, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return VD3D_OK;
+  return stage_finish(ctx, dst, o_d, obytes, mem);
 }
 
 // host-only test hook: the cv2 computeResizeAreaTab restatement used by the fractional INTER_AREA fit.
@@ -2183,41 +2081,15 @@ int vd3d_dof_grade(vd3d_ctx* ctx, const uint8_t* eye_bgr, int h, int w, const fl
     if ((r = copy_in(ctx, ctx->in_depthf, depth01, sizeof(float) * (size_t)dh * dw, mem, s, &dp_d))) return r;
     if ((r = ensure_dof_kernels(ctx, max_sigma, 5))) return r;
   }
-  uint8_t* o_d = dst;
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = ensure(ctx, ctx->out_dev[0], bytes))) return r;
-    o_d = (uint8_t*)ctx->out_dev[0].p;
-  }
-  DofArgs da;
-  memset(&da, 0, sizeof da);
+  void* o_d;
+  if ((r = stage_out(ctx, ctx->out_dev[0], dst, bytes, mem, &o_d))) return r;
+  DofArgs da = dof_args(ctx, dof ? 5 : 1, h, w, (const float*)dp_d, dh, dw, sat, con, bri);
   da.src_l = da.src_r = (const uint8_t*)s_d;
-  da.dst_l = da.dst_r = o_d;
-  da.H = h;
-  da.W = w;
-  da.depth = (const float*)dp_d;
-  da.dh = dh;
-  da.dw = dw;
+  da.dst_l = da.dst_r = (uint8_t*)o_d;
   da.focal = (float)focal;
-  da.focus_w = (float)(0.35 + 1e-6);
-  da.idx_max = (float)(5 - 1 - 1e-6);
-  da.nlevels = dof ? 5 : 1;
-  if (dof) {
-    for (int i = 0; i < 8; ++i) {
-      da.ksize[i] = ctx->dof_ksize[i];
-      da.koff[i] = ctx->dof_koff[i];
-    }
-    da.kern = (const float*)ctx->dof_kern.p;
-    da.halo = ctx->dof_halo;
-  }
-  da.sat = (float)sat;
-  da.con = (float)con;
-  da.bri = (float)bri;
   launch_dof(da, 1, s);
   ctx->launches += 1;
-  CK(cudaGetLastError());
-  if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(dst, o_d, bytes, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  return VD3D_OK;
+  return stage_finish(ctx, dst, o_d, bytes, mem);
 }
 
 }  // extern "C"
