@@ -94,6 +94,12 @@ typedef struct {
   int32_t enable_dynamic_convergence;
   double ipd_factor;
   double color_saturation, color_contrast, color_brightness;
+  /* detect_black_bars + crop_black_bars_torch on every frame (core/render_3d.py:293-326,1238-1242): the rows of the
+   * top / bottom black bars found on the colour frame are cut from the frame and the depth map before the aspect crop.
+   * Sizes do not change per frame.  The reference sizes a preserve_original_aspect output with original_video_* = None
+   * from the cropped first frame; here 0 means the uncropped source size, so callers pass that size explicitly
+   * (vd3d_detect_black_bars on the first frame). */
+  int32_t auto_crop_black_bars;
 } vd3d_render_params;
 
 /* sizes derived at core/render_3d.py:1074-1138,1250-1259 */
@@ -115,6 +121,7 @@ typedef struct {
   double focal_depth, motion_metric;
   double stable_zero;
   int32_t bar_width, bar_side; /* side: 0 none, 1 right, 2 left */
+  int32_t crop_top, crop_bottom; /* black-bar rows detected on the frame (0 without auto_crop_black_bars) */
 } vd3d_frame_info;
 
 /* sizeof() of the ABI structs, so bindings can verify their layout:
@@ -186,6 +193,16 @@ int vd3d_render_clip(vd3d_ctx* ctx, int n, const uint8_t* const* frames, const u
  * in-memory replacement of the reference's XVID depth-video round trip (SURVEY 0.5). */
 int vd3d_render_clip_depth(vd3d_ctx* ctx, vd3d_depth* depth, int n, const uint8_t* const* frames, int src_h,
                            int src_w, const vd3d_render_params* rp, uint8_t* const* outs, int mem);
+
+/* (top, bottom) of each of the n frames of the last vd3d_render_clip / vd3d_render_clip_depth call, as int32 pairs.
+ * The per-frame values are copied behind the output frames on the device-to-host stream (no synchronisation inside the
+ * clip).  VD3D_ERR_STATE when that call had auto_crop_black_bars off or rendered fewer than n frames. */
+int vd3d_last_crops(vd3d_ctx* ctx, int32_t* top_bottom, int n);
+
+/* detect_black_bars (core/render_3d.py:293-316) on one u8 BGR frame [h,w,3]: top = first row whose cv2 gray mean is
+ * above 10, bottom = h-1-last such row, both 0 when there is none.  The kernel the frame loop runs for
+ * auto_crop_black_bars; synchronises. */
+int vd3d_detect_black_bars(vd3d_ctx* ctx, const uint8_t* frame_bgr, int h, int w, int mem, int* top, int* bottom);
 
 /* ---- exact frame sharding (SURVEY 8(e)) --------------------------------------------------
  * The loop is stateful (7 EMAs / trackers + the temporal depth plane).  A rank that renders frames

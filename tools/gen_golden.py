@@ -122,7 +122,8 @@ def run_loop(r3d, torch, cv2, src_w, src_h, n_frames, kind, rp):
             color_brightness=rp.get("color_brightness", 0.0),
             **{k: rp[k] for k in ("enable_edge_masking", "enable_feathering",
                                   "convergence_strength", "enable_dynamic_convergence", "ipd_factor",
-                                  "parallax_balance", "depth_pop_gamma", "fg_pop_multiplier") if k in rp},
+                                  "parallax_balance", "depth_pop_gamma", "fg_pop_multiplier", "auto_crop_black_bars")
+               if k in rp},
         )
     finally:
         cv2.VideoCapture, cv2.VideoWriter = real_cap, real_wr
@@ -376,6 +377,51 @@ def gen_signatures():
     print(p, os.path.getsize(p))
 
 
+def gen_autocrop():
+    """R. auto_crop_black_bars on the letterbox set (visiondepth3d_b200/synth.py), `python tools/gen_golden.py autocrop`.
+    The reference's detect_black_bars is wrapped so that each fixture also records every (top, bottom) it returned, the
+    probe frame's first (`crops` [n, 2]).  Final frames keep every `rows`-th row to stay under 1 MB."""
+    mods = refshim.load_reference(("render_3d",))
+    r3d = mods["render_3d"]
+    import cv2
+    import torch
+    import torchvision
+    torch.set_num_threads(os.cpu_count())
+    meta = dict(torch=torch.__version__, torchvision=torchvision.__version__, cv2=cv2.__version__,
+                numpy=np.__version__)
+    base = dict(output_width=320, output_height=180, sharpness_factor=0.2, output_format="Half-SBS",
+                dof_strength=0.0, feather_strength=10.0, blur_ksize=9, use_subject_tracking=True,
+                use_floating_window=True, preserve_original_aspect=False, zero_parallax_strength=0.01,
+                auto_crop_black_bars=True)
+    real = r3d.detect_black_bars
+    cases = (
+        # Half-SBS: the fused k_render path; all eight frames of the schedule (the first is the probe)
+        ("loop_autocrop_halfsbs_320x180.npz", 8, base, 1),
+        # Full-SBS, preserve_original_aspect, original_video_* None: the output size comes from the cropped probe frame
+        ("loop_autocrop_fullsbs_320x180.npz", 6, dict(base, output_format="Full-SBS", preserve_original_aspect=True), 2),
+        # DOF on the Half-SBS path: the non-fused post chain
+        ("loop_autocrop_dof_halfsbs_320x180.npz", 6, dict(base, dof_strength=1.5), 2),
+    )
+    for name, n, rp, step in cases:
+        crops = []
+
+        def wrapped(frame_tensor, threshold=10):
+            tb = real(frame_tensor, threshold)
+            crops.append(tb)
+            return tb
+
+        r3d.detect_black_bars = wrapped
+        try:
+            g = run_loop(r3d, torch, cv2, 320, 180, n, "letterbox", rp)
+        finally:
+            r3d.detect_black_bars = real
+        assert len(crops) == n and len(g) == n - 1, (len(crops), len(g))
+        out = {k: v[::step] for k, v in g.items()}
+        p = os.path.join(OUT, name)
+        np.savez_compressed(p, **out, crops=np.array(crops, dtype=np.int32), rows=np.int32(step), **meta)
+        print(name, os.path.getsize(p), crops, {k: v.shape for k, v in g.items()})
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "signatures":
         gen_signatures()
@@ -387,5 +433,7 @@ if __name__ == "__main__":
         gen_vr()
     elif len(sys.argv) > 1 and sys.argv[1] == "natural":
         gen_natural()
+    elif len(sys.argv) > 1 and sys.argv[1] == "autocrop":
+        gen_autocrop()
     else:
         main()

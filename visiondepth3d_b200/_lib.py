@@ -54,6 +54,7 @@ class RenderParams(C.Structure):
         ("enable_dynamic_convergence", C.c_int32),
         ("ipd_factor", C.c_double),
         ("color_saturation", C.c_double), ("color_contrast", C.c_double), ("color_brightness", C.c_double),
+        ("auto_crop_black_bars", C.c_int32),
     ]
 
 
@@ -73,6 +74,7 @@ class FrameInfo(C.Structure):
         ("focal_depth", C.c_double), ("motion_metric", C.c_double),
         ("stable_zero", C.c_double),
         ("bar_width", C.c_int32), ("bar_side", C.c_int32),
+        ("crop_top", C.c_int32), ("crop_bottom", C.c_int32),
     ]
 
 
@@ -92,6 +94,7 @@ SYMBOLS = [
     "vd3d_set_depth_batch", "vd3d_get_depth_batch", "vd3d_render_clip_depth", "vd3d_depth_add_launches", "vd3d_depth_clone", "vd3d_release_depth",
     "vd3d_depth_profile", "vd3d_depth_profile_collect", "vd3d_depth_profile_spans",
     "vd3d_advance_state", "vd3d_state_bytes", "vd3d_export_state", "vd3d_import_state",
+    "vd3d_last_crops", "vd3d_detect_black_bars",
 ]
 
 _lib = None
@@ -161,6 +164,10 @@ def load():
     lib.vd3d_render_clip.restype = i
     lib.vd3d_render_clip_depth.argtypes = [vp, vp, i, C.POINTER(vp), i, i, C.POINTER(RenderParams), C.POINTER(vp), i]
     lib.vd3d_render_clip_depth.restype = i
+    lib.vd3d_last_crops.argtypes = [vp, C.POINTER(C.c_int32), i]
+    lib.vd3d_last_crops.restype = i
+    lib.vd3d_detect_black_bars.argtypes = [vp, u8p, i, i, i, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    lib.vd3d_detect_black_bars.restype = i
     lib.vd3d_heal.argtypes = [vp, fp, fp, fp, i, i, C.c_double, fp, i]
     lib.vd3d_heal.restype = i
     lib.vd3d_pack.argtypes = [vp, u8p, u8p, i, i, i, u8p, i]

@@ -52,6 +52,7 @@ struct StatsSmem {
   SelState sel[3];
   DevState st;
   FrameScalars fs;
+  int crop[4];        // ingest source rectangle {x0, y0, w, h} of this frame (the fixed crop, or auto_crop_black_bars)
 };
 
 __device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
@@ -421,7 +422,24 @@ __global__ void __launch_bounds__(NT, 1) k_stats(StatsArgs a) {
     zero_pass1(S);
     {
       const IngestArgs& ia = a.ia;
-      const bool ident = (ia.tw == ia.cw && ia.th == ia.ch);
+      if (tid == 0) {
+        if (ia.bars) {  // auto_crop_black_bars: this frame's rectangle from the words of k_black_bars
+          int top, bottom;
+          black_bar_crop(ia.src_w, ia.src_h, ia.bars[0], ia.bars[1], ia.aspect, S.crop, &top, &bottom);
+          if (blockIdx.x == 0 && ia.crop_out) {
+            ia.crop_out[0] = top;
+            ia.crop_out[1] = bottom;
+          }
+        } else {
+          S.crop[0] = ia.cx0;
+          S.crop[1] = ia.cy0;
+          S.crop[2] = ia.cw;
+          S.crop[3] = ia.ch;
+        }
+      }
+      __syncthreads();
+      const int cx0 = S.crop[0], cy0 = S.crop[1], cw = S.crop[2], ch = S.crop[3];
+      const bool ident = (ia.tw == cw && ia.th == ch);
       const int tdf_init = S.st.tdf_init;
       const FastDiv fdt = fast_div((uint32_t)tw, (uint32_t)ntp);
       for (int base = blockIdx.x * (NT * UNR); base < ntp; base += gridDim.x * (NT * UNR)) {
@@ -436,14 +454,14 @@ __global__ void __launch_bounds__(NT, 1) k_stats(StatsArgs a) {
             float cur;
             RsAxis ax, ay;
             if (ident && !a.rgbx_s) {
-              cur = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, ia.cy0 + y, ia.cx0 + x);
+              cur = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, cy0 + y, cx0 + x);
             } else {
-              ax = rs_axis(x, ia.cw, ia.tw);
-              ay = rs_axis(y, ia.ch, ia.th);
-              float v00 = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, ia.cy0 + ay.i0, ia.cx0 + ax.i0);
-              float v01 = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, ia.cy0 + ay.i0, ia.cx0 + ax.i1);
-              float v10 = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, ia.cy0 + ay.i1, ia.cx0 + ax.i0);
-              float v11 = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, ia.cy0 + ay.i1, ia.cx0 + ax.i1);
+              ax = rs_axis(x, cw, ia.tw);
+              ay = rs_axis(y, ch, ia.th);
+              float v00 = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, cy0 + ay.i0, cx0 + ax.i0);
+              float v01 = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, cy0 + ay.i0, cx0 + ax.i1);
+              float v10 = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, cy0 + ay.i1, cx0 + ax.i0);
+              float v11 = depth_lut01(S.lut, ia.depth, ia.depth_ch, ia.src_w, cy0 + ay.i1, cx0 + ax.i1);
               cur = rs_combine(v00, v01, v10, v11, ax, ay);
             }
             float prev = tdf_init ? __ldcg(ia.tdf + idx) : cur;
@@ -454,10 +472,10 @@ __global__ void __launch_bounds__(NT, 1) k_stats(StatsArgs a) {
 #pragma unroll
               for (int ch = 0; ch < 3; ++ch) {  // ch: 0=R 1=G 2=B ; source is BGR
                 const uint8_t* f = ia.frame + (2 - ch);
-                float v00 = S.lut[f[((size_t)(ia.cy0 + ay.i0) * ia.src_w + ia.cx0 + ax.i0) * 3]];
-                float v01 = S.lut[f[((size_t)(ia.cy0 + ay.i0) * ia.src_w + ia.cx0 + ax.i1) * 3]];
-                float v10 = S.lut[f[((size_t)(ia.cy0 + ay.i1) * ia.src_w + ia.cx0 + ax.i0) * 3]];
-                float v11 = S.lut[f[((size_t)(ia.cy0 + ay.i1) * ia.src_w + ia.cx0 + ax.i1) * 3]];
+                float v00 = S.lut[f[((size_t)(cy0 + ay.i0) * ia.src_w + cx0 + ax.i0) * 3]];
+                float v01 = S.lut[f[((size_t)(cy0 + ay.i0) * ia.src_w + cx0 + ax.i1) * 3]];
+                float v10 = S.lut[f[((size_t)(cy0 + ay.i1) * ia.src_w + cx0 + ax.i0) * 3]];
+                float v11 = S.lut[f[((size_t)(cy0 + ay.i1) * ia.src_w + cx0 + ax.i1) * 3]];
                 c[ch] = rs_combine(v00, v01, v10, v11, ax, ay);
               }
               a.rgbx_s[idx] = make_float4(c[0], c[1], c[2], 0.f);

@@ -16,18 +16,31 @@ __global__ void __launch_bounds__(256) k_ingest(IngestArgs a) {
   int x = blockIdx.x * 32 + (threadIdx.x & 31);
   int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= a.tw || y >= a.th) return;
+  int cx0 = a.cx0, cy0 = a.cy0, cw = a.cw, ch = a.ch;
+  if (a.bars) {  // auto_crop_black_bars: this frame's rectangle from the words of k_black_bars
+    int rect[4], top, bottom;
+    black_bar_crop(a.src_w, a.src_h, a.bars[0], a.bars[1], a.aspect, rect, &top, &bottom);
+    cx0 = rect[0];
+    cy0 = rect[1];
+    cw = rect[2];
+    ch = rect[3];
+    if (x == 0 && y == 0 && a.crop_out) {
+      a.crop_out[0] = top;
+      a.crop_out[1] = bottom;
+    }
+  }
   float cur;
   RsAxis ax, ay;
-  bool fast = (a.tw == a.cw && a.th == a.ch) && !a.rgb_s;
+  bool fast = (a.tw == cw && a.th == ch) && !a.rgb_s;
   if (fast) {
-    cur = depth_src01(a.depth, a.depth_ch, a.src_w, a.cy0 + y, a.cx0 + x);
+    cur = depth_src01(a.depth, a.depth_ch, a.src_w, cy0 + y, cx0 + x);
   } else {  // same-size axes degenerate to i0 = d, l1 = 0: an exact identity
-    ax = rs_axis(x, a.cw, a.tw);
-    ay = rs_axis(y, a.ch, a.th);
-    float v00 = depth_src01(a.depth, a.depth_ch, a.src_w, a.cy0 + ay.i0, a.cx0 + ax.i0);
-    float v01 = depth_src01(a.depth, a.depth_ch, a.src_w, a.cy0 + ay.i0, a.cx0 + ax.i1);
-    float v10 = depth_src01(a.depth, a.depth_ch, a.src_w, a.cy0 + ay.i1, a.cx0 + ax.i0);
-    float v11 = depth_src01(a.depth, a.depth_ch, a.src_w, a.cy0 + ay.i1, a.cx0 + ax.i1);
+    ax = rs_axis(x, cw, a.tw);
+    ay = rs_axis(y, ch, a.th);
+    float v00 = depth_src01(a.depth, a.depth_ch, a.src_w, cy0 + ay.i0, cx0 + ax.i0);
+    float v01 = depth_src01(a.depth, a.depth_ch, a.src_w, cy0 + ay.i0, cx0 + ax.i1);
+    float v10 = depth_src01(a.depth, a.depth_ch, a.src_w, cy0 + ay.i1, cx0 + ax.i0);
+    float v11 = depth_src01(a.depth, a.depth_ch, a.src_w, cy0 + ay.i1, cx0 + ax.i1);
     cur = rs_combine(v00, v01, v10, v11, ax, ay);
   }
   size_t o = (size_t)y * a.tw + x;
@@ -40,12 +53,60 @@ __global__ void __launch_bounds__(256) k_ingest(IngestArgs a) {
     for (int c = 0; c < 3; ++c) {  // c: 0=R 1=G 2=B ; source is BGR
       int sc = 2 - c;
       const uint8_t* f = a.frame + sc;
-      float v00 = (float)f[((size_t)(a.cy0 + ay.i0) * a.src_w + a.cx0 + ax.i0) * 3] / 255.0f;
-      float v01 = (float)f[((size_t)(a.cy0 + ay.i0) * a.src_w + a.cx0 + ax.i1) * 3] / 255.0f;
-      float v10 = (float)f[((size_t)(a.cy0 + ay.i1) * a.src_w + a.cx0 + ax.i0) * 3] / 255.0f;
-      float v11 = (float)f[((size_t)(a.cy0 + ay.i1) * a.src_w + a.cx0 + ax.i1) * 3] / 255.0f;
+      float v00 = (float)f[((size_t)(cy0 + ay.i0) * a.src_w + cx0 + ax.i0) * 3] / 255.0f;
+      float v01 = (float)f[((size_t)(cy0 + ay.i0) * a.src_w + cx0 + ax.i1) * 3] / 255.0f;
+      float v10 = (float)f[((size_t)(cy0 + ay.i1) * a.src_w + cx0 + ax.i0) * 3] / 255.0f;
+      float v11 = (float)f[((size_t)(cy0 + ay.i1) * a.src_w + cx0 + ax.i1) * 3] / 255.0f;
       a.rgb_s[c * plane + o] = rs_combine(v00, v01, v10, v11, ax, ay);
     }
+  }
+}
+
+// ---------------------------------------------------------------------------
+// detect_black_bars (core/render_3d.py:293-316): one warp per row of the u8 BGR frame.  The row sum of cv2 BGR2GRAY is
+// an exact integer, and np.mean(gray[y]) > threshold  <=>  sum > threshold * w.  Rows whose start is 16-byte aligned
+// (w % 16 == 0 on an aligned frame) are read 48 bytes = 16 pixels per lane and step; others one pixel at a time.
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t gray_u8(uint32_t b, uint32_t g, uint32_t r) {
+  return (b * 3735u + g * 19235u + r * 9798u + (1u << 14)) >> 15;
+}
+
+__global__ void __launch_bounds__(256) k_black_bars(const uint8_t* __restrict__ frame, int h, int w, int threshold,
+                                                    uint32_t* __restrict__ words) {
+  __shared__ uint32_t s_first, s_last;
+  const int lane = threadIdx.x & 31;
+  const int y = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (threadIdx.x == 0) s_first = s_last = 0u;
+  __syncthreads();
+  if (y < h) {
+    const uint8_t* row = frame + (size_t)y * w * 3;
+    uint32_t sum = 0;
+    int x0 = 0;
+    if (((uintptr_t)row & 15) == 0) {
+      const int chunks = w / 16;
+      const uint4* v = reinterpret_cast<const uint4*>(row);
+      for (int c = lane; c < chunks; c += 32) {
+        uint4 q[3];
+        q[0] = __ldg(v + 3 * c);
+        q[1] = __ldg(v + 3 * c + 1);
+        q[2] = __ldg(v + 3 * c + 2);
+        const uint8_t* p = reinterpret_cast<const uint8_t*>(q);
+#pragma unroll
+        for (int k = 0; k < 16; ++k) sum += gray_u8(p[3 * k], p[3 * k + 1], p[3 * k + 2]);
+      }
+      x0 = chunks * 16;
+    }
+    for (int x = x0 + lane; x < w; x += 32) sum += gray_u8(row[3 * x], row[3 * x + 1], row[3 * x + 2]);
+    sum = __reduce_add_sync(0xffffffffu, sum);
+    if (lane == 0 && sum > (uint32_t)threshold * (uint32_t)w) {
+      atomicMax(&s_first, (uint32_t)(h - y));
+      atomicMax(&s_last, (uint32_t)(y + 1));
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && s_first) {
+    atomicMax(words, s_first);
+    atomicMax(words + 1, s_last);
   }
 }
 
@@ -1072,6 +1133,9 @@ void launch_heal(const float* warped, const float* orig, const float* edge, floa
 static inline dim3 grid2d(int w, int h) { return dim3((w + 31) / 32, (h + 7) / 8); }
 
 void launch_ingest(const IngestArgs& a, cudaStream_t s) { k_ingest<<<grid2d(a.tw, a.th), 256, 0, s>>>(a); }
+void launch_black_bars(const uint8_t* frame, int h, int w, int threshold, uint32_t* words, cudaStream_t s) {
+  k_black_bars<<<(h + 7) / 8, 256, 0, s>>>(frame, h, w, threshold, words);
+}
 
 void launch_resize_planar(const float* src, int C, int sh, int sw, float* dst, int oh, int ow, cudaStream_t s) {
   k_resize_planar<<<grid2d(ow, oh), 256, 0, s>>>(src, C, sh, sw, dst, oh, ow);

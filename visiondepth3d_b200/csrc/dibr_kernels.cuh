@@ -63,6 +63,8 @@ struct FrameScalars {  // recomputed every frame
   float c_fg, c_fgm, c_mg, c_bg, c_bgm, c_pb, c_half, c_mid, c_gamma;
   float c_zpo, c_max, c_conv, c_m1, c_m2;
   int use_zpo, use_conv;
+  // auto_crop_black_bars (k_black_bars): max(H - y) and max(y + 1) over the bright rows y of the frame; 0 = none
+  uint32_t bars[2];
 };
 
 struct SelTarget {

@@ -20,7 +20,50 @@ struct IngestArgs {
   float* rgb_s;          // resized RGB planes [3, th, tw] or null on the identity path
   float alpha, one_minus_alpha;
   const DevState* st;
+  // auto_crop_black_bars: the crop of this frame is derived on the device from the two words k_black_bars left in
+  // bars (FrameScalars::bars) and the aspect ratio; cx0 .. ch above are then unused.  null: the fixed crop above.
+  const uint32_t* bars;
+  double aspect;
+  int32_t* crop_out;  // (top, bottom) of the frame, written once (may be null)
 };
+
+// centre crop of a w x h frame to `ratio` (core/render_3d.py:1236-1248), fp64 like the reference's Python floats;
+// rect = {x0, y0, w, h}
+__host__ __device__ inline void aspect_crop(int w, int h, double ratio, int* rect) {
+  rect[0] = 0;
+  rect[1] = 0;
+  rect[2] = w;
+  rect[3] = h;
+  const double cur = (double)w / (double)h;
+  if (fabs(cur - ratio) > 0.01) {
+    if (cur > ratio) {
+      rect[2] = (int)(h * ratio);
+      rect[0] = (w - rect[2]) / 2;
+    } else {
+      rect[3] = (int)(w / ratio);
+      rect[1] = (h - rect[3]) / 2;
+    }
+  }
+}
+// (top, bottom) of detect_black_bars from the two words of k_black_bars (0: no bright row)
+__host__ __device__ inline void bar_rows(int h, uint32_t first, uint32_t last, int* top, int* bottom) {
+  *top = first ? h - (int)first : 0;
+  *bottom = last ? h - (int)last : 0;
+}
+// The source rectangle of one auto-cropped frame: the rows of the black bars off (crop_black_bars_torch, which keeps the
+// frame when top + bottom >= H), then the aspect crop on what is left (1238-1248).  first / last: the words of
+// k_black_bars.
+__host__ __device__ inline void black_bar_crop(int src_w, int src_h, uint32_t first, uint32_t last, double ratio,
+                                               int* rect, int* top, int* bottom) {
+  bar_rows(src_h, first, last, top, bottom);
+  int y0 = *top, rows = src_h - *top - *bottom;
+  if (*top + *bottom >= src_h) {
+    y0 = 0;
+    rows = src_h;
+  }
+  aspect_crop(src_w, rows, ratio, rect);
+  rect[1] += y0;
+}
 
 struct LoopArgs {
   double fg, mg, bg;  // render_sbs_3d arguments
@@ -100,6 +143,10 @@ struct PostArgs {
 };
 
 void launch_ingest(const IngestArgs& a, cudaStream_t s);
+// detect_black_bars (core/render_3d.py:293-316) on a u8 BGR frame [h, w, 3]: integer row sums of cv2 gray, row y bright
+// when sum > threshold * w; atomicMax(words[0], h - y) and atomicMax(words[1], y + 1) over the bright rows (the caller
+// zeroes words).  One warp per row.
+void launch_black_bars(const uint8_t* frame, int h, int w, int threshold, uint32_t* words, cudaStream_t s);
 void launch_resize_planar(const float* src, int C, int sh, int sw, float* dst, int oh, int ow, cudaStream_t s);
 // 3 histogram passes + 3 bin searches; b may be null.  b's region must lie inside a's
 // and share a.data.  nblocks = grid of the pass kernels.

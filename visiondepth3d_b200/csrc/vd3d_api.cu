@@ -49,6 +49,12 @@ struct vd3d_ctx {
   int prof_depth_frames = 0;  // frames covered by the stage-2 (depth) samples since the last collect
   uint64_t dclone_wver = 0;
   unsigned* bar = nullptr;  // grid barrier counter of k_stats (inside jobwords: zeroed by begin_frame)
+  // auto_crop_black_bars: (top, bottom) written by the ingest of each staging slot [kSlots][2], their copies for the
+  // frames of the last clip call (pinned, crops_n frames), and the two words of vd3d_detect_black_bars
+  int32_t* crops_dev = nullptr;
+  int32_t* crops_host = nullptr;
+  int crops_cap = 0, crops_n = 0;
+  uint32_t* detect_words = nullptr;
 
   DevState* st = nullptr;
   FrameScalars* fs = nullptr;
@@ -463,10 +469,16 @@ int begin_frame(vd3d_ctx* ctx) {
   return VD3D_OK;
 }
 
-int fetch_info(vd3d_ctx* ctx, vd3d_frame_info* info) {
+// crop_slot >= 0: the frame was auto-cropped, its (top, bottom) sits in crops_dev[crop_slot]
+int fetch_info(vd3d_ctx* ctx, vd3d_frame_info* info, int crop_slot = -1) {
+  int32_t tb[2] = {0, 0};
   CK(cudaMemcpyAsync(ctx->fs_pinned, ctx->fs, sizeof(FrameScalars), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(ctx->st_pinned, ctx->st, sizeof(DevState), cudaMemcpyDeviceToHost, ctx->stream));
+  if (crop_slot >= 0)
+    CK(cudaMemcpyAsync(tb, ctx->crops_dev + 2 * crop_slot, sizeof tb, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
+  info->crop_top = tb[0];
+  info->crop_bottom = tb[1];
   const FrameScalars& f = *ctx->fs_pinned;
   const DevState& t = *ctx->st_pinned;
   info->pct_lo = t.pct_lo;
@@ -891,6 +903,9 @@ int vd3d_create(int device, vd3d_ctx** out) {
     return bail("cudaMalloc", e);
   ctx->bar = ctx->jobwords + kJobs * kJobWords;
   if ((e = cudaMalloc(&ctx->tgs, sizeof(SelTarget) * kJobs * 4)) != cudaSuccess) return bail("cudaMalloc", e);
+  if ((e = cudaMalloc(&ctx->crops_dev, sizeof(int32_t) * 2 * kSlots)) != cudaSuccess) return bail("cudaMalloc", e);
+  if ((e = cudaMalloc(&ctx->detect_words, sizeof(uint32_t) * 2)) != cudaSuccess) return bail("cudaMalloc", e);
+  cudaMemset(ctx->crops_dev, 0, sizeof(int32_t) * 2 * kSlots);
   cudaMemset(ctx->st, 0, sizeof(DevState));
   cudaMemset(ctx->fs, 0, sizeof(FrameScalars));
   cudaMemset(ctx->jobwords, 0, sizeof(uint32_t) * (kJobs * kJobWords + kBarWords));
@@ -950,6 +965,9 @@ void vd3d_destroy(vd3d_ctx* ctx) {
   cudaFree(ctx->fs);
   cudaFree(ctx->jobwords);
   cudaFree(ctx->tgs);
+  cudaFree(ctx->crops_dev);
+  cudaFree(ctx->detect_words);
+  if (ctx->crops_host) cudaFreeHost(ctx->crops_host);
   cudaFreeHost(ctx->fs_pinned);
   cudaFreeHost(ctx->st_pinned);
   for (int i = 0; i < kSlots; ++i) {
@@ -1129,17 +1147,8 @@ int vd3d_pixel_shift(vd3d_ctx* ctx, const float* rgb, const float* depth, int in
 int vd3d_plan_sizes(int src_w, int src_h, const vd3d_render_params* rp, vd3d_size_plan* o) {
   if (!rp || !o || src_w < 2 || src_h < 2) return VD3D_ERR_ARG;
   double target_ratio = rp->aspect_ratio;
-  int cw = src_w, ch = src_h, cx0 = 0, cy0 = 0;
-  double cur = (double)src_w / (double)src_h;
-  if (fabs(cur - target_ratio) > 0.01) {
-    if (cur > target_ratio) {
-      cw = (int)(src_h * target_ratio);
-      cx0 = (src_w - cw) / 2;
-    } else {
-      ch = (int)(src_w / target_ratio);
-      cy0 = (src_h - ch) / 2;
-    }
-  }
+  int crop[4];
+  aspect_crop(src_w, src_h, target_ratio, crop);
   int rw, rh, pw, ph, outw, outh, tew, teh;
   int fmt = rp->output_format;
   if (rp->preserve_original_aspect) {
@@ -1179,10 +1188,10 @@ int vd3d_plan_sizes(int src_w, int src_h, const vd3d_render_params* rp, vd3d_siz
     teh = (int)(pw / target_ratio);
     if (teh % 2 != 0) teh += 1;
   }
-  o->crop_x0 = cx0;
-  o->crop_y0 = cy0;
-  o->crop_w = cw;
-  o->crop_h = ch;
+  o->crop_x0 = crop[0];
+  o->crop_y0 = crop[1];
+  o->crop_w = crop[2];
+  o->crop_h = crop[3];
   o->target_eye_w = tew;
   o->target_eye_h = teh;
   o->resized_width = rw;
@@ -1378,10 +1387,11 @@ static int enqueue_dof_post(vd3d_ctx* ctx, const vd3d_render_params* rp, const v
   return VD3D_OK;
 }
 
-// enqueue one loop iteration on ctx->stream; inputs/outputs are DEVICE pointers
+// enqueue one loop iteration on ctx->stream; inputs/outputs are DEVICE pointers.  slot: the staging slot whose
+// crops_dev entry receives the frame's (top, bottom) under auto_crop_black_bars.
 static int enqueue_frame(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_t* depth_d, int depth_channels,
                          int src_h, int src_w, const vd3d_render_params* rp, const vd3d_size_plan& pl,
-                         uint8_t* out_d) {
+                         uint8_t* out_d, int slot) {
   int r;
   ProfScope frame_scope(ctx, 0);
   const int tw = pl.target_eye_w, th = pl.target_eye_h;
@@ -1397,6 +1407,11 @@ static int enqueue_frame(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_t* d
     if ((r = vd3d_reset_state(ctx, VD3D_STATE_CLIP))) return r;
   }
   if ((r = begin_frame(ctx))) return r;
+  const bool autocrop = rp->auto_crop_black_bars != 0;
+  if (autocrop) {  // detect_black_bars on the frame; the ingest derives the crop from the two words on the device
+    launch_black_bars(frame_d, src_h, src_w, 10, ctx->fs->bars, ctx->stream);
+    ctx->launches += 1;
+  }
 
   // ---- loop-level inputs: ingest + TemporalDepthFilter, trackers, normalised-depth ping-pong, pixel_shift_cuda
   IngestArgs ia;
@@ -1416,6 +1431,11 @@ static int enqueue_frame(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_t* d
   ia.alpha = 0.5f;
   ia.one_minus_alpha = (float)(1 - 0.5);
   ia.st = ctx->st;
+  if (autocrop) {
+    ia.bars = ctx->fs->bars;
+    ia.aspect = rp->aspect_ratio;
+    ia.crop_out = ctx->crops_dev + 2 * slot;
+  }
   LoopArgs la;
   la.fg = rp->fg_shift;
   la.mg = rp->mg_shift;
@@ -1430,7 +1450,9 @@ static int enqueue_frame(vd3d_ctx* ctx, const uint8_t* frame_d, const uint8_t* d
   la.dyn_span = (float)(1.15 - 0.90);
   float* dn = (float*)(ctx->frame_parity ? ctx->dn1.p : ctx->dn0.p);
   const float* dn_prev = (const float*)(ctx->frame_parity ? ctx->dn0.p : ctx->dn1.p);
-  const bool ident = (tw == pl.crop_w && th == pl.crop_h && W == tw && H == th);
+  // identity (the eyes sample the u8 frame directly): not under auto-crop, whose crop is only known on the device; its
+  // bilinear resize at scale 1 is an exact identity too, like F.interpolate
+  const bool ident = !autocrop && (tw == pl.crop_w && th == pl.crop_h && W == tw && H == th);
   CoreIn ci;
   memset(&ci, 0, sizeof ci);
   ci.depth = dn;
@@ -1551,7 +1573,7 @@ static int run_frame_slot(vd3d_ctx* ctx, int b, int depth_channels, int src_h, i
   const uint8_t* f_d = (const uint8_t*)ctx->in_frame[b].p;
   uint8_t* d_d = (uint8_t*)ctx->in_depth[b].p;
   uint8_t* o_d = (uint8_t*)ctx->out_dev[b].p;
-  auto eager = [&]() { return enqueue_frame(ctx, f_d, d_d, depth_channels, src_h, src_w, rp, pl, o_d); };
+  auto eager = [&]() { return enqueue_frame(ctx, f_d, d_d, depth_channels, src_h, src_w, rp, pl, o_d, b); };
   bool same = ctx->fg_h == src_h && ctx->fg_w == src_w && ctx->fg_dch == depth_channels &&
               memcmp(&ctx->fg_rp, rp, sizeof *rp) == 0;
   if (ctx->fg_epoch != ctx->res_epoch) {  // another entry point moved / rewrote something the graphs bake in
@@ -1596,6 +1618,55 @@ static size_t out_bytes(const vd3d_render_params* rp, const vd3d_size_plan& pl) 
   return (size_t)packed_w(rp, pl) * pl.per_eye_h * 3;
 }
 
+// vd3d_last_crops bookkeeping of a clip call: room for n (top, bottom) pairs in pinned memory (auto-crop only)
+static int begin_crops(vd3d_ctx* ctx, const vd3d_render_params* rp, int n) {
+  ctx->crops_n = 0;
+  if (!rp->auto_crop_black_bars) return VD3D_OK;
+  if (n > ctx->crops_cap) {
+    CK(cudaStreamSynchronize(ctx->s_d2h));  // copies of an earlier call may still target the old block
+    if (ctx->crops_host) CK(cudaFreeHost(ctx->crops_host));
+    ctx->crops_host = nullptr;
+    ctx->crops_cap = 0;
+    CK(cudaMallocHost(&ctx->crops_host, sizeof(int32_t) * 2 * (size_t)n));
+    ctx->crops_cap = n;
+  }
+  ctx->crops_n = n;
+  return VD3D_OK;
+}
+
+// behind the output frame of clip frame i (staging slot b) on the D2H stream: its (top, bottom)
+static int copy_crop(vd3d_ctx* ctx, const vd3d_render_params* rp, int i, int b) {
+  if (!rp->auto_crop_black_bars) return VD3D_OK;
+  CK(cudaMemcpyAsync(ctx->crops_host + 2 * (size_t)i, ctx->crops_dev + 2 * b, 2 * sizeof(int32_t),
+                     cudaMemcpyDeviceToHost, ctx->s_d2h));
+  return VD3D_OK;
+}
+
+int vd3d_last_crops(vd3d_ctx* ctx, int32_t* top_bottom, int n) {
+  if (!ctx || !top_bottom || n < 0) return fail(ctx, VD3D_ERR_ARG, "bad argument");
+  if (n > ctx->crops_n) return fail(ctx, VD3D_ERR_STATE, "the last clip call did not auto-crop that many frames");
+  memcpy(top_bottom, ctx->crops_host, sizeof(int32_t) * 2 * (size_t)n);  // the clip call synchronised its D2H stream
+  return VD3D_OK;
+}
+
+int vd3d_detect_black_bars(vd3d_ctx* ctx, const uint8_t* frame_bgr, int h, int w, int mem, int* top, int* bottom) {
+  if (!ctx || !frame_bgr || !top || !bottom || h < 1 || w < 1) return fail(ctx, VD3D_ERR_ARG, "bad argument");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  const void* f_d;
+  int r;
+  if ((r = copy_in(ctx, ctx->in_frame[0], frame_bgr, (size_t)h * w * 3, mem, s, &f_d))) return r;
+  CK(cudaMemsetAsync(ctx->detect_words, 0, 2 * sizeof(uint32_t), s));
+  launch_black_bars((const uint8_t*)f_d, h, w, 10, ctx->detect_words, s);
+  ctx->launches += 2;
+  CK(cudaGetLastError());
+  uint32_t words[2];
+  CK(cudaMemcpyAsync(words, ctx->detect_words, sizeof words, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  bar_rows(h, words[0], words[1], top, bottom);
+  return VD3D_OK;
+}
+
 int vd3d_render_frame(vd3d_ctx* ctx, const uint8_t* frame_bgr, const uint8_t* depth, int depth_channels,
                       int src_h, int src_w, const vd3d_render_params* rp, uint8_t* out_bgr, int mem,
                       vd3d_frame_info* info) {
@@ -1614,10 +1685,10 @@ int vd3d_render_frame(vd3d_ctx* ctx, const uint8_t* frame_bgr, const uint8_t* de
   void* o_d;
   if ((r = stage_out(ctx, ctx->out_dev[0], out_bgr, ob, mem, &o_d))) return r;
   if ((r = enqueue_frame(ctx, (const uint8_t*)f_d, (const uint8_t*)d_d, depth_channels, src_h, src_w, rp, pl,
-                         (uint8_t*)o_d)))
+                         (uint8_t*)o_d, 0)))
     return r;
   if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(out_bgr, o_d, ob, cudaMemcpyDeviceToHost, s));
-  if (info) return fetch_info(ctx, info);
+  if (info) return fetch_info(ctx, info, rp->auto_crop_black_bars ? 0 : -1);
   CK(cudaStreamSynchronize(s));
   return VD3D_OK;
 }
@@ -1638,6 +1709,7 @@ int vd3d_render_clip(vd3d_ctx* ctx, int n, const uint8_t* const* frames, const u
     if ((r = ensure(ctx, ctx->in_depth[b], db))) return r;
     if ((r = ensure(ctx, ctx->out_dev[b], ob))) return r;
   }
+  if ((r = begin_crops(ctx, rp, n))) return r;
   for (int i = 0; i < n; ++i) {
     int b = i % kSlots;
     if (mem == VD3D_MEM_DEVICE) {
@@ -1655,11 +1727,12 @@ int vd3d_render_clip(vd3d_ctx* ctx, int n, const uint8_t* const* frames, const u
       if (i >= kSlots) CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_d2h[b], 0));
     }
     if ((r = run_frame_slot(ctx, b, depth_channels, src_h, src_w, rp, pl))) return r;
-    if (infos && (r = fetch_info(ctx, &infos[i]))) return r;
+    if (infos && (r = fetch_info(ctx, &infos[i], rp->auto_crop_black_bars ? b : -1))) return r;
     CK(cudaEventRecord(ctx->ev_done[b], ctx->stream));
     CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[b], 0));
     CK(cudaMemcpyAsync(outs[i], ctx->out_dev[b].p, ob,
                        mem == VD3D_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->s_d2h));
+    if ((r = copy_crop(ctx, rp, i, b))) return r;
     CK(cudaEventRecord(ctx->ev_d2h[b], ctx->s_d2h));
   }
   CK(cudaStreamSynchronize(ctx->stream));
@@ -1681,6 +1754,7 @@ int vd3d_render_clip_depth(vd3d_ctx* ctx, vd3d_depth* depth, int n, const uint8_
     if ((r = ensure(ctx, ctx->in_depth[b], db))) return r;
     if ((r = ensure(ctx, ctx->out_dev[b], ob))) return r;
   }
+  if ((r = begin_crops(ctx, rp, n))) return r;
   // Frames travel in groups of `depth_batch`: one batched depth forward per group on one of two engine instances
   // (group g+1's forward overlaps the neck / head tail of group g and the DIBR kernels of group g's frames), then the
   // DIBR loop body frame by frame on the main stream (sequential temporal state), D2H behind it.
@@ -1736,6 +1810,7 @@ int vd3d_render_clip_depth(vd3d_ctx* ctx, vd3d_depth* depth, int n, const uint8_
       CK(cudaEventRecord(ctx->ev_done[sl], ctx->stream));
       CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[sl], 0));
       CK(cudaMemcpyAsync(outs[i0 + j], ctx->out_dev[sl].p, ob, kout, ctx->s_d2h));
+      if ((r = copy_crop(ctx, rp, i0 + j, sl))) return r;
       CK(cudaEventRecord(ctx->ev_d2h[sl], ctx->s_d2h));
     }
   }
@@ -1774,7 +1849,7 @@ int vd3d_advance_state(vd3d_ctx* ctx, const uint8_t* frame_bgr, const uint8_t* d
   if ((r = copy_in(ctx, ctx->in_frame[0], frame_bgr, fb, mem, s, &f_d))) return r;
   if ((r = copy_in(ctx, ctx->in_depth[0], depth, db, mem, s, &d_d))) return r;
   ctx->stats_only = 1;
-  r = enqueue_frame(ctx, (const uint8_t*)f_d, (const uint8_t*)d_d, depth_channels, src_h, src_w, rp, pl, nullptr);
+  r = enqueue_frame(ctx, (const uint8_t*)f_d, (const uint8_t*)d_d, depth_channels, src_h, src_w, rp, pl, nullptr, 0);
   ctx->stats_only = 0;
   if (r) return r;
   CK(cudaStreamSynchronize(s));

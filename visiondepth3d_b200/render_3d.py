@@ -276,7 +276,7 @@ def make_render_params(output_width, output_height, fg_shift, mg_shift, bg_shift
                        preserve_original_aspect=False, zero_parallax_strength=0.0, enable_edge_masking=True,
                        enable_feathering=True, original_video_width=None, original_video_height=None,
                        convergence_strength=0.0, enable_dynamic_convergence=True, ipd_factor=1.0,
-                       color_saturation=1.0, color_contrast=1.0, color_brightness=0.0):
+                       color_saturation=1.0, color_contrast=1.0, color_brightness=0.0, auto_crop_black_bars=False):
     """vd3d_render_params from render_sbs_3d's arguments (core/render_3d.py:933-985)."""
     if output_format not in _lib.FMT:
         output_format = "Half-SBS"  # format_3d_output's fallback is hstack (860)
@@ -288,7 +288,7 @@ def make_render_params(output_width, output_height, fg_shift, mg_shift, bg_shift
         float(zero_parallax_strength), int(bool(enable_edge_masking)), int(bool(enable_feathering)),
         int(original_video_width or 0), int(original_video_height or 0), float(convergence_strength),
         int(bool(enable_dynamic_convergence)), float(ipd_factor), float(color_saturation),
-        float(color_contrast), float(color_brightness))
+        float(color_contrast), float(color_brightness), int(bool(auto_crop_black_bars)))
 
 
 def plan_sizes(src_w, src_h, rp):
@@ -443,13 +443,15 @@ def render_sbs_3d(
     streams, CUDA-graph replay), and a writer thread pushes the packed frames of the previous batch as raw bgr24 into
     an ffmpeg pipe (use_ffmpeg, when the binary exists) or a cv2.VideoWriter.  Sequencing follows the reference:
     first pair of the window dropped, pop controls and parallax_balance not forwarded (1284-1331), no exception
-    escapes (1477-1478).  auto_crop_black_bars / skip_blank_frames (ffmpeg blackdetect, letterbox tracker) are outside
-    the hot path: refused with a message before any file is created."""
+    escapes (1477-1478).  auto_crop_black_bars detects and crops the black bars of every frame on the GPU
+    (vd3d_detect_black_bars on the dropped first frame, then per frame inside vd3d_render_clip) and prints the
+    reference's lines; skip_blank_frames (an external ffmpeg blackdetect pass) is outside the hot path: refused with a
+    message before any file is created."""
     import queue
     import shutil
     import cv2
-    if auto_crop_black_bars or skip_blank_frames:
-        print("⚠️ auto_crop_black_bars / skip_blank_frames are outside the GPU hot path")
+    if skip_blank_frames:
+        print("⚠️ skip_blank_frames (ffmpeg blackdetect) is outside the GPU hot path")
         return
     if use_ffmpeg and shutil.which("ffmpeg") is None:
         print("⚠️ ffmpeg binary not found: writing through cv2.VideoWriter instead")
@@ -476,17 +478,28 @@ def render_sbs_3d(
         suspend_flag = suspend_flag or globals()["suspend_flag"]
         cancel_flag = cancel_flag or globals()["cancel_flag"]
         ratio = aspect_ratios.get(selected_aspect_ratio.get(), 16 / 9)
+        sh, sw = probe.shape[:2]
+        ctx = _ctx()
+        if auto_crop_black_bars:  # detected on the first pair, the one the loop drops (1065-1070)
+            top, bottom = C.c_int(), C.c_int()
+            probe = np.ascontiguousarray(probe)
+            ctx.check(ctx.lib.vd3d_detect_black_bars(ctx.h, probe.ctypes.data, sh, sw, _lib.MEM_HOST, C.byref(top),
+                                                     C.byref(bottom)))
+            print(f"Auto-crop: Top {top.value}px | Bottom {bottom.value}px")
+            if preserve_original_aspect and (original_video_width is None or original_video_height is None):
+                # the output size falls back to the cropped first frame (1086-1090)
+                original_video_width = sw
+                original_video_height = sh - top.value - bottom.value if top.value + bottom.value < sh else sh
         rp = make_render_params(
             output_width, output_height, fg_shift, mg_shift, bg_shift, sharpness_factor, output_format, ratio,
             dof_strength, feather_strength, blur_ksize, use_subject_tracking, use_floating_window,
             max_pixel_shift_percent, preserve_original_aspect, zero_parallax_strength, enable_edge_masking,
             enable_feathering, original_video_width, original_video_height, convergence_strength,
-            enable_dynamic_convergence, ipd_factor, color_saturation, color_contrast, color_brightness)
-        sh, sw = probe.shape[:2]
+            enable_dynamic_convergence, ipd_factor, color_saturation, color_contrast, color_brightness,
+            auto_crop_black_bars)
         dch = 1 if probe_d.ndim == 2 else probe_d.shape[2]
         pl = plan_sizes(sw, sh, rp)                     # raises before any output file exists
         oshape = output_shape(rp, pl)
-        ctx = _ctx()
         ctx.check(ctx.lib.vd3d_check_config(ctx.h, sh, sw, C.byref(rp)))   # eye fit / DOF limits, still no file
         sink = _FrameSink(output_path, (oshape[1], oshape[0]), fps, selected_codec, use_ffmpeg, selected_ffmpeg_codec,
                           crf_value)
@@ -627,6 +640,11 @@ def render_sbs_3d(
             dp = (C.c_void_p * n)(*[ring_in[1].ptrs[k] for k in slots])
             op = (C.c_void_p * n)(*[ring_out.ptrs[half * _BATCH + j] for j in range(n)])
             ctx.check(ctx.lib.vd3d_render_clip(ctx.h, n, fp, dp, dch, sh, sw, C.byref(rp), op, _lib.MEM_HOST, None))
+            if auto_crop_black_bars:  # the reference prints one line per frame (1238-1240)
+                tb = (C.c_int32 * (2 * n))()
+                ctx.check(ctx.lib.vd3d_last_crops(ctx.h, tb, n))
+                for j in range(n):
+                    print(f"🔪 Cropping top: {tb[2 * j]}px, bottom: {tb[2 * j + 1]}px")
             for k in slots:
                 free_in.put(k)
             to_write.put((half, n))
