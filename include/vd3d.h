@@ -274,7 +274,7 @@ typedef struct {
 } vd3d_depth_config;
 int vd3d_depth_create(const vd3d_depth_config* cfg, void* cuda_stream, vd3d_depth** out);
 void vd3d_depth_destroy(vd3d_depth* e);
-/* CUDA-event timing of the fc1 GEMM launches (k_umma_gemm<128,3>; M = tokens, N = 4*hidden, K = hidden) */
+/* CUDA-event timing of the fc1 GEMM launches (k_umma_gemm<128,4>; M = tokens, N = 4*hidden, K = hidden) */
 int vd3d_depth_profile(vd3d_depth* e, int enable);
 int vd3d_depth_profile_collect(vd3d_depth* e, double* total_ms, int* count, double* gflop_per_launch);
 /* tuning aid: after vd3d_depth_profile(e, 2), every launch class of an eager forward is bracketed by CUDA events; this
@@ -323,7 +323,7 @@ int vd3d_gemm_f16(vd3d_depth* e, const void* A_f16, const void* B_f16, int M, in
 /* tuning hook: average launch time (ms) of one M x N x K GEMM on device-resident operands, on the 128 x 128 tile
    kernel with an operand ring of 4 (variant 0, the default), 3 (variant 1) or 2 (variant 2) stages; other variants
    return VD3D_ERR_ARG.  dbg (low 3 bits): 0 normal, 2 no TMA loads (MMA rate), 3 prologue + teardown only, 4 no
-   epilogue, other values VD3D_ERR_ARG; bit 3: poll barriers with test_wait.  act: 0 none, 1 GELU; 0x100 selects the
+   epilogue (the epilogue warpgroup only releases the staging tile), other values VD3D_ERR_ARG; bit 3: poll barriers with test_wait.  act: 0 none, 1 GELU; 0x100 selects the
    residual (proj / fc2) epilogue */
 int vd3d_gemm_bench(vd3d_depth* e, int M, int N, int K, int variant, int dbg, int act, int iters, float* ms_out);
 int vd3d_conv_f16(vd3d_depth* e, const void* in_nhwc_f16, int H, int W, int cin, const void* w_f16, int cout,

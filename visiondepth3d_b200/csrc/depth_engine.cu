@@ -243,7 +243,7 @@ int vd3d_depth_create(const vd3d_depth_config* cfg, void* stream, vd3d_depth** o
   return VD3D_OK;
 }
 
-// device timing of the fc1 GEMM launches (k_umma_gemm<128,3>, M=tokens, N=4D, K=D): bench.py roofline
+// device timing of the fc1 GEMM launches (k_umma_gemm<128,4>, M=tokens, N=4D, K=D): bench.py roofline
 int vd3d_depth_profile(vd3d_depth* e, int enable) {
   if (!e) return VD3D_ERR_ARG;
   e->prof = enable == 1;

@@ -472,7 +472,8 @@ cudaError_t launch_gemm(int bn, const CUtensorMap& a, const CUtensorMap& b, cons
   g.nt = (g.N + bn - 1) / bn;
   g.mt = m_tiles;
   g.nz = batch;
-  // persistent grid: one CTA per SM (two consumer warpgroups, up to 144 KB of operand ring), each walks its tiles
+  // persistent grid: one CTA per SM (producer, epilogue and two consumer warpgroups, up to 144 KB of operand ring),
+  // each walks its tiles
   const int total = g.nt * g.mt * g.nz, sms = sm_count();
   dim3 grid(total < sms ? total : sms, 1, 1);
   switch (bn) {

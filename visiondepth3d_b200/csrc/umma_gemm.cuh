@@ -7,10 +7,11 @@
 // * two consumer warpgroups each own 64 rows of the 128 x BN tile and issue
 //   wgmma.mma_async m64nBNk16 (A and B read from shared memory through matrix descriptors),
 //   accumulating in registers; a ring slot is released once the wgmmas reading it retired;
-// * the accumulator is staged through shared memory so that one thread owns 32 consecutive
-//   columns of one row, and the fused epilogue (bias, GELU, LayerScale+residual, QKV head
-//   split with V transposed, pixel-shuffle for ConvTranspose, ReLU / residual for convs,
-//   DPT head) runs on that chunk.
+// * the finished accumulator is staged through shared memory and handed (mbarriers) to a
+//   dedicated epilogue warpgroup, one thread per tile row, which runs the fused epilogue
+//   (bias, GELU, LayerScale+residual, QKV head split with V transposed, pixel-shuffle for
+//   ConvTranspose, ReLU / residual for convs, DPT head) on 32-column chunks of its row while
+//   the consumers already run the next tile's mainloop.
 // * A can also be an NHWC activation read through a 3-D tensor map (C, W, H): the K loop
 //   then walks the 3x3 taps and channel blocks (implicit GEMM); out-of-image taps are
 //   zero-filled by TMA, so no im2col buffer and no padding copies exist.
@@ -67,7 +68,8 @@ struct GemmArgs {
   const float* w3;
   const float* b3p;
   // tuning hook (vd3d_gemm_bench), low 3 bits: 0 = normal, 2 = skip the TMA loads (MMA rate), 3 = prologue +
-  // teardown only, 4 = no epilogue; bit 3 (8): poll barriers with test_wait instead of try_wait
+  // teardown only, 4 = no epilogue (the epilogue warpgroup only releases the staging tile); bit 3 (8): poll barriers
+  // with test_wait instead of try_wait
   int dbg;
 };
 
@@ -467,11 +469,22 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmArgs& g, const uin
   }
 }
 
-// warp 0: TMA producer; warps 4-11: two consumer warpgroups (64 accumulator rows each).  Warps 1-3 only fill the
-// producer's warpgroup so that the consumers are whole, aligned warpgroups.
-constexpr int kGemmThreads = 384;
+// Four warpgroups:
+//   WG0 (warps 0-3)   TMA producer; warp 0 issues, warps 1-3 only make the other warpgroups whole and aligned;
+//   WG1 (warps 4-7)   epilogue: thread t owns row t of the 128 x BN tile;
+//   WG2-3 (warps 8-15) MMA consumers, 64 accumulator rows each.
+// The consumers hand each finished tile to the epilogue warpgroup through the fp32 staging tile and go straight on to
+// the next tile's mainloop, so the tensor cores stay busy while the epilogue of the previous tile runs.
+constexpr int kGemmThreads = 512;
 constexpr int kBK = 64;  // 64 f16 = 128 B = one swizzle row
 constexpr int kPromote = 4;  // k-blocks (K = 256) per tensor-core accumulation group
+// setmaxnreg split of the 64 K-register file: 128 x producer + 128 x epilogue + 256 x consumer <= 65536.  A consumer
+// holds acc + tot (BN registers) and the loop state; the epilogue holds one 32-column chunk (~100 live values for the
+// LayerScale + residual read-modify-write).
+constexpr int kProducerRegs = 40;
+constexpr int kEpilogueRegs = 120;
+constexpr int kConsumerRegs = 176;
+static_assert(128 * kProducerRegs + 128 * kEpilogueRegs + 256 * kConsumerRegs <= 65536, "register file overcommitted");
 
 template <int BN, int STAGES>
 struct GemmSmem {
@@ -479,7 +492,7 @@ struct GemmSmem {
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStage = kABytes + kBBytes;
   static constexpr int kPitch = BN + 4;  // floats per staged row (+4: no bank conflicts on the row reads)
-  static constexpr int kEpi = 2 * 64 * kPitch * 4;  // one 64 x BN fp32 staging tile per consumer warpgroup
+  static constexpr int kEpi = 128 * kPitch * 4;  // the 128 x BN fp32 staging tile (consumers -> epilogue warpgroup)
   static constexpr int kTotal = STAGES * kStage + kEpi + 1024 /*align*/ + 256 /*barriers*/;
 };
 
@@ -494,6 +507,8 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   uint64_t* bars = (uint64_t*)(smem + STAGES * S::kStage + S::kEpi);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
+  uint64_t* epi_full = bars + 2 * STAGES;  // staging tile written by both consumer warpgroups
+  uint64_t* epi_empty = epi_full + 1;      // staging tile read by the epilogue warpgroup
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -509,6 +524,8 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       umma::mbar_init(umma::smem_u32(&full[s]), 1);
       umma::mbar_init(umma::smem_u32(&empty[s]), 2);  // one arrive per consumer warpgroup
     }
+    umma::mbar_init(umma::smem_u32(epi_full), 256);  // every consumer thread, after its own staging stores
+    umma::mbar_init(umma::smem_u32(epi_empty), 128);  // every epilogue thread, after its own staging reads
     umma::fence_barrier_init();
   }
   __syncthreads();
@@ -530,7 +547,7 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     // tuning: prologue + teardown only
   } else if (warp < 4) {
     // ===================== TMA producer =====================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");  // hand registers to the consumer warpgroups
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));  // registers go to the consumers
     if (warp == 0 && lane == 0) {
       int kit = 0;  // k-block counter across tiles (ring position)
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -564,17 +581,58 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
     }
+  } else if (warp < 8) {
+    // ===================== epilogue warpgroup =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kEpilogueRegs));
+    const int r = threadIdx.x & 127;  // accumulator row inside the tile
+    int j = 0;                        // staging round (tiles of this CTA)
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++j) {
+      int n_blk, m_blk, z, px0, py0;
+      decode(tile, n_blk, m_blk, z, px0, py0);
+      int m;  // logical output row
+      bool row_ok;
+      if (g.conv) {
+        int ly = r / g.tw, lx = r % g.tw;
+        int y = py0 + ly, x = px0 + lx;
+        row_ok = (y < g.imgH) && (x < g.imgW);
+        m = y * g.imgW + x;
+      } else {
+        m = m_blk * 128 + r;
+        row_ok = m < g.M;
+      }
+      umma::mbar_wait_dbg(umma::smem_u32(epi_full), j & 1, spin);
+      if (dmode != 4) {
+        // the fused epilogue on the row's BN / 32 chunks of 32 consecutive columns, in column order
+        float head_acc = 0.f;
+#pragma unroll 1
+        for (int ci = 0; ci < BN / 32; ++ci) {
+          uint32_t v[32];
+          const float4* src = (const float4*)(epi_buf + r * S::kPitch + ci * 32);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const float4 f = src[i];
+            v[4 * i] = __float_as_uint(f.x);
+            v[4 * i + 1] = __float_as_uint(f.y);
+            v[4 * i + 2] = __float_as_uint(f.z);
+            v[4 * i + 3] = __float_as_uint(f.w);
+          }
+          gemm_epilogue_chunk(g, v, m, z, n_blk * BN + ci * 32, row_ok, head_acc);
+        }
+        // DPT head: N == 32 is a single chunk
+        if (g.epi == EPI_HEAD && row_ok && n_blk == 0) g.out_f32[m] = fmaxf(head_acc + g.b3p[0], 0.f);
+      }
+      umma::mbar_arrive(umma::smem_u32(epi_empty));
+    }
   } else {
-    // ===================== consumers: MMA + epilogue =====================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");  // 128 x 40 + 256 x 232 <= 64 K registers
-    const int wg = (warp >> 2) - 1;      // consumer warpgroup: accumulator rows 64 wg .. 64 wg + 63
+    // ===================== consumers: MMA, then hand the tile to the epilogue warpgroup =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+    const int wg = (warp >> 2) - 2;      // consumer warpgroup: accumulator rows 64 wg .. 64 wg + 63
     const int t = threadIdx.x & 127;     // thread in the warpgroup
     const int wq = t >> 5;               // warp in the warpgroup: fragment rows 16 wq .. 16 wq + 15
     float* ebuf = epi_buf + wg * 64 * S::kPitch;
     int kit = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      int n_blk, m_blk, z, px0, py0;
-      decode(tile, n_blk, m_blk, z, px0, py0);
+    int j = 0;  // staging round
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++j) {
       // The tensor core adds each k16 product sum into its accumulator with truncation, so over long reductions (fc2:
       // K = 4D) the error grows with K.  Each group of kPromote k-blocks is therefore accumulated from zero in `acc`
       // and then added into the fp32 total `tot` in the FP32 pipe.
@@ -609,50 +667,18 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         for (int i = 0; i < BN / 2; ++i) tot[i] += acc[i];
       }
       if (prev >= 0 && t == 0) umma::mbar_arrive(umma::smem_u32(&empty[prev]));
-      if (dmode == 4) continue;
 
-      // ---- epilogue: the warpgroup's 64 x BN accumulator goes through shared memory, then thread
-      // (row t & 63, chunks t >> 6, +2, ...) runs the fused epilogue on 32 consecutive columns of its row ----
-      const int er = t & 63, ec = t >> 6;
-      const int r = wg * 64 + er;  // accumulator row inside the tile
-      int m;                       // logical output row
-      bool row_ok;
-      if (g.conv) {
-        int ly = r / g.tw, lx = r % g.tw;
-        int y = py0 + ly, x = px0 + lx;
-        row_ok = (y < g.imgH) && (x < g.imgW);
-        m = y * g.imgW + x;
-      } else {
-        m = m_blk * 128 + r;
-        row_ok = m < g.M;
-      }
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // staging buffer free (previous tile read)
-      // fragment of m64nN: tot[4 j + i] is row 16 wq + lane/4 + 8 (i >> 1), column 8 j + 2 (lane & 3) + (i & 1)
+      // ---- hand-off: once the epilogue warpgroup has read the previous tile, stage this one ----
+      umma::mbar_wait_dbg(umma::smem_u32(epi_empty), (j & 1) ^ 1, spin);
+      // fragment of m64nN: tot[4 i + q] is row 16 wq + lane/4 + 8 (q >> 1), column 8 i + 2 (lane & 3) + (q & 1)
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int c = 8 * j + 2 * (lane & 3);
+      for (int i = 0; i < BN / 8; ++i) {
+        const int c = 8 * i + 2 * (lane & 3);
         const int r0 = 16 * wq + (lane >> 2);
-        *(float2*)(ebuf + r0 * S::kPitch + c) = make_float2(tot[4 * j], tot[4 * j + 1]);
-        *(float2*)(ebuf + (r0 + 8) * S::kPitch + c) = make_float2(tot[4 * j + 2], tot[4 * j + 3]);
+        *(float2*)(ebuf + r0 * S::kPitch + c) = make_float2(tot[4 * i], tot[4 * i + 1]);
+        *(float2*)(ebuf + (r0 + 8) * S::kPitch + c) = make_float2(tot[4 * i + 2], tot[4 * i + 3]);
       }
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-      float head_acc = 0.f;
-#pragma unroll 1
-      for (int ci = ec; ci < BN / 32; ci += 2) {
-        uint32_t v[32];
-        const float4* src = (const float4*)(ebuf + er * S::kPitch + ci * 32);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 f = src[i];
-          v[4 * i] = __float_as_uint(f.x);
-          v[4 * i + 1] = __float_as_uint(f.y);
-          v[4 * i + 2] = __float_as_uint(f.z);
-          v[4 * i + 3] = __float_as_uint(f.w);
-        }
-        gemm_epilogue_chunk(g, v, m, z, n_blk * BN + ci * 32, row_ok, head_acc);
-      }
-      // DPT head: N == 32 is a single chunk, owned by the chunk-0 threads
-      if (g.epi == EPI_HEAD && ec == 0 && row_ok && n_blk == 0) g.out_f32[m] = fmaxf(head_acc + g.b3p[0], 0.f);
+      umma::mbar_arrive(umma::smem_u32(epi_full));
     }
   }
 }
