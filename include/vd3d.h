@@ -204,6 +204,27 @@ int vd3d_last_crops(vd3d_ctx* ctx, int32_t* top_bottom, int n);
  * auto_crop_black_bars; synchronises. */
 int vd3d_detect_black_bars(vd3d_ctx* ctx, const uint8_t* frame_bgr, int h, int w, int mem, int* top, int* bottom);
 
+/* ---- letterbox tracker of the depth-video pass (core/render_depth.py:273-573, 1919-1933) ---------------------------
+ * Per-frame statistics of n u8 BGR frames [n,h,w,3] (contiguous; host or device memory per `mem`, w <= 8192), from
+ * which the host-side tracker decides the bar rows:
+ *   row_y_mean / row_y_var [n,h]: float32 mean and variance of the Rec.709 luma 0.2126 r + 0.7152 g + 0.0722 b, equal
+ *     to numpy's float32 y.mean(axis=1) / y.var(axis=1) bit for bit (pairwise summation order);
+ *   row_s_mean [n,h]: float32 mean of cv2 BGR2HSV's S; row_edges [n,h]: edge pixels of cv2.Canny(gray, 30, 90,
+ *     apertureSize=3, L2gradient=True) per row;
+ *   frame_y_mean [n]: float32 y.mean() of the whole frame; frame_hist [n,64]: 64-bin histogram of cv2 BGR2GRAY
+ *     (bin = gray >> 2); frame_absdiff [n]: sum |gray - previous gray|, the previous gray being frame i-1, and for
+ *     frame 0 prev_gray [h,w] (0 when prev_gray is null).
+ * The records are host memory.  last_gray (optional, `mem` space) receives the gray plane of frame n-1.  Synchronises. */
+int vd3d_letterbox_stats(vd3d_ctx* ctx, int n, const uint8_t* frames, int h, int w, const uint8_t* prev_gray, int mem,
+                         float* row_y_mean, float* row_y_var, float* row_s_mean, int32_t* row_edges,
+                         float* frame_y_mean, uint32_t* frame_hist, uint64_t* frame_absdiff, uint8_t* last_gray);
+/* cv2.Canny(gray [h,w], low, high, apertureSize=3, L2gradient=True) -> dst [h,w] of 0/255, bit for bit */
+int vd3d_canny_u8(vd3d_ctx* ctx, const uint8_t* gray, int h, int w, double low, double high, uint8_t* dst, int mem);
+/* process_video2's depth re-pad: u8 depth [h,w] -> dst [h,w] with the INTER_CUBIC resize of the depth to
+ * (w, h - top - bottom) at rows [top, h - bottom) and the bar rows filled with int(np.median(core)).  No bars, or
+ * h - top - bottom <= 0 (the reference then drops the bars), copies the depth.  src and dst must not alias. */
+int vd3d_letterbox_repad(vd3d_ctx* ctx, const uint8_t* src, int h, int w, int top, int bottom, uint8_t* dst, int mem);
+
 /* ---- exact frame sharding (SURVEY 8(e)) --------------------------------------------------
  * The loop is stateful (7 EMAs / trackers + the temporal depth plane).  A rank that renders frames
  * [a, b) exactly needs the state after frame a-1: vd3d_advance_state runs one loop iteration

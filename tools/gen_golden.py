@@ -422,6 +422,120 @@ def gen_autocrop():
         print(name, os.path.getsize(p), crops, {k: v.shape for k, v in g.items()})
 
 
+def gen_letterbox():
+    """S. the depth-video letterbox tracker: the unmodified process_video2 with ignore_letterbox_bars=True on the
+    letterbox_track sets (visiondepth3d_b200/synth.py), `python tools/gen_golden.py letterbox`.  An in-memory capture
+    (frame count, fps 2, size, POS_FRAMES seeks) feeds it, a recording writer collects the u8 frames it writes, and
+    `pipe` is a deterministic stub (pipe_type "hf", tensor output: depth = 0.5 * green + row) that the tests
+    reproduce.  LetterboxTracker.bootstrap / update and detect_letterbox_multiframe_confidence are wrapped to record
+    the bootstrap (bars, confidence, locks) and every per-frame (top, bottom).  Batches of 4 frames: neither clip
+    length is a multiple of 4."""
+    import json
+    import tempfile
+    import types
+    import cv2
+    import torch
+    from PIL import Image
+    for n in ("diffusers.configuration_utils", "core.unet", "core.depthcrafter_adapter"):
+        refshim._stub(n)
+    rd = refshim.load_reference(("render_depth",))["render_depth"]
+    from visiondepth3d_b200 import synth
+    meta = dict(torch=torch.__version__, cv2=cv2.__version__, numpy=np.__version__)
+
+    def stub_pipe(images, inference_size=None):
+        out = []
+        for img in images:
+            g = np.asarray(img.convert("RGB"), dtype=np.float32)[..., 1]
+            out.append({"predicted_depth": torch.from_numpy(0.5 * g + np.arange(g.shape[0], dtype=np.float32)[:, None])})
+        return out
+
+    for kind, sched in (("letterbox_track", synth._TRACK), ("letterbox_track_nobars", synth._TRACK_NOBARS)):
+        n_frames = len(sched)
+        frames = [synth_frame(i, 320, 180, kind)[0] for i in range(n_frames)]
+
+        class Cap:
+            def __init__(self, *a):
+                self.pos = 0
+
+            def isOpened(self):
+                return True
+
+            def get(self, prop):
+                return float({cv2.CAP_PROP_FRAME_COUNT: n_frames, cv2.CAP_PROP_FPS: 2.0, cv2.CAP_PROP_FRAME_WIDTH: 320,
+                              cv2.CAP_PROP_FRAME_HEIGHT: 180, cv2.CAP_PROP_POS_FRAMES: self.pos}.get(prop, 0.0))
+
+            def set(self, prop, v):
+                if prop == cv2.CAP_PROP_POS_FRAMES:
+                    self.pos = int(v)
+                return True
+
+            def read(self):
+                if self.pos >= n_frames:
+                    return False, None
+                self.pos += 1
+                return True, frames[self.pos - 1].copy()
+
+            def release(self):
+                pass
+
+        written = []
+
+        class Writer:
+            def __init__(self, *a, **k):
+                pass
+
+            def isOpened(self):
+                return True
+
+            def write(self, f):
+                written.append(f[..., 0].copy())
+
+            def release(self):
+                pass
+
+        rec = {"boot": None, "conf": None, "bars": []}
+        real_boot, real_upd = rd.LetterboxTracker.bootstrap, rd.LetterboxTracker.update
+        real_conf = rd.detect_letterbox_multiframe_confidence
+
+        def conf(*a, **k):
+            r = real_conf(*a, **k)
+            rec["conf"] = r[1]
+            return r
+
+        def boot(self, cap):
+            r = real_boot(self, cap)
+            rec["boot"] = (r[0], r[1], bool(r[2][0]), bool(r[2][1]))
+            return r
+
+        def upd(self, frame, idx):
+            r = real_upd(self, frame, idx)
+            rec["bars"].append(r)
+            return r
+
+        real_cap, real_wr = cv2.VideoCapture, cv2.VideoWriter
+        rd.detect_letterbox_multiframe_confidence = conf
+        rd.LetterboxTracker.bootstrap, rd.LetterboxTracker.update = boot, upd
+        cv2.VideoCapture, cv2.VideoWriter = Cap, Writer
+        rd.pipe, rd.pipe_type = stub_pipe, "hf"
+        status = types.SimpleNamespace(config=lambda **k: None, update_idletasks=lambda: None)
+        try:
+            with tempfile.TemporaryDirectory() as td:
+                rd.process_video2(os.path.join(td, kind + ".mkv"), n_frames, 0, 4, Var(td), Var("Original"), status,
+                                  {}, threading.Event(), Var(False), ignore_letterbox_bars=True)
+                side = json.load(open(os.path.join(td, kind + "_depth.letterbox.json")))
+        finally:
+            cv2.VideoCapture, cv2.VideoWriter = real_cap, real_wr
+            rd.detect_letterbox_multiframe_confidence = real_conf
+            rd.LetterboxTracker.bootstrap, rd.LetterboxTracker.update = real_boot, real_upd
+        assert len(written) == n_frames and len(rec["bars"]) == n_frames, (len(written), len(rec["bars"]))
+        p = os.path.join(OUT, kind.replace("letterbox_track", "letterbox") + "_320x180.npz")
+        np.savez_compressed(p, kind=kind, batch_size=np.int32(4), fps=np.float64(2.0),
+                            boot_bars=np.array(rec["boot"][:2], np.int32), boot_locks=np.array(rec["boot"][2:], bool),
+                            boot_conf=np.float64(rec["conf"]), bars=np.array(rec["bars"], np.int32),
+                            sidecar=json.dumps(side, sort_keys=True), written=np.stack(written), **meta)
+        print(p, os.path.getsize(p), rec["boot"], rec["conf"], side)
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "signatures":
         gen_signatures()
@@ -435,5 +549,7 @@ if __name__ == "__main__":
         gen_natural()
     elif len(sys.argv) > 1 and sys.argv[1] == "autocrop":
         gen_autocrop()
+    elif len(sys.argv) > 1 and sys.argv[1] == "letterbox":
+        gen_letterbox()
     else:
         main()

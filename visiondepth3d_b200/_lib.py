@@ -95,6 +95,7 @@ SYMBOLS = [
     "vd3d_depth_profile", "vd3d_depth_profile_collect", "vd3d_depth_profile_spans",
     "vd3d_advance_state", "vd3d_state_bytes", "vd3d_export_state", "vd3d_import_state",
     "vd3d_last_crops", "vd3d_detect_black_bars",
+    "vd3d_letterbox_stats", "vd3d_canny_u8", "vd3d_letterbox_repad",
 ]
 
 _lib = None
@@ -168,6 +169,12 @@ def load():
     lib.vd3d_last_crops.restype = i
     lib.vd3d_detect_black_bars.argtypes = [vp, u8p, i, i, i, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.vd3d_detect_black_bars.restype = i
+    lib.vd3d_letterbox_stats.argtypes = [vp, i, u8p, i, i, u8p, i, fp, fp, fp, vp, fp, vp, vp, u8p]
+    lib.vd3d_letterbox_stats.restype = i
+    lib.vd3d_canny_u8.argtypes = [vp, u8p, i, i, C.c_double, C.c_double, u8p, i]
+    lib.vd3d_canny_u8.restype = i
+    lib.vd3d_letterbox_repad.argtypes = [vp, u8p, i, i, i, i, u8p, i]
+    lib.vd3d_letterbox_repad.restype = i
     lib.vd3d_heal.argtypes = [vp, fp, fp, fp, i, i, C.c_double, fp, i]
     lib.vd3d_heal.restype = i
     lib.vd3d_pack.argtypes = [vp, u8p, u8p, i, i, i, u8p, i]

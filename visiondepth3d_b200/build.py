@@ -16,6 +16,7 @@ UNITS = [
     ("dibr_kernels.cu", ["-fmad=false"]),
     ("dibr_fast.cu", ["-fmad=false"]),
     ("vd3d_api.cu", ["-fmad=false"]),
+    ("letterbox.cu", ["-fmad=false"]),
     ("depth_kernels.cu", []),
     ("depth_engine.cu", []),
 ]

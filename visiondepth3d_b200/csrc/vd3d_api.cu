@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "dibr_launch.h"
+#include "letterbox_launch.h"
 
 using namespace vd3d;
 
@@ -55,6 +56,11 @@ struct vd3d_ctx {
   int32_t* crops_host = nullptr;
   int crops_cap = 0, crops_n = 0;
   uint32_t* detect_words = nullptr;
+  // letterbox tracker statistics, Canny and depth re-pad (letterbox.cu): inputs, planes, per-row/per-frame records
+  // and the cut nodes of the frame-wide pairwise luma sum (cached per pixel count)
+  Buf lb_in, lb_prev, lb_gray, lb_mag, lb_label, lb_flag, lb_rec, lb_nodes, lb_node_sum, lb_out, lb_hist;
+  int64_t lb_nodes_npix = -1;
+  int lb_nodes_n = 0;
 
   DevState* st = nullptr;
   FrameScalars* fs = nullptr;
@@ -946,7 +952,9 @@ void vd3d_destroy(vd3d_ctx* ctx) {
   Buf* bufs[] = {&ctx->xs,    &ctx->ys,    &ctx->tdf,   &ctx->dn0,   &ctx->dn1,      &ctx->rgb_s,
                  &ctx->frameB, &ctx->d,     &ctx->shift, &ctx->e2,    &ctx->eyeL,     &ctx->eyeR,
                  &ctx->eyeL2, &ctx->eyeR2, &ctx->in_rgbf, &ctx->in_depthf, &ctx->dof_kern,
-                 &ctx->area_tab[0], &ctx->area_tab[1]};
+                 &ctx->area_tab[0], &ctx->area_tab[1], &ctx->lb_in, &ctx->lb_prev, &ctx->lb_gray, &ctx->lb_mag,
+                 &ctx->lb_label, &ctx->lb_flag, &ctx->lb_rec, &ctx->lb_nodes, &ctx->lb_node_sum, &ctx->lb_out,
+                 &ctx->lb_hist};
   for (Buf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (int i = 0; i < kSlots; ++i) {
@@ -2165,6 +2173,149 @@ int vd3d_dof_grade(vd3d_ctx* ctx, const uint8_t* eye_bgr, int h, int w, const fl
   launch_dof(da, 1, s);
   ctx->launches += 1;
   return stage_finish(ctx, dst, o_d, bytes, mem);
+}
+
+// ---- letterbox tracker (core/render_depth.py:273-573) and depth re-pad (1919-1933); kernels in letterbox.cu ----
+
+// cv2.Canny's integer thresholds with L2gradient: clamp to 32767, square, floor; low > high is swapped
+static void canny_thresholds(double low, double high, int* low2, int* high2) {
+  if (low > high) {
+    const double t = low;
+    low = high;
+    high = t;
+  }
+  low = fmin(32767.0, low);
+  high = fmin(32767.0, high);
+  if (low > 0) low *= low;
+  if (high > 0) high *= high;
+  *low2 = (int)floor(low);
+  *high2 = (int)floor(high);
+}
+
+static int lb_canny_scratch(vd3d_ctx* ctx, size_t npx) {
+  int r;
+  if ((r = ensure(ctx, ctx->lb_mag, npx * 4)) || (r = ensure(ctx, ctx->lb_label, npx * 4)) ||
+      (r = ensure(ctx, ctx->lb_flag, npx * 2)))
+    return r;
+  return VD3D_OK;
+}
+
+int vd3d_canny_u8(vd3d_ctx* ctx, const uint8_t* gray, int h, int w, double low, double high, uint8_t* dst, int mem) {
+  if (!ctx || !gray || !dst || h < 1 || w < 1 || (size_t)h * w >= (1u << 31)) return fail(ctx, VD3D_ERR_ARG, "bad argument");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  const size_t npx = (size_t)h * w;
+  const void* g_d;
+  void* o_d;
+  int r;
+  if ((r = copy_in(ctx, ctx->lb_prev, gray, npx, mem, s, &g_d))) return r;
+  if ((r = stage_out(ctx, ctx->lb_out, dst, npx, mem, &o_d))) return r;
+  if ((r = lb_canny_scratch(ctx, npx))) return r;
+  int low2, high2;
+  canny_thresholds(low, high, &low2, &high2);
+  launch_canny((const uint8_t*)g_d, 1, h, w, low2, high2, (int32_t*)ctx->lb_mag.p, (int32_t*)ctx->lb_label.p,
+               (uint8_t*)ctx->lb_flag.p, (uint8_t*)o_d, nullptr, s);
+  ctx->launches += 5;
+  return stage_finish(ctx, dst, o_d, npx, mem);
+}
+
+int vd3d_letterbox_stats(vd3d_ctx* ctx, int n, const uint8_t* frames, int h, int w, const uint8_t* prev_gray, int mem,
+                         float* row_y_mean, float* row_y_var, float* row_s_mean, int32_t* row_edges,
+                         float* frame_y_mean, uint32_t* frame_hist, uint64_t* frame_absdiff, uint8_t* last_gray) {
+  if (!ctx || !frames || n < 1 || h < 1 || w < 1 || w > 8192 || !row_y_mean || !row_y_var || !row_s_mean ||
+      !row_edges || !frame_y_mean || !frame_hist || !frame_absdiff)
+    return fail(ctx, VD3D_ERR_ARG, "bad argument (frames of 1..8192 columns, every record pointer set)");
+  const size_t npix = (size_t)h * w, npx = npix * n, rows = (size_t)h * n;
+  if (npx >= (1u << 31)) return fail(ctx, VD3D_ERR_ARG, "n * h * w must stay below 2^31");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  const void *f_d, *p_d = nullptr;
+  int r;
+  if ((r = copy_in(ctx, ctx->lb_in, frames, npx * 3, mem, s, &f_d))) return r;
+  if (prev_gray && (r = copy_in(ctx, ctx->lb_prev, prev_gray, npix, mem, s, &p_d))) return r;
+  if ((r = ensure(ctx, ctx->lb_gray, npx)) || (r = lb_canny_scratch(ctx, npx))) return r;
+  if (ctx->lb_nodes_npix != (int64_t)npix) {
+    int cnt = 0;
+    lb_cut_nodes((int64_t)npix, nullptr, nullptr, &cnt, 0);
+    std::vector<int64_t> st(cnt);
+    std::vector<int> ln(cnt);
+    lb_cut_nodes((int64_t)npix, st.data(), ln.data(), &cnt, cnt);
+    if ((r = ensure(ctx, ctx->lb_nodes, (size_t)cnt * 12))) return r;
+    CK(cudaMemcpyAsync(ctx->lb_nodes.p, st.data(), (size_t)cnt * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync((char*)ctx->lb_nodes.p + (size_t)cnt * 8, ln.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaStreamSynchronize(s));
+    ctx->lb_nodes_npix = (int64_t)npix;
+    ctx->lb_nodes_n = cnt;
+  }
+  const int nodes = ctx->lb_nodes_n;
+  if ((r = ensure(ctx, ctx->lb_node_sum, (size_t)nodes * n * 4))) return r;
+  // one record block, one D2H: absdiff u64 [n] | y_mean, y_var, s_mean f32 [rows] | edges i32 [rows] | hist u32 [n,64]
+  // | frame y_mean f32 [n]
+  const size_t o_mean = 8 * (size_t)n, o_var = o_mean + 4 * rows, o_sat = o_var + 4 * rows, o_edge = o_sat + 4 * rows,
+               o_hist = o_edge + 4 * rows, o_fmean = o_hist + 256 * (size_t)n, rec = o_fmean + 4 * (size_t)n;
+  if ((r = ensure(ctx, ctx->lb_rec, rec))) return r;
+  char* R = (char*)ctx->lb_rec.p;
+  CK(cudaMemsetAsync(R, 0, rec, s));
+  LbRowArgs a;
+  a.frames = (const uint8_t*)f_d;
+  a.prev_gray = (const uint8_t*)p_d;
+  a.n = n;
+  a.h = h;
+  a.w = w;
+  a.gray = (uint8_t*)ctx->lb_gray.p;
+  a.y_mean = (float*)(R + o_mean);
+  a.y_var = (float*)(R + o_var);
+  a.s_mean = (float*)(R + o_sat);
+  a.hist = (uint32_t*)(R + o_hist);
+  a.absdiff = (unsigned long long*)R;
+  launch_lb_rows(a, s);
+  launch_lb_frame_mean(a.frames, n, (int64_t)npix, (const int64_t*)ctx->lb_nodes.p,
+                       (const int*)((char*)ctx->lb_nodes.p + (size_t)nodes * 8), nodes, (float*)ctx->lb_node_sum.p,
+                       (float*)(R + o_fmean), s);
+  launch_canny(a.gray, n, h, w, 900, 8100, (int32_t*)ctx->lb_mag.p, (int32_t*)ctx->lb_label.p,
+               (uint8_t*)ctx->lb_flag.p, nullptr, (int32_t*)(R + o_edge), s);
+  ctx->launches += 8;
+  CK(cudaGetLastError());
+  std::vector<char> host(rec);
+  CK(cudaMemcpyAsync(host.data(), R, rec, cudaMemcpyDeviceToHost, s));
+  if (last_gray)
+    CK(cudaMemcpyAsync(last_gray, a.gray + npix * (n - 1), npix,
+                       mem == VD3D_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, s));
+  CK(cudaStreamSynchronize(s));
+  memcpy(frame_absdiff, host.data(), 8 * (size_t)n);
+  memcpy(row_y_mean, host.data() + o_mean, 4 * rows);
+  memcpy(row_y_var, host.data() + o_var, 4 * rows);
+  memcpy(row_s_mean, host.data() + o_sat, 4 * rows);
+  memcpy(row_edges, host.data() + o_edge, 4 * rows);
+  memcpy(frame_hist, host.data() + o_hist, 256 * (size_t)n);
+  memcpy(frame_y_mean, host.data() + o_fmean, 4 * (size_t)n);
+  return VD3D_OK;
+}
+
+int vd3d_letterbox_repad(vd3d_ctx* ctx, const uint8_t* src, int h, int w, int top, int bottom, uint8_t* dst, int mem) {
+  if (!ctx || !src || !dst || h < 1 || w < 1 || top < 0 || bottom < 0) return fail(ctx, VD3D_ERR_ARG, "bad argument");
+  if (mem == VD3D_MEM_DEVICE && src == dst) return fail(ctx, VD3D_ERR_ARG, "src and dst must not alias");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  const size_t npx = (size_t)h * w;
+  const void* s_d;
+  void* o_d;
+  int r;
+  if ((r = copy_in(ctx, ctx->lb_prev, src, npx, mem, s, &s_d))) return r;
+  if ((r = stage_out(ctx, ctx->lb_out, dst, npx, mem, &o_d))) return r;
+  const int core_h = h - top - bottom;
+  if ((top == 0 && bottom == 0) || core_h <= 0) {
+    // no bars, or the reference's fallback (bars dropped, core = the whole frame): cv2.resize to the same size copies
+    CK(cudaMemcpyAsync(o_d, s_d, npx, cudaMemcpyDeviceToDevice, s));
+    ctx->launches += 1;
+  } else {
+    if ((r = ensure(ctx, ctx->lb_hist, 256 * 4))) return r;
+    CK(cudaMemsetAsync(ctx->lb_hist.p, 0, 256 * 4, s));
+    launch_resize_cubic_u8((const uint8_t*)s_d, h, w, 1, (uint8_t*)o_d + (size_t)top * w, core_h, w, s);
+    launch_lb_pad((uint8_t*)o_d, h, w, top, core_h, (uint32_t*)ctx->lb_hist.p, s);
+    ctx->launches += 4;
+  }
+  return stage_finish(ctx, dst, o_d, npx, mem);
 }
 
 }  // extern "C"

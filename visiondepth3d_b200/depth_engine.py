@@ -56,6 +56,8 @@ def _bind(lib):
     lib.vd3d_depth_infer_device.restype = i
     lib.vd3d_depth_infer_batch.argtypes = [vp, i, C.POINTER(vp), i, i, C.POINTER(vp), C.POINTER(vp), i]
     lib.vd3d_depth_infer_batch.restype = i
+    lib.vd3d_depth_infer_batch_device.argtypes = [vp, i, C.POINTER(vp), i, i, C.POINTER(vp), C.POINTER(vp), i]
+    lib.vd3d_depth_infer_batch_device.restype = i
     lib.vd3d_depth_profile.argtypes = [vp, i]
     lib.vd3d_depth_profile.restype = i
     lib.vd3d_depth_profile_collect.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(i), C.POINTER(C.c_double)]
@@ -149,6 +151,19 @@ class DepthEngine:
             self.check(self.lib.vd3d_depth_infer_batch(self.h, n, fp, h, w, p32, p8, int(bool(invert))))
             out += list(zip(d32, d8))
         return out
+
+    def infer_batch_u8_device(self, frame_ptrs, h, w, u8_ptrs, invert=False):
+        """Device form of infer_batch: up to 8 BGR frames [h,w,3] at device pointers -> min-max u8 depth [h,w] at
+        device pointers.  Enqueued on the context's stream; no synchronisation."""
+        n = len(frame_ptrs)
+        if not 1 <= n <= 8 or len(u8_ptrs) != n:
+            raise ValueError("infer_batch_u8_device takes 1..8 frames and one output per frame")
+        if processed_size(w, h) != (self.image_h, self.image_w):
+            raise ValueError(f"engine built for processed size {(self.image_h, self.image_w)}, a {w}x{h} frame needs "
+                             f"{processed_size(w, h)}")
+        fp = (C.c_void_p * n)(*frame_ptrs)
+        p8 = (C.c_void_p * n)(*u8_ptrs)
+        self.check(self.lib.vd3d_depth_infer_batch_device(self.h, n, fp, h, w, p8, None, int(bool(invert))))
 
     def get_buffer(self, name, shape, dtype):
         out = np.empty(shape, dtype=dtype)

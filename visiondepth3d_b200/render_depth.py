@@ -1,7 +1,7 @@
 """Drop-in for the hot-path surface of the reference's core/render_depth.py: the `pipe`
 callable protocol and the depth -> uint8 normalisation, backed by the libvd3d depth engine
-(Depth-Anything-V2 on wgmma tensor cores).  GUI, ONNX, Marigold, DepthCrafter and the
-letterbox tracker are outside the GPU hot path (SURVEY.md section 2).
+(Depth-Anything-V2 on wgmma tensor cores), and the letterbox tracker of the depth-video pass with its pixel work on
+the GPU (letterbox.cu).  GUI, ONNX, Marigold and DepthCrafter are outside the GPU hot path (SURVEY.md section 2).
 
 Protocol kept (core/render_depth.py:1113-1119, consumers 201-268 and 1894-1917):
     pipe(images: list[PIL.Image], inference_size: (W, H) | None) -> list[{"predicted_depth": Tensor[h, w]}]
@@ -334,58 +334,443 @@ def read_letterbox_sidecar(video_path):
         return json.load(f)
 
 
-def depth_video_from_video(input_path, output_path, invert=False, inference_size=None, batch_size=8,
-                           status=None, max_frames=None):
-    """Frames of `input_path` -> depth video `output_path` in the reference's format (process_video2's `hf` branch
-    without the letterbox tracker, i.e. bars 0/0 in the sidecar): each frame through the depth engine, min-max u8
-    (convert_depth_to_grayscale), optional inversion, INTER_CUBIC resize back when inference_size was given, grey ->
-    BGR, XVID.  Returns the number of frames written."""
+# ---------------------------------------------------------------------------
+# letterbox tracker (core/render_depth.py:273-573): the pixel statistics come from the GPU (vd3d_letterbox_stats, one
+# small record per frame); the scan, the gates, the bootstrap median and the hysteresis are host scalar logic
+# ---------------------------------------------------------------------------
+class _FrameStats:
+    """GPU statistics of one u8 BGR frame: what the reference's helpers compute from its pixels.  has_prev: a
+    previous gray plane was compared (absdiff is meaningful); prev_shape_differs: the previous plane had another
+    shape, which is_scene_cut counts as a cut."""
+    __slots__ = ("h", "w", "y_mean", "y_var", "s_mean", "edges", "frame_y_mean", "hist", "absdiff", "has_prev",
+                 "prev_shape_differs")
+
+    def row_edge_density(self):
+        # _horizontal_edge_density: edges.mean(axis=1) / 255.0 on the 0/255 Canny map, built as numpy builds it
+        return (self.edges.astype(np.float64) * 255.0) / np.intp(self.w) / 255.0
+
+
+def _is_cuda_tensor(x):
+    return torch is not None and isinstance(x, torch.Tensor) and x.is_cuda
+
+
+def letterbox_stats(frames, prev_gray=None):
+    """Statistics of same-shape u8 BGR frames in one GPU pass -> (list of _FrameStats, gray plane of the last frame).
+    frames: a list of host frames [h,w,3], or a CUDA uint8 tensor [n,h,w,3] (the statistics then read device memory and
+    the returned gray plane is a CUDA tensor).  prev_gray: the gray plane before the first frame (host array or CUDA
+    tensor), or None.  Only the per-row / per-frame records come back to the host, in one copy."""
+    from . import _lib
+    ctx = _lib.default_context(0)
+    device = _is_cuda_tensor(frames)
+    if device:
+        fr = frames.contiguous()
+        if fr.dtype != torch.uint8 or fr.dim() != 4 or fr.shape[3] != 3:
+            raise ValueError("Expected a uint8 CUDA tensor [n, h, w, 3] of BGR frames")
+        n, h, w = (int(v) for v in fr.shape[:3])
+    else:
+        fr = np.ascontiguousarray(np.stack([np.asarray(f, dtype=np.uint8) for f in frames]))
+        if fr.ndim != 4 or fr.shape[3] != 3:
+            raise ValueError("Expected BGR uint8 image with 3 channels")
+        n, h, w = fr.shape[:3]
+    ym = np.empty((n, h), np.float32)
+    yv = np.empty((n, h), np.float32)
+    sm = np.empty((n, h), np.float32)
+    ed = np.empty((n, h), np.int32)
+    fm = np.empty(n, np.float32)
+    hist = np.empty((n, 64), np.uint32)
+    ad = np.empty(n, np.uint64)
+    pg = None
+    shape_differs = prev_gray is not None and tuple(prev_gray.shape) != (h, w)
+    if prev_gray is not None and not shape_differs:
+        if device:
+            pg = (prev_gray if _is_cuda_tensor(prev_gray) else torch.from_numpy(np.asarray(prev_gray))).to(
+                fr.device, torch.uint8).contiguous()
+        else:
+            pg = np.ascontiguousarray(prev_gray.cpu().numpy() if _is_cuda_tensor(prev_gray) else prev_gray,
+                                      dtype=np.uint8)
+    if device:
+        last = torch.empty((h, w), dtype=torch.uint8, device=fr.device)
+        torch.cuda.current_stream().synchronize()  # the frames may come from work queued on torch's stream
+        fp, pp, lp, mem = fr.data_ptr(), pg.data_ptr() if pg is not None else None, last.data_ptr(), _lib.MEM_DEVICE
+    else:
+        last = np.empty((h, w), np.uint8)
+        fp, pp, lp, mem = fr.ctypes.data, pg.ctypes.data if pg is not None else None, last.ctypes.data, _lib.MEM_HOST
+    ctx.check(ctx.lib.vd3d_letterbox_stats(ctx.h, n, fp, h, w, pp, mem, ym.ctypes.data, yv.ctypes.data,
+                                           sm.ctypes.data, ed.ctypes.data, fm.ctypes.data, hist.ctypes.data,
+                                           ad.ctypes.data, lp))
+    out = []
+    for i in range(n):
+        st = _FrameStats()
+        st.h, st.w = h, w
+        st.y_mean, st.y_var, st.s_mean, st.edges = ym[i], yv[i], sm[i], ed[i]
+        st.frame_y_mean, st.hist, st.absdiff = fm[i], hist[i], int(ad[i])
+        st.has_prev = i > 0 or pg is not None
+        st.prev_shape_differs = i == 0 and shape_differs
+        out.append(st)
+    return out, last
+
+
+def _stats1(frame_bgr):
+    if frame_bgr is None or frame_bgr.ndim != 3 or frame_bgr.shape[2] != 3:
+        raise ValueError("Expected BGR uint8 image with 3 channels")
+    return letterbox_stats([frame_bgr])[0][0]
+
+
+def _scene_cut_from_stats(st, prev_hist, mad_thresh=28.0, corr_thresh=0.60):
     import cv2
+    if st.prev_shape_differs:
+        return True
+    if not st.has_prev:
+        return False
+    mad = float(np.float64(st.absdiff) / np.intp(st.h * st.w))
+    if mad > mad_thresh:
+        return True
+    h1 = prev_hist.astype(np.float32).reshape(64, 1)
+    h2 = st.hist.astype(np.float32).reshape(64, 1)
+    cv2.normalize(h1, h1)
+    cv2.normalize(h2, h2)
+    return float(cv2.compareHist(h1, h2, cv2.HISTCMP_CORREL)) < corr_thresh
+
+
+def _near_black_from_stats(st, mean_thresh=18, edge_thresh=0.02):
+    return float(st.frame_y_mean) < mean_thresh and st.row_edge_density().mean() < edge_thresh
+
+
+def _strict_robust_from_stats(st, y_thresh=16, var_thresh=3.0, sat_thresh=6.0, max_scan_frac=0.25,
+                              min_band_frac=0.06, edge_max=0.04):
+    h, w = st.h, st.w
+    if h < 64 or w < 64:
+        return 0, 0
+    y_mean, y_var, s_mean, row_edge = st.y_mean, st.y_var, st.s_mean, st.row_edge_density()
+
+    def scan(rows):
+        run = 0
+        for i in rows:
+            if y_mean[i] < y_thresh and y_var[i] < var_thresh and s_mean[i] < sat_thresh and row_edge[i] <= edge_max:
+                run += 1
+            else:
+                break
+        if run < int(h * min_band_frac):
+            run = 0
+        if run % 2 == 1:
+            run -= 1
+        return max(run, 0)
+
+    H = int(h * max_scan_frac)
+    top = scan(range(0, H))
+    bot = scan(range(h - 1, h - 1 - H, -1))
+    if top + bot >= h * 0.6:  # absurd
+        return 0, 0
+    return int(top), int(bot)
+
+
+def is_scene_cut(prev_gray, gray, mad_thresh=28.0, corr_thresh=0.60):
+    """core/render_depth.py:295-319 on two gray planes: MAD above mad_thresh, else 64-bin histogram correlation below
+    corr_thresh."""
+    import cv2
+    if prev_gray is None or gray is None:
+        return False
+    if prev_gray.shape != gray.shape:
+        return True
+    mad = float(np.mean(np.abs(prev_gray.astype(np.int16) - gray.astype(np.int16))))
+    if mad > mad_thresh:
+        return True
+    h1 = cv2.calcHist([prev_gray], [0], None, [64], [0, 256])
+    h2 = cv2.calcHist([gray], [0], None, [64], [0, 256])
+    cv2.normalize(h1, h1)
+    cv2.normalize(h2, h2)
+    return float(cv2.compareHist(h1, h2, cv2.HISTCMP_CORREL)) < corr_thresh
+
+
+def detect_letterbox_strict_robust(frame_bgr, y_thresh=16, var_thresh=3.0, sat_thresh=6.0, max_scan_frac=0.25,
+                                   min_band_frac=0.06, edge_max=0.04):
+    """core/render_depth.py:336-385: (top, bottom) bar rows of one frame, or (0, 0)."""
+    h, w = frame_bgr.shape[:2]
+    if h < 64 or w < 64:
+        return 0, 0
+    return _strict_robust_from_stats(_stats1(frame_bgr), y_thresh, var_thresh, sat_thresh, max_scan_frac,
+                                     min_band_frac, edge_max)
+
+
+def is_near_black_frame(frame_bgr, mean_thresh=18, edge_thresh=0.02):
+    """core/render_depth.py:387-392: dark (luma mean) and nearly edge-free."""
+    return _near_black_from_stats(_stats1(frame_bgr), mean_thresh, edge_thresh)
+
+
+def detect_letterbox_multiframe_confidence(cap, original_height, fps, max_seconds=3, samples=9):
+    """core/render_depth.py:394-455: ((top, bottom), confidence) from up to `samples` frames of the first
+    max_seconds, skipping near-black frames and scene cuts; the capture position is restored."""
+    import cv2
+    try:
+        total = int(cap.get(cv2.CAP_PROP_FRAME_COUNT))
+    except Exception:
+        total = 0
+    window = max(min(total, int((fps if fps and fps > 0 else 30) * max_seconds)), 1)
+    tops, bottoms = [], []
+    prev_gray, prev_hist = None, None
+    pos_backup = cap.get(cv2.CAP_PROP_POS_FRAMES)
+    for i in np.linspace(0, max(0, window - 1), num=min(samples, window), dtype=int):
+        cap.set(cv2.CAP_PROP_POS_FRAMES, int(i))
+        ok, frame = cap.read()
+        if not ok:
+            continue
+        (st,), gray = letterbox_stats([frame], prev_gray)
+        if not (_near_black_from_stats(st) or _scene_cut_from_stats(st, prev_hist)):
+            t, b = _strict_robust_from_stats(st)
+            if 0 <= t < original_height and 0 <= b < original_height and (t + b) < original_height:
+                tops.append(t)
+                bottoms.append(b)
+        prev_gray, prev_hist = gray, st.hist
+    cap.set(cv2.CAP_PROP_POS_FRAMES, pos_backup or 0)
+    if not tops:
+        return (0, 0), 0.0
+    t_med, b_med = int(np.median(tops)), int(np.median(bottoms))
+    if t_med % 2:
+        t_med -= 1
+    if b_med % 2:
+        b_med -= 1
+    t_med, b_med = max(t_med, 0), max(b_med, 0)
+    if t_med + b_med >= original_height * 0.6:
+        return (0, 0), 0.0
+    agree = sum(1 for t, b in zip(tops, bottoms) if abs(t - t_med) <= 4 and abs(b - b_med) <= 4)
+    return (t_med, b_med), float(agree / max(1, len(tops)))
+
+
+class LetterboxTracker:
+    """core/render_depth.py:458-573: tracks and freezes letterbox bars, re-checking only at scene cuts on non-black
+    frames, with a cooldown and confirm_needed-fold hysteresis.  States: locked_zero (no bars) and locked_bars.
+    update() takes one frame; update_batch() takes a batch in one GPU pass with the same result frame by frame."""
+
+    def __init__(self, h, fps, min_change=8, confirm_needed=3, max_total_frac=0.35, conf_enable=0.7,
+                 conf_disable=0.6, cooldown_sec=3.0):
+        self.h = int(h)
+        self.fps = float(fps) if fps and fps > 0 else 30.0
+        self.min_change = int(min_change)
+        self.confirm_needed = int(confirm_needed)
+        self.max_total_frac = float(max_total_frac)
+        self.conf_enable = float(conf_enable)
+        self.conf_disable = float(conf_disable)
+        self.cooldown_frames = int(self.fps * cooldown_sec)
+        self.top = 0
+        self.bot = 0
+        self.locked_zero = True
+        self.locked_bars = False
+        self._cand = (0, 0)
+        self._streak = 0
+        self._cooldown = 0
+        self.prev_gray = None
+        self._prev_hist = None
+
+    def bootstrap(self, cap):
+        (t, b), conf = detect_letterbox_multiframe_confidence(cap, self.h, self.fps)
+        if conf >= self.conf_enable and (t + b) > 0:
+            self.top, self.bot = t, b
+            self.locked_bars, self.locked_zero = True, False
+        else:
+            self.top, self.bot = 0, 0
+            self.locked_zero, self.locked_bars = True, False
+        self._cooldown = self.cooldown_frames
+        return self.top, self.bot, (self.locked_bars, self.locked_zero)
+
+    def should_recheck(self, frame_idx):
+        return self._cooldown <= 0
+
+    def update(self, frame_bgr, frame_idx):
+        return self.update_batch([frame_bgr], frame_idx)[-1]
+
+    def update_batch(self, frames_bgr, first_idx=0):
+        """update() on each frame in order (indices first_idx, first_idx + 1, ...) -> list of (top, bottom).  frames_bgr:
+        a list of host frames or a CUDA uint8 tensor [n, h, w, 3] (the previous gray plane then stays on the device)."""
+        stats, gray = letterbox_stats(frames_bgr, self.prev_gray)
+        out = []
+        for k, st in enumerate(stats):
+            out.append(self._step(st, first_idx + k))
+            self._prev_hist = st.hist
+        self.prev_gray = gray
+        return out
+
+    def _step(self, st, frame_idx):
+        if self._cooldown > 0:
+            self._cooldown -= 1
+        if _near_black_from_stats(st):
+            return self.top, self.bot
+        if not _scene_cut_from_stats(st, self._prev_hist):
+            return self.top, self.bot
+        if not self.should_recheck(frame_idx):
+            return self.top, self.bot
+        mt, mb = _strict_robust_from_stats(st)
+        if (mt + mb) > int(self.h * self.max_total_frac):
+            mt, mb = 0, 0
+        if mt % 2:
+            mt -= 1
+        if mb % 2:
+            mb -= 1
+        mt, mb = max(mt, 0), max(mb, 0)
+        if abs(mt - self.top) + abs(mb - self.bot) < self.min_change:
+            self._streak = 0
+            self._cand = (self.top, self.bot)
+            return self.top, self.bot
+        cand = (mt, mb)
+        if cand == self._cand:
+            self._streak += 1
+        else:
+            self._cand = cand
+            self._streak = 1
+        if self._streak >= self.confirm_needed:
+            if self.locked_zero and (mt + mb) > 0:
+                self.top, self.bot = mt, mb
+                self.locked_zero, self.locked_bars = False, True
+                self._cooldown = self.cooldown_frames
+            elif self.locked_bars:
+                self.top, self.bot = mt, mb
+                self.locked_zero = (mt + mb) == 0
+                self.locked_bars = (mt + mb) > 0
+                self._cooldown = self.cooldown_frames
+        return self.top, self.bot
+
+
+def crop_by_bars(frame_bgr, top, bottom):
+    """core/render_depth.py:577-583: drop the bar rows, unless that would leave nothing."""
+    h = frame_bgr.shape[0]
+    top, bottom = max(int(top), 0), max(int(bottom), 0)
+    if top + bottom >= h:
+        return frame_bgr
+    return frame_bgr[top:h - bottom, :]
+
+
+def letterbox_repad(depth_u8, top, bottom):
+    """process_video2's re-pad of a u8 depth plane (core/render_depth.py:1919-1933) on the GPU
+    (vd3d_letterbox_repad): INTER_CUBIC resize into the core rows, bar rows filled with the core's median."""
+    from . import _lib
+    ctx = _lib.default_context(0)
+    src = np.ascontiguousarray(depth_u8, dtype=np.uint8)
+    out = np.empty_like(src)
+    ctx.check(ctx.lib.vd3d_letterbox_repad(ctx.h, src.ctypes.data, src.shape[0], src.shape[1], int(top), int(bottom),
+                                           out.ctypes.data, _lib.MEM_HOST))
+    return out
+
+
+def _repad_device(src, top, bottom, dst):
+    """vd3d_letterbox_repad on CUDA planes (src, dst: uint8 tensors [h, w], distinct)."""
+    from . import _lib
+    ctx = _lib.default_context(0)
+    h, w = (int(v) for v in src.shape)
+    ctx.check(ctx.lib.vd3d_letterbox_repad(ctx.h, src.data_ptr(), h, w, int(top), int(bottom), dst.data_ptr(),
+                                           _lib.MEM_DEVICE))
+
+
+_staging = {}  # (n, H, W) -> pinned host tensor [n, H, W, 3]: the upload buffer of the tracked batch path
+
+
+def _tracked_batch_device(batch, W, H, invert, tracker):
+    """One tracked depth batch on one device copy of its frames: the tracker's statistics and the depth forward read
+    the same upload, the re-pad works on the device depth, and the written planes come back in one download."""
+    eng = _engine_for(W, H)
+    n = len(batch)
+    host = _staging.get((n, H, W))
+    if host is None:
+        host = _staging[(n, H, W)] = torch.empty((n, H, W, 3), dtype=torch.uint8).pin_memory()
+    hn = host.numpy()
+    for k, f in enumerate(batch):
+        hn[k] = f
+    dev = host.to("cuda", non_blocking=True)
+    bars = tracker.update_batch(dev)[-1]  # synchronises torch's stream before the statistics read `dev`
+    d8 = torch.empty((n, H, W), dtype=torch.uint8, device=dev.device)
+    for i0 in range(0, n, 8):
+        idx = range(i0, min(n, i0 + 8))
+        eng.infer_batch_u8_device([dev[k].data_ptr() for k in idx], H, W, [d8[k].data_ptr() for k in idx], invert)
+    if bars[0] or bars[1]:
+        out = torch.empty_like(d8)
+        for k in range(n):
+            _repad_device(d8[k], bars[0], bars[1], out[k])
+        d8 = out
+    eng.ctx.check(eng.lib.vd3d_sync(eng.ctx.h))
+    return list(d8.cpu().numpy())
+
+
+def iter_depth_frames(cap, W, H, invert=False, inference_size=None, batch_size=8, max_frames=None, tracker=None,
+                      status=None):
+    """The u8 depth planes depth_video_from_video writes, in order, from the frames cap.read() returns.  With a
+    bootstrapped `tracker` (ignore_letterbox_bars), every frame read goes through tracker.update and each frame of a
+    batch is re-padded with the bars the tracker holds after the batch's last frame, as process_video2 does."""
     from PIL import Image
-    cap = cv2.VideoCapture(input_path)
-    if not cap.isOpened():
-        print(f"❌ Cannot open {input_path}")
-        return 0
-    fps = cap.get(cv2.CAP_PROP_FPS) or 24.0
-    W, H = int(cap.get(cv2.CAP_PROP_FRAME_WIDTH)), int(cap.get(cv2.CAP_PROP_FRAME_HEIGHT))
-    write_letterbox_sidecar(output_path, 0, 0, W, H)
-    out = cv2.VideoWriter(output_path, cv2.VideoWriter_fourcc(*"XVID"), fps, (W, H))
-    if not out.isOpened():
-        print(f"❌ Failed to open video writer for {os.path.basename(output_path)}")
-        cap.release()
-        return 0
     n, batch = 0, []
 
     def flush():
-        nonlocal n
+        if tracker is not None and inference_size is None:
+            d8s = _tracked_batch_device(batch, W, H, invert, tracker)
+            batch.clear()
+            return d8s
+        bars = (0, 0)
+        if tracker is not None:
+            bars = tracker.update_batch(batch, n + 1)[-1]
         if inference_size is None:
-            eng = _engine_for(W, H)
-            for _, d8 in eng.infer_batch(batch, invert=invert):
-                out.write(cv2.cvtColor(d8, cv2.COLOR_GRAY2BGR))
-                n += 1
+            d8s = [d8 for _, d8 in _engine_for(W, H).infer_batch(batch, invert=invert)]
         else:
+            d8s = []
             pil = [Image.fromarray(f[..., ::-1].copy()) for f in batch]
             for res in hf_batch_safe_pipe(pil, inference_size):
                 d8 = convert_depth_to_grayscale(res["predicted_depth"])
                 if invert:
                     d8 = 255 - d8
-                d8 = resize_cubic_u8(d8, W, H)
-                out.write(cv2.cvtColor(d8, cv2.COLOR_GRAY2BGR))
-                n += 1
+                d8s.append(resize_cubic_u8(d8, W, H))
         batch.clear()
+        if tracker is not None and (bars[0] or bars[1]):
+            d8s = [letterbox_repad(d8, bars[0], bars[1]) for d8 in d8s]
+        return d8s
+
+    while not cancel_requested.is_set():
+        ok, frame = cap.read()
+        if not ok or (max_frames is not None and n + len(batch) >= max_frames):
+            break
+        batch.append(frame)
+        if len(batch) >= batch_size:
+            for d8 in flush():
+                n += 1
+                yield d8
+            if status is not None:
+                _notify(status, f"📸 Processed: {n}")
+    if batch and not cancel_requested.is_set():
+        for d8 in flush():
+            n += 1
+            yield d8
         if status is not None:
             _notify(status, f"📸 Processed: {n}")
 
+
+def depth_video_from_video(input_path, output_path, invert=False, inference_size=None, batch_size=8,
+                           status=None, max_frames=None, ignore_letterbox_bars=False):
+    """Frames of `input_path` -> depth video `output_path` in the reference's format (process_video2's `hf` branch):
+    each frame through the depth engine, min-max u8 (convert_depth_to_grayscale), optional inversion, INTER_CUBIC
+    resize back when inference_size was given, grey -> BGR, XVID.  Returns the number of frames written.
+    ignore_letterbox_bars=False writes bars 0/0 to the sidecar.  True runs the reference's letterbox tracker: a
+    bootstrap on the first int(fps * 3) frames decides the sidecar's bars, every frame updates the tracker, and each
+    depth frame is re-padded to the tracked bars (iter_depth_frames)."""
+    import cv2
+    cap = cv2.VideoCapture(input_path)
+    if not cap.isOpened():
+        print(f"❌ Cannot open {input_path}")
+        return 0
+    raw_fps = cap.get(cv2.CAP_PROP_FPS)
+    fps = raw_fps or 24.0
+    W, H = int(cap.get(cv2.CAP_PROP_FRAME_WIDTH)), int(cap.get(cv2.CAP_PROP_FRAME_HEIGHT))
+    tracker = None
+    top = bottom = 0
+    if ignore_letterbox_bars:
+        tracker = LetterboxTracker(H, raw_fps)
+        top, bottom, (locked_bars, locked_zero) = tracker.bootstrap(cap)
+        print(f"[VD3D] Bootstrap bars: top={top} bottom={bottom} | locked_bars={locked_bars} locked_zero={locked_zero}")
+    write_letterbox_sidecar(output_path, top, bottom, W, H)
+    out = cv2.VideoWriter(output_path, cv2.VideoWriter_fourcc(*"XVID"), fps, (W, H))
+    if not out.isOpened():
+        print(f"❌ Failed to open video writer for {os.path.basename(output_path)}")
+        cap.release()
+        return 0
+    n = 0
     try:
-        while not cancel_requested.is_set():
-            ok, frame = cap.read()
-            if not ok or (max_frames is not None and n + len(batch) >= max_frames):
-                break
-            batch.append(frame)
-            if len(batch) >= batch_size:
-                flush()
-        if batch and not cancel_requested.is_set():
-            flush()
+        for d8 in iter_depth_frames(cap, W, H, invert, inference_size, batch_size, max_frames, tracker, status):
+            out.write(cv2.cvtColor(d8, cv2.COLOR_GRAY2BGR))
+            n += 1
     finally:
         cap.release()
         out.release()

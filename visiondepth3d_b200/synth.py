@@ -4,6 +4,8 @@ smooth set: ramps + moving disc (parity gate);  noise set: white-noise RGB
 (throughput / adversarial LSB case).  Frame i uses default_rng(1000+i).
 letterbox set: the natural content inside top / bottom black bars whose heights change per frame, with the edge cases
 of render_sbs_3d's black-bar detection (auto_crop_black_bars) on a fixed eight-frame schedule (_letterbox).
+letterbox_track / letterbox_track_nobars sets: clips for the depth-video letterbox tracker at a small fps (2: a
+six-frame bootstrap window and cooldown), on the schedule of _TRACK / _TRACK_NOBARS.
 natural set: band-limited random colour / depth fields with fine texture, translating 3 px per frame (temporally
 coherent like footage).  Sub-pixel warps of such content land on generic values, not on the k/255 truncation
 boundaries the ramps of the smooth set sit on, so it is the set the 1-LSB gate against the reference is meant for.
@@ -69,8 +71,66 @@ def _letterbox(i, w, h, rgb):
     return rgb
 
 
+# (scene, top, bottom, bar content) per frame.  Scenes 0 and 1 differ in brightness, so a switch between them is a
+# scene cut by mean absolute difference; consecutive frames of one scene are not cuts.  "black" is all black, "fade"
+# near-black; "flat" is scene 0 squeezed to 15 % contrast around its mean (a cut by histogram correlation alone).
+# Bar content: "zero" black, "noise" gray noise (fails the variance gate only), "blue" dark saturated blue (saturation
+# gate only), "gray40" (luma gate only), "edge" black with one gray-24 row, which puts Canny edges on a black row
+# (edge gate only).  Bars of b rows are detected as b - 2 rows (the two rows next to the picture carry its edges).
+_TRACK = (
+    [(0, 22, 22, "zero")] * 6                                    # 0-5: bootstrap window, locks (20, 20)
+    + [("black", 0, 0, "zero"), (1, 22, 22, "zero")]             # 6 near-black; 7 cut, change below min_change
+    + [(0, 31, 31, "zero"), (1, 31, 31, "zero"), (0, 31, 31, "zero")]  # 8-10 odd bars -> (30, 30), confirmed at 3
+    + [(1, 12, 12, "zero"), (1, 12, 12, "zero"), (0, 12, 12, "zero"), (0, 12, 12, "zero"), (0, 12, 12, "zero")]
+    #                                                              11-15 cuts inside the cooldown: ignored
+    + [(1, 16, 16, "zero"), (0, 16, 16, "zero"), (1, 31, 31, "zero")]  # 16-18 candidate (14, 14) breaks off after 2
+    + [(0, 27, 31, "zero")]                                      # 19 (26, 30): change 4, below min_change
+    + [(1, 42, 42, "zero"), (0, 42, 42, "zero"), (1, 42, 42, "zero")]  # 20-22 (40, 40) > max_total_frac -> (0, 0)
+    + [(0, 31, 31, "noise"), (1, 31, 31, "blue"), (0, 31, 31, "gray40"), (1, 31, 31, "edge")]  # 23-26 gates
+    + [(1, 0, 0, "zero"), (1, 0, 0, "zero"), (0, 0, 0, "zero"), (0, 0, 0, "zero"), ("flat", 0, 0, "zero")]
+    #                                                              27-31: 31 is a histogram-only cut
+    + [("fade", 0, 0, "zero"), (0, 22, 22, "zero"), (1, 22, 22, "zero"), (0, 22, 22, "zero")]  # 32 fade; 33-35
+    #                                                              locked_zero -> bars (20, 20), confirmed at 3
+    + [(0, 22, 22, "zero")]                                      # 36
+)
+_TRACK_NOBARS = [(0, 0, 0, "zero")] * 6 + [(1, 0, 0, "zero"), (0, 0, 0, "zero")]
+
+
+def _track_frame(i, w, h, sched):
+    scene, top, bot, bar = sched[i]
+    if scene == "black":
+        return np.zeros((h, w, 3), np.uint8)
+    base = _natural(i, w, h)[0][..., ::-1].astype(np.float64)
+    if scene == "fade":
+        f = base * 0.05
+    elif scene == "flat":
+        f = base * 0.45
+        f = (f - f.mean()) * 0.15 + f.mean()
+    else:
+        f = base * 0.45 if scene == 0 else base * 0.6 + 90
+    f = np.clip(f, 0, 255).astype(np.uint8)
+    rng = np.random.default_rng(6000 + i)
+    for rows, inner in ((slice(0, top), 1), (slice(h - bot, h), h - 2)):
+        n = f[rows].shape[0]
+        if n == 0:
+            continue
+        f[rows] = 0
+        if bar == "noise":
+            f[rows] = rng.integers(0, 14, (n, w, 1), dtype=np.uint8)
+        elif bar == "blue":
+            f[rows] = (30, 0, 0)
+        elif bar == "gray40":
+            f[rows] = 40
+        elif bar == "edge":
+            f[inner + (1 if inner == 1 else -1)] = 24
+    return np.ascontiguousarray(f)
+
+
 def synth_frame(i: int, w: int, h: int, kind: str = "smooth"):
     """Return (frame_bgr u8 [h,w,3], depth_bgr u8 [h,w,3]) for frame index i."""
+    if kind in ("letterbox_track", "letterbox_track_nobars"):
+        f = _track_frame(i, w, h, _TRACK if kind == "letterbox_track" else _TRACK_NOBARS)
+        return f, np.ascontiguousarray(np.repeat(f[..., 1:2], 3, axis=2))
     rng = np.random.default_rng(1000 + i)
     y, x = np.mgrid[0:h, 0:w]
     cx = (w // 4 + 20 * i) % w
