@@ -125,7 +125,7 @@ typedef struct {
 } vd3d_frame_info;
 
 /* sizeof() of the ABI structs, so bindings can verify their layout:
- * 0 vd3d_shift_params, 1 vd3d_render_params, 2 vd3d_size_plan, 3 vd3d_frame_info */
+ * 0 vd3d_shift_params, 1 vd3d_render_params, 2 vd3d_size_plan, 3 vd3d_frame_info, 4 vd3d_upscale_params */
 int vd3d_struct_size(int which);
 
 /* ---- lifecycle ------------------------------------------------------- */
@@ -337,6 +337,23 @@ int vd3d_get_depth_batch(vd3d_ctx* ctx);
  * implicit-GEMM convs, f16 activations, fp32 accumulate, fp32 last layer) -> PixelShuffle + input -> postprocess_esr. */
 int vd3d_sr_create(void* cuda_stream, vd3d_depth** out);
 int vd3d_sr_forward(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, int num_conv, uint8_t* out_bgr, int mem);
+/* arguments of run_esrgan (core/merged_pipeline.py:240-267) without tiling.  input_res_pct and blend_alpha are Python
+ * floats there (double here, rounded where the reference's cv2 calls round them). */
+typedef struct {
+  double input_res_pct;       /* < 100 INTER_AREA, > 100 INTER_CUBIC, 100 none (247-249) */
+  int32_t scale;              /* 4, or 2 when the reference's model_name contains "x2" (262) */
+  int32_t target_w, target_h; /* 0, 0 = no target_size (265-266) */
+  double blend_alpha;         /* < 0: mode "OFF" (no addWeighted); else the alpha of blend_images (233-238) */
+} vd3d_upscale_params;
+/* run_esrgan's whole untiled chain for n frames BGR u8 [h,w,3] -> outs [target or h,w,3], every step on the device:
+ * input resize (the INTER_AREA kernels of vd3d_fit_eye / INTER_CUBIC), the network of vd3d_sr_forward, the x4 image
+ * resampled with INTER_CUBIC straight from the last conv to the original size (to 2x the network input for scale 2,
+ * then INTER_CUBIC to the original size) without materialising it, INTER_CUBIC to the target, addWeighted.  Same-size
+ * resizes are skipped (cv2 copies).  A blend of two different sizes is VD3D_ERR_ARG (cv2.addWeighted raises).  sr must
+ * have been created on vd3d_stream(ctx).  Host memory: one upload and one download per frame, overlapping the compute
+ * of the neighbouring frames (page-locked buffers for full overlap); device memory: no PCIe traffic.  Synchronises. */
+int vd3d_sr_upscale(vd3d_ctx* ctx, vd3d_depth* sr, int n, const uint8_t* const* frames, int h, int w, int num_conv,
+                    const vd3d_upscale_params* p, uint8_t* const* outs, int mem);
 /* copy an internal activation buffer to the host (parity triage: "x", "tap0.0".., "f0".., "fused3") */
 int vd3d_depth_get_buffer(vd3d_depth* e, const char* name, void* host_out, size_t bytes);
 /* unit-test hooks for the tensor-core kernels */

@@ -536,6 +536,86 @@ def gen_letterbox():
         print(p, os.path.getsize(p), rec["boot"], rec["conf"], side)
 
 
+def gen_merged():
+    """The unmodified start_merged_pipeline (core/merged_pipeline.py:287-386) on the synth frames folder,
+    `python tools/gen_golden.py merged`.  Stand-ins: an onnxruntime module whose InferenceSession raises for the RIFE
+    file (the reference then runs without RIFE) and runs oracle/sr.py's srvgg_forward for the ESRGAN file;
+    start_ffmpeg_writer replaced by a recorder of (width, height, fps, codec) and every frame written;
+    natural_sort wrapped to record the file order."""
+    import importlib.machinery
+    import json
+    import tempfile
+    import types
+    import cv2
+    import torch
+    from oracle import sr as S
+    from tests.merged_oracle import MERGED_BASE, MERGED_CASES, MERGED_SR
+    from visiondepth3d_b200 import synth
+    sd = S.srvgg_state_dict(**MERGED_SR)
+
+    class Session:
+        def __init__(self, path, sess_options=None, providers=None):
+            if "RIFE" in os.path.basename(path):
+                raise FileNotFoundError(path)
+
+        def get_inputs(self):
+            return [types.SimpleNamespace(name="input")]
+
+        def run(self, _outputs, feeds):
+            with torch.no_grad():
+                return [S.srvgg_forward(sd, torch.from_numpy(feeds["input"])).numpy()]
+
+    ort = types.ModuleType("onnxruntime")
+    ort.__spec__ = importlib.machinery.ModuleSpec("onnxruntime", None)
+    ort.SessionOptions = type("SessionOptions", (), {})
+    ort.GraphOptimizationLevel = types.SimpleNamespace(ORT_ENABLE_ALL=99)
+    ort.get_available_providers = lambda: ["CPUExecutionProvider"]
+    ort.InferenceSession = Session
+    sys.modules["onnxruntime"] = ort
+    mp = refshim.load_reference(("merged_pipeline",))["merged_pipeline"]
+    meta = dict(torch=torch.__version__, cv2=cv2.__version__, numpy=np.__version__)
+    real_sort = mp.natural_sort
+    for name, case in MERGED_CASES.items():
+        rec = {"frames": []}
+
+        class Proc:
+            class stdin:  # noqa: N801
+                write = staticmethod(lambda b: rec["frames"].append(bytes(b)))
+                close = staticmethod(lambda: None)
+
+            def wait(self):
+                return 0
+
+        def writer(path, w, h, fps, codec):
+            rec["args"] = (w, h, fps, codec)
+            return Proc()
+
+        def sort(files):
+            out = real_sort(files)
+            rec["files"] = [os.path.basename(f) for f in out]
+            return out
+
+        mp.start_ffmpeg_writer, mp.natural_sort = writer, sort
+        with tempfile.TemporaryDirectory() as td:
+            folder = synth.merged_frames_folder(os.path.join(td, "frames"))
+            model = os.path.join(td, "weights", "RealESR_Gx4_fp16.onnx")
+            if case.get("model") != "missing":
+                os.makedirs(os.path.dirname(model))
+                open(model, "wb").close()
+            settings = dict(MERGED_BASE, frames_folder=folder, output_file=os.path.join(td, "out.mp4"), model_path=model)
+            settings.update({k: v for k, v in case.items() if k != "model"})
+            mp.start_merged_pipeline(settings, None, None)
+        w, h = rec["args"][:2]
+        frames = np.stack([np.frombuffer(b, np.uint8).reshape((h, w, 3) if len(b) == w * h * 3 else (72, 128, 3))
+                           for b in rec["frames"]])
+        p = os.path.join(OUT, name)
+        np.savez_compressed(p, frames=frames, writer_size=np.array(rec["args"][:2], np.int32),
+                            writer_fps=np.float64(rec["args"][2]), codec=rec["args"][3], files=json.dumps(rec["files"]),
+                            settings=json.dumps({k: v for k, v in case.items()}), **meta)
+        print(p, os.path.getsize(p), frames.shape, rec["args"], rec["files"])
+    mp.natural_sort = real_sort
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "signatures":
         gen_signatures()
@@ -551,5 +631,7 @@ if __name__ == "__main__":
         gen_autocrop()
     elif len(sys.argv) > 1 and sys.argv[1] == "letterbox":
         gen_letterbox()
+    elif len(sys.argv) > 1 and sys.argv[1] == "merged":
+        gen_merged()
     else:
         main()

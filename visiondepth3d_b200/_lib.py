@@ -78,6 +78,15 @@ class FrameInfo(C.Structure):
     ]
 
 
+class UpscaleParams(C.Structure):
+    _fields_ = [
+        ("input_res_pct", C.c_double),
+        ("scale", C.c_int32),
+        ("target_w", C.c_int32), ("target_h", C.c_int32),
+        ("blend_alpha", C.c_double),
+    ]
+
+
 # every symbol declared in include/vd3d.h (tests/test_abi.py checks the header against this)
 SYMBOLS = [
     "vd3d_create", "vd3d_destroy", "vd3d_last_error", "vd3d_reset_state", "vd3d_host_alloc",
@@ -86,7 +95,7 @@ SYMBOLS = [
     "vd3d_pixel_shift", "vd3d_plan_sizes", "vd3d_render_frame", "vd3d_render_clip",
     "vd3d_sharpen", "vd3d_dof_grade", "vd3d_struct_size", "vd3d_pack", "vd3d_fit_eye", "vd3d_area_table", "vd3d_area_linear_table", "vd3d_heal",
     "vd3d_profile", "vd3d_profile_collect", "vd3d_check_config", "vd3d_color_grade", "vd3d_resize_cubic_u8", "vd3d_resize_cubic", "vd3d_add_weighted",
-    "vd3d_sr_create", "vd3d_sr_forward",
+    "vd3d_sr_create", "vd3d_sr_forward", "vd3d_sr_upscale",
     # depth forward (bound in depth_engine.py)
     "vd3d_depth_create", "vd3d_depth_destroy", "vd3d_depth_last_error", "vd3d_depth_launch_count",
     "vd3d_depth_set_tensor", "vd3d_depth_forward", "vd3d_depth_get_buffer", "vd3d_gemm_f16", "vd3d_gemm_bench", "vd3d_conv_f16",
@@ -114,7 +123,7 @@ def load():
     vp, i, u8p, fp = C.c_void_p, C.c_int, C.c_void_p, C.c_void_p
     lib.vd3d_struct_size.argtypes = [i]
     lib.vd3d_struct_size.restype = i
-    for which, st in enumerate((ShiftParams, RenderParams, SizePlan, FrameInfo)):
+    for which, st in enumerate((ShiftParams, RenderParams, SizePlan, FrameInfo, UpscaleParams)):
         if lib.vd3d_struct_size(which) != C.sizeof(st):
             raise OSError(f"libvd3d ABI mismatch for {st.__name__}: "
                           f"{lib.vd3d_struct_size(which)} != {C.sizeof(st)}")
@@ -207,6 +216,8 @@ def load():
     lib.vd3d_sr_create.restype = i
     lib.vd3d_sr_forward.argtypes = [vp, u8p, i, i, i, u8p, i]
     lib.vd3d_sr_forward.restype = i
+    lib.vd3d_sr_upscale.argtypes = [vp, vp, i, C.POINTER(vp), i, i, i, C.POINTER(UpscaleParams), C.POINTER(vp), i]
+    lib.vd3d_sr_upscale.restype = i
     lib.vd3d_color_grade.argtypes = [vp, fp, i, i, C.c_double, C.c_double, C.c_double, fp, i]
     lib.vd3d_color_grade.restype = i
     lib.vd3d_sharpen.argtypes = [vp, u8p, i, i, C.c_double, u8p, i]

@@ -17,6 +17,7 @@ UNITS = [
     ("dibr_fast.cu", ["-fmad=false"]),
     ("vd3d_api.cu", ["-fmad=false"]),
     ("letterbox.cu", ["-fmad=false"]),
+    ("sr_kernels.cu", ["-fmad=false"]),
     ("depth_kernels.cu", []),
     ("depth_engine.cu", []),
 ]

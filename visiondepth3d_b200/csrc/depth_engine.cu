@@ -18,6 +18,7 @@
 
 #include "../../include/vd3d.h"
 #include "depth_launch.h"
+#include "sr_engine.h"
 #include "umma_gemm.cuh"
 
 using namespace vd3d;
@@ -973,24 +974,27 @@ int vd3d_sr_create(void* stream, vd3d_depth** out) {
   return VD3D_OK;
 }
 
-// frame BGR u8 [h,w,3] -> BGR u8 [4h,4w,3] (preprocess_esr -> network -> postprocess_esr).  Weights: "sr.c{i}.w" f16
-// [Cout, 9*64] (tap-major, input channels padded to 64), "sr.c{i}.b" f32 [Cout], "sr.a{i}" f32 [64] (PReLU slopes),
-// i = 0 .. num_conv+1.
-int vd3d_sr_forward(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, int num_conv, uint8_t* out_bgr, int mem) {
-  if (!e || !frame_bgr || !out_bgr || h < 8 || w < 8 || num_conv < 1 || num_conv > 64) return VD3D_ERR_ARG;
+}  // extern "C"
+
+namespace vd3d {
+
+cudaStream_t sr_stream(vd3d_depth* e) { return e->stream; }
+
+int sr_buffer(vd3d_depth* e, const char* name, size_t bytes, void** out) { return get_buf(e, name, bytes, out); }
+
+// Weights: "sr.c{i}.w" f16 [Cout, 9*64] (tap-major, input channels padded to 64), "sr.c{i}.b" f32 [Cout], "sr.a{i}" f32
+// [64] (PReLU slopes), i = 0 .. num_conv+1.
+int sr_network(vd3d_depth* e, const uint8_t* fd, int h, int w, int num_conv, const float** conv_out) {
+  if (!e || !fd || !conv_out || h < 8 || w < 8 || num_conv < 1 || num_conv > 64) return VD3D_ERR_ARG;
   cudaStream_t s = e->stream;
   const size_t npix = (size_t)h * w;
-  void *fd = (void*)frame_bgr, *od = out_bgr, *x0, *x1, *cvo;
+  void *x0, *x1, *cvo;
   int r;
   char nm[32];
-  if (mem == VD3D_MEM_HOST) {
-    if ((r = get_buf(e, "sr.in", npix * 3, &fd)) || (r = get_buf(e, "sr.outu8", npix * 48, &od))) return r;
-    DCK(cudaMemcpyAsync(fd, frame_bgr, npix * 3, cudaMemcpyHostToDevice, s));
-  }
   if ((r = get_buf(e, "sr.x0", npix * 64 * 2, &x0)) || (r = get_buf(e, "sr.x1", npix * 64 * 2, &x1)) ||
       (r = get_buf(e, "sr.cv", npix * 48 * 4, &cvo)))
     return r;
-  launch_sr_in((const uint8_t*)fd, (__half*)x0, (int)npix, s);
+  launch_sr_in(fd, (__half*)x0, (int)npix, s);
   e->launches++;
   __half *cur = (__half*)x0, *nxt = (__half*)x1;
   for (int i = 0; i <= num_conv + 1; ++i) {
@@ -1024,7 +1028,28 @@ int vd3d_sr_forward(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, int n
       nxt = t;
     }
   }
-  launch_sr_out((const float*)cvo, 48, (const uint8_t*)fd, (uint8_t*)od, h, w, s);
+  *conv_out = (const float*)cvo;
+  return VD3D_OK;
+}
+
+}  // namespace vd3d
+
+extern "C" {
+
+// frame BGR u8 [h,w,3] -> BGR u8 [4h,4w,3] (preprocess_esr -> network -> postprocess_esr)
+int vd3d_sr_forward(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, int num_conv, uint8_t* out_bgr, int mem) {
+  if (!e || !frame_bgr || !out_bgr || h < 8 || w < 8 || num_conv < 1 || num_conv > 64) return VD3D_ERR_ARG;
+  cudaStream_t s = e->stream;
+  const size_t npix = (size_t)h * w;
+  void *fd = (void*)frame_bgr, *od = out_bgr;
+  const float* cvo;
+  int r;
+  if (mem == VD3D_MEM_HOST) {
+    if ((r = get_buf(e, "sr.in", npix * 3, &fd)) || (r = get_buf(e, "sr.outu8", npix * 48, &od))) return r;
+    DCK(cudaMemcpyAsync(fd, frame_bgr, npix * 3, cudaMemcpyHostToDevice, s));
+  }
+  if ((r = sr_network(e, (const uint8_t*)fd, h, w, num_conv, &cvo))) return r;
+  launch_sr_out(cvo, 48, (const uint8_t*)fd, (uint8_t*)od, h, w, s);
   e->launches++;
   DCK(cudaGetLastError());
   if (mem == VD3D_MEM_HOST) {

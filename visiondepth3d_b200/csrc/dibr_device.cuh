@@ -73,6 +73,30 @@ __device__ __forceinline__ uint8_t rhe_u8(float v) {  // cvRound + saturate_cast
   return (uint8_t)(i < 0 ? 0 : (i > 255 ? 255 : i));
 }
 
+// cv2 INTER_CUBIC taps of destination index d (ssize -> dsize): source indices clamped to the border and the float32
+// coefficients (A = -0.75), as k_resize_cubic_u8 (dibr_kernels.cu) and k_sr_tail_cubic (sr_kernels.cu) apply them
+struct CubicTap {
+  int o[4];
+  float c[4];
+};
+__device__ __forceinline__ CubicTap cubic_tap(int d, int ssize, int dsize) {
+  CubicTap t;
+  const double scale = (double)ssize / (double)dsize;
+  float fx = (float)(((double)d + 0.5) * scale - 0.5);
+  float fl = floorf(fx);
+  int sx = (int)fl;
+  float x = fx - fl;
+  const float A = -0.75f;
+  float x1 = x + 1.0f, xm = 1.0f - x;
+  t.c[0] = ((((A * x1) - (5.0f * A)) * x1) + (8.0f * A)) * x1 - (4.0f * A);
+  t.c[1] = ((((A + 2.0f) * x) - (A + 3.0f)) * x) * x + 1.0f;
+  t.c[2] = ((((A + 2.0f) * xm) - (A + 3.0f)) * xm) * xm + 1.0f;
+  t.c[3] = ((1.0f - t.c[0]) - t.c[1]) - t.c[2];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) t.o[k] = min(max(sx - 1 + k, 0), ssize - 1);
+  return t;
+}
+
 __device__ __forceinline__ int reflect101(int i, int n) {
   if (i < 0) i = -i;
   if (i >= n) i = 2 * n - 2 - i;

@@ -1044,28 +1044,7 @@ __global__ void __launch_bounds__(256) k_heal(const float* __restrict__ warped, 
 }
 
 // cv2.resize(u8 plane, INTER_CUBIC) (core/render_depth.py:1917): float32 bicubic, A = -0.75, rows then columns,
-// round half to even -- the arithmetic of oracle.resize_cubic_u8 (pinned to the installed cv2 / IPP)
-struct CubicTap {
-  int o[4];
-  float c[4];
-};
-__device__ __forceinline__ CubicTap cubic_tap(int d, int ssize, int dsize) {
-  CubicTap t;
-  const double scale = (double)ssize / (double)dsize;
-  float fx = (float)(((double)d + 0.5) * scale - 0.5);
-  float fl = floorf(fx);
-  int sx = (int)fl;
-  float x = fx - fl;
-  const float A = -0.75f;
-  float x1 = x + 1.0f, xm = 1.0f - x;
-  t.c[0] = ((((A * x1) - (5.0f * A)) * x1) + (8.0f * A)) * x1 - (4.0f * A);
-  t.c[1] = ((((A + 2.0f) * x) - (A + 3.0f)) * x) * x + 1.0f;
-  t.c[2] = ((((A + 2.0f) * xm) - (A + 3.0f)) * xm) * xm + 1.0f;
-  t.c[3] = ((1.0f - t.c[0]) - t.c[1]) - t.c[2];
-#pragma unroll
-  for (int k = 0; k < 4; ++k) t.o[k] = min(max(sx - 1 + k, 0), ssize - 1);
-  return t;
-}
+// round half to even -- the arithmetic of oracle.resize_cubic_u8 (pinned to the installed cv2 / IPP); taps: cubic_tap
 __global__ void __launch_bounds__(256) k_resize_cubic_u8(const uint8_t* __restrict__ src, int h, int w, int ch,
                                                          uint8_t* __restrict__ dst, int oh, int ow) {
   int x = blockIdx.x * 32 + (threadIdx.x & 31);

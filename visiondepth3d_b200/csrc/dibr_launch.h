@@ -177,6 +177,10 @@ void launch_grade_f32(const float* src, float* dst, int n, float sat, float con,
 void launch_resize_cubic_u8(const uint8_t* src, int h, int w, int ch, uint8_t* dst, int oh, int ow, cudaStream_t s);
 void launch_add_weighted(const uint8_t* a, float alpha, const uint8_t* b, float beta, uint8_t* dst, size_t n,
                          cudaStream_t s);
+// sr_kernels.cu: the x4 output of the SR network (last conv f32 NHWC [h*w, 48] + network input BGR u8 [h,w,3]) resampled
+// with INTER_CUBIC straight to [oh, ow, 3] without materialising the 4h x 4w image
+void launch_sr_tail_cubic(const float* conv, const uint8_t* bgr, int h, int w, uint8_t* dst, int oh, int ow,
+                          cudaStream_t s);
 void launch_heal(const float* warped, const float* orig, const float* edge, float* out, int H, int W, float hs,
                  cudaStream_t s);
 

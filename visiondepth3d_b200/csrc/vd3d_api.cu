@@ -12,6 +12,7 @@
 
 #include "dibr_launch.h"
 #include "letterbox_launch.h"
+#include "sr_engine.h"
 
 using namespace vd3d;
 
@@ -27,6 +28,7 @@ struct Buf {
 constexpr int kSlots = 16;   // staging slots: two depth batches of up to kMaxDepthBatch frames in flight
 constexpr int kClones = 2;   // depth engine instances (own activation buffers / stream), alternating per batch
 constexpr int kMaxDepthBatch = 8;
+constexpr int kSrSlots = 3;  // vd3d_sr_upscale: upload of frame i+1 | compute of frame i | download of frame i-1
 constexpr int kJobs = 5;  // pct, subj(norm), quantile(d0), subj(d0), subj(shaped)
 constexpr size_t kJobWords = 4096 + 4 * 4096 + 4 * 64 + 64 + 64;  // + count (padded)
 constexpr size_t kBarWords = 64;
@@ -78,6 +80,8 @@ struct vd3d_ctx {
   Buf tdf, dn0, dn1, rgb_s, frameB, d, shift, e2, eyeL, eyeR, eyeL2, eyeR2;
   Buf in_frame[kSlots], in_depth[kSlots], out_dev[kSlots], in_rgbf, in_depthf;
   Buf dof_kern;
+  // host-memory staging of vd3d_sr_upscale (frame in, result out), apart from the frame path's slots
+  Buf sr_in[kSrSlots], sr_out[kSrSlots];
   // cv2 ResizeArea_ tables of the current non-integer eye fit (device) + the sizes they were built for
   // ([0]: the frame path, whose CUDA graphs bake the pointers in; [1]: the stage entry points vd3d_fit_eye ...)
   Buf area_tab[2];
@@ -869,6 +873,7 @@ int vd3d_struct_size(int which) {
     case 1: return (int)sizeof(vd3d_render_params);
     case 2: return (int)sizeof(vd3d_size_plan);
     case 3: return (int)sizeof(vd3d_frame_info);
+    case 4: return (int)sizeof(vd3d_upscale_params);
     default: return -1;
   }
 }
@@ -961,6 +966,10 @@ void vd3d_destroy(vd3d_ctx* ctx) {
     if (ctx->in_frame[i].p) cudaFree(ctx->in_frame[i].p);
     if (ctx->in_depth[i].p) cudaFree(ctx->in_depth[i].p);
     if (ctx->out_dev[i].p) cudaFree(ctx->out_dev[i].p);
+  }
+  for (int i = 0; i < kSrSlots; ++i) {
+    if (ctx->sr_in[i].p) cudaFree(ctx->sr_in[i].p);
+    if (ctx->sr_out[i].p) cudaFree(ctx->sr_out[i].p);
   }
   drop_graphs(ctx);
   drop_depth_graphs(ctx);
@@ -2002,6 +2011,106 @@ int vd3d_add_weighted(vd3d_ctx* ctx, const uint8_t* a, double alpha, const uint8
   launch_add_weighted((const uint8_t*)a_d, (float)alpha, (const uint8_t*)b_d, (float)beta, (uint8_t*)o_d, n, s);
   ctx->launches += 1;
   return stage_finish(ctx, dst, o_d, n, mem);
+}
+
+// run_esrgan (core/merged_pipeline.py:240-267) without tiling on n frames.  Per frame, on ctx->stream: the input resize
+// (247-249), the network, k_sr_tail_cubic from the last conv straight to the size of the first non-identity INTER_CUBIC
+// resize of 263-264, the remaining INTER_CUBIC resizes (264-266) and addWeighted (233-238).  The chain never needs the
+// 4h x 4w image: the reference's 4x resize is the identity for scale 4, and its next resize reads each of those pixels
+// through 16 taps that k_sr_tail_cubic computes from the conv output.
+int vd3d_sr_upscale(vd3d_ctx* ctx, vd3d_depth* sr, int n, const uint8_t* const* frames, int h, int w, int num_conv,
+                    const vd3d_upscale_params* p, uint8_t* const* outs, int mem) {
+  if (!ctx || !sr || !frames || !p || !outs || n < 0 || h < 1 || w < 1) return fail(ctx, VD3D_ERR_ARG, "bad argument");
+  if (sr_stream(sr) != ctx->stream) return fail(ctx, VD3D_ERR_ARG, "the SR engine must be created on vd3d_stream(ctx)");
+  if (p->scale != 4 && p->scale != 2) return fail(ctx, VD3D_ERR_ARG, "scale must be 4 or 2");
+  if (p->target_w < 0 || p->target_h < 0 || (p->target_w == 0) != (p->target_h == 0))
+    return fail(ctx, VD3D_ERR_ARG, "target size: both positive, or both 0 for none");
+  const double pct = p->input_res_pct;
+  int rw = w, rh = h;  // network input: int(w * input_res_pct / 100) in double, as the reference computes it
+  if (pct != 100.0) {
+    rw = (int)((double)w * pct / 100.0);
+    rh = (int)((double)h * pct / 100.0);
+  }
+  if (rw < 8 || rh < 8) return fail(ctx, VD3D_ERR_ARG, "network input below 8 x 8 pixels");
+  const int t1w = p->scale == 4 ? w : 2 * rw, t1h = p->scale == 4 ? h : 2 * rh;  // k_sr_tail_cubic output
+  const bool to_orig = t1w != w || t1h != h;                                     // scale 2: then to the original size
+  const int fw = p->target_w ? p->target_w : w, fh = p->target_h ? p->target_h : h;
+  const bool to_target = fw != w || fh != h;
+  const bool blend = p->blend_alpha >= 0.0;
+  if (blend && to_target) return fail(ctx, VD3D_ERR_ARG, "blend of two different sizes (cv2.addWeighted raises)");
+  const int nst = 1 + (int)to_orig + (int)to_target + (int)blend;  // kernels after the network
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  int r;
+  FitPlan fp;
+  if (pct < 100.0 && (r = plan_fit(ctx, VD3D_FMT_HALF_SBS, w, h, rw, rh, fp, 1))) return r;
+  const size_t fb = (size_t)h * w * 3, ob = (size_t)fh * fw * 3;
+  const size_t tb = (size_t)(t1w * t1h > w * h ? t1w * t1h : w * h) * 3;
+  void *rs = nullptr, *tmp[2] = {nullptr, nullptr};
+  if (pct != 100.0 && (r = sr_buffer(sr, "up.in", (size_t)rw * rh * 3, &rs))) return r;
+  if (nst > 1 && (r = sr_buffer(sr, "up.0", tb, &tmp[0]))) return r;
+  if (nst > 2 && (r = sr_buffer(sr, "up.1", tb, &tmp[1]))) return r;
+  if (mem == VD3D_MEM_HOST)
+    for (int b = 0; b < kSrSlots; ++b)
+      if ((r = ensure(ctx, ctx->sr_in[b], fb)) || (r = ensure(ctx, ctx->sr_out[b], ob))) return r;
+  for (int i = 0; i < n; ++i) {
+    const int b = i % kSrSlots;
+    const uint8_t* f_d = frames[i];
+    uint8_t* o_d = outs[i];
+    if (mem == VD3D_MEM_HOST) {  // three streams: H2D(i+1) | kernels(i) | D2H(i-1)
+      if (i >= kSrSlots) CK(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_done[b], 0));
+      CK(cudaMemcpyAsync(ctx->sr_in[b].p, frames[i], fb, cudaMemcpyHostToDevice, ctx->s_h2d));
+      CK(cudaEventRecord(ctx->ev_h2d[b], ctx->s_h2d));
+      CK(cudaStreamWaitEvent(s, ctx->ev_h2d[b], 0));
+      if (i >= kSrSlots) CK(cudaStreamWaitEvent(s, ctx->ev_d2h[b], 0));
+      f_d = (const uint8_t*)ctx->sr_in[b].p;
+      o_d = (uint8_t*)ctx->sr_out[b].p;
+    }
+    const uint8_t* x = f_d;
+    if (pct < 100.0) {
+      PostArgs pa = single_eye_post(f_d, h, w, (uint8_t*)rs, rw, rh);
+      set_fit(pa, fp);
+      launch_post(pa, s);
+      ctx->launches += 1;
+      x = (const uint8_t*)rs;
+    } else if (pct > 100.0) {
+      launch_resize_cubic_u8(f_d, h, w, 3, (uint8_t*)rs, rh, rw, s);
+      ctx->launches += 1;
+      x = (const uint8_t*)rs;
+    }
+    const float* cv;
+    if ((r = sr_network(sr, x, rh, rw, num_conv, &cv))) {
+      ctx->err = std::string("SR engine: ") + vd3d_depth_last_error(sr);
+      return r;
+    }
+    int k = 0;
+    auto next = [&]() { return ++k == nst ? o_d : (uint8_t*)tmp[(k - 1) & 1]; };
+    uint8_t* cur = next();
+    launch_sr_tail_cubic(cv, x, rh, rw, cur, t1h, t1w, s);
+    if (to_orig) {
+      uint8_t* d = next();
+      launch_resize_cubic_u8(cur, t1h, t1w, 3, d, h, w, s);
+      cur = d;
+    }
+    if (to_target) {
+      uint8_t* d = next();
+      launch_resize_cubic_u8(cur, h, w, 3, d, fh, fw, s);
+      cur = d;
+    }
+    if (blend)
+      launch_add_weighted(cur, (float)p->blend_alpha, f_d, (float)(1.0 - p->blend_alpha), next(), fb, s);
+    ctx->launches += nst;
+    if (mem == VD3D_MEM_HOST) {
+      CK(cudaEventRecord(ctx->ev_done[b], s));
+      CK(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_done[b], 0));
+      CK(cudaMemcpyAsync(outs[i], o_d, ob, cudaMemcpyDeviceToHost, ctx->s_d2h));
+      CK(cudaEventRecord(ctx->ev_d2h[b], ctx->s_d2h));
+    }
+  }
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(s));
+  CK(cudaStreamSynchronize(ctx->s_d2h));
+  return VD3D_OK;
 }
 
 // apply_color_grade (core/render_3d.py:734-767) on f32 RGB planes [3,h,w] in 0..1

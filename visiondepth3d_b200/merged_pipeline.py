@@ -1,19 +1,33 @@
-"""Drop-in for the Real-ESRGAN upscale stage of the reference's core/merged_pipeline.py (run_esrgan and its helpers,
-lines 221-284), backed by libvd3d.so: the SRVGGNetCompact network on wgmma implicit-GEMM convolutions, cv2's INTER_AREA
-/ INTER_CUBIC resizes and addWeighted as CUDA kernels.  RIFE interpolation, the image-folder driver and the ffmpeg
-writer of that module are outside the hot path.
+"""Drop-in for the reference's core/merged_pipeline.py, backed by libvd3d.so: the SRVGGNetCompact network on wgmma
+implicit-GEMM convolutions, and run_esrgan's whole untiled chain (input resize, network, INTER_CUBIC resizes,
+addWeighted) as one device call, vd3d_sr_upscale.  start_merged_pipeline drives an image folder through it into ffmpeg.
 
-The reference loads `weights/RealESR_Gx4_fp16.onnx` through ONNXRuntime (VisionDepth3D.py:1094-1100); here the model is
-an upstream-format state_dict (`body.{i}.weight` ...: realesr-general-x4v3 / realesr-animevideov3 .pth files) handed to
-load_esrgan(); without one a random-init model is built (no checkpoints offline).
+    from visiondepth3d_b200 import merged_pipeline as core_merged_pipeline
+    core_merged_pipeline.start_merged_pipeline(settings, progress_bar, status_label)
+
+The reference loads `weights/RealESR_Gx4_fp16.onnx` through ONNXRuntime (VisionDepth3D.py:1094-1100).  ONNX files are
+not read here: the model is an upstream-format state_dict (`body.{i}.weight` ...: realesr-general-x4v3 /
+realesr-animevideov3), either handed to load_esrgan() or found as `<stem>.pth` / `<stem>.safetensors` next to the
+settings' model_path.  RIFE frame interpolation is not built: its network is not part of the reference (it loads a
+`RIFE_fp32.onnx` it does not ship), so rife_session stays None and run_rife returns [] -- what the reference does
+without that file.
 """
 import ctypes as C
+import os
+import re
+import threading
+import time
 
 import numpy as np
 
 from . import _lib
 
 esrgan_session = None  # the reference's module global: truthy once a model is loaded
+rife_session = None    # RIFE is not built (see the module docstring)
+suspend_flag = threading.Event()
+cancel_flag = threading.Event()
+progress_bar = None
+status_label = None
 
 
 class SrEngine:
@@ -61,6 +75,22 @@ class SrEngine:
         out = np.empty((4 * h, 4 * w, 3), dtype=np.uint8)
         self.check(self.lib.vd3d_sr_forward(self.h, f.ctypes.data, h, w, self.num_conv, out.ctypes.data, _lib.MEM_HOST))
         return out
+
+    def upscale_ptrs(self, frames, h, w, params, outs, mem):
+        """vd3d_sr_upscale on len(frames) frames BGR u8 [h,w,3] given as addresses in `mem` (host / device) memory."""
+        n = len(frames)
+        fp = (C.c_void_p * n)(*frames)
+        op = (C.c_void_p * n)(*outs)
+        self.ctx.check(self.lib.vd3d_sr_upscale(self.ctx.h, self.h, n, fp, int(h), int(w), self.num_conv,
+                                                C.byref(params), op, mem))
+
+    def upscale_chain(self, frames, params, out_size):
+        """run_esrgan's untiled chain on a list of same-size host frames; returns new arrays of out_size (w, h)."""
+        fr = [np.ascontiguousarray(f, dtype=np.uint8) for f in frames]
+        h, w = fr[0].shape[:2]
+        outs = [np.empty((out_size[1], out_size[0], 3), dtype=np.uint8) for _ in fr]
+        self.upscale_ptrs([f.ctypes.data for f in fr], h, w, params, [o.ctypes.data for o in outs], _lib.MEM_HOST)
+        return outs
 
     def close(self):
         if getattr(self, "h", None):
@@ -155,12 +185,38 @@ def _esrgan_tiled(img, tile, pad):
     return out
 
 
+_BLEND_ALPHA = {"LOW": 0.85, "MEDIUM": 0.5, "HIGH": 0.25}
+
+
+def upscale_params(blend_mode="OFF", input_res_pct=100, model_name="RealESR_Gx4_fp16", target_size=None):
+    """vd3d_upscale_params of a run_esrgan call: blend_images' alpha (exactly "OFF": none; an unknown mode: 1.0),
+    the x2 model-name quirk, target_size (w, h) or None."""
+    tw, th = (int(target_size[0]), int(target_size[1])) if target_size else (0, 0)
+    alpha = -1.0 if blend_mode == "OFF" else _BLEND_ALPHA.get(blend_mode.upper(), 1.0)
+    return _lib.UpscaleParams(float(input_res_pct), 2 if "x2" in model_name.lower() else 4, tw, th, float(alpha))
+
+
 def run_esrgan(frame, blend_mode="OFF", input_res_pct=100, model_name="RealESR_Gx4_fp16", target_size=None, tile=None,
                tile_pad=8):
-    """core/merged_pipeline.py:240-267.  Returns the input frame when no model is loaded or the engine fails, like the
-    reference."""
+    """core/merged_pipeline.py:240-267.  Untiled: one vd3d_sr_upscale call (one upload, one download).  Returns the
+    input frame when no model is loaded or the engine fails, like the reference."""
     if not esrgan_session:
         return frame
+    if not tile:
+        h, w = frame.shape[:2]
+        p = upscale_params(blend_mode, input_res_pct, model_name, target_size)
+        size = (p.target_w, p.target_h) if target_size else (w, h)
+        if blend_mode != "OFF":
+            assert size == (w, h)  # blend_images: cv2.addWeighted raises on two different sizes
+        # the caller's sizes raise here, as the reference's cv2.resize calls do; only the engine takes the fallback
+        nw, nh = int(w * input_res_pct / 100), int(h * input_res_pct / 100)
+        if nw < 1 or nh < 1 or size[0] < 1 or size[1] < 1:
+            raise ValueError(f"run_esrgan: empty size (input {nw}x{nh}, output {size[0]}x{size[1]})")
+        try:
+            return esrgan_session.upscale_chain([frame], p, size)[0]
+        except _lib.Vd3dError as e:
+            print(f"❌ ESRGAN failed: {e}")
+            return frame
     from . import render_3d as R
     original = frame
     if input_res_pct != 100:
@@ -178,3 +234,405 @@ def run_esrgan(frame, blend_mode="OFF", input_res_pct=100, model_name="RealESR_G
     if target_size:
         upscaled = _resize_cubic(upscaled, target_size[0], target_size[1])
     return blend_images(original, upscaled, mode=blend_mode)
+
+
+# ---------------------------------------------------------------------------
+# RIFE (core/merged_pipeline.py:196-219): the helpers as the reference defines them; without a RIFE network
+# rife_session is None and run_rife interpolates nothing
+# ---------------------------------------------------------------------------
+def concatenate_images(frame1, frame2):
+    """Both frames as float32 / 255, stacked on the channel axis."""
+    return np.concatenate([frame1.astype(np.float32) / 255.0, frame2.astype(np.float32) / 255.0], axis=2)
+
+
+def preprocess_rife(frame):
+    """HWC -> NCHW float32 with a batch axis of one."""
+    return np.expand_dims(np.transpose(frame, (2, 0, 1)), 0).astype(np.float32)
+
+
+def run_rife(frame1, frame2, multiplier):
+    """multiplier - 1 frames between frame1 and frame2 from rife_session, or [] without one (or when it fails)."""
+    if not rife_session:
+        return []
+    batch = np.repeat(preprocess_rife(concatenate_images(frame1, frame2)), multiplier - 1, axis=0)
+    try:
+        out = rife_session.run(None, {rife_session.get_inputs()[0].name: batch})[0]
+    except Exception as e:
+        print(f"❌ RIFE inference error: {e}")
+        return []
+    return [(f * 255).astype(np.uint8) for f in np.transpose(np.clip(out, 0, 1), (0, 2, 3, 1))]
+
+
+# ---------------------------------------------------------------------------
+# folder helpers and progress (core/merged_pipeline.py:64-80, 189-194)
+# ---------------------------------------------------------------------------
+def extract_frame_number(filename):
+    """The first run of digits in the basename as an int; inf when there is none (such names sort last)."""
+    m = re.search(r"\d+", os.path.basename(filename))
+    return float("inf") if m is None else int(m.group(0))
+
+
+def natural_sort(files):
+    """Stable sort on extract_frame_number."""
+    return sorted(files, key=extract_frame_number)
+
+
+def update_progress(done, total, start):
+    """Progress bar value and "Progress: done/total | FPS | ETA" on the status label, marshalled with .after(0, ...);
+    nothing without both widgets."""
+    if not progress_bar or not status_label:
+        return
+    el = time.time() - start
+    rate = done / el if el > 0 else 0
+    eta = (total - done) / rate if rate > 0 else float("inf")
+    eta_s = "--:--" if eta == float("inf") else time.strftime("%H:%M:%S", time.gmtime(eta))
+    pct = done / total * 100 if total else 0
+    try:
+        progress_bar.after(0, lambda: progress_bar.configure(value=pct))
+        status_label.after(0, lambda: status_label.configure(
+            text=f"Progress: {done}/{total} | FPS: {rate:.2f} | ETA: {eta_s}"))
+    except Exception:
+        pass
+
+
+def _gui_only(name):
+    def f(*_a, **_k):
+        raise RuntimeError(f"{name} is a Tk GUI helper of the reference (core/merged_pipeline.py); pass paths to "
+                           "start_merged_pipeline's settings instead")
+    f.__name__ = name
+    return f
+
+
+# Tk dialogs the reference's main window imports (VisionDepth3D.py:55-61); the import list must resolve
+select_video_and_generate_frames = _gui_only("select_video_and_generate_frames")
+select_output_file = _gui_only("select_output_file")
+select_frames_folder = _gui_only("select_frames_folder")
+
+
+def _encoder_args(codec):
+    if "nvenc" in (codec or "").lower():
+        return ["-c:v", "h264_nvenc", "-preset", "p4", "-tune", "hq", "-rc", "vbr", "-cq", "19", "-rc-lookahead", "20",
+                "-bf:v", "3", "-b_ref_mode", "middle", "-pix_fmt", "yuv420p"]
+    return ["-c:v", "libx264", "-preset", "medium", "-crf", "18", "-pix_fmt", "yuv420p"]
+
+
+def start_ffmpeg_writer(output_path, width, height, fps, codec):
+    """core/merged_pipeline.py:390-426: an ffmpeg process reading raw bgr24 frames of width x height on stdin."""
+    import subprocess
+    cmd = ["ffmpeg", "-y", "-f", "rawvideo", "-vcodec", "rawvideo", "-pix_fmt", "bgr24", "-s", f"{width}x{height}",
+           "-r", str(fps), "-i", "-"] + _encoder_args(codec) + [output_path]
+    return subprocess.Popen(cmd, stdin=subprocess.PIPE)
+
+
+# ---------------------------------------------------------------------------
+# model loading
+# ---------------------------------------------------------------------------
+def _read_state_dict(path):
+    if path.lower().endswith(".safetensors"):
+        from safetensors.numpy import load_file
+        sd = load_file(path)
+    else:
+        import torch
+        sd = torch.load(path, map_location="cpu", weights_only=True)
+    for key in ("params_ema", "params"):  # upstream Real-ESRGAN checkpoints wrap the state dict
+        if isinstance(sd, dict) and key in sd and isinstance(sd[key], dict):
+            sd = sd[key]
+            break
+    sd = {k: (v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)) for k, v in sd.items()}
+    n = len([k for k in sd if k.startswith("body.") and k.endswith(".bias")])
+    ok = n >= 3
+    for i in range(n if ok else 0):
+        w = sd.get(f"body.{2 * i}.weight")
+        ci, co = (3 if i == 0 else 64), (48 if i == n - 1 else 64)
+        ok = ok and w is not None and tuple(w.shape) == (co, ci, 3, 3) and (i == n - 1 or f"body.{2 * i + 1}.weight" in sd)
+    if not ok:
+        raise ValueError(f"{path}: not an SRVGGNetCompact x4 state dict (num_feat 64)")
+    return sd
+
+
+def _model_files(model_path):
+    stem, ext = os.path.splitext(model_path)
+    if ext.lower() in (".pth", ".safetensors"):
+        return [model_path]
+    return [stem + ".pth", stem + ".safetensors"]
+
+
+def load_esrgan_from(model_path):
+    """The settings' model_path: the path itself when it is a .pth / .safetensors file, else <stem>.pth or
+    <stem>.safetensors next to it (the ONNX file is not read).  None, with the reference's message, when there is
+    none; a state dict that is not SRVGGNetCompact raises."""
+    global esrgan_session
+    for f in _model_files(model_path):
+        if os.path.exists(f):
+            return load_esrgan(_read_state_dict(f))
+    print(f"❌ ESRGAN model missing: {model_path}")
+    esrgan_session = None
+    return None
+
+
+# ---------------------------------------------------------------------------
+# the image-folder driver (core/merged_pipeline.py:85-104, 287-386)
+# ---------------------------------------------------------------------------
+_SR_BATCH = 4  # frames per vd3d_sr_upscale call
+
+
+class _MergedPlan:
+    def __init__(self, settings):
+        self.frames_dir = settings["frames_folder"]
+        self.output_path = settings["output_file"]
+        self.codec = settings["codec"]
+        self.width, self.height = int(settings["width"]), int(settings["height"])
+        self.fps = settings["fps"]
+        self.fps_mult = settings["fps_multiplier"]
+        self.enable_rife = settings["enable_rife"]
+        self.enable_upscale = settings["enable_upscale"]
+        self.blend_mode = settings.get("blend_mode", "OFF")
+        self.input_res_pct = settings.get("input_res_pct", 100)
+        self.model_path = settings.get("model_path", "weights/RealESR_Gx4_fp16.onnx")
+        self.output_fps = self.fps * self.fps_mult if self.enable_rife else self.fps
+        self.files = []
+
+    def prepare(self):
+        """Model (before any file is listed or written) and the frame list; False when there are no frames."""
+        if self.enable_upscale:
+            load_esrgan_from(self.model_path)
+        self.files = natural_sort([os.path.join(self.frames_dir, f) for f in os.listdir(self.frames_dir)
+                                   if f.lower().endswith((".jpg", ".jpeg", ".png"))])
+        if not self.files:
+            print("❌ No frames found in selected folder.")
+            return False
+        return True
+
+
+def _prefetch(files, ring, free, out_q, stop):
+    """Reader thread: decode each file (unreadable ones are skipped), copy it into a free slot of the pinned ring when
+    it has the ring's shape, and queue (slot, None) or (None, array); None ends the stream."""
+    import cv2
+    try:
+        for fp in files:
+            if stop.is_set():
+                break
+            img = cv2.imread(fp, cv2.IMREAD_COLOR)
+            if img is None:
+                continue
+            if ring is not None and img.shape == ring.arrays[0].shape:
+                k = free.get()
+                if k is None:
+                    break
+                np.copyto(ring.arrays[k], img)
+                out_q.put((k, None))
+            else:
+                out_q.put((None, img))
+    finally:
+        out_q.put(None)
+
+
+def _close_rings(pinned):
+    while pinned:
+        pinned.pop().close()
+
+
+def _merged_batches(plan, stop, pinned):
+    """Frames for the writer, in order, as (list of frames, release) pairs: release() returns pinned output slots.
+    The pinned rings are appended to `pinned` instead of being freed here: the frames handed out are views into them,
+    and whoever consumes those views (a writer thread may still be writing them after this generator has finished)
+    frees the rings with _close_rings once it is done with every frame.
+    Upscaling on with a model: batches of up to _SR_BATCH same-size frames through vd3d_sr_upscale (target size
+    (width, height), scale 4, the settings' blend and input_res_pct).  Upscaling on without a model: the source
+    frames.  Upscaling off: the loader's resize to (width, height) on the GPU (INTER_AREA when the source is wider than
+    the target, else INTER_CUBIC).  cancel_flag is read once per source frame after the first."""
+    import cv2
+    import queue
+    from . import render_3d as R
+    sr = esrgan_session if plan.enable_upscale else None
+    target = (plan.width, plan.height)
+    probe, i0 = None, 0
+    for i0, fp in enumerate(plan.files):  # the ring is shaped by the first readable frame, which goes in first
+        probe = cv2.imread(fp, cv2.IMREAD_COLOR)
+        if probe is not None:
+            break
+    if probe is None:
+        print("❌ No readable frames.")
+        return
+    lib = _lib.load()
+    ring = outs = None
+    if sr:
+        ring = R._PinnedRing(lib, 3 * _SR_BATCH, probe.shape)
+        pinned.append(ring)
+        outs = R._PinnedRing(lib, 2 * _SR_BATCH, (plan.height, plan.width, 3))
+        pinned.append(outs)
+    params = upscale_params(plan.blend_mode, plan.input_res_pct, target_size=target) if sr else None
+    free, free_out, q = queue.Queue(), queue.Queue(), queue.Queue(maxsize=3 * _SR_BATCH)
+    for k in range(3 * _SR_BATCH if sr else 0):
+        free.put(k)
+    free_out.put(0)
+    free_out.put(1)
+    if sr:
+        k = free.get()
+        np.copyto(ring.arrays[k], probe)
+        q.put((k, None))
+    else:
+        q.put((None, probe))
+    th = threading.Thread(target=_prefetch, args=(plan.files[i0 + 1:], ring, free, q, stop), daemon=True)
+    th.start()
+    try:
+        n_src, pending, done = 0, None, False
+        while not done:
+            batch = [pending] if pending is not None else []
+            pending = None
+            while len(batch) < (_SR_BATCH if sr else 1):
+                if batch and q.empty():
+                    break  # hand over what is there rather than wait for a full batch
+                item = q.get()
+                if item is None:
+                    done = True
+                    break
+                if n_src > 0 and cancel_flag.is_set():
+                    done = True
+                    break
+                n_src += 1
+                if batch and (item[0] is None or batch[0][0] is None):  # arrays travel alone
+                    pending = item
+                    break
+                batch.append(item)
+            if not batch:
+                break
+            if not sr:
+                frames = [img for _, img in batch]
+                if not plan.enable_upscale:
+                    frames = [R.resize_area(f, *target) if f.shape[1] > target[0] else _resize_cubic(f, *target)
+                              for f in frames]
+                yield frames, (lambda: None)
+                continue
+            if batch[0][0] is None:  # a frame of another size than the first one: host memory, alone
+                yield sr.upscale_chain([batch[0][1]], params, target), (lambda: None)
+                continue
+            half = free_out.get()
+            ks = [k for k, _ in batch]
+            optrs = [outs.ptrs[half * _SR_BATCH + j] for j in range(len(ks))]
+            sr.upscale_ptrs([ring.ptrs[k] for k in ks], probe.shape[0], probe.shape[1], params, optrs, _lib.MEM_HOST)
+            for k in ks:
+                free.put(k)
+            yield ([outs.arrays[half * _SR_BATCH + j] for j in range(len(ks))],
+                   (lambda h=half: free_out.put(h)))
+    finally:
+        stop.set()
+        free.put(None)
+        while th.is_alive():  # unblock a reader waiting on a full queue
+            try:
+                q.get(timeout=0.05)
+            except queue.Empty:
+                pass
+        th.join()
+
+
+def _merged_stream(plan, stop, pinned):
+    """(frame, release, is_source_frame) in writer order, with the reference's sequencing: the first frame, then for every further
+    source frame run_rife(prev, curr)'s frames (when enable_rife) followed by the frame itself."""
+    prev = None
+    for frames, release in _merged_batches(plan, stop, pinned):
+        for j, f in enumerate(frames):
+            last = j == len(frames) - 1
+            if prev is not None and plan.enable_rife:
+                for g in run_rife(prev, f, plan.fps_mult):
+                    yield g, None, False
+            prev = f
+            yield f, (release if last else None), True
+
+
+def iter_merged_frames(settings):
+    """Every frame start_merged_pipeline hands its writer, in order (copies), without a codec: for tests and for
+    callers that encode themselves."""
+    plan = _MergedPlan(settings)
+    if not plan.prepare():
+        return
+    stop, pinned = threading.Event(), []
+    gen = _merged_stream(plan, stop, pinned)
+    try:
+        for f, release, _ in gen:
+            out = np.array(f, copy=True)
+            if release:
+                release()
+            yield out
+    finally:
+        gen.close()
+        _close_rings(pinned)
+
+
+class _PipeWriter:
+    def __init__(self, proc):
+        self.proc = proc
+
+    def write(self, frame):
+        self.proc.stdin.write(memoryview(np.ascontiguousarray(frame)).cast("B"))
+
+    def close(self):
+        try:
+            self.proc.stdin.close()
+        except Exception:
+            pass
+        self.proc.wait()
+
+
+def start_merged_pipeline(settings, progress_widget, status_label_widget):
+    """core/merged_pipeline.py:287-386: an image folder -> (RIFE) -> Real-ESRGAN -> video.
+
+    A reader thread decodes the frames into a pinned ring, the calling thread hands batches to vd3d_sr_upscale (or the
+    GPU resize when upscaling is off), and a writer thread pipes bgr24 into start_ffmpeg_writer's process -- or, where
+    the ffmpeg binary is missing, a cv2.VideoWriter (mp4v).  The writer is opened at (width, height) and output fps
+    fps * fps_multiplier whenever enable_rife, as in the reference."""
+    global progress_bar, status_label
+    import queue
+    import shutil
+    from . import render_3d as R
+    progress_bar, status_label = progress_widget, status_label_widget
+    plan = _MergedPlan(settings)
+    print("⚠️ RIFE interpolation is not built: no frames are interpolated")
+    if not plan.prepare():
+        return
+    if shutil.which("ffmpeg") is not None:
+        sink = _PipeWriter(start_ffmpeg_writer(plan.output_path, plan.width, plan.height, plan.output_fps, plan.codec))
+    else:
+        print("⚠️ ffmpeg binary not found: writing through cv2.VideoWriter instead")
+        sink = R._FrameSink(plan.output_path, (plan.width, plan.height), plan.output_fps, "mp4v", False, None, 0)
+    to_write, errors = queue.Queue(maxsize=4 * _SR_BATCH), []
+
+    def writer():
+        while True:
+            item = to_write.get()
+            if item is None:
+                return
+            f, release = item
+            try:
+                if not errors:
+                    sink.write(f)
+            except Exception as e:
+                print(f"❌ write error: {e}")
+                errors.append(e)
+            if release:
+                release()
+
+    th = threading.Thread(target=writer, daemon=True)
+    th.start()
+    stop, pinned = threading.Event(), []
+    start = time.time()
+    total = len(plan.files) if not plan.enable_rife else len(plan.files) - 1
+    n = 0
+    gen = _merged_stream(plan, stop, pinned)
+    try:
+        for f, release, src in gen:
+            to_write.put((f, release))
+            n += src
+            if src and n > 1:  # progress per source frame after the first
+                update_progress(n, total, start)
+    finally:
+        gen.close()
+        to_write.put(None)
+        th.join()          # every queued frame is written (or dropped after a write error) ...
+        _close_rings(pinned)  # ... before the pinned buffers they point into are freed
+        sink.close()
+    update_progress(total, total, start)
+    try:
+        status_label.after(0, lambda: status_label.configure(text="✅ Processing Complete!"))
+    except Exception:
+        pass

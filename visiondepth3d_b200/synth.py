@@ -10,6 +10,8 @@ natural set: band-limited random colour / depth fields with fine texture, transl
 coherent like footage).  Sub-pixel warps of such content land on generic values, not on the k/255 truncation
 boundaries the ramps of the smooth set sit on, so it is the set the 1-LSB gate against the reference is meant for.
 """
+import os
+
 import numpy as np
 
 
@@ -158,3 +160,25 @@ def synth_frame(i: int, w: int, h: int, kind: str = "smooth"):
     d[disc] = 230
     depth = np.repeat(d[..., None], 3, axis=2)
     return np.ascontiguousarray(rgb), np.ascontiguousarray(depth)
+
+
+# the frames folder of the merged_pipeline fixtures (tools/gen_golden.py merged): numbered PNGs (frame_9 before
+# frame_10 only under the number sort), an upper-case .JPG, a name without digits (sorts last), one corrupt PNG (skipped
+# by the loader), and files the extension filter drops
+MERGED_FOLDER = (("frame_10.png", 0), ("frame_9.png", 1), ("frame_2.JPG", 2), ("shot_b.png", 3), ("frame_11.png", 4),
+                 ("frame_1.png", 5))
+MERGED_DECOYS = {"notes.txt": b"not a frame", "frame_5.png": b"\x89PNG corrupt", "frame_3.bmp": None}
+
+
+def merged_frames_folder(path, w=128, h=72):
+    """Write the fixture folder into `path` (created) and return it."""
+    import cv2
+    os.makedirs(path, exist_ok=True)
+    for name, seed in MERGED_FOLDER:
+        ext = os.path.splitext(name)[1].lower()
+        with open(os.path.join(path, name), "wb") as f:
+            f.write(cv2.imencode(ext, synth_frame(seed, w, h, "natural")[0])[1].tobytes())
+    for name, data in MERGED_DECOYS.items():
+        with open(os.path.join(path, name), "wb") as f:
+            f.write(data if data is not None else cv2.imencode(".bmp", synth_frame(7, w, h, "natural")[0])[1].tobytes())
+    return path
