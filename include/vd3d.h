@@ -125,7 +125,8 @@ typedef struct {
 } vd3d_frame_info;
 
 /* sizeof() of the ABI structs, so bindings can verify their layout:
- * 0 vd3d_shift_params, 1 vd3d_render_params, 2 vd3d_size_plan, 3 vd3d_frame_info, 4 vd3d_upscale_params */
+ * 0 vd3d_shift_params, 1 vd3d_render_params, 2 vd3d_size_plan, 3 vd3d_frame_info, 4 vd3d_upscale_params,
+ * 5 vd3d_tile */
 int vd3d_struct_size(int which);
 
 /* ---- lifecycle ------------------------------------------------------- */
@@ -224,6 +225,40 @@ int vd3d_canny_u8(vd3d_ctx* ctx, const uint8_t* gray, int h, int w, double low, 
  * (w, h - top - bottom) at rows [top, h - bottom) and the bar rows filled with int(np.median(core)).  No bars, or
  * h - top - bottom <= 0 (the reference then drops the bars), copies the depth.  src and dst must not alias. */
 int vd3d_letterbox_repad(vd3d_ctx* ctx, const uint8_t* src, int h, int w, int top, int bottom, uint8_t* dst, int mem);
+
+/* ---- tiled depth inference (core/render_depth.py:46-51, 62-194) ----------------------------------------------------
+ * The plan of an [h,w] image for (tile, pad) is infer_depth_tile's loop: core = max(1, tile - 2*pad), tiles start every
+ * core rows / columns, row-major; each is a core rect of up to `tile` pixels, padded by `pad` and clipped to the image,
+ * and the padded crop is INTER_CUBIC-resized to the next multiples of 14 (copied when it is one already).  Every entry
+ * point checks that `tiles` is exactly that plan. */
+typedef struct {
+  int32_t y0, y1, x0, x1;     /* core rect [y0, y1) x [x0, x1) */
+  int32_t yp0, yp1, xp0, xp1; /* padded crop */
+  int32_t rh, rw;             /* crop size rounded up to multiples of 14: the engine's input and prediction size */
+  int32_t cls;                /* index of the engine serving this tile (vd3d_depth_tiled); tiles of a class share rh, rw */
+} vd3d_tile;
+/* the crops the engine sees, of one u8 BGR frame [h,w,3], concatenated in plan order: out [sum(rh*rw*3)] */
+int vd3d_tile_crops(vd3d_ctx* ctx, const uint8_t* frame, int h, int w, int tile, int pad, const vd3d_tile* tiles,
+                    int n_tiles, uint8_t* out, int mem);
+/* infer_depth_tile's blend: preds[t] f32 [rh,rw] (the prediction of tile t), weights[t] f32 [y1-y0, x1-x0] (its Hann
+ * weights) -> out f32 [h,w] = sum(center * w) / max(sum(w), 1e-8f) with center = pred[y0-yp0 :, x0-xp0 :], accumulated
+ * in plan order with float32 rounding.  minmax (optional, host) receives np.nanmin / np.nanmax of out. */
+int vd3d_tile_blend(vd3d_ctx* ctx, int h, int w, int tile, int pad, const vd3d_tile* tiles, int n_tiles,
+                    const float* const* preds, const float* const* weights, float* out, float* minmax, int mem);
+/* _normalize_to_u8(d, (ow, oh), invert, (p_lo, p_hi)) on d f32 [h,w]: nan_to_num, np.percentile (linear, float32) at
+ * p_lo and p_hi by exact selection, clip to [lo, hi] (min-max when hi - lo < 1e-6, flat 128 when that is flat too),
+ * x255 truncated to u8, 255 - u8 when inverted, INTER_CUBIC to [oh,ow] -> out.  stats_out (optional, host): lo, hi,
+ * min, max. */
+int vd3d_normalize_u8(vd3d_ctx* ctx, const float* d, int h, int w, double p_lo, double p_hi, int invert, uint8_t* out,
+                      int oh, int ow, float* stats_out, int mem);
+/* The tiled depth-video step on n u8 BGR frames [h,w,3]: every tile crop of every frame in one launch, forwards of up
+ * to 8 tiles per class through vd3d_depth_infer_batch_device on engines[cls] (created on vd3d_stream(ctx)), the blend
+ * and _normalize_to_u8(p1, p99) of each frame to out_u8[i] [oh,ow].  weights[t]: device memory (uploaded once per
+ * plan).  out_f32[i] (optional) receives the blended depth [h,w], minmax (optional, host) [n,2] its extremes.  Host
+ * memory: one upload and one download per frame; device memory: nothing crosses PCIe.  Synchronises. */
+int vd3d_depth_tiled(vd3d_ctx* ctx, vd3d_depth* const* engines, int n_classes, int n, const uint8_t* const* frames,
+                     int h, int w, int tile, int pad, const vd3d_tile* tiles, int n_tiles, const float* const* weights,
+                     int invert, int oh, int ow, uint8_t* const* out_u8, float* const* out_f32, float* minmax, int mem);
 
 /* ---- exact frame sharding (SURVEY 8(e)) --------------------------------------------------
  * The loop is stateful (7 EMAs / trackers + the temporal depth plane).  A rank that renders frames

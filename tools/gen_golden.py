@@ -615,6 +615,177 @@ def gen_merged():
         print(p, os.path.getsize(p), frames.shape, rec["args"], rec["files"])
     mp.natural_sort = real_sort
 
+TILED_CASES = [  # name, frame (w, h), inference_size, tile, pad, invert, prediction
+    ("256x144_t96p16", (256, 144), None, 96, 16, False, "ramp"),
+    ("odd_203x117_t96p16_inv", (203, 117), None, 96, 16, True, "ramp"),
+    ("small_80x60_t96p16", (80, 60), None, 96, 16, False, "ramp"),
+    ("bigpad_100x64_t64p24", (100, 64), None, 64, 24, False, "ramp"),
+    ("shrink_256x144_to_200x112", (256, 144), (200, 112), 96, 16, False, "ramp"),
+    ("grow_160x90_to_208x117", (160, 90), (208, 117), 96, 16, True, "ramp"),
+    ("flat_128x96_t64p16", (128, 96), None, 64, 16, False, "flat"),
+    ("outliers_200x120_t96p16", (200, 120), None, 96, 16, False, "outliers"),
+]
+
+
+def tiled_prediction(crop_rgb, kind):
+    """The stand-in depth of a tile crop (RGB u8 [h, w, 3]): integer-valued float32 arithmetic, exact in any order.
+    ramp: R + 2G + B + x + 2y (tile seams stay visible); flat: 7; outliers: 5 everywhere but 3 (the first of every
+    fifth row's first two columns), so p1 == p99 while the range is not flat."""
+    h, w = crop_rgb.shape[:2]
+    if kind == "flat":
+        return np.full((h, w), 7.0, np.float32)
+    if kind == "outliers":
+        d = np.full((h, w), 5.0, np.float32)
+        d[::5, :2] = 3.0
+        return d
+    c = crop_rgb.astype(np.float32)
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float32)
+    return c[..., 0] + 2.0 * c[..., 1] + c[..., 2] + xx + 2.0 * yy
+
+
+def gen_tiled():
+    """T. tiled depth: the unmodified infer_depth_tile, _run_pipe_or_tile and _normalize_to_u8 with the module's
+    USE_TILED_DEPTH / TILE_* set as attributes, `python tools/gen_golden.py tiled`.  `pipe` is a recording stand-in
+    whose prediction is tiled_prediction of the crop; the fixtures hold the crops it was handed, the blended float32
+    depth, its percentiles, the written u8 frame and the printed lines."""
+    import contextlib
+    import io
+    import cv2
+    import torch
+    for n in ("diffusers.configuration_utils", "core.unet", "core.depthcrafter_adapter"):
+        refshim._stub(n)
+    rd = refshim.load_reference(("render_depth",))["render_depth"]
+    from PIL import Image
+    meta = dict(torch=torch.__version__, cv2=cv2.__version__, numpy=np.__version__)
+    for name, (w, h), inf, tile, pad, invert, kind in TILED_CASES:
+        rng = np.random.default_rng(len(name) * 7919 + w * 31 + h)
+        rgb = np.clip(rng.normal(128, 60, (h, w, 3)), 0, 255).astype(np.uint8)
+        crops, sizes = [], []
+
+        def stub_pipe(images, inference_size=None):
+            out = []
+            for img in images:
+                a = np.asarray(img.convert("RGB"))
+                assert inference_size == (a.shape[1], a.shape[0])
+                crops.append(a.copy())
+                sizes.append(inference_size)
+                out.append({"predicted_depth": torch.from_numpy(tiled_prediction(a, kind))})
+            return out
+
+        rd.pipe, rd.pipe_type = stub_pipe, "hf"
+        rd.USE_TILED_DEPTH, rd.TILE_SIZE, rd.TILE_PAD, rd.TILE_DEBUG = True, tile, pad, True
+        # the tile defaults are bound at import: pass them as _run_pipe_or_tile does, through the attributes above
+        rd.infer_depth_tile.__defaults__ = (tile, pad)
+        buf = io.StringIO()
+        with contextlib.redirect_stdout(buf):
+            res = rd._run_pipe_or_tile([Image.fromarray(rgb)], inf)
+        depth = res[0]["predicted_depth"]
+        assert depth.dtype == np.float32
+        u8 = rd._normalize_to_u8(depth, (w, h), invert=invert)
+        dn = np.nan_to_num(depth, nan=0.0, posinf=0.0, neginf=0.0)
+        pct = np.array([np.percentile(dn, 1.0), np.percentile(dn, 99.0)], np.float32)
+        p = os.path.join(OUT, f"tiled_{name}.npz")
+        np.savez_compressed(p, rgb=rgb, size=np.array([w, h], np.int32),
+                            inference_size=np.array(inf if inf else (0, 0), np.int32), tile=np.int32(tile),
+                            pad=np.int32(pad), invert=np.bool_(invert), kind=kind,
+                            crop_sizes=np.array(sizes, np.int32), crops=np.concatenate([c.ravel() for c in crops]),
+                            depth=depth, pct=pct, u8=u8, log=buf.getvalue(), **meta)
+        print(p, os.path.getsize(p), len(crops), "tiles")
+    gen_tiled_video(rd, torch, cv2, meta)
+
+
+def gen_tiled_video(rd, torch, cv2, meta):
+    """The tiled branch of the unmodified process_video2 (USE_TILED_DEPTH, tile 96, pad 16) on the first 13 frames of
+    the letterbox_track clip at 2 fps, in batches of 4, with and without ignore_letterbox_bars: an in-memory capture
+    and a recording writer as in gen_letterbox, the stand-in pipe's "ramp" prediction.  Records every per-frame
+    (top, bottom), every written frame and the printed [tile] lines."""
+    import contextlib
+    import io
+    import json
+    import tempfile
+    import types
+    n_frames = 13
+    frames = [synth_frame(i, 320, 180, "letterbox_track")[0] for i in range(n_frames)]
+
+    def stub_pipe(images, inference_size=None):
+        return [{"predicted_depth": torch.from_numpy(tiled_prediction(np.asarray(img.convert("RGB")), "ramp"))}
+                for img in images]
+
+    for ignore in (True, False):
+        class Cap:
+            def __init__(self, *a):
+                self.pos = 0
+
+            def isOpened(self):
+                return True
+
+            def get(self, prop):
+                return float({cv2.CAP_PROP_FRAME_COUNT: n_frames, cv2.CAP_PROP_FPS: 2.0, cv2.CAP_PROP_FRAME_WIDTH: 320,
+                              cv2.CAP_PROP_FRAME_HEIGHT: 180, cv2.CAP_PROP_POS_FRAMES: self.pos}.get(prop, 0.0))
+
+            def set(self, prop, v):
+                if prop == cv2.CAP_PROP_POS_FRAMES:
+                    self.pos = int(v)
+                return True
+
+            def read(self):
+                if self.pos >= n_frames:
+                    return False, None
+                self.pos += 1
+                return True, frames[self.pos - 1].copy()
+
+            def release(self):
+                pass
+
+        written, bars = [], []
+
+        class Writer:
+            def __init__(self, *a, **k):
+                pass
+
+            def isOpened(self):
+                return True
+
+            def write(self, f):
+                written.append(f[..., 0].copy())
+
+            def release(self):
+                pass
+
+        real_upd = rd.LetterboxTracker.update
+
+        def upd(self, frame, idx):
+            r = real_upd(self, frame, idx)
+            bars.append(r)
+            return r
+
+        real_cap, real_wr = cv2.VideoCapture, cv2.VideoWriter
+        rd.LetterboxTracker.update = upd
+        cv2.VideoCapture, cv2.VideoWriter = Cap, Writer
+        rd.pipe, rd.pipe_type = stub_pipe, "hf"
+        rd.USE_TILED_DEPTH, rd.TILE_SIZE, rd.TILE_PAD, rd.TILE_DEBUG = True, 96, 16, False
+        rd.infer_depth_tile.__defaults__ = (96, 16)
+        status = types.SimpleNamespace(config=lambda **k: None, update_idletasks=lambda: None)
+        buf = io.StringIO()
+        try:
+            with tempfile.TemporaryDirectory() as td, contextlib.redirect_stdout(buf):
+                rd.process_video2(os.path.join(td, "clip.mkv"), n_frames, 0, 4, Var(td), Var("Original"), status,
+                                  {}, threading.Event(), Var(False), ignore_letterbox_bars=ignore)
+                side = json.load(open(os.path.join(td, "clip_depth.letterbox.json")))
+        finally:
+            cv2.VideoCapture, cv2.VideoWriter = real_cap, real_wr
+            rd.LetterboxTracker.update = real_upd
+        assert len(written) == n_frames, len(written)
+        if not ignore:
+            bars = [(0, 0)] * n_frames
+        ranges = [ln for ln in buf.getvalue().splitlines() if ln.startswith("[tile] range")]
+        p = os.path.join(OUT, "tiled_video_%s_320x180.npz" % ("bars" if ignore else "nobars"))
+        np.savez_compressed(p, batch_size=np.int32(4), tile=np.int32(96), pad=np.int32(16),
+                            ignore_letterbox_bars=np.bool_(ignore), bars=np.array(bars, np.int32),
+                            sidecar=json.dumps(side, sort_keys=True), written=np.stack(written),
+                            ranges="\n".join(ranges), **meta)
+        print(p, os.path.getsize(p), side, sorted(set(map(tuple, bars))))
+
 
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "signatures":
@@ -633,5 +804,7 @@ if __name__ == "__main__":
         gen_letterbox()
     elif len(sys.argv) > 1 and sys.argv[1] == "merged":
         gen_merged()
+    elif len(sys.argv) > 1 and sys.argv[1] == "tiled":
+        gen_tiled()
     else:
         main()

@@ -87,6 +87,11 @@ class UpscaleParams(C.Structure):
     ]
 
 
+class Tile(C.Structure):
+    """vd3d_tile: one tile of infer_depth_tile's plan (core rect, padded crop, crop size rounded to 14, engine class)."""
+    _fields_ = [(n, C.c_int32) for n in ("y0", "y1", "x0", "x1", "yp0", "yp1", "xp0", "xp1", "rh", "rw", "cls")]
+
+
 # every symbol declared in include/vd3d.h (tests/test_abi.py checks the header against this)
 SYMBOLS = [
     "vd3d_create", "vd3d_destroy", "vd3d_last_error", "vd3d_reset_state", "vd3d_host_alloc",
@@ -105,6 +110,7 @@ SYMBOLS = [
     "vd3d_advance_state", "vd3d_state_bytes", "vd3d_export_state", "vd3d_import_state",
     "vd3d_last_crops", "vd3d_detect_black_bars",
     "vd3d_letterbox_stats", "vd3d_canny_u8", "vd3d_letterbox_repad",
+    "vd3d_tile_crops", "vd3d_tile_blend", "vd3d_normalize_u8", "vd3d_depth_tiled",
 ]
 
 _lib = None
@@ -123,7 +129,7 @@ def load():
     vp, i, u8p, fp = C.c_void_p, C.c_int, C.c_void_p, C.c_void_p
     lib.vd3d_struct_size.argtypes = [i]
     lib.vd3d_struct_size.restype = i
-    for which, st in enumerate((ShiftParams, RenderParams, SizePlan, FrameInfo, UpscaleParams)):
+    for which, st in enumerate((ShiftParams, RenderParams, SizePlan, FrameInfo, UpscaleParams, Tile)):
         if lib.vd3d_struct_size(which) != C.sizeof(st):
             raise OSError(f"libvd3d ABI mismatch for {st.__name__}: "
                           f"{lib.vd3d_struct_size(which)} != {C.sizeof(st)}")
@@ -184,6 +190,16 @@ def load():
     lib.vd3d_canny_u8.restype = i
     lib.vd3d_letterbox_repad.argtypes = [vp, u8p, i, i, i, i, u8p, i]
     lib.vd3d_letterbox_repad.restype = i
+    tp = C.POINTER(Tile)
+    lib.vd3d_tile_crops.argtypes = [vp, u8p, i, i, i, i, tp, i, u8p, i]
+    lib.vd3d_tile_crops.restype = i
+    lib.vd3d_tile_blend.argtypes = [vp, i, i, i, i, tp, i, C.POINTER(vp), C.POINTER(vp), fp, fp, i]
+    lib.vd3d_tile_blend.restype = i
+    lib.vd3d_normalize_u8.argtypes = [vp, fp, i, i, C.c_double, C.c_double, i, u8p, i, i, fp, i]
+    lib.vd3d_normalize_u8.restype = i
+    lib.vd3d_depth_tiled.argtypes = [vp, C.POINTER(vp), i, i, C.POINTER(vp), i, i, i, i, tp, i, C.POINTER(vp), i, i, i,
+                                     C.POINTER(vp), C.POINTER(vp), fp, i]
+    lib.vd3d_depth_tiled.restype = i
     lib.vd3d_heal.argtypes = [vp, fp, fp, fp, i, i, C.c_double, fp, i]
     lib.vd3d_heal.restype = i
     lib.vd3d_pack.argtypes = [vp, u8p, u8p, i, i, i, u8p, i]

@@ -18,6 +18,7 @@ UNITS = [
     ("vd3d_api.cu", ["-fmad=false"]),
     ("letterbox.cu", ["-fmad=false"]),
     ("sr_kernels.cu", ["-fmad=false"]),
+    ("tiled_depth.cu", ["-fmad=false"]),
     ("depth_kernels.cu", []),
     ("depth_engine.cu", []),
 ]

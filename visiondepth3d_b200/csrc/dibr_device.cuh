@@ -97,6 +97,27 @@ __device__ __forceinline__ CubicTap cubic_tap(int d, int ssize, int dsize) {
   return t;
 }
 
+// output pixel (x, y) of cv2.resize(u8 [h, w, ch] -> [oh, ow, ch], INTER_CUBIC): float32 bicubic, rows then columns,
+// round half to even.  src rows are `pitch` bytes apart, so a crop of a larger image is resized in place.
+__device__ __forceinline__ void resize_cubic_u8_px(const uint8_t* __restrict__ src, size_t pitch, int h, int w, int ch,
+                                                   uint8_t* __restrict__ dst, int oh, int ow, int x, int y) {
+  CubicTap tx = cubic_tap(x, w, ow), ty = cubic_tap(y, h, oh);
+  for (int c = 0; c < ch; ++c) {
+    float col[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {  // rows first: the value of column tx.o[k] at output row y
+      const size_t xc = (size_t)tx.o[k] * ch + c;
+      float v = (float)src[(size_t)ty.o[0] * pitch + xc] * ty.c[0];
+      v = v + ((float)src[(size_t)ty.o[1] * pitch + xc] * ty.c[1]);
+      v = v + ((float)src[(size_t)ty.o[2] * pitch + xc] * ty.c[2]);
+      v = v + ((float)src[(size_t)ty.o[3] * pitch + xc] * ty.c[3]);
+      col[k] = v;
+    }
+    float r = (((col[0] * tx.c[0]) + (col[1] * tx.c[1])) + (col[2] * tx.c[2])) + (col[3] * tx.c[3]);
+    dst[((size_t)y * ow + x) * ch + c] = rhe_u8(r);
+  }
+}
+
 __device__ __forceinline__ int reflect101(int i, int n) {
   if (i < 0) i = -i;
   if (i >= n) i = 2 * n - 2 - i;

@@ -1050,21 +1050,7 @@ __global__ void __launch_bounds__(256) k_resize_cubic_u8(const uint8_t* __restri
   int x = blockIdx.x * 32 + (threadIdx.x & 31);
   int y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= ow || y >= oh) return;
-  CubicTap tx = cubic_tap(x, w, ow), ty = cubic_tap(y, h, oh);
-  for (int c = 0; c < ch; ++c) {
-    float col[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {  // rows first: the value of column tx.o[k] at output row y
-      const int xc = tx.o[k];
-      float v = (float)src[((size_t)ty.o[0] * w + xc) * ch + c] * ty.c[0];
-      v = v + ((float)src[((size_t)ty.o[1] * w + xc) * ch + c] * ty.c[1]);
-      v = v + ((float)src[((size_t)ty.o[2] * w + xc) * ch + c] * ty.c[2]);
-      v = v + ((float)src[((size_t)ty.o[3] * w + xc) * ch + c] * ty.c[3]);
-      col[k] = v;
-    }
-    float r = (((col[0] * tx.c[0]) + (col[1] * tx.c[1])) + (col[2] * tx.c[2])) + (col[3] * tx.c[3]);
-    dst[((size_t)y * ow + x) * ch + c] = rhe_u8(r);
-  }
+  resize_cubic_u8_px(src, (size_t)w * ch, h, w, ch, dst, oh, ow, x, y);
 }
 void launch_resize_cubic_u8(const uint8_t* src, int h, int w, int ch, uint8_t* dst, int oh, int ow, cudaStream_t s) {
   dim3 g((ow + 31) / 32, (oh + 7) / 8);

@@ -13,6 +13,7 @@
 #include "dibr_launch.h"
 #include "letterbox_launch.h"
 #include "sr_engine.h"
+#include "tiled_launch.h"
 
 using namespace vd3d;
 
@@ -63,6 +64,9 @@ struct vd3d_ctx {
   Buf lb_in, lb_prev, lb_gray, lb_mag, lb_label, lb_flag, lb_rec, lb_nodes, lb_node_sum, lb_out, lb_hist;
   int64_t lb_nodes_npix = -1;
   int lb_nodes_n = 0;
+  // tiled depth (tiled_depth.cu): frames, tile crops, per-tile predictions and weights, tile jobs, blended depth, u8
+  // planes before the output resize, selection scratch, extremes, outputs staged for host memory
+  Buf td_frames, td_crops, td_preds, td_wgt, td_jobs, td_depth, td_u8, td_sel, td_mm, td_stats, td_out, td_outf;
 
   DevState* st = nullptr;
   FrameScalars* fs = nullptr;
@@ -874,6 +878,7 @@ int vd3d_struct_size(int which) {
     case 2: return (int)sizeof(vd3d_size_plan);
     case 3: return (int)sizeof(vd3d_frame_info);
     case 4: return (int)sizeof(vd3d_upscale_params);
+    case 5: return (int)sizeof(vd3d_tile);
     default: return -1;
   }
 }
@@ -959,7 +964,8 @@ void vd3d_destroy(vd3d_ctx* ctx) {
                  &ctx->eyeL2, &ctx->eyeR2, &ctx->in_rgbf, &ctx->in_depthf, &ctx->dof_kern,
                  &ctx->area_tab[0], &ctx->area_tab[1], &ctx->lb_in, &ctx->lb_prev, &ctx->lb_gray, &ctx->lb_mag,
                  &ctx->lb_label, &ctx->lb_flag, &ctx->lb_rec, &ctx->lb_nodes, &ctx->lb_node_sum, &ctx->lb_out,
-                 &ctx->lb_hist};
+                 &ctx->lb_hist, &ctx->td_frames, &ctx->td_crops, &ctx->td_preds, &ctx->td_wgt, &ctx->td_jobs,
+                 &ctx->td_depth, &ctx->td_u8, &ctx->td_sel, &ctx->td_mm, &ctx->td_stats, &ctx->td_out, &ctx->td_outf};
   for (Buf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (int i = 0; i < kSlots; ++i) {
@@ -2425,6 +2431,332 @@ int vd3d_letterbox_repad(vd3d_ctx* ctx, const uint8_t* src, int h, int w, int to
     ctx->launches += 4;
   }
   return stage_finish(ctx, dst, o_d, npx, mem);
+}
+
+}  // extern "C"
+
+// ===========================================================================
+// tiled depth inference (core/render_depth.py:102-194)
+// ===========================================================================
+namespace {
+
+int r14(int v) { return (v + 13) / 14 * 14; }
+
+// the plan infer_depth_tile walks for an [h,w] image: tiles must be exactly it.  n_classes > 0 also checks that every
+// tile names a class and that the tiles of one class share their rounded size.
+int check_plan(vd3d_ctx* ctx, int h, int w, int tile, int pad, const vd3d_tile* tiles, int n_tiles, int n_classes,
+               int* step, int* nx, int* ny) {
+  if (h < 1 || w < 1 || tile < 1 || pad < 0 || !tiles) return fail(ctx, VD3D_ERR_ARG, "bad tile plan argument");
+  const int core = tile - 2 * pad > 1 ? tile - 2 * pad : 1;
+  *step = core;
+  *nx = (w + core - 1) / core;
+  *ny = (h + core - 1) / core;
+  if (n_tiles != *nx * *ny) return fail(ctx, VD3D_ERR_ARG, "tile count does not match the plan");
+  std::vector<int> cls_h(n_classes > 0 ? n_classes : 0, -1), cls_w(cls_h.size(), -1);
+  for (int i = 0; i < *ny; ++i)
+    for (int j = 0; j < *nx; ++j) {
+      const vd3d_tile& t = tiles[i * *nx + j];
+      const int y0 = i * core, x0 = j * core, y1 = std::min(y0 + tile, h), x1 = std::min(x0 + tile, w);
+      const int yp0 = std::max(0, y0 - pad), xp0 = std::max(0, x0 - pad);
+      const int yp1 = std::min(h, y1 + pad), xp1 = std::min(w, x1 + pad);
+      if (t.y0 != y0 || t.y1 != y1 || t.x0 != x0 || t.x1 != x1 || t.yp0 != yp0 || t.yp1 != yp1 || t.xp0 != xp0 ||
+          t.xp1 != xp1 || t.rh != r14(yp1 - yp0) || t.rw != r14(xp1 - xp0))
+        return fail(ctx, VD3D_ERR_ARG, "tile does not match the plan");
+      if (n_classes > 0) {
+        if (t.cls < 0 || t.cls >= n_classes) return fail(ctx, VD3D_ERR_ARG, "tile class out of range");
+        if (cls_h[t.cls] < 0) {
+          cls_h[t.cls] = t.rh;
+          cls_w[t.cls] = t.rw;
+        } else if (cls_h[t.cls] != t.rh || cls_w[t.cls] != t.rw) {
+          return fail(ctx, VD3D_ERR_ARG, "tiles of one class differ in size");
+        }
+      }
+    }
+  return VD3D_OK;
+}
+
+// jobs of n frames (frame-major, plan order); crops and predictions are packed per frame at the offsets of the plan
+void tile_jobs(const uint8_t* const* frames, int n, const vd3d_tile* tiles, int n_tiles, uint8_t* crops,
+               float* preds, const float* const* weights, std::vector<TileJob>& jobs, size_t* crop_bytes,
+               size_t* pred_count) {
+  size_t cb = 0, pc = 0;
+  for (int t = 0; t < n_tiles; ++t) {
+    cb += (size_t)tiles[t].rh * tiles[t].rw * 3;
+    pc += (size_t)tiles[t].rh * tiles[t].rw;
+  }
+  *crop_bytes = cb;
+  *pred_count = pc;
+  jobs.resize((size_t)n * n_tiles);
+  for (int f = 0; f < n; ++f) {
+    size_t co = cb * f, po = pc * f;
+    for (int t = 0; t < n_tiles; ++t) {
+      const vd3d_tile& s = tiles[t];
+      TileJob& j = jobs[(size_t)f * n_tiles + t];
+      j.frame = frames ? frames[f] : nullptr;
+      j.crop = crops ? crops + co : nullptr;
+      j.pred = preds ? preds + po : nullptr;
+      j.wgt = weights ? weights[t] : nullptr;
+      j.y0 = s.y0;
+      j.x0 = s.x0;
+      j.ch = s.y1 - s.y0;
+      j.cw = s.x1 - s.x0;
+      j.yp0 = s.yp0;
+      j.xp0 = s.xp0;
+      j.pch = s.yp1 - s.yp0;
+      j.pcw = s.xp1 - s.xp0;
+      j.rh = s.rh;
+      j.rw = s.rw;
+      co += (size_t)s.rh * s.rw * 3;
+      po += (size_t)s.rh * s.rw;
+    }
+  }
+}
+
+int upload_jobs(vd3d_ctx* ctx, const std::vector<TileJob>& jobs, const TileJob** dev) {
+  int r;
+  if ((r = ensure(ctx, ctx->td_jobs, jobs.size() * sizeof(TileJob)))) return r;
+  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `jobs` may go out of scope afterwards
+  CK(cudaMemcpyAsync(ctx->td_jobs.p, jobs.data(), jobs.size() * sizeof(TileJob), cudaMemcpyHostToDevice, ctx->stream));
+  *dev = (const TileJob*)ctx->td_jobs.p;
+  return VD3D_OK;
+}
+
+void gather(vd3d_ctx* ctx, const TileJob* jobs_dev, const vd3d_tile* tiles, int n_tiles, int njobs, int w) {
+  int mh = 0, mw = 0;
+  for (int t = 0; t < n_tiles; ++t) {
+    mh = std::max(mh, tiles[t].rh);
+    mw = std::max(mw, tiles[t].rw);
+  }
+  launch_tile_gather(jobs_dev, njobs, mh, mw, w, ctx->stream);
+  ctx->launches += 1;
+}
+
+// numpy's percentile bookkeeping for a plane of npix values (numpy 2.x, float32 data): q = float32(p) / float32(100),
+// virtual index float32(npix - 1) * q in float32, neighbours floor(v) and floor(v) + 1 (both the last element when
+// v >= npix - 1), gamma = v - floor(v) in float32
+void pct_targets(int64_t npix, double p, uint32_t* k0, uint32_t* k1, float* gamma) {
+  const float q = (float)p / 100.0f;
+  const float nm1 = (float)(npix - 1);
+  const float v = nm1 * q;
+  if (v >= nm1) {
+    *k0 = *k1 = (uint32_t)(npix - 1);
+    *gamma = (float)((double)v + 1.0);  // gamma against the index -1 numpy substitutes; b - a is 0 there
+    return;
+  }
+  const float fl = floorf(v);
+  *k0 = (uint32_t)fl;
+  *k1 = (uint32_t)std::min<int64_t>((int64_t)fl + 1, npix - 1);
+  *gamma = v - fl;
+}
+
+// _normalize_to_u8 of n planes at d_dev [n, h*w] -> outs[f] [oh, ow] (device); stats_host (optional) [n, 4]
+int normalize_planes(vd3d_ctx* ctx, const float* d_dev, int n, int h, int w, double p_lo, double p_hi, int invert,
+                     uint8_t* const* outs, int oh, int ow, float* stats_host) {
+  cudaStream_t s = ctx->stream;
+  const int64_t npix = (int64_t)h * w;
+  if (npix > 0xffffffffLL) return fail(ctx, VD3D_ERR_ARG, "plane too large");
+  NormArgs a;
+  pct_targets(npix, p_lo, &a.rank[0], &a.rank[1], &a.gamma_lo);
+  pct_targets(npix, p_hi, &a.rank[2], &a.rank[3], &a.gamma_hi);
+  a.rank[4] = 0;
+  a.rank[5] = (uint32_t)(npix - 1);
+  a.invert = invert ? 1 : 0;
+  int r;
+  if ((r = ensure(ctx, ctx->td_sel, (size_t)n * normalize_scratch_words() * 4)) ||
+      (r = ensure(ctx, ctx->td_u8, (size_t)n * npix)) || (r = ensure(ctx, ctx->td_stats, (size_t)n * 16)))
+    return r;
+  launch_normalize_u8(d_dev, n, npix, a, (uint32_t*)ctx->td_sel.p, (uint8_t*)ctx->td_u8.p,
+                      stats_host ? (float*)ctx->td_stats.p : nullptr, s);
+  ctx->launches += 10;  // four histogram + pick passes, the scalars, the u8 write
+  for (int f = 0; f < n; ++f) {
+    const uint8_t* u = (const uint8_t*)ctx->td_u8.p + (size_t)f * npix;
+    if (oh == h && ow == w)
+      CK(cudaMemcpyAsync(outs[f], u, npix, cudaMemcpyDeviceToDevice, s));  // cv2.resize copies on equal sizes
+    else
+      launch_resize_cubic_u8(u, h, w, 1, outs[f], oh, ow, s);
+    ctx->launches += 1;
+  }
+  if (stats_host) CK(cudaMemcpyAsync(stats_host, ctx->td_stats.p, (size_t)n * 16, cudaMemcpyDeviceToHost, s));
+  return VD3D_OK;
+}
+
+// blend of n frames from the jobs at jobs_dev into ctx->td_depth [n, h, w]; minmax_host (optional) [n, 2]
+int blend_frames(vd3d_ctx* ctx, const TileJob* jobs_dev, int n, int h, int w, int tile, int step, int nx, int ny,
+                 float* minmax_host) {
+  cudaStream_t s = ctx->stream;
+  int r;
+  if ((r = ensure(ctx, ctx->td_depth, (size_t)n * h * w * 4)) || (r = ensure(ctx, ctx->td_mm, (size_t)n * 16)))
+    return r;
+  uint32_t* keys = (uint32_t*)ctx->td_mm.p;
+  launch_tile_blend(jobs_dev, n, h, w, step, tile, nx, ny, (float*)ctx->td_depth.p, keys, s);
+  ctx->launches += 2;
+  if (minmax_host) {
+    float* mmf = (float*)(keys + 2 * n);
+    launch_keys_to_float(keys, 2 * n, mmf, s);
+    ctx->launches += 1;
+    CK(cudaMemcpyAsync(minmax_host, mmf, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+  }
+  return VD3D_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vd3d_tile_crops(vd3d_ctx* ctx, const uint8_t* frame, int h, int w, int tile, int pad, const vd3d_tile* tiles,
+                    int n_tiles, uint8_t* out, int mem) {
+  if (!ctx || !frame || !out) return fail(ctx, VD3D_ERR_ARG, "bad argument");
+  int step, nx, ny, r;
+  if ((r = check_plan(ctx, h, w, tile, pad, tiles, n_tiles, 0, &step, &nx, &ny))) return r;
+  CK(cudaSetDevice(ctx->device));
+  const void* f_d;
+  if ((r = copy_in(ctx, ctx->td_frames, frame, (size_t)h * w * 3, mem, ctx->stream, &f_d))) return r;
+  std::vector<TileJob> jobs;
+  size_t cb, pc;
+  tile_jobs(nullptr, 1, tiles, n_tiles, nullptr, nullptr, nullptr, jobs, &cb, &pc);
+  void* o_d;
+  if ((r = stage_out(ctx, ctx->td_out, out, cb, mem, &o_d))) return r;
+  const uint8_t* fp = (const uint8_t*)f_d;
+  tile_jobs(&fp, 1, tiles, n_tiles, (uint8_t*)o_d, nullptr, nullptr, jobs, &cb, &pc);
+  const TileJob* jd;
+  if ((r = upload_jobs(ctx, jobs, &jd))) return r;
+  gather(ctx, jd, tiles, n_tiles, n_tiles, w);
+  return stage_finish(ctx, out, o_d, cb, mem);
+}
+
+int vd3d_tile_blend(vd3d_ctx* ctx, int h, int w, int tile, int pad, const vd3d_tile* tiles, int n_tiles,
+                    const float* const* preds, const float* const* weights, float* out, float* minmax, int mem) {
+  if (!ctx || !preds || !weights || !out) return fail(ctx, VD3D_ERR_ARG, "bad argument");
+  int step, nx, ny, r;
+  if ((r = check_plan(ctx, h, w, tile, pad, tiles, n_tiles, 0, &step, &nx, &ny))) return r;
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  std::vector<TileJob> jobs;
+  size_t cb, pc;
+  tile_jobs(nullptr, 1, tiles, n_tiles, nullptr, nullptr, nullptr, jobs, &cb, &pc);
+  std::vector<const float*> wd(weights, weights + n_tiles);
+  float* pred_base = nullptr;
+  if (mem == VD3D_MEM_HOST) {  // pack the predictions and the weights into device buffers
+    size_t wc = 0;
+    for (int t = 0; t < n_tiles; ++t) wc += (size_t)(tiles[t].y1 - tiles[t].y0) * (tiles[t].x1 - tiles[t].x0);
+    if ((r = ensure(ctx, ctx->td_preds, pc * 4)) || (r = ensure(ctx, ctx->td_wgt, wc * 4))) return r;
+    pred_base = (float*)ctx->td_preds.p;
+    size_t po = 0, wo = 0;
+    for (int t = 0; t < n_tiles; ++t) {
+      const size_t np = (size_t)tiles[t].rh * tiles[t].rw;
+      const size_t nw = (size_t)(tiles[t].y1 - tiles[t].y0) * (tiles[t].x1 - tiles[t].x0);
+      CK(cudaMemcpyAsync(pred_base + po, preds[t], np * 4, cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync((float*)ctx->td_wgt.p + wo, weights[t], nw * 4, cudaMemcpyHostToDevice, s));
+      wd[t] = (const float*)ctx->td_wgt.p + wo;
+      po += np;
+      wo += nw;
+    }
+  }
+  tile_jobs(nullptr, 1, tiles, n_tiles, nullptr, pred_base, wd.data(), jobs, &cb, &pc);
+  if (mem != VD3D_MEM_HOST)
+    for (int t = 0; t < n_tiles; ++t) jobs[t].pred = preds[t];
+  const TileJob* jd;
+  if ((r = upload_jobs(ctx, jobs, &jd))) return r;
+  if ((r = blend_frames(ctx, jd, 1, h, w, tile, step, nx, ny, minmax))) return r;
+  const size_t bytes = (size_t)h * w * 4;
+  CK(cudaMemcpyAsync(out, ctx->td_depth.p, bytes,
+                     mem == VD3D_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, s));
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(s));
+  return VD3D_OK;
+}
+
+int vd3d_normalize_u8(vd3d_ctx* ctx, const float* d, int h, int w, double p_lo, double p_hi, int invert, uint8_t* out,
+                      int oh, int ow, float* stats_out, int mem) {
+  if (!ctx || !d || !out || h < 1 || w < 1 || oh < 1 || ow < 1) return fail(ctx, VD3D_ERR_ARG, "bad argument");
+  CK(cudaSetDevice(ctx->device));
+  const void* d_d;
+  void* o_d;
+  int r;
+  if ((r = copy_in(ctx, ctx->td_depth, d, (size_t)h * w * 4, mem, ctx->stream, &d_d))) return r;
+  if ((r = stage_out(ctx, ctx->td_out, out, (size_t)oh * ow, mem, &o_d))) return r;
+  uint8_t* outs[1] = {(uint8_t*)o_d};
+  if ((r = normalize_planes(ctx, (const float*)d_d, 1, h, w, p_lo, p_hi, invert, outs, oh, ow, stats_out))) return r;
+  return stage_finish(ctx, out, o_d, (size_t)oh * ow, mem);
+}
+
+int vd3d_depth_tiled(vd3d_ctx* ctx, vd3d_depth* const* engines, int n_classes, int n, const uint8_t* const* frames,
+                     int h, int w, int tile, int pad, const vd3d_tile* tiles, int n_tiles, const float* const* weights,
+                     int invert, int oh, int ow, uint8_t* const* out_u8, float* const* out_f32, float* minmax,
+                     int mem) {
+  if (!ctx || !engines || n_classes < 1 || n < 1 || !frames || !weights || !out_u8 || oh < 1 || ow < 1)
+    return fail(ctx, VD3D_ERR_ARG, "bad argument");
+  for (int c = 0; c < n_classes; ++c) {
+    if (!engines[c]) return fail(ctx, VD3D_ERR_ARG, "missing engine");
+    // the gather and the blend run on ctx->stream: an engine on another stream would race them
+    if (sr_stream(engines[c]) != ctx->stream)
+      return fail(ctx, VD3D_ERR_ARG, "the depth engines must be created on vd3d_stream(ctx)");
+  }
+  int step, nx, ny, r;
+  if ((r = check_plan(ctx, h, w, tile, pad, tiles, n_tiles, n_classes, &step, &nx, &ny))) return r;
+  for (int t = 0; t < n_tiles; ++t)
+    if (tiles[t].rh < 16 || tiles[t].rw < 16)
+      return fail(ctx, VD3D_ERR_ARG, "a tile crop is below the depth engine's 16 x 16 minimum");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  const size_t fbytes = (size_t)h * w * 3, npix = (size_t)h * w, obytes = (size_t)oh * ow;
+  std::vector<const uint8_t*> fd(frames, frames + n);
+  if (mem == VD3D_MEM_HOST) {
+    if ((r = ensure(ctx, ctx->td_frames, fbytes * n))) return r;
+    for (int f = 0; f < n; ++f) {
+      fd[f] = (const uint8_t*)ctx->td_frames.p + fbytes * f;
+      CK(cudaMemcpyAsync((void*)fd[f], frames[f], fbytes, cudaMemcpyHostToDevice, s));
+    }
+  }
+  std::vector<TileJob> jobs;
+  size_t cb, pc;
+  tile_jobs(nullptr, 1, tiles, n_tiles, nullptr, nullptr, nullptr, jobs, &cb, &pc);
+  if ((r = ensure(ctx, ctx->td_crops, cb * n)) || (r = ensure(ctx, ctx->td_preds, pc * 4 * n))) return r;
+  tile_jobs(fd.data(), n, tiles, n_tiles, (uint8_t*)ctx->td_crops.p, (float*)ctx->td_preds.p, weights, jobs, &cb, &pc);
+  const TileJob* jd;
+  if ((r = upload_jobs(ctx, jobs, &jd))) return r;
+  gather(ctx, jd, tiles, n_tiles, n * n_tiles, w);
+  // forwards: the tiles of each class, frame-major in plan order, up to 8 per batch
+  for (int c = 0; c < n_classes; ++c) {
+    const uint8_t* cin[8];
+    float* cout_[8];
+    int b = 0, rh = 0, rw = 0;
+    for (size_t k = 0; k <= jobs.size(); ++k) {
+      const bool take = k < jobs.size() && tiles[k % n_tiles].cls == c;
+      if (take) {
+        cin[b] = jobs[k].crop;
+        cout_[b] = (float*)jobs[k].pred;
+        rh = jobs[k].rh;
+        rw = jobs[k].rw;
+        ++b;
+      }
+      if (b == 8 || (k == jobs.size() && b > 0)) {
+        if ((r = vd3d_depth_infer_batch_device(engines[c], b, cin, rh, rw, nullptr, cout_, 0))) {
+          ctx->err = std::string("tile forward: ") + vd3d_depth_last_error(engines[c]);
+          return r;
+        }
+        b = 0;
+      }
+    }
+  }
+  if ((r = blend_frames(ctx, jd, n, h, w, tile, step, nx, ny, minmax))) return r;
+  std::vector<uint8_t*> od(out_u8, out_u8 + n);
+  if (mem == VD3D_MEM_HOST) {
+    if ((r = ensure(ctx, ctx->td_out, obytes * n))) return r;
+    for (int f = 0; f < n; ++f) od[f] = (uint8_t*)ctx->td_out.p + obytes * f;
+  }
+  if ((r = normalize_planes(ctx, (const float*)ctx->td_depth.p, n, h, w, 1.0, 99.0, invert, od.data(), oh, ow,
+                            nullptr)))
+    return r;
+  for (int f = 0; f < n; ++f) {
+    const cudaMemcpyKind k = mem == VD3D_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+    if (mem == VD3D_MEM_HOST) CK(cudaMemcpyAsync(out_u8[f], od[f], obytes, k, s));
+    if (out_f32 && out_f32[f])
+      CK(cudaMemcpyAsync(out_f32[f], (const float*)ctx->td_depth.p + npix * f, npix * 4, k, s));
+  }
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(s));
+  return VD3D_OK;
 }
 
 }  // extern "C"

@@ -11,6 +11,7 @@ transformers' DepthEstimationPipeline.postprocess does.
 import os
 import threading
 import time
+from ctypes import c_void_p as C_void_p
 
 import numpy as np
 
@@ -200,25 +201,259 @@ def resize_cubic_u8(plane, width, height):
 
 
 def _normalize_to_u8(depth_f, out_size, invert=False, pclip=(1.0, 99.0)):
-    """core/render_depth.py:173-194 (the ndarray / tiled-depth front end): non-finite values -> 0, clip to the
-    [p1, p99] percentiles (np.percentile, linear), fall back to min-max when they coincide and to flat 128 when the
-    frame is flat, truncate to u8, optional inversion, INTER_CUBIC resize to out_size = (W, H) on the GPU.  The
-    percentile front end is a host helper: the HF tensor path of the hot loop never takes it (1907-1917)."""
-    d = np.asarray(depth_f, dtype=np.float32)
-    if not np.isfinite(d).all():
-        d = np.nan_to_num(d, nan=0.0, posinf=0.0, neginf=0.0)
-    lo, hi = np.percentile(d, pclip[0]), np.percentile(d, pclip[1])
-    if hi - lo >= 1e-6:
-        u8 = (np.clip((d - lo) / (hi - lo), 0.0, 1.0) * 255.0).astype(np.uint8)
+    """core/render_depth.py:173-194 (the ndarray / tiled-depth front end) on the GPU (vd3d_normalize_u8): non-finite
+    values -> 0, clip to the [p1, p99] percentiles (np.percentile, linear, float32), fall back to min-max when they
+    coincide and to flat 128 when the frame is flat, truncate to u8, optional inversion, INTER_CUBIC resize to
+    out_size = (W, H)."""
+    from . import _lib
+    ctx = _lib.default_context(0)
+    d = np.ascontiguousarray(depth_f, dtype=np.float32)
+    if d.ndim != 2:
+        raise ValueError(f"depth must be a 2D plane, got shape {d.shape}")
+    ow, oh = int(out_size[0]), int(out_size[1])
+    out = np.empty((oh, ow), dtype=np.uint8)
+    ctx.check(ctx.lib.vd3d_normalize_u8(ctx.h, d.ctypes.data, d.shape[0], d.shape[1], float(pclip[0]), float(pclip[1]),
+                                        int(bool(invert)), out.ctypes.data, oh, ow, None, _lib.MEM_HOST))
+    return out
+
+
+# ---------------------------------------------------------------------------
+# tiled depth inference (core/render_depth.py:46-51, 62-268): the tile crops, the batched per-tile forwards, the Hann
+# blend and the percentile normalisation run on the GPU in one call (vd3d_depth_tiled)
+# ---------------------------------------------------------------------------
+USE_TILED_DEPTH = False   # read at call time by _run_pipe_or_tile and the depth-video pass
+TILE_SIZE = 512
+TILE_PAD = 32
+TILE_DEBUG = False        # print one line per tile
+
+assert TILE_SIZE > 2 * TILE_PAD, "TILE_SIZE must be larger than 2*TILE_PAD"
+
+
+def _hann2d(h, w):
+    """core/render_depth.py:62-66: outer product of two np.hanning windows, divided by (max + 1e-8), float32."""
+    wy = np.hanning(max(2, h))
+    wx = np.hanning(max(2, w))
+    m = np.outer(wy, wx).astype(np.float32)
+    mmax = float(m.max()) if m.size else 1.0
+    return m / (mmax + 1e-8)
+
+
+def _ensure_depth_np(pred):
+    """core/render_depth.py:68-100: a prediction (tensor / ndarray, optionally in a dict or list) -> float32 [H, W]."""
+    if isinstance(pred, list):
+        pred = pred[0]
+    if isinstance(pred, dict) and "predicted_depth" in pred:
+        pred = pred["predicted_depth"]
+    if torch is not None and isinstance(pred, torch.Tensor):
+        arr = pred.detach().cpu().float().numpy()
+    elif isinstance(pred, np.ndarray):
+        arr = pred.astype(np.float32, copy=False)
     else:
-        mn, mx = float(d.min()), float(d.max())
-        if mx - mn >= 1e-6:
-            u8 = (((d - mn) / (mx - mn + 1e-6)) * 255.0).astype(np.uint8)
+        raise TypeError(f"Unexpected depth type: {type(pred)}")
+    if arr.ndim == 3:
+        if arr.shape[0] in (1, 3):
+            arr = arr[0] if arr.shape[0] == 1 else arr.mean(axis=0)
+        elif arr.shape[2] in (1, 3):
+            arr = arr[..., 0] if arr.shape[2] == 1 else arr.mean(axis=-1)
         else:
-            u8 = np.full_like(d, 128, dtype=np.uint8)
-    if invert:
-        u8 = 255 - u8
-    return resize_cubic_u8(u8, out_size[0], out_size[1])
+            arr = np.squeeze(arr)
+    elif arr.ndim > 2:
+        arr = np.squeeze(arr)
+    if arr.ndim != 2:
+        raise ValueError(f"Depth must be 2D after squeeze; got shape {arr.shape}")
+    return arr.astype(np.float32, copy=False)
+
+
+def tile_plan(width, height, tile=TILE_SIZE, pad=TILE_PAD):
+    """infer_depth_tile's loop over a (width, height) image: [(y0, y1, x0, x1, yp0, yp1, xp0, xp1, rh, rw)] in
+    row-major order -- core rect, padded crop, and the crop size rounded up to multiples of 14."""
+    core = max(1, int(tile) - 2 * int(pad))
+    r14 = lambda v: ((int(v) + 13) // 14) * 14  # noqa: E731
+    out = []
+    for y0 in range(0, height, core):
+        for x0 in range(0, width, core):
+            y1, x1 = min(y0 + tile, height), min(x0 + tile, width)
+            yp0, xp0 = max(0, y0 - pad), max(0, x0 - pad)
+            yp1, xp1 = min(height, y1 + pad), min(width, x1 + pad)
+            out.append((y0, y1, x0, x1, yp0, yp1, xp0, xp1, r14(yp1 - yp0), r14(xp1 - xp0)))
+    return out
+
+
+def tile_weights(ch, cw, tile=TILE_SIZE, pad=TILE_PAD):
+    """The Hann weights of a tile whose core rect is ch x cw, as infer_depth_tile builds them (cv2 INTER_CUBIC from
+    the core x core window when the shapes differ)."""
+    import cv2
+    core = max(1, int(tile) - 2 * int(pad))
+    w = _hann2d(core, core)
+    if w.shape != (ch, cw):
+        w = cv2.resize(w, (cw, ch), interpolation=cv2.INTER_CUBIC)
+    return np.ascontiguousarray(w, dtype=np.float32)
+
+
+class _TilePlan:
+    """Set-up of one (width, height, tile, pad): the tiles (vd3d_tile array), one class per rounded crop size (in order
+    of first use), and the Hann weights uploaded once, one map per core-rect shape."""
+
+    def __init__(self, width, height, tile, pad):
+        from . import _lib
+        self.width, self.height, self.tile, self.pad = width, height, tile, pad
+        self.rects = tile_plan(width, height, tile, pad)
+        self.classes = []
+        for r in self.rects:
+            if (r[8], r[9]) not in self.classes:
+                self.classes.append((r[8], r[9]))
+        self.tiles = (_lib.Tile * len(self.rects))()
+        maps = {}
+        self._weights = []  # keeps the CUDA tensors alive
+        for k, r in enumerate(self.rects):
+            self.tiles[k] = _lib.Tile(*r, self.classes.index((r[8], r[9])))
+            shape = (r[1] - r[0], r[3] - r[2])
+            if shape not in maps:
+                maps[shape] = torch.from_numpy(tile_weights(*shape, tile, pad)).cuda()
+                self._weights.append(maps[shape])
+        self.weight_ptrs = (C_void_p * len(self.rects))(*[maps[(r[1] - r[0], r[3] - r[2])].data_ptr()
+                                                           for r in self.rects])
+        torch.cuda.current_stream().synchronize()
+
+    def engines(self):
+        """The engine of each class (through _engine_for, so they follow the loaded model)."""
+        return [_engine_for(rw, rh) for rh, rw in self.classes]
+
+    def debug_lines(self):
+        return [f"[tile] ({y0}:{y1},{x0}:{x1}) crop={(rh, rw)} center={(y1 - y0, x1 - x0)} acc={(y1 - y0, x1 - x0)}"
+                for y0, y1, x0, x1, _a, _b, _c, _d, rh, rw in self.rects]
+
+
+_tile_plans = {}  # (width, height, tile, pad) -> _TilePlan
+
+
+def _plan_for(width, height, tile, pad):
+    key = (int(width), int(height), int(tile), int(pad))
+    plan = _tile_plans.get(key)
+    if plan is None:
+        plan = _tile_plans[key] = _TilePlan(*key)
+    return plan
+
+
+def depth_tiled(frames, width, height, out_size, invert=False, tile=None, pad=None, want_f32=False):
+    """vd3d_depth_tiled on n same-shape u8 BGR frames [height, width, 3]: the tiled depth of each frame, normalised
+    by _normalize_to_u8 to out_size = (W, H).  frames: a list of host frames or a CUDA uint8 tensor [n, h, w, 3] (the
+    results are then CUDA tensors).  Returns (u8 planes, float32 depth planes or None, [(min, max)] per frame)."""
+    from . import _lib
+    tile = TILE_SIZE if tile is None else int(tile)
+    pad = TILE_PAD if pad is None else int(pad)
+    ctx = _lib.default_context(0)
+    plan = _plan_for(width, height, tile, pad)
+    engines = plan.engines()
+    ow, oh = int(out_size[0]), int(out_size[1])
+    device = _is_cuda_tensor(frames)
+    if device:
+        fr = frames.contiguous()
+        n = int(fr.shape[0])
+        u8 = torch.empty((n, oh, ow), dtype=torch.uint8, device=fr.device)
+        f32 = torch.empty((n, height, width), dtype=torch.float32, device=fr.device) if want_f32 else None
+        fptr = [fr[k].data_ptr() for k in range(n)]
+        uptr = [u8[k].data_ptr() for k in range(n)]
+        dptr = [f32[k].data_ptr() for k in range(n)] if want_f32 else None
+        mem = _lib.MEM_DEVICE
+        torch.cuda.current_stream().synchronize()  # the frames may come from work queued on torch's stream
+    else:
+        fr = [np.ascontiguousarray(f, dtype=np.uint8) for f in frames]
+        n = len(fr)
+        u8 = [np.empty((oh, ow), np.uint8) for _ in range(n)]
+        f32 = [np.empty((height, width), np.float32) for _ in range(n)] if want_f32 else None
+        fptr = [f.ctypes.data for f in fr]
+        uptr = [u.ctypes.data for u in u8]
+        dptr = [d.ctypes.data for d in f32] if want_f32 else None
+        mem = _lib.MEM_HOST
+    mm = np.empty((n, 2), np.float32)
+    vp = C_void_p
+    ctx.check(ctx.lib.vd3d_depth_tiled(
+        ctx.h, (vp * len(engines))(*[e.h for e in engines]), len(engines), n, (vp * n)(*fptr), height, width, tile,
+        pad, plan.tiles, len(plan.rects), plan.weight_ptrs, int(bool(invert)), oh, ow, (vp * n)(*uptr),
+        (vp * n)(*dptr) if want_f32 else None, mm.ctypes.data, mem))
+    return u8, f32, [(float(a), float(b)) for a, b in mm]
+
+
+def _print_tile_log(width, height, ranges):
+    """What _run_pipe_or_tile prints per image, image after image: the TILE_DEBUG lines of the plan, then the range."""
+    for lo, hi in ranges:
+        if TILE_DEBUG:
+            for line in _plan_for(width, height, TILE_SIZE, TILE_PAD).debug_lines():
+                print(line)
+        print(f"[tile] range min={lo:.6f} max={hi:.6f}")
+
+
+def _outer_resize(rgb, tgt_w, tgt_h):
+    """infer_depth_tile's first step on the GPU: cv2 INTER_AREA when the image shrinks (vd3d_fit_eye), INTER_CUBIC when
+    it grows (vd3d_resize_cubic), a copy at the same size; returns BGR.  One axis shrinking while the other grows is
+    refused: cv2 takes neither path there."""
+    from . import _lib
+    h, w = rgb.shape[:2]
+    bgr = np.ascontiguousarray(rgb[:, :, ::-1])
+    if (tgt_w, tgt_h) == (w, h):
+        return bgr
+    ctx = _lib.default_context(0)
+    out = np.empty((tgt_h, tgt_w, 3), np.uint8)
+    if tgt_w <= w and tgt_h <= h:
+        ctx.check(ctx.lib.vd3d_fit_eye(ctx.h, bgr.ctypes.data, h, w, tgt_w, tgt_h, 0, out.ctypes.data, _lib.MEM_HOST))
+    elif tgt_w >= w and tgt_h >= h:
+        ctx.check(ctx.lib.vd3d_resize_cubic(ctx.h, bgr.ctypes.data, h, w, 3, out.ctypes.data, tgt_h, tgt_w,
+                                            _lib.MEM_HOST))
+    else:
+        raise ValueError(f"inference_size {(tgt_w, tgt_h)} shrinks one axis of a {w}x{h} image and enlarges the other: "
+                         "cv2's INTER_AREA takes no area path there, which the GPU path does not reproduce")
+    return out
+
+
+def infer_depth_tile(model_call, rgb_np, inference_size, tile=TILE_SIZE, pad=TILE_PAD):
+    """core/render_depth.py:102-170 for this module's `pipe`: resize to inference_size, tile with `pad` of context,
+    run every tile crop through the depth engine (batched per crop size), blend the predictions with Hann weights.
+    Returns float32 [tgtH, tgtW].  Other model callables are refused: the tiles never leave the GPU."""
+    if model_call is not hf_batch_safe_pipe:
+        raise TypeError("infer_depth_tile runs this module's depth pipe on the GPU (vd3d_depth_tiled); load a model with "
+                        "load_depth_model() / update_pipeline() and pass render_depth.pipe")
+    if rgb_np.dtype != np.uint8:
+        rgb_np = rgb_np.astype(np.uint8, copy=False)
+    H, W = rgb_np.shape[:2]
+    tgt_w, tgt_h = (inference_size or (W, H))
+    bgr = _outer_resize(rgb_np, int(tgt_w), int(tgt_h))
+    _u8, f32, _mm = depth_tiled([bgr], int(tgt_w), int(tgt_h), (int(tgt_w), int(tgt_h)), tile=tile, pad=pad,
+                                want_f32=True)
+    if TILE_DEBUG:
+        for line in _plan_for(int(tgt_w), int(tgt_h), tile, pad).debug_lines():
+            print(line)
+    return f32[0]
+
+
+def _run_pipe_or_tile(images_pil, inference_size):
+    """core/render_depth.py:201-268 for the HF pipe: with USE_TILED_DEPTH each image goes through infer_depth_tile
+    (one "[tile] range" line per image), otherwise the whole list through pipe."""
+    if USE_TILED_DEPTH:
+        preds = []
+        for img in images_pil:
+            rgb = np.array(img.convert("RGB"))
+            dep = infer_depth_tile(pipe, rgb, inference_size, tile=TILE_SIZE, pad=TILE_PAD)
+            dep_min, dep_max = float(np.nanmin(dep)), float(np.nanmax(dep))
+            print(f"[tile] range min={dep_min:.6f} max={dep_max:.6f}")
+            preds.append({"predicted_depth": dep})
+        return preds
+    try:
+        res = pipe(images_pil, inference_size=inference_size)
+        if isinstance(res, list):
+            return res
+        elif isinstance(res, dict):
+            return [res]
+        else:
+            return [{"predicted_depth": res}]
+    except TypeError:
+        outs = []
+        for img in images_pil:
+            r = pipe(img, inference_size=inference_size)
+            if isinstance(r, list):
+                r = r[0]
+            outs.append(r if isinstance(r, dict) else {"predicted_depth": r})
+        return outs
 
 
 # ---------------------------------------------------------------------------
@@ -695,8 +930,27 @@ def iter_depth_frames(cap, W, H, invert=False, inference_size=None, batch_size=8
     batch is re-padded with the bars the tracker holds after the batch's last frame, as process_video2 does."""
     from PIL import Image
     n, batch = 0, []
+    tiled = USE_TILED_DEPTH
+
+    def flush_tiled():
+        # process_video2's tiled branch: _run_pipe_or_tile -> infer_depth_tile on each (PIL-resized) frame, then
+        # _normalize_to_u8 to the frame size and the re-pad, in one vd3d_depth_tiled call per batch
+        bars = tracker.update_batch(batch, n + 1)[-1] if tracker is not None else (0, 0)
+        frames = batch
+        if inference_size is not None:
+            frames = [np.ascontiguousarray(np.asarray(Image.fromarray(f[..., ::-1].copy()).resize(
+                tuple(inference_size), Image.BICUBIC))[..., ::-1]) for f in batch]
+        th, tw = frames[0].shape[:2]
+        d8s, _, ranges = depth_tiled(frames, tw, th, (W, H), invert)
+        _print_tile_log(tw, th, ranges)
+        batch.clear()
+        if bars[0] or bars[1]:
+            d8s = [letterbox_repad(d8, bars[0], bars[1]) for d8 in d8s]
+        return d8s
 
     def flush():
+        if tiled:
+            return flush_tiled()
         if tracker is not None and inference_size is None:
             d8s = _tracked_batch_device(batch, W, H, invert, tracker)
             batch.clear()
