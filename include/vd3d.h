@@ -361,6 +361,27 @@ int vd3d_depth_infer_batch(vd3d_depth* e, int B, const uint8_t* const* frames_bg
                            uint8_t* const* depth_u8, int invert);
 int vd3d_depth_infer_batch_device(vd3d_depth* e, int B, const uint8_t* const* frames_bgr_dev, int h, int w,
                                   uint8_t* const* depth_u8_dev, float* const* depth_f32_dev, int invert);
+/* ---- still images (process_image / process_images_in_folder, core/render_depth.py:1229-1477) ----------------------
+ * Image.resize((ow, oh), Image.BICUBIC) of one u8 RGB image [h,w,3] -> [oh,ow,3], bit for bit with Pillow's 8-bit
+ * resampling: width pass then height pass (a pass is skipped when its axis keeps its size), fixed-point weights with 22
+ * fractional bits from tables built on the host once per (in, out) size pair and cached by the engine, integer sums.
+ * Host memory synchronises; device memory is enqueued on the engine stream. */
+int vd3d_depth_resize_pil(vd3d_depth* e, const uint8_t* src, int h, int w, uint8_t* dst, int oh, int ow, int mem);
+/* host-only test hook (no GPU needed): the table of one axis, in_size -> out_size: bounds [2*out_size] = (first input,
+ * tap count) per output index, kk [out_size*cap] fixed-point weights.  Returns the taps per output (ksize); with bounds or
+ * kk NULL only that; VD3D_ERR_ARG when cap < ksize. */
+int vd3d_pil_bicubic_table(int in_size, int out_size, int32_t* bounds, int32_t* kk, int cap);
+/* B (1..8) u8 RGB images, each of its own size, through ONE batched forward.  sizes [B][4] = src_h, src_w, in_h, in_w:
+ * the image's size and its input size (the inference size, or the source size again).  Every input size must map to the
+ * engine's processed size (the DPT processor's keep-aspect multiple-of-14 size), else VD3D_ERR_ARG.  Per image: the
+ * Pillow resize to the input size when it differs, the DPT processor into the image's slot of the batch; then the
+ * forward on the stacked token matrix (as vd3d_depth_infer_batch); then per image bicubic back to the input size, min-max
+ * u8 (255 - u8 when invert) and cv2 INTER_CUBIC to the source size when it differs -> depth_u8[b] [src_h,src_w].
+ * depth_f32 (optional; the array or single entries may be NULL): the predicted depth at the input size [in_h,in_w].
+ * Host memory: one upload per image and one download per output, synchronises; device memory: enqueued on the engine
+ * stream. */
+int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_rgb, const int32_t* sizes,
+                            uint8_t* const* depth_u8, float* const* depth_f32, int invert, int mem);
 /* frames per depth forward inside vd3d_render_clip_depth (1..8, default 4; env VD3D_DEPTH_BATCH) */
 int vd3d_set_depth_batch(vd3d_ctx* ctx, int frames);
 int vd3d_get_depth_batch(vd3d_ctx* ctx);

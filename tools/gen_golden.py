@@ -787,6 +787,111 @@ def gen_tiled_video(rd, torch, cv2, meta):
         print(p, os.path.getsize(p), side, sorted(set(map(tuple, bars))))
 
 
+IMAGE_VARIANTS = (("original", "Original", False), ("384x384", "384x384", False), ("invert", "Original", True))
+
+
+def image_depth_weights():
+    """The random-init Depth-Anything-V2-Small of the depth tests (seed 0; the head's last 1x1 conv made non-negative
+    so that its output does not cancel, tests/test_depth_gpu.py _model)."""
+    import torch
+    from transformers import DepthAnythingForDepthEstimation
+    from visiondepth3d_b200.depth_weights import hf_config
+    torch.manual_seed(0)
+    sd = DepthAnythingForDepthEstimation(hf_config("vits")).eval().state_dict()
+    sd["head.conv3.weight"] = sd["head.conv3.weight"].abs() + 0.02
+    sd["head.conv3.bias"] = torch.zeros_like(sd["head.conv3.bias"])
+    return sd
+
+
+def gen_images():
+    """I. still images: the unmodified process_images_in_folder and process_image on the photo folder of
+    visiondepth3d_b200.synth.image_folder, for Original, "384x384" and invert (`python tools/gen_golden.py images`).
+    `pipe` is the reference's HF branch: a transformers depth-estimation pipeline over image_depth_weights() and the
+    DA-V2 image processor, behind the pipe protocol (PIL bicubic to the inference size first).  Records the written
+    file names and their u8 arrays and modes."""
+    import contextlib
+    import io
+    import tempfile
+    import zlib
+    import torch
+    from PIL import Image
+    from transformers import DepthAnythingForDepthEstimation, pipeline
+    from transformers.models.dpt.image_processing_dpt import DPTImageProcessor
+    from visiondepth3d_b200.depth_weights import hf_config
+    from visiondepth3d_b200.synth import IMAGE_FOLDER, image_folder
+    for n in ("diffusers.configuration_utils", "core.unet", "core.depthcrafter_adapter"):
+        refshim._stub(n)
+    rd = refshim.load_reference(("render_depth",))["render_depth"]
+    model = DepthAnythingForDepthEstimation(hf_config("vits")).eval()
+    model.load_state_dict(image_depth_weights())
+    proc = DPTImageProcessor(do_resize=True, size={"height": 518, "width": 518}, keep_aspect_ratio=True,
+                             ensure_multiple_of=14, resample=3, do_rescale=True, do_normalize=True,
+                             image_mean=[0.485, 0.456, 0.406], image_std=[0.229, 0.224, 0.225], do_pad=False)
+    raw = pipeline("depth-estimation", model=model, image_processor=proc, device=-1)
+
+    def hf_pipe(images, inference_size=None):  # the pipe protocol of the reference's HF branch
+        if inference_size:
+            images = [img.resize(inference_size, Image.BICUBIC) for img in images]
+        return raw(images) if isinstance(images, list) else [raw(images)]
+
+    class Widget:
+        def __init__(self):
+            self.kw = {}
+
+        def after(self, _ms, fn):
+            fn()
+
+        def config(self, **kw):
+            self.kw.update(kw)
+
+        def __getitem__(self, k):
+            return self.kw.get(k)
+
+        def start(self, *_a):
+            pass
+
+        def stop(self):
+            pass
+
+    rd.pipe, rd.pipe_type, rd.USE_TILED_DEPTH = hf_pipe, "hf", False
+    import json
+    p = os.path.join(OUT, "images_resolutions.json")  # the choices parse_inference_resolution must read as it does
+    json.dump({k: (list(v) if v else None) for k, v in rd.INFERENCE_RESOLUTIONS.items()}, open(p, "w"), indent=1)
+    meta = dict(torch=torch.__version__, numpy=np.__version__, pillow=Image.__version__)
+    with tempfile.TemporaryDirectory() as tmp:
+        src = image_folder(os.path.join(tmp, "in"))
+        inputs = {name: np.asarray(Image.open(os.path.join(src, name)).convert("RGB")) for name, *_ in IMAGE_FOLDER}
+        crc = np.array([zlib.crc32(inputs[name].tobytes()) for name, *_ in IMAGE_FOLDER], np.uint32)
+        for tag, res, invert in IMAGE_VARIANTS:
+            out = {}
+            for mode in ("folder", "single"):
+                dst = os.path.join(tmp, f"{tag}_{mode}")
+                log = io.StringIO()
+                with torch.no_grad(), contextlib.redirect_stdout(log):
+                    if mode == "folder":
+                        rd.process_images_in_folder(src, Var("4"), Var(dst), Var(res), Widget(), Widget(), Widget(),
+                                                    Var(invert))
+                    else:
+                        for name, *_ in IMAGE_FOLDER:
+                            rd.process_image(os.path.join(src, name), Var("Default"), Var(invert), Var(dst), Var(res),
+                                             Widget(), Widget(), Widget(), Widget())
+                names = sorted(os.listdir(dst))
+                out[f"{mode}_names"] = np.array(names)
+                for n in names:
+                    im = Image.open(os.path.join(dst, n))
+                    out[f"{mode}_mode_{n}"] = im.mode
+                    out[f"{mode}_{n}"] = np.asarray(im)
+            # every 4th row and column of the folder outputs (keeps the fixture small); process_image wrote the same
+            for n in out["folder_names"]:
+                full = out.pop(f"folder_{n}")
+                assert np.array_equal(out.pop(f"single_{n}"), full) and out.pop(f"single_mode_{n}") == "L"
+                out[f"shape_{n}"] = np.array(full.shape, np.int32)
+                out[f"u8_{n}"] = full[::4, ::4]
+            p = os.path.join(OUT, f"images_{tag}.npz")
+            np.savez_compressed(p, resolution=res, invert=np.bool_(invert), input_crc=crc, **out, **meta)
+            print(p, os.path.getsize(p), list(out["folder_names"]))
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "signatures":
         gen_signatures()
@@ -806,5 +911,7 @@ if __name__ == "__main__":
         gen_merged()
     elif len(sys.argv) > 1 and sys.argv[1] == "tiled":
         gen_tiled()
+    elif len(sys.argv) > 1 and sys.argv[1] == "images":
+        gen_images()
     else:
         main()

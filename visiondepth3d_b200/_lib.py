@@ -111,6 +111,7 @@ SYMBOLS = [
     "vd3d_last_crops", "vd3d_detect_black_bars",
     "vd3d_letterbox_stats", "vd3d_canny_u8", "vd3d_letterbox_repad",
     "vd3d_tile_crops", "vd3d_tile_blend", "vd3d_normalize_u8", "vd3d_depth_tiled",
+    "vd3d_depth_resize_pil", "vd3d_pil_bicubic_table", "vd3d_depth_infer_images",
 ]
 
 _lib = None

@@ -8,16 +8,19 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <string>
 #include <vector>
 
 #include "../../include/vd3d.h"
 #include "depth_launch.h"
+#include "dibr_launch.h"  // launch_resize_cubic_u8 (cv2 INTER_CUBIC) for the image path
 #include "sr_engine.h"
 #include "umma_gemm.cuh"
 
@@ -862,6 +865,106 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
   return VD3D_OK;
 }
 
+// Pillow's precompute_coeffs + normalize_coeffs_8bpc for the bicubic filter (a = -0.5, support 2 widened by the scale
+// when shrinking), in double as Pillow computes them: tab = (first input, tap count) per output index, then ksize
+// weights per output index in fixed point with 22 fractional bits, rounded away from zero.  Returns ksize.
+double pil_bicubic(double x) {
+  const double a = -0.5;
+  if (x < 0.0) x = -x;
+  if (x < 1.0) return ((a + 2.0) * x - (a + 3.0)) * x * x + 1;
+  if (x < 2.0) return (((x - 5) * x + 8) * x - 4) * a;
+  return 0.0;
+}
+int pil_bicubic_table(int in_size, int out_size, std::vector<int>& tab) {
+  const double scale = (double)in_size / out_size;
+  const double filterscale = scale < 1.0 ? 1.0 : scale;
+  const double support = 2.0 * filterscale, ss = 1.0 / filterscale;
+  const int ksize = (int)ceil(support) * 2 + 1;
+  tab.assign((size_t)out_size * (2 + ksize), 0);
+  std::vector<double> w(ksize);
+  for (int xx = 0; xx < out_size; ++xx) {
+    const double center = (xx + 0.5) * scale;
+    int xmin = (int)(center - support + 0.5);
+    if (xmin < 0) xmin = 0;
+    int xmax = (int)(center + support + 0.5);
+    if (xmax > in_size) xmax = in_size;
+    xmax -= xmin;
+    double ww = 0.0;
+    for (int x = 0; x < xmax; ++x) {
+      w[x] = pil_bicubic((x + xmin - center + 0.5) * ss);
+      ww += w[x];
+    }
+    int* k = &tab[(size_t)2 * out_size + (size_t)xx * ksize];
+    for (int x = 0; x < xmax; ++x) {
+      const double v = ww != 0.0 ? w[x] / ww : w[x];
+      k[x] = v < 0 ? (int)(-0.5 + v * (1 << 22)) : (int)(0.5 + v * (1 << 22));
+    }
+    tab[2 * xx] = xmin;
+    tab[2 * xx + 1] = xmax;
+  }
+  return ksize;
+}
+
+// the device table of one (in, out) axis, built and uploaded on first use, then cached by the engine
+int pil_table(vd3d_depth* e, int in_size, int out_size, const int** out, int* ksize) {
+  char nm[48];
+  snprintf(nm, sizeof nm, "pil.%d.%d", in_size, out_size);
+  const double scale = (double)in_size / out_size;
+  *ksize = (int)ceil(2.0 * (scale < 1.0 ? 1.0 : scale)) * 2 + 1;
+  const size_t bytes = (size_t)out_size * (2 + *ksize) * sizeof(int);
+  void* d;
+  int r;
+  if (e->buf.find(nm) == e->buf.end()) {
+    std::vector<int> tab;
+    pil_bicubic_table(in_size, out_size, tab);
+    if ((r = get_buf(e, nm, bytes, &d))) return r;
+    // pageable source: the copy returns once the table is staged, so `tab` may go out of scope
+    DCK(cudaMemcpyAsync(d, tab.data(), bytes, cudaMemcpyHostToDevice, e->stream));
+  } else if ((r = get_buf(e, nm, bytes, &d))) {
+    return r;
+  }
+  *out = (const int*)d;
+  return VD3D_OK;
+}
+
+// Pillow's resize of u8 [h,w,3] -> [oh,ow,3]: width pass into tmp (>= h*ow*3 bytes), then height pass; a pass whose
+// axis keeps its size is skipped.  src != dst.
+int pil_resize(vd3d_depth* e, const uint8_t* src, int h, int w, uint8_t* tmp, uint8_t* dst, int oh, int ow) {
+  const int *tx = nullptr, *ty = nullptr;
+  int kx = 0, ky = 0, r;
+  if (ow != w && (r = pil_table(e, w, ow, &tx, &kx))) return r;
+  if (oh != h && (r = pil_table(e, h, oh, &ty, &ky))) return r;
+  cudaStream_t s = e->stream;
+  if (ow == w && oh == h) {
+    DCK(cudaMemcpyAsync(dst, src, (size_t)h * w * 3, cudaMemcpyDeviceToDevice, s));
+    return VD3D_OK;
+  }
+  if (ow != w) {
+    launch_resize_pil_u8(src, h, w, oh == h ? dst : tmp, h, ow, tx, kx, 0, s);
+    e->launches++;
+    src = tmp;
+  }
+  if (oh != h) {
+    launch_resize_pil_u8(src, h, ow, dst, oh, ow, ty, ky, 1, s);
+    e->launches++;
+  }
+  DCK(cudaGetLastError());
+  return VD3D_OK;
+}
+
+// (h, w) the DPT image processor resizes an image to (depth_engine.py processed_size): keep the aspect ratio, scale the
+// side closer to 518, round to multiples of 14 (Python's round: half to even)
+void processed_size(int h, int w, int* ph, int* pw) {
+  double sh = 518.0 / h, sw = 518.0 / w;
+  if (fabs(1 - sw) < fabs(1 - sh))
+    sh = sw;
+  else
+    sw = sh;
+  auto rnd = [](double v) { int r = (int)nearbyint(v / 14) * 14; return r < 14 ? 14 : r; };
+  *ph = rnd(sh * h);
+  *pw = rnd(sw * w);
+}
+
 }  // namespace
 
 extern "C" {
@@ -955,6 +1058,147 @@ int vd3d_depth_infer_batch(vd3d_depth* e, int B, const uint8_t* const* frames_bg
       DCK(cudaMemcpyAsync(depth_u8[b], u8d[b], (size_t)h * w, cudaMemcpyDeviceToHost, e->stream));
   }
   DCK(cudaStreamSynchronize(e->stream));
+  return VD3D_OK;
+}
+
+// host-only: the table pil_resize builds for one axis (tests pin it to Pillow)
+int vd3d_pil_bicubic_table(int in_size, int out_size, int32_t* bounds, int32_t* kk, int cap) {
+  if (in_size < 1 || out_size < 1) return VD3D_ERR_ARG;
+  std::vector<int> tab;
+  const int ksize = pil_bicubic_table(in_size, out_size, tab);
+  if (!bounds || !kk) return ksize;
+  if (cap < ksize) return VD3D_ERR_ARG;
+  for (int o = 0; o < out_size; ++o) {
+    bounds[2 * o] = tab[2 * o];
+    bounds[2 * o + 1] = tab[2 * o + 1];
+    for (int j = 0; j < cap; ++j) kk[(size_t)o * cap + j] = j < ksize ? tab[(size_t)2 * out_size + (size_t)o * ksize + j] : 0;
+  }
+  return ksize;
+}
+
+// Image.resize((ow, oh), Image.BICUBIC) of one u8 RGB image [h,w,3] -> [oh,ow,3]
+int vd3d_depth_resize_pil(vd3d_depth* e, const uint8_t* src, int h, int w, uint8_t* dst, int oh, int ow, int mem) {
+  if (!e || !src || !dst || h < 1 || w < 1 || oh < 1 || ow < 1) return VD3D_ERR_ARG;
+  const size_t nin = (size_t)h * w * 3, nout = (size_t)oh * ow * 3;
+  void *s_d = (void*)src, *d_d = dst, *tmp;
+  int r;
+  if ((r = get_buf(e, "pil.tmp", (size_t)h * ow * 3, &tmp))) return r;
+  if (mem == VD3D_MEM_HOST) {
+    if ((r = get_buf(e, "pil.src", nin, &s_d)) || (r = get_buf(e, "pil.dst", nout, &d_d))) return r;
+    DCK(cudaMemcpyAsync(s_d, src, nin, cudaMemcpyHostToDevice, e->stream));
+  }
+  if ((r = pil_resize(e, (const uint8_t*)s_d, h, w, (uint8_t*)tmp, (uint8_t*)d_d, oh, ow))) return r;
+  if (mem == VD3D_MEM_HOST) {
+    DCK(cudaMemcpyAsync(dst, d_d, nout, cudaMemcpyDeviceToHost, e->stream));
+    DCK(cudaStreamSynchronize(e->stream));
+  }
+  return VD3D_OK;
+}
+
+// Still images of their own sizes through ONE batched forward: per image the Pillow resize to its input size, the DPT
+// processor into its slot of the batch; the forward; per image bicubic back to the input size + min-max u8, and
+// cv2 INTER_CUBIC to the source size when that differs.  sizes: [B][4] = src_h, src_w, in_h, in_w.
+int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_rgb, const int32_t* sizes,
+                            uint8_t* const* depth_u8, float* const* depth_f32, int invert, int mem) {
+  if (!e || !images_rgb || !sizes || !depth_u8 || B < 1 || B > kMaxBatch) return VD3D_ERR_ARG;
+  const int IH = e->cfg.image_h, IW = e->cfg.image_w;
+  cudaStream_t s = e->stream;
+  const bool host = mem == VD3D_MEM_HOST;
+  size_t src_max = 0, rs_max = 0, tmp_max = 0, pp_max = 0, in_max = 0;
+  for (int b = 0; b < B; ++b) {
+    const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
+    if (!images_rgb[b] || !depth_u8[b] || sh < 1 || sw < 1 || ih < 16 || iw < 16) return VD3D_ERR_ARG;
+    int ph, pw;
+    processed_size(ih, iw, &ph, &pw);
+    if (ph != IH || pw != IW) {
+      char m[160];
+      snprintf(m, sizeof m, "image %d: a %dx%d input maps to processed size %dx%d, the engine serves %dx%d", b, iw, ih,
+               pw, ph, IW, IH);
+      return dfail(e, VD3D_ERR_ARG, m);
+    }
+    src_max = std::max(src_max, (size_t)sh * sw * 3);
+    if (ih != sh || iw != sw) {
+      rs_max = std::max(rs_max, (size_t)ih * iw * 3);
+      tmp_max = std::max(tmp_max, (size_t)sh * iw * 3);
+    }
+    pp_max = std::max(pp_max, (size_t)ih * IW * 3);
+    in_max = std::max(in_max, (size_t)ih * iw);
+  }
+  // every buffer first, so that no reallocation lands between enqueued launches
+  void *src_d = nullptr, *rs = nullptr, *ptmp = nullptr, *tmp, *rgb, *mm, *up, *u8in;
+  int r;
+  char nm[32];
+  if ((host && (r = get_buf(e, "im.src", src_max, &src_d))) || (rs_max && (r = get_buf(e, "im.rs", rs_max, &rs))) ||
+      (tmp_max && (r = get_buf(e, "pil.tmp", tmp_max, &ptmp))) || (r = get_buf(e, "pp.tmp", pp_max, &tmp)) ||
+      (r = get_buf(e, "pp.rgb", (size_t)IH * IW * 3, &rgb)) || (r = get_buf(e, "post.mm", 64, &mm)) ||
+      (r = get_buf(e, "im.up", in_max * 4, &up)) || (r = get_buf(e, "im.u8in", in_max, &u8in)))
+    return r;
+  const float* pxs[kMaxBatch];
+  float* dds[kMaxBatch];
+  uint8_t* o8[kMaxBatch];
+  float* o32[kMaxBatch];
+  for (int b = 0; b < B; ++b) {
+    const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
+    void *px, *dd;
+    snprintf(nm, sizeof nm, b ? "px.%d" : "px", b);
+    if ((r = get_buf(e, nm, (size_t)3 * IH * IW * 4, &px))) return r;
+    snprintf(nm, sizeof nm, b ? "depth.%d" : "depth", b);
+    if ((r = get_buf(e, nm, (size_t)IH * IW * 4, &dd))) return r;
+    pxs[b] = (const float*)px;
+    dds[b] = (float*)dd;
+    o8[b] = depth_u8[b];
+    o32[b] = depth_f32 ? depth_f32[b] : nullptr;
+    if (host) {
+      void* p;
+      snprintf(nm, sizeof nm, "im.u8.%d", b);
+      if ((r = get_buf(e, nm, (size_t)sh * sw, &p))) return r;
+      o8[b] = (uint8_t*)p;
+      if (o32[b]) {
+        snprintf(nm, sizeof nm, "im.f32.%d", b);
+        if ((r = get_buf(e, nm, (size_t)ih * iw * 4, &p))) return r;
+        o32[b] = (float*)p;
+      }
+    }
+    // the Pillow tables of this image, so that a first use uploads before anything of this call is enqueued
+    const int* t;
+    int k;
+    if ((iw != sw && (r = pil_table(e, sw, iw, &t, &k))) || (ih != sh && (r = pil_table(e, sh, ih, &t, &k)))) return r;
+  }
+  for (int b = 0; b < B; ++b) {
+    const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
+    const uint8_t* img = images_rgb[b];
+    if (host) {
+      DCK(cudaMemcpyAsync(src_d, img, (size_t)sh * sw * 3, cudaMemcpyHostToDevice, s));
+      img = (const uint8_t*)src_d;
+    }
+    if (ih != sh || iw != sw) {
+      if ((r = pil_resize(e, img, sh, sw, (uint8_t*)ptmp, (uint8_t*)rs, ih, iw))) return r;
+      img = (const uint8_t*)rs;
+    }
+    launch_preprocess(img, ih, iw, (uint8_t*)tmp, (uint8_t*)rgb, (float*)pxs[b], IH, IW, s, 0);
+    e->launches += 3;
+  }
+  if ((r = forward_core(e, B, pxs, dds))) return r;
+  for (int b = 0; b < B; ++b) {
+    const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
+    const bool back = ih != sh || iw != sw;
+    launch_depth_post(dds[b], IH, IW, o32[b] ? o32[b] : (float*)up, ih, iw, (unsigned*)mm,
+                      back ? (uint8_t*)u8in : o8[b], invert, s);
+    e->launches += 3;
+    if (back) {
+      launch_resize_cubic_u8((const uint8_t*)u8in, ih, iw, 1, o8[b], sh, sw, s);
+      e->launches++;
+    }
+  }
+  DCK(cudaGetLastError());
+  if (host) {
+    for (int b = 0; b < B; ++b) {
+      const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
+      DCK(cudaMemcpyAsync(depth_u8[b], o8[b], (size_t)sh * sw, cudaMemcpyDeviceToHost, s));
+      if (o32[b]) DCK(cudaMemcpyAsync(depth_f32[b], o32[b], (size_t)ih * iw * 4, cudaMemcpyDeviceToHost, s));
+    }
+    DCK(cudaStreamSynchronize(s));
+  }
   return VD3D_OK;
 }
 

@@ -189,6 +189,34 @@ __global__ void __launch_bounds__(256) k_resize_aa_u8(const uint8_t* __restrict_
   }
 }
 
+// one pass of Pillow's 8-bit bicubic resize (ImagingResample{Horizontal,Vertical}_8bpc) on interleaved u8 [IH, IW, 3]
+// -> [OH, OW, 3] along x (axis_y = 0) or y.  tab: the host-built table of the axis (vd3d_pil_bicubic_table): (first
+// input, tap count) per output index, then ksize fixed-point weights per output index.  Integer arithmetic only: sums
+// start at 1 << 21, then >> 22 and clip to 0..255.
+__global__ void __launch_bounds__(256) k_resize_pil_u8(const uint8_t* __restrict__ src, int IH, int IW,
+                                                       uint8_t* __restrict__ dst, int OH, int OW,
+                                                       const int* __restrict__ tab, int ksize, int axis_y) {
+  int ox = blockIdx.x * 32 + (threadIdx.x & 31);
+  int oy = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (ox >= OW || oy >= OH) return;
+  const int o = axis_y ? oy : ox, out_sz = axis_y ? OH : OW;
+  const int x0 = tab[2 * o], cnt = tab[2 * o + 1];
+  const int* k = tab + 2 * out_sz + (size_t)o * ksize;
+  const size_t step = axis_y ? (size_t)IW * 3 : 3;
+  const uint8_t* q = axis_y ? src + ((size_t)x0 * IW + ox) * 3 : src + ((size_t)oy * IW + x0) * 3;
+  int s0 = 1 << 21, s1 = 1 << 21, s2 = 1 << 21;
+  for (int j = 0; j < cnt; ++j, q += step) {
+    const int w = k[j];
+    s0 += (int)q[0] * w;
+    s1 += (int)q[1] * w;
+    s2 += (int)q[2] * w;
+  }
+  uint8_t* d = dst + ((size_t)oy * OW + ox) * 3;
+  d[0] = (uint8_t)min(max(s0 >> 22, 0), 255);
+  d[1] = (uint8_t)min(max(s1 >> 22, 0), 255);
+  d[2] = (uint8_t)min(max(s2 >> 22, 0), 255);
+}
+
 // u8 RGB interleaved [H, W, 3] -> f32 CHW normalised pixel_values
 __global__ void __launch_bounds__(256) k_normalize_px(const uint8_t* __restrict__ rgb, int H, int W,
                                                       float* __restrict__ px) {
@@ -318,11 +346,16 @@ __global__ void __launch_bounds__(256) k_add_relu_f16(const __half* __restrict__
 // launchers
 // ---------------------------------------------------------------------------
 void launch_preprocess(const uint8_t* frame_bgr, int H, int W, uint8_t* tmp_u8, uint8_t* rgb_u8, float* px, int OH,
-                       int OW, cudaStream_t s) {
+                       int OW, cudaStream_t s, int swap_rb) {
   dim3 g1((OW + 31) / 32, (H + 7) / 8), g2((OW + 31) / 32, (OH + 7) / 8);
   k_resize_aa_u8<<<g1, 256, 0, s>>>(frame_bgr, H, W, tmp_u8, H, OW, 0, 0);       // width pass
-  k_resize_aa_u8<<<g2, 256, 0, s>>>(tmp_u8, H, OW, rgb_u8, OH, OW, 1, 1);       // height pass (+BGR->RGB)
+  k_resize_aa_u8<<<g2, 256, 0, s>>>(tmp_u8, H, OW, rgb_u8, OH, OW, 1, swap_rb);  // height pass (+BGR->RGB)
   k_normalize_px<<<(OH * OW + 255) / 256, 256, 0, s>>>(rgb_u8, OH, OW, px);
+}
+void launch_resize_pil_u8(const uint8_t* src, int IH, int IW, uint8_t* dst, int OH, int OW, const int* tab, int ksize,
+                          int axis_y, cudaStream_t s) {
+  dim3 g((OW + 31) / 32, (OH + 7) / 8);
+  k_resize_pil_u8<<<g, 256, 0, s>>>(src, IH, IW, dst, OH, OW, tab, ksize, axis_y);
 }
 void launch_depth_post(const float* depth, int IH, int IW, float* up, int OH, int OW, unsigned* mm, uint8_t* out_u8,
                        int invert, cudaStream_t s) {

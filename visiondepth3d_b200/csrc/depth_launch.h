@@ -13,9 +13,12 @@ void launch_patch_im2col(const float* px, int IH, int IW, int ph, int pw, __half
 void launch_set_cls(float* x, const float* cls, const float* pos, int D, cudaStream_t s);
 void launch_im2col_s2(const __half* in, int H, int W, int C, int ldc, __half* out, int OH, int OW, cudaStream_t s);
 void launch_upsample_ac(const __half* in, int H, int W, int C, __half* out, int OH, int OW, cudaStream_t s);
-// DPT image processor: BGR u8 [H,W,3] -> pixel_values f32 [3,OH,OW] (3 launches)
+// DPT image processor: BGR u8 [H,W,3] -> pixel_values f32 [3,OH,OW] (3 launches); swap_rb = 0 takes RGB input
 void launch_preprocess(const uint8_t* frame_bgr, int H, int W, uint8_t* tmp_u8, uint8_t* rgb_u8, float* px, int OH,
-                       int OW, cudaStream_t s);
+                       int OW, cudaStream_t s, int swap_rb = 1);
+// one pass of Pillow's 8-bit bicubic resize on u8 [IH,IW,3] (axis_y = 0: width, 1: height) with a host-built table
+void launch_resize_pil_u8(const uint8_t* src, int IH, int IW, uint8_t* dst, int OH, int OW, const int* tab, int ksize,
+                          int axis_y, cudaStream_t s);
 // bicubic to (OH,OW) + min/max (+ u8 quantisation when out_u8 != null) (2-3 launches)
 void launch_depth_post(const float* depth, int IH, int IW, float* up, int OH, int OW, unsigned* mm, uint8_t* out_u8,
                        int invert, cudaStream_t s);

@@ -58,6 +58,13 @@ def _bind(lib):
     lib.vd3d_depth_infer_batch.restype = i
     lib.vd3d_depth_infer_batch_device.argtypes = [vp, i, C.POINTER(vp), i, i, C.POINTER(vp), C.POINTER(vp), i]
     lib.vd3d_depth_infer_batch_device.restype = i
+    lib.vd3d_depth_infer_images.argtypes = [vp, i, C.POINTER(vp), C.POINTER(C.c_int32), C.POINTER(vp), C.POINTER(vp), i,
+                                            i]
+    lib.vd3d_depth_infer_images.restype = i
+    lib.vd3d_depth_resize_pil.argtypes = [vp, vp, i, i, vp, i, i, i]
+    lib.vd3d_depth_resize_pil.restype = i
+    lib.vd3d_pil_bicubic_table.argtypes = [i, i, vp, vp, i]
+    lib.vd3d_pil_bicubic_table.restype = i
     lib.vd3d_depth_profile.argtypes = [vp, i]
     lib.vd3d_depth_profile.restype = i
     lib.vd3d_depth_profile_collect.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(i), C.POINTER(C.c_double)]
@@ -164,6 +171,65 @@ class DepthEngine:
         fp = (C.c_void_p * n)(*frame_ptrs)
         p8 = (C.c_void_p * n)(*u8_ptrs)
         self.check(self.lib.vd3d_depth_infer_batch_device(self.h, n, fp, h, w, p8, None, int(bool(invert))))
+
+    def infer_images(self, images_rgb, input_sizes=None, invert=False, want_f32=False):
+        """vd3d_depth_infer_images: up to 8 RGB u8 images [h,w,3] of their own sizes -> list of (min-max u8 depth at
+        the image's size, predicted_depth f32 at its input size or None), with one batched forward.  input_sizes: one
+        (W, H) or None (the image's own size) per image; every input size must map to this engine's processed size.
+        images_rgb: host arrays, or CUDA uint8 tensors (the results are then CUDA tensors)."""
+        import torch
+        n = len(images_rgb)
+        if not 1 <= n <= 8:
+            raise ValueError("infer_images takes 1..8 images")
+        input_sizes = list(input_sizes) if input_sizes is not None else [None] * n
+        if len(input_sizes) != n:
+            raise ValueError("one input size (or None) per image")
+        device = isinstance(images_rgb[0], torch.Tensor) and images_rgb[0].is_cuda
+        if device:
+            imgs = [t.contiguous() for t in images_rgb]
+            if any(t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3 or not t.is_cuda for t in imgs):
+                raise ValueError("expected CUDA uint8 tensors [h, w, 3]")
+        else:
+            imgs = [np.ascontiguousarray(a, dtype=np.uint8) for a in images_rgb]
+            if any(a.ndim != 3 or a.shape[2] != 3 for a in imgs):
+                raise ValueError("expected RGB uint8 arrays [h, w, 3]")
+        sizes = np.empty((n, 4), np.int32)
+        for k, (img, ins) in enumerate(zip(imgs, input_sizes)):
+            sh, sw = int(img.shape[0]), int(img.shape[1])
+            iw, ih = (sw, sh) if ins is None else (int(ins[0]), int(ins[1]))
+            if processed_size(iw, ih) != (self.image_h, self.image_w):
+                raise ValueError(f"engine built for processed size {(self.image_h, self.image_w)}, a {iw}x{ih} input "
+                                 f"needs {processed_size(iw, ih)}")
+            sizes[k] = sh, sw, ih, iw
+        if device:
+            dev = imgs[0].device
+            u8 = [torch.empty((int(s[0]), int(s[1])), dtype=torch.uint8, device=dev) for s in sizes]
+            f32 = [torch.empty((int(s[2]), int(s[3])), dtype=torch.float32, device=dev) for s in sizes] if want_f32 else None
+            ptr, mem = (lambda t: t.data_ptr()), _lib.MEM_DEVICE
+            torch.cuda.current_stream().synchronize()  # the images may come from work queued on torch's stream
+        else:
+            u8 = [np.empty((int(s[0]), int(s[1])), np.uint8) for s in sizes]
+            f32 = [np.empty((int(s[2]), int(s[3])), np.float32) for s in sizes] if want_f32 else None
+            ptr, mem = (lambda a: a.ctypes.data), _lib.MEM_HOST
+        vp = C.c_void_p
+        self.check(self.lib.vd3d_depth_infer_images(
+            self.h, n, (vp * n)(*[ptr(a) for a in imgs]), sizes.ctypes.data_as(C.POINTER(C.c_int32)),
+            (vp * n)(*[ptr(a) for a in u8]), (vp * n)(*[ptr(a) for a in f32]) if want_f32 else None,
+            int(bool(invert)), mem))
+        if device:
+            self.ctx.check(self.lib.vd3d_sync(self.ctx.h))
+        return list(zip(u8, f32 if want_f32 else [None] * n))
+
+    def resize_pil(self, rgb, width, height):
+        """vd3d_depth_resize_pil: Image.fromarray(rgb).resize((width, height), Image.BICUBIC) on a host RGB u8
+        [h,w,3] array, on the GPU."""
+        src = np.ascontiguousarray(rgb, dtype=np.uint8)
+        if src.ndim != 3 or src.shape[2] != 3:
+            raise ValueError("expected an RGB uint8 array [h, w, 3]")
+        out = np.empty((int(height), int(width), 3), np.uint8)
+        self.check(self.lib.vd3d_depth_resize_pil(self.h, src.ctypes.data, src.shape[0], src.shape[1], out.ctypes.data,
+                                                  int(height), int(width), _lib.MEM_HOST))
+        return out
 
     def get_buffer(self, name, shape, dtype):
         out = np.empty(shape, dtype=dtype)

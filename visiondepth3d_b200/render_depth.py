@@ -1,7 +1,8 @@
 """Drop-in for the hot-path surface of the reference's core/render_depth.py: the `pipe`
 callable protocol and the depth -> uint8 normalisation, backed by the libvd3d depth engine
 (Depth-Anything-V2 on wgmma tensor cores), and the letterbox tracker of the depth-video pass with its pixel work on
-the GPU (letterbox.cu).  GUI, ONNX, Marigold and DepthCrafter are outside the GPU hot path (SURVEY.md section 2).
+the GPU (letterbox.cu), and the still-image drivers of the Depth tab (depth_images, vd3d_depth_infer_images).  GUI,
+ONNX, Marigold and DepthCrafter are outside the GPU hot path (SURVEY.md section 2).
 
 Protocol kept (core/render_depth.py:1113-1119, consumers 201-268 and 1894-1917):
     pipe(images: list[PIL.Image], inference_size: (W, H) | None) -> list[{"predicted_depth": Tensor[h, w]}]
@@ -9,6 +10,7 @@ with `predicted_depth` already resized (bicubic) to the PIL image size, as
 transformers' DepthEstimationPipeline.postprocess does.
 """
 import os
+import re
 import threading
 import time
 from ctypes import c_void_p as C_void_p
@@ -17,6 +19,7 @@ import numpy as np
 
 from .depth_engine import DepthEngine, processed_size as _processed_size
 from .depth_weights import CONFIGS, hf_config
+from .render_3d import _dialog, _val
 
 try:
     import torch
@@ -1031,6 +1034,233 @@ def depth_video_from_video(input_path, output_path, invert=False, inference_size
     return n
 
 
+# ---------------------------------------------------------------------------
+# still images (core/render_depth.py:1196-1213, 1215-1340, 1353-1515): the drivers of the Depth tab's image modes.  The
+# pixel work of the `pipe` path -- the inference-size resize, the DPT processor, one batched forward per processed
+# size, the bicubic post-resize, min-max u8 and the resize back -- runs on the GPU in one call per batch
+# (vd3d_depth_infer_images)
+# ---------------------------------------------------------------------------
+IMAGE_EXTENSIONS = (".jpeg", ".jpg", ".png")
+_RESOLUTION = re.compile(r"^\s*(\d+)\s*x\s*(\d+)")
+
+
+def parse_inference_resolution(res_string, fallback=(384, 384)):
+    """core/render_depth.py:1196-1197: the (W, H) of a resolution choice of the Depth tab, read from its "<W>x<H>"
+    prefix ("910x518 (Depth Anything)" -> (910, 518)); "Original" -> None (each image at its own size); anything
+    else -> fallback."""
+    s = res_string.strip()
+    if s == "Original":
+        return None
+    m = _RESOLUTION.match(s)
+    return (int(m.group(1)), int(m.group(2))) if m else fallback
+
+
+def get_dynamic_batch_size(base=4, scale_factor=1.0, max_limit=32, reserve_vram_gb=1.0):
+    """core/render_depth.py:1206-1213: base images per GB of device memory beyond reserve_vram_gb, capped at
+    max_limit; base without a GPU."""
+    if torch is not None and torch.cuda.is_available():
+        total = torch.cuda.get_device_properties(0).total_memory / (1024 ** 3)
+        return min(int(base * max(0, total - reserve_vram_gb) * scale_factor), max_limit)
+    return base
+
+
+def _rgb_array(img):
+    if isinstance(img, np.ndarray):
+        if img.ndim != 3 or img.shape[2] != 3:
+            raise ValueError(f"expected an RGB array [h, w, 3], got shape {img.shape}")
+        return np.ascontiguousarray(img, dtype=np.uint8)
+    return np.asarray(img.convert("RGB"), dtype=np.uint8)
+
+
+def depth_images(images, inference_size=None, invert=False):
+    """Still images -> u8 depth planes, each at its image's own size: what _run_pipe_or_tile + the image drivers'
+    min-max normalisation, inversion and cv2 INTER_CUBIC resize back compute for the `pipe` path.  images: PIL
+    images or RGB u8 arrays.  Images whose input size (inference_size, or their own size) maps to the same DPT
+    processed size share one batched forward (up to 8 per forward), whatever their source sizes."""
+    rgbs = [_rgb_array(img) for img in images]
+    groups = {}
+    for k, a in enumerate(rgbs):
+        iw, ih = inference_size if inference_size is not None else (a.shape[1], a.shape[0])
+        groups.setdefault(_processed_size(int(iw), int(ih)), []).append(k)
+    out = [None] * len(rgbs)
+    for (ph, pw), idxs in groups.items():
+        iw, ih = inference_size if inference_size is not None else (rgbs[idxs[0]].shape[1], rgbs[idxs[0]].shape[0])
+        eng = _engine_for(int(iw), int(ih))
+        for i0 in range(0, len(idxs), 8):
+            chunk = idxs[i0:i0 + 8]
+            ins = [inference_size] * len(chunk)
+            for k, (d8, _) in zip(chunk, eng.infer_images([rgbs[k] for k in chunk], ins, invert=invert)):
+                out[k] = d8
+    return out
+
+
+def _progress(bar, **kw):
+    if bar is not None:
+        bar.config(**kw)
+
+
+def _grayscale_image(depth_u8, colormap_name):
+    """The written image: grayscale ("L").  Colour maps come from matplotlib in the reference, which this package
+    does not use: any other name falls back to grayscale with the reference's message."""
+    from PIL import Image
+    if colormap_name != "default":
+        print(f"⚠️ Unknown colormap '{colormap_name}', defaulting to grayscale.")
+    return Image.fromarray(np.ascontiguousarray(depth_u8, dtype=np.uint8))  # 2-D u8 -> mode "L"
+
+
+def _ensure_output_dir(output_dir, status_label):
+    """The output-directory checks of the image drivers: True when output_dir exists or was created."""
+    if not output_dir:
+        print("⚠️ Please select an output directory before processing.")
+        _notify(status_label, "❌ Output directory not selected.")
+        return False
+    if not os.path.exists(output_dir):
+        try:
+            os.makedirs(output_dir)
+        except Exception as e:
+            print(f"❌ Could not create output directory:\n{e}")
+            _notify(status_label, "❌ Failed to create output directory.")
+            return False
+    return True
+
+
+def _depth_output_path(output_dir, file_path):
+    return os.path.join(output_dir, f"{os.path.splitext(os.path.basename(file_path))[0]}_depth.png")
+
+
+def process_images_in_folder(folder_path, batch_size_widget, output_dir_var, inference_res_var, status_label,
+                             progress_bar, root, invert_var):
+    """core/render_depth.py:1229-1340: every .jpeg / .jpg / .png of folder_path (os.listdir order) -> <stem>_depth.png
+    (u8 grayscale, the image's size) in the output directory, in chunks of the batch size.  GUI variables may be Tk
+    variables or plain values; status text goes to status_label (or stdout), root is not used.  With USE_TILED_DEPTH
+    each image goes through infer_depth_tile and _normalize_to_u8, otherwise through depth_images."""
+    output_dir = str(_val(output_dir_var) or "").strip()
+    if not _ensure_output_dir(output_dir, status_label):
+        return
+    inference_size = parse_inference_resolution(_val(inference_res_var))
+    try:
+        user_value = str(_val(batch_size_widget) or "").strip()
+        batch_size = int(user_value) if user_value else get_dynamic_batch_size()
+        if batch_size <= 0:
+            raise ValueError
+    except Exception:
+        batch_size = get_dynamic_batch_size()
+        _notify(status_label, f"⚠️ Invalid batch size. Using dynamic batch size: {batch_size}")
+    image_files = [os.path.join(folder_path, f) for f in os.listdir(folder_path) if f.lower().endswith(IMAGE_EXTENSIONS)]
+    if not image_files:
+        _notify(status_label, "⚠️ No image files found.")
+        return
+    total = len(image_files)
+    invert = bool(_val(invert_var))
+    _notify(status_label, f"📂 Processing {total} images...")
+    _progress(progress_bar, maximum=total, value=0)
+    from PIL import Image
+    start = time.time()
+    for i in range(0, total, batch_size):
+        if cancel_requested.is_set():
+            _notify(status_label, "❌ Cancelled by user.")
+            return
+        batch_files = image_files[i:i + batch_size]
+        images = [Image.open(f).convert("RGB") for f in batch_files]
+        print(f"🚀 Running batch of {len(images)} images at {inference_size}")
+        if USE_TILED_DEPTH:
+            planes = [p["predicted_depth"] for p in _run_pipe_or_tile(images, inference_size)]
+        else:
+            planes = depth_images(images, inference_size, invert)
+        for j, plane in enumerate(planes):
+            if cancel_requested.is_set():
+                _notify(status_label, "❌ Cancelled during batch.")
+                return
+            file_path = batch_files[j]
+            try:
+                d8 = _normalize_to_u8(plane, images[j].size, invert=invert) if USE_TILED_DEPTH else plane
+                _grayscale_image(d8, "default").save(_depth_output_path(output_dir, file_path))
+            except Exception as e:
+                print(f"❌ Error processing {file_path}: {e}")
+                continue
+            done = i + j + 1
+            elapsed = time.time() - start
+            fps = done / elapsed if elapsed > 0 else 0
+            eta = (total - done) / fps if fps > 0 else 0
+            if progress_bar is not None and status_label is not None:
+                update_progress(done, total, fps, eta, progress_bar, status_label)
+    _notify(status_label, "✅ All images processed successfully!")
+    _progress(progress_bar, value=total)
+
+
+def process_image(file_path, colormap_var, invert_var, output_dir_var, inference_res_var, input_label, output_label,
+                  status_label, progress_bar, folder=False):
+    """core/render_depth.py:1353-1477: one image -> <stem>_depth.png in the output directory, the same file the folder
+    driver writes for it.  The Tk previews (input_label / output_label thumbnails) are not produced; colour maps fall
+    back to grayscale."""
+    from PIL import Image
+    image = Image.open(file_path).convert("RGB")
+    inference_size = parse_inference_resolution(_val(inference_res_var))
+    print("📏 Using inference size:", inference_size)
+    invert = bool(_val(invert_var))
+    colormap_name = str(_val(colormap_var)).strip().lower()
+    if USE_TILED_DEPTH:
+        dep = _run_pipe_or_tile([image], inference_size)[0]["predicted_depth"]
+    else:
+        dep = depth_images([image], inference_size, invert)[0]
+    try:
+        d8 = _normalize_to_u8(dep, image.size, invert=invert) if USE_TILED_DEPTH else dep
+        depth_image = _grayscale_image(d8, colormap_name)
+    except Exception as e:
+        print(f"❌ Error extracting depth: {e}")
+        return
+    output_dir = str(_val(output_dir_var) or "").strip()
+    if not _ensure_output_dir(output_dir, status_label):
+        return
+    path = _depth_output_path(output_dir, file_path)
+    depth_image.save(path)
+    if not folder:
+        cancel_requested.clear()
+        _notify(status_label, f"✅ Image saved: {path}")
+        _progress(progress_bar, value=100)
+        if progress_bar is not None and hasattr(progress_bar, "stop"):
+            progress_bar.stop()
+
+
+def open_image(status_label_widget, progress_bar_widget, colormap_var, invert_var, output_dir_var, inference_res_var,
+               input_label_widget, output_label_widget):
+    """core/render_depth.py:1480-1514: pick an image (Tk file dialog) and run process_image on a worker thread.
+    Returns the thread, or None when no file was picked."""
+    file_path = _dialog("askopenfilename", filetypes=[("Image Files", "*.jpeg;*.jpg;*.png")])
+    if not file_path:
+        return None
+    cancel_requested.clear()
+    _notify(status_label_widget, "🔄 Processing image...")
+    if progress_bar_widget is not None and hasattr(progress_bar_widget, "start"):
+        progress_bar_widget.start(10)
+
+    def work():
+        process_image(file_path, colormap_var, invert_var, output_dir_var, inference_res_var, input_label_widget,
+                      output_label_widget, status_label_widget, progress_bar_widget)
+        if progress_bar_widget is not None and hasattr(progress_bar_widget, "stop"):
+            progress_bar_widget.stop()
+
+    t = threading.Thread(target=work, daemon=True)
+    t.start()
+    return t
+
+
+def process_image_folder(batch_size_widget, output_dir_var, inference_res_var, status_label, progress_bar, invert_var,
+                         root):
+    """core/render_depth.py:1215-1226: pick a folder (Tk directory dialog) and run process_images_in_folder on a
+    worker thread.  Returns the thread, or None when no folder was picked."""
+    folder_path = _dialog("askdirectory", title="Select Folder Containing Images")
+    if not folder_path:
+        cancel_requested.clear()
+        _notify(status_label, "⚠️ No folder selected.")
+        return None
+    t = threading.Thread(target=process_images_in_folder, args=(folder_path, batch_size_widget, output_dir_var,
+                                                                 inference_res_var, status_label, progress_bar, root,
+                                                                 invert_var), daemon=True)
+    t.start()
+    return t
+
+
 def _gui_only(name):
     def f(*_a, **_k):
         raise RuntimeError(f"{name} is a Tk GUI driver of the reference (core/render_depth.py); on the GPU path use "
@@ -1040,10 +1270,6 @@ def _gui_only(name):
 
 
 # GUI batch drivers the reference's main window imports (VisionDepth3D.py:41-53); the import list must resolve
-open_image = _gui_only("open_image")
 open_video = _gui_only("open_video")
-process_image = _gui_only("process_image")
-process_image_folder = _gui_only("process_image_folder")
-process_images_in_folder = _gui_only("process_images_in_folder")
 process_video_folder = _gui_only("process_video_folder")
 process_videos_in_folder = _gui_only("process_videos_in_folder")

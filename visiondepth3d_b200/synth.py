@@ -182,3 +182,28 @@ def merged_frames_folder(path, w=128, h=72):
         with open(os.path.join(path, name), "wb") as f:
             f.write(data if data is not None else cv2.imencode(".bmp", synth_frame(7, w, h, "natural")[0])[1].tobytes())
     return path
+
+
+# the photo folder of the image-depth fixtures (tools/gen_golden.py images): two landscape sizes of one processed size
+# (640x480 PNG, 1024x768 upper-case .JPG), a portrait and an odd size, and files the extension filter drops
+IMAGE_FOLDER = (("a_room.png", 640, 480, 11), ("b_street.JPG", 1024, 768, 12), ("c_portrait.png", 480, 854, 13),
+                ("d_odd.jpeg", 333, 517, 14))
+IMAGE_DECOYS = {"notes.txt": b"not an image", "scan.bmp": None}
+
+
+def image_folder(path):
+    """Write the photo fixture folder into `path` (created; Pillow encoders, default quality) and return it."""
+    from PIL import Image
+    os.makedirs(path, exist_ok=True)
+    for name, w, h, seed in IMAGE_FOLDER:
+        rgb = synth_frame(seed, w, h, "natural")[0][..., ::-1]
+        Image.fromarray(np.ascontiguousarray(rgb)).save(os.path.join(path, name), format="JPEG" if name.lower().endswith(
+            (".jpg", ".jpeg")) else "PNG")
+    for name, data in IMAGE_DECOYS.items():
+        p = os.path.join(path, name)
+        if data is None:
+            Image.fromarray(synth_frame(15, 64, 48, "natural")[0]).save(p, format="BMP")
+        else:
+            with open(p, "wb") as f:
+                f.write(data)
+    return path
