@@ -393,6 +393,16 @@ int vd3d_get_depth_batch(vd3d_ctx* ctx);
  * implicit-GEMM convs, f16 activations, fp32 accumulate, fp32 last layer) -> PixelShuffle + input -> postprocess_esr. */
 int vd3d_sr_create(void* cuda_stream, vd3d_depth** out);
 int vd3d_sr_forward(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, int num_conv, uint8_t* out_bgr, int mem);
+/* Make an SR engine an RRDBNet (the generator of ESRGAN / Real-ESRGAN RealESRGAN_x4plus / BSRGAN: num_feat 64, growth
+ * 32, nb RRDB blocks of three dense blocks, net_scale 4 = two nearest-x2 up-convs or 2 = one), or SRVGGNetCompact
+ * again with nb = 0.  Weights (vd3d_depth_set_tensor, ".w" f16 [Cout, 9 * Cin_padded] tap-major, ".b" f32 [Cout]):
+ * "rr.first" (Cin 3 padded to 64), "rr.{i}.{j}.{k}" for block i, dense block j = 0..2 and conv k = 1..5 (input
+ * channels laid out as 64 + 64 per 32-channel growth slice, zero columns in the padding: Cin_padded = 64 k), "rr.body",
+ * "rr.up1" / "rr.up2" (nearest x2 + conv as four phase convs: [4 * 64, 9 * 64], rows (py * 2 + px) * 64 + co),
+ * "rr.hr", "rr.last" ([32, 9 * 64], rows 3..31 zero).  vd3d_sr_forward then returns BGR u8 [net_scale h,
+ * net_scale w, 3] and vd3d_sr_upscale runs the reference's resize chain on it (scale stays the model-name quirk);
+ * num_conv is ignored.  VD3D_ERR_ARG for nb outside 0..64 or another net_scale. */
+int vd3d_sr_set_rrdb(vd3d_depth* e, int nb, int net_scale);
 /* arguments of run_esrgan (core/merged_pipeline.py:240-267) without tiling.  input_res_pct and blend_alpha are Python
  * floats there (double here, rounded where the reference's cv2 calls round them). */
 typedef struct {

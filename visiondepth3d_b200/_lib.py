@@ -100,7 +100,7 @@ SYMBOLS = [
     "vd3d_pixel_shift", "vd3d_plan_sizes", "vd3d_render_frame", "vd3d_render_clip",
     "vd3d_sharpen", "vd3d_dof_grade", "vd3d_struct_size", "vd3d_pack", "vd3d_fit_eye", "vd3d_area_table", "vd3d_area_linear_table", "vd3d_heal",
     "vd3d_profile", "vd3d_profile_collect", "vd3d_check_config", "vd3d_color_grade", "vd3d_resize_cubic_u8", "vd3d_resize_cubic", "vd3d_add_weighted",
-    "vd3d_sr_create", "vd3d_sr_forward", "vd3d_sr_upscale",
+    "vd3d_sr_create", "vd3d_sr_forward", "vd3d_sr_upscale", "vd3d_sr_set_rrdb",
     # depth forward (bound in depth_engine.py)
     "vd3d_depth_create", "vd3d_depth_destroy", "vd3d_depth_last_error", "vd3d_depth_launch_count",
     "vd3d_depth_set_tensor", "vd3d_depth_forward", "vd3d_depth_get_buffer", "vd3d_gemm_f16", "vd3d_gemm_bench", "vd3d_conv_f16",
@@ -235,6 +235,8 @@ def load():
     lib.vd3d_sr_forward.restype = i
     lib.vd3d_sr_upscale.argtypes = [vp, vp, i, C.POINTER(vp), i, i, i, C.POINTER(UpscaleParams), C.POINTER(vp), i]
     lib.vd3d_sr_upscale.restype = i
+    lib.vd3d_sr_set_rrdb.argtypes = [vp, i, i]
+    lib.vd3d_sr_set_rrdb.restype = i
     lib.vd3d_color_grade.argtypes = [vp, fp, i, i, C.c_double, C.c_double, C.c_double, fp, i]
     lib.vd3d_color_grade.restype = i
     lib.vd3d_sharpen.argtypes = [vp, u8p, i, i, C.c_double, u8p, i]

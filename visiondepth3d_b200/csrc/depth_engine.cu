@@ -87,6 +87,8 @@ struct vd3d_depth {
     if (i >= 0) cudaEventRecord(spans[i].e1, s);
   }
   bool prof_spans = false;
+  // SR engines: RRDBNet with rr_nb blocks and network scale rr_scale (vd3d_sr_set_rrdb); 0: SRVGGNetCompact
+  int rr_nb = 0, rr_scale = 0;
 };
 
 namespace {
@@ -194,8 +196,10 @@ void pick_tile(int W, int H, int& tw, int& th) {
   }
 }
 
-// conv over an NHWC f16 map [H, W, cin] (3x3 pad 1 when k3, else 1x1); weights [N, taps*cin]
-int conv(vd3d_depth* e, const __half* in, int H, int W, int cin, const __half* wt, bool k3, GemmArgs g, int bn = 0) {
+// conv over an NHWC f16 map [H, W, cin] (3x3 pad 1 when k3, else 1x1); weights [N, taps*cin].  pitch: channels per
+// pixel of the map when it holds more than the cin read (0: cin); sr: the RRDBNet epilogue (EPI_SR)
+int conv(vd3d_depth* e, const __half* in, int H, int W, int cin, const __half* wt, bool k3, GemmArgs g, int bn = 0,
+         int pitch = 0, bool sr = false) {
   if (cin % 64) return dfail(e, VD3D_ERR_ARG, "conv: cin must be a multiple of 64");
   if (!bn) bn = pick_bn(g.N);
   int tw, th;
@@ -210,10 +214,12 @@ int conv(vd3d_depth* e, const __half* in, int H, int W, int cin, const __half* w
   g.K = (k3 ? 9 : 1) * cin;
   CUtensorMap ma, mb;
   int r;
-  if ((r = make_map(e, &ma, in, cin, W, H, cin, (uint64_t)cin * W, tw, th))) return r;
+  if (!pitch) pitch = cin;
+  if ((r = make_map(e, &ma, in, cin, W, H, pitch, (uint64_t)pitch * W, tw, th))) return r;
   if ((r = make_map(e, &mb, wt, g.K, g.N, 1, g.K, (uint64_t)g.K * g.N, bn, 1))) return r;
   int m_tiles = ((W + tw - 1) / tw) * ((H + th - 1) / th);
-  cudaError_t ce = launch_gemm(bn, ma, mb, g, m_tiles, 1, e->cur ? e->cur : e->stream);
+  cudaStream_t s = e->cur ? e->cur : e->stream;
+  cudaError_t ce = sr ? launch_gemm_sr(bn, ma, mb, g, m_tiles, s) : launch_gemm(bn, ma, mb, g, m_tiles, 1, s);
   if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("conv launch: ") + cudaGetErrorString(ce));
   e->launches++;
   return VD3D_OK;
@@ -1218,11 +1224,22 @@ int vd3d_sr_create(void* stream, vd3d_depth** out) {
   return VD3D_OK;
 }
 
+// Make an SR engine an RRDBNet (ESRGAN / Real-ESRGAN / BSRGAN: num_feat 64, growth 32) with nb RRDB blocks and
+// network scale 2 or 4; nb = 0 makes it an SRVGGNetCompact again.
+int vd3d_sr_set_rrdb(vd3d_depth* e, int nb, int net_scale) {
+  if (!e || nb < 0 || nb > 64 || (nb && net_scale != 2 && net_scale != 4)) return VD3D_ERR_ARG;
+  e->rr_nb = nb;
+  e->rr_scale = nb ? net_scale : 0;
+  return VD3D_OK;
+}
+
 }  // extern "C"
 
 namespace vd3d {
 
 cudaStream_t sr_stream(vd3d_depth* e) { return e->stream; }
+
+int sr_net_scale(vd3d_depth* e) { return e->rr_scale; }
 
 int sr_buffer(vd3d_depth* e, const char* name, size_t bytes, void** out) { return get_buf(e, name, bytes, out); }
 
@@ -1276,18 +1293,134 @@ int sr_network(vd3d_depth* e, const uint8_t* fd, int h, int w, int num_conv, con
   return VD3D_OK;
 }
 
+// RRDBNet (ESRGAN, Wang et al. 2018; Real-ESRGAN and BSRGAN use the same generator), every 3x3 conv on the wgmma
+// implicit GEMM with the EPI_SR epilogue, f16 NHWC activations, fp32 accumulate:
+//   feat = conv_first(x);  nb x RRDB;  feat = feat + conv_body(trunk);  (scale / 2) x [lrelu(conv_up(nearest x2))];
+//   out = conv_last(lrelu(conv_hr(.)))  (f32).
+// Dense blocks without copies: each RDB owns one [h*w, 320] buffer, x in channels 0..63 and growth slice k (32
+// channels) at 64 k, padded to 64 (the padding channels are zero from allocation and never written; the packed
+// weights have zero columns there), so conv k reads the channel prefix 64 k through its tensor map and writes only its
+// own slice.  The RDB output x + 0.2 x5 goes to channels 0..63 of the next RDB's buffer; the third RDB of an RRDB adds
+// the RRDB residual in the same epilogue (x_rrdb + 0.2 (x + 0.2 x5)) in place over x_rrdb, which no conv of that
+// launch reads.  Three buffers rotate: RDB j reads d[j] and writes d[(j + 1) % 3].  nearest x2 + conv is four phase
+// convs on the low-resolution map, one 3x3 GEMM with N = 4 x 64 (combined weights) and the pixel-shuffle scatter.
+// Weights "rr.first", "rr.{i}.{j}.{k}" (block i, RDB j = 0..2, conv k = 1..5: f16 [32 or 64, 9 * 64 k]), "rr.body",
+// "rr.up1", "rr.up2" (f16 [256, 576]), "rr.hr", "rr.last" (f16 [32, 576], rows 3.. zero) with ".w" / ".b" (f32 [N]).
+// *rgb: f32 [scale h * scale w, 32], RGB in columns 0..2.
+int rrdb_network(vd3d_depth* e, const uint8_t* fd, int h, int w, const float** rgb) {
+  if (!e || !fd || !rgb || h < 8 || w < 8 || !e->rr_nb) return VD3D_ERR_ARG;
+  constexpr int P = 320;  // channels per pixel of a dense buffer
+  cudaStream_t s = e->stream;
+  const int ns = e->rr_scale, nb = e->rr_nb;
+  const size_t npix = (size_t)h * w, nhr = npix * ns * ns;
+  void *x0, *feat, *body, *d[3], *u[2];
+  int r;
+  if ((r = get_buf(e, "rr.x0", npix * 64 * 2, &x0)) || (r = get_buf(e, "rr.feat", npix * 64 * 2, &feat)) ||
+      (r = get_buf(e, "rr.body", npix * 64 * 2, &body)) || (r = get_buf(e, "rr.d0", npix * P * 2, &d[0])) ||
+      (r = get_buf(e, "rr.d1", npix * P * 2, &d[1])) || (r = get_buf(e, "rr.d2", npix * P * 2, &d[2])) ||
+      (r = get_buf(e, "rr.u0", nhr * 64 * 2, &u[0])) || (r = get_buf(e, "rr.u1", nhr * 64 * 2, &u[1])))
+    return r;
+  __half* D[3] = {(__half*)d[0], (__half*)d[1], (__half*)d[2]};
+  __half* U[2] = {(__half*)u[0], (__half*)u[1]};
+  auto run = [&](const char* nm, const __half* in, int H, int Wd, int cin, int pitch, GemmArgs g) {
+    const __half* wt;
+    const float* b;
+    int rr;
+    if ((rr = W(e, std::string(nm) + ".w", &wt, (size_t)g.N * 9 * cin)) || (rr = W(e, std::string(nm) + ".b", &b, g.N)))
+      return rr;
+    g.bias = b;
+    return conv(e, in, H, Wd, cin, wt, true, g, 0, pitch, true);
+  };
+  launch_sr_in(fd, (__half*)x0, (int)npix, s);
+  e->launches++;
+  GemmArgs g = base_args(0, 64, 0, EPI_SR);
+  g.out_f16 = (__half*)feat;
+  if ((r = run("rr.first", (const __half*)x0, h, w, 64, 64, g))) return r;
+  DCK(cudaMemcpy2DAsync(D[0], P * 2, feat, 64 * 2, 64 * 2, npix, cudaMemcpyDeviceToDevice, s));
+  char nm[48];
+  for (int i = 0; i < nb; ++i)
+    for (int j = 0; j < 3; ++j) {
+      __half *X = D[j], *Y = D[(j + 1) % 3];
+      for (int k = 1; k <= 5; ++k) {
+        snprintf(nm, sizeof nm, "rr.%d.%d.%d", i, j, k);
+        g = base_args(0, k < 5 ? 32 : 64, 0, EPI_SR);
+        g.ldc = P;
+        if (k < 5) {
+          g.out_f16 = X + 64 * k;
+          g.act = 4;
+        } else {
+          g.out_f16 = Y;
+          g.res_f16 = X;
+          g.rs = 0.2f;
+          if (j == 2) {  // Y is the RRDB's input
+            g.res2_f16 = Y;
+            g.rs2 = 0.2f;
+          }
+        }
+        if ((r = run(nm, X, h, w, 64 * k, P, g))) return r;
+      }
+    }
+  g = base_args(0, 64, 0, EPI_SR);
+  g.out_f16 = (__half*)body;
+  g.res_f16 = (const __half*)feat;
+  g.rs = 1.f;
+  if ((r = run("rr.body", D[0], h, w, 64, P, g))) return r;
+  const __half* src = (const __half*)body;
+  int H = h, Wd = w, ui = 1;
+  for (int k = 1; 1 << k <= ns; ++k) {
+    snprintf(nm, sizeof nm, "rr.up%d", k);
+    g = base_args(0, 256, 0, EPI_SR);
+    g.out_f16 = U[ui];
+    g.act = 4;
+    g.ct_k = 2;
+    g.ct_cout = 64;
+    g.ct_w = Wd;
+    if ((r = run(nm, src, H, Wd, 64, 64, g))) return r;
+    src = U[ui];
+    ui ^= 1;
+    H *= 2;
+    Wd *= 2;
+  }
+  g = base_args(0, 64, 0, EPI_SR);
+  g.out_f16 = U[ui];
+  g.act = 4;
+  if ((r = run("rr.hr", src, H, Wd, 64, 64, g))) return r;
+  g = base_args(0, 32, 0, EPI_SR);
+  g.out_f32 = (float*)src;  // the last up-conv's output is no longer read: its buffer holds [H * Wd, 32] floats
+  if ((r = run("rr.last", U[ui], H, Wd, 64, 64, g))) return r;
+  *rgb = (const float*)src;
+  return VD3D_OK;
+}
+
 }  // namespace vd3d
 
 extern "C" {
 
 // frame BGR u8 [h,w,3] -> BGR u8 [4h,4w,3] (preprocess_esr -> network -> postprocess_esr)
 int vd3d_sr_forward(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, int num_conv, uint8_t* out_bgr, int mem) {
-  if (!e || !frame_bgr || !out_bgr || h < 8 || w < 8 || num_conv < 1 || num_conv > 64) return VD3D_ERR_ARG;
+  if (!e || !frame_bgr || !out_bgr || h < 8 || w < 8 || (!e->rr_nb && (num_conv < 1 || num_conv > 64)))
+    return VD3D_ERR_ARG;
   cudaStream_t s = e->stream;
   const size_t npix = (size_t)h * w;
   void *fd = (void*)frame_bgr, *od = out_bgr;
   const float* cvo;
   int r;
+  if (e->rr_nb) {  // RRDBNet: BGR u8 [scale h, scale w, 3]
+    const size_t nout = npix * e->rr_scale * e->rr_scale;
+    if (mem == VD3D_MEM_HOST) {
+      if ((r = get_buf(e, "sr.in", npix * 3, &fd)) || (r = get_buf(e, "sr.outu8", nout * 3, &od))) return r;
+      DCK(cudaMemcpyAsync(fd, frame_bgr, npix * 3, cudaMemcpyHostToDevice, s));
+    }
+    if ((r = rrdb_network(e, (const uint8_t*)fd, h, w, &cvo))) return r;
+    launch_rrdb_out(cvo, 32, (uint8_t*)od, nout, s);
+    e->launches++;
+    DCK(cudaGetLastError());
+    if (mem == VD3D_MEM_HOST) {
+      DCK(cudaMemcpyAsync(out_bgr, od, nout * 3, cudaMemcpyDeviceToHost, s));
+      DCK(cudaStreamSynchronize(s));
+    }
+    return VD3D_OK;
+  }
   if (mem == VD3D_MEM_HOST) {
     if ((r = get_buf(e, "sr.in", npix * 3, &fd)) || (r = get_buf(e, "sr.outu8", npix * 48, &od))) return r;
     DCK(cudaMemcpyAsync(fd, frame_bgr, npix * 3, cudaMemcpyHostToDevice, s));

@@ -437,17 +437,18 @@ void launch_relu_f16(const __half* in, __half* out, size_t n, cudaStream_t s) {
   k_relu_f16<<<(unsigned)((n8 + 255) / 256), 256, 0, s>>>(in, out, n8);
 }
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool kSr = false>
 static cudaError_t launch_gemm_t(const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, dim3 grid,
                                  cudaStream_t s) {
   static bool attr_set = false;
   constexpr int smem = GemmSmem<BN, STAGES>::kTotal;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(k_umma_gemm<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e =
+        cudaFuncSetAttribute(k_umma_gemm<BN, STAGES, kSr>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  k_umma_gemm<BN, STAGES><<<grid, kGemmThreads, smem, s>>>(a, b, g);
+  k_umma_gemm<BN, STAGES, kSr><<<grid, kGemmThreads, smem, s>>>(a, b, g);
   return cudaGetLastError();
 }
 
@@ -513,6 +514,23 @@ cudaError_t launch_gemm(int bn, const CUtensorMap& a, const CUtensorMap& b, cons
     case 128: return launch_gemm_t<128, 4>(a, b, g, grid, s);
     case 64: return launch_gemm_t<64, 6>(a, b, g, grid, s);
     case 32: return launch_gemm_t<32, 6>(a, b, g, grid, s);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+// the RRDBNet convs: launch_gemm's tiles and grid with the EPI_SR epilogue (k_umma_gemm<BN, STAGES, true>)
+cudaError_t launch_gemm_sr(int bn, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g_in, int m_tiles,
+                           cudaStream_t s) {
+  GemmArgs g = g_in;
+  g.nt = (g.N + bn - 1) / bn;
+  g.mt = m_tiles;
+  g.nz = 1;
+  const int total = g.nt * g.mt, sms = sm_count();
+  dim3 grid(total < sms ? total : sms, 1, 1);
+  switch (bn) {
+    case 128: return launch_gemm_t<128, 4, true>(a, b, g, grid, s);
+    case 64: return launch_gemm_t<64, 6, true>(a, b, g, grid, s);
+    case 32: return launch_gemm_t<32, 6, true>(a, b, g, grid, s);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -35,4 +35,7 @@ cudaError_t launch_gemm(int bn, const CUtensorMap& a, const CUtensorMap& b, cons
                         int batch, cudaStream_t s);
 cudaError_t launch_gemm_variant(int variant, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, int m_tiles,
                         int batch, cudaStream_t s);
+// launch_gemm for the RRDBNet convs (epilogue EPI_SR), batch 1
+cudaError_t launch_gemm_sr(int bn, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, int m_tiles,
+                           cudaStream_t s);
 }  // namespace vd3d

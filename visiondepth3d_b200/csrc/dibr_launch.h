@@ -179,6 +179,8 @@ void launch_add_weighted(const uint8_t* a, float alpha, const uint8_t* b, float 
                          cudaStream_t s);
 // sr_kernels.cu: the x4 output of the SR network (last conv f32 NHWC [h*w, 48] + network input BGR u8 [h,w,3]) resampled
 // with INTER_CUBIC straight to [oh, ow, 3] without materialising the 4h x 4w image
+// postprocess_esr of an RRDBNet output: f32 RGB rows of ld floats -> clip [0,1], x255, truncate, BGR u8 [npix, 3]
+void launch_rrdb_out(const float* rgb, int ld, uint8_t* bgr, size_t npix, cudaStream_t s);
 void launch_sr_tail_cubic(const float* conv, const uint8_t* bgr, int h, int w, uint8_t* dst, int oh, int ow,
                           cudaStream_t s);
 void launch_heal(const float* warped, const float* orig, const float* edge, float* out, int H, int W, float hs,

@@ -79,6 +79,24 @@ __global__ void __launch_bounds__(256) k_sr_tail_cubic(const float* __restrict__
   }
 }
 
+// postprocess_esr (core/merged_pipeline.py:227-231) of the RRDBNet output, whose network output has no base add:
+// one thread per pixel.
+__global__ void __launch_bounds__(256) k_rrdb_out(const float* __restrict__ rgb, int ld, uint8_t* __restrict__ bgr,
+                                                  size_t npix) {
+  const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+  if (i >= npix) return;
+  const float* p = rgb + i * ld;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float v = fminf(fmaxf(__ldg(p + c), 0.f), 1.f) * 255.0f;
+    bgr[i * 3 + 2 - c] = (uint8_t)(int)v;
+  }
+}
+
+void launch_rrdb_out(const float* rgb, int ld, uint8_t* bgr, size_t npix, cudaStream_t s) {
+  k_rrdb_out<<<(unsigned)((npix + 255) / 256), 256, 0, s>>>(rgb, ld, bgr, npix);
+}
+
 void launch_sr_tail_cubic(const float* conv, const uint8_t* bgr, int h, int w, uint8_t* dst, int oh, int ow,
                           cudaStream_t s) {
   dim3 g((ow + 31) / 32, (oh + 7) / 8);

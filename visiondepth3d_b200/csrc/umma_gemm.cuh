@@ -34,6 +34,7 @@ enum Epi : int {
   EPI_PATCH = 4,      // x_f32[m+1, n] = acc + bias[n] + pos[m+1, n]       (patch embedding)
   EPI_CONVT = 5,      // ConvTranspose2d(k=s): pixel-shuffle scatter into NHWC f16
   EPI_HEAD = 6,       // depth[m] = relu(sum_n relu(acc+bias)[n] * w3[n] + b3)
+  EPI_SR = 7,         // RRDBNet convs (k_umma_gemm<.., .., true> only): see sr_epilogue_chunk
 };
 
 struct GemmArgs {
@@ -71,6 +72,9 @@ struct GemmArgs {
   // teardown only, 4 = no epilogue (the epilogue warpgroup only releases the staging tile); bit 3 (8): poll barriers
   // with test_wait instead of try_wait
   int dbg;
+  // EPI_SR: second scaled residual and the two residual scales (act 4 = LeakyReLU(0.2) there)
+  const __half* res2_f16;
+  float rs, rs2;
 };
 
 namespace umma {
@@ -282,9 +286,83 @@ __device__ __forceinline__ void pack16(const float (&a)[32], int base, bool relu
 
 }  // namespace umma
 
+// EPI_SR, the epilogue of the RRDBNet convs (a = acc + bias of one 32-column chunk):
+//   out_f32 set:  out_f32[m, n] = a                                  (conv_last, ldc floats per row)
+//   otherwise:    a = res + rs a (res_f16 set); a = res2 + rs2 a (res2_f16 set); a = LeakyReLU_0.2(a) (act 4);
+//                 f16 at out_f16[m, n] (ldc), or with ct_k the pixel-shuffle scatter of EPI_CONVT (nearest x2 + conv
+//                 as four phase convs).  The residuals are read at the output's own offset, so out may alias a
+//                 residual (the RRDB add writes in place): each element is read and then written by one thread.
+__device__ __forceinline__ void sr_epilogue_chunk(const GemmArgs& g, float (&a)[32], const int m, const int n0,
+                                                  const int nvalid, const bool full) {
+  if (g.out_f32) {
+    float* dst = g.out_f32 + (size_t)m * g.ldc + n0;
+    if (full && ((((size_t)m * g.ldc + n0) & 3) == 0)) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) ((float4*)dst)[j] = make_float4(a[4 * j], a[4 * j + 1], a[4 * j + 2], a[4 * j + 3]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 32; ++j)
+        if (j < nvalid) dst[j] = a[j];
+    }
+    return;
+  }
+  size_t o;
+  if (g.ct_k) {
+    const int tap = n0 / g.ct_cout, co = n0 % g.ct_cout;
+    const int dy = tap / g.ct_k, dx = tap % g.ct_k;
+    const int y = m / g.ct_w, x = m % g.ct_w;
+    o = ((size_t)(y * g.ct_k + dy) * (g.ct_w * g.ct_k) + (x * g.ct_k + dx)) * g.ct_cout + co;
+  } else {
+    o = (size_t)m * g.ldc + n0;
+  }
+  const bool vec = full && ((o & 15) == 0);
+#pragma unroll
+  for (int q = 0; q < 2; ++q) {
+    const __half* res = q == 0 ? g.res_f16 : g.res2_f16;
+    if (!res) continue;
+    const float sc = q == 0 ? g.rs : g.rs2;
+    float rv[32];
+    if (vec) {
+      uint32_t u[2][8];
+      umma::ldg_v8(res + o, u[0]);
+      umma::ldg_v8(res + o + 16, u[1]);
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int t = 0; t < 8; ++t) {
+          const float2 f = __half22float2(*(const __half2*)&u[j][t]);
+          rv[16 * j + 2 * t] = f.x;
+          rv[16 * j + 2 * t + 1] = f.y;
+        }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 32; ++j) rv[j] = (j < nvalid) ? __half2float(res[o + j]) : 0.f;
+    }
+#pragma unroll
+    for (int j = 0; j < 32; ++j) a[j] = rv[j] + sc * a[j];
+  }
+  if (g.act == 4) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) a[j] = a[j] > 0.f ? a[j] : 0.2f * a[j];
+  }
+  if (vec) {
+    uint32_t u[8];
+    umma::pack16(a, 0, false, u);
+    umma::stg_v8(g.out_f16 + o, u);
+    umma::pack16(a, 16, false, u);
+    umma::stg_v8(g.out_f16 + o + 16, u);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 32; ++j)
+      if (j < nvalid) g.out_f16[o + j] = __float2half_rn(a[j]);
+  }
+}
+
 // Fused epilogue of one 32-column chunk of one accumulator row (thread == row): v = raw fp32 accumulator bits,
 // m = logical output row, n0 = first output column.  Every
-// register array is indexed with compile-time constants only so the chunk stays in registers.
+// register array is indexed with compile-time constants only so the chunk stays in registers.  kSr: the RRDBNet
+// instantiations, whose only epilogue is EPI_SR (the others compile exactly as without it).
+template <bool kSr>
 __device__ __forceinline__ void gemm_epilogue_chunk(const GemmArgs& g, const uint32_t (&v)[32], const int m, const int z,
                                                     const int n0, const bool row_ok, float& head_acc) {
   if (!row_ok || n0 >= g.N) return;
@@ -308,6 +386,10 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmArgs& g, const uin
   } else {
 #pragma unroll
     for (int j = 0; j < 32; ++j) a[j] = __uint_as_float(v[j]);
+  }
+  if constexpr (kSr) {
+    sr_epilogue_chunk(g, a, m, n0, nvalid, full);
+    return;
   }
   switch (g.epi) {
     case EPI_F16: {
@@ -496,7 +578,7 @@ struct GemmSmem {
   static constexpr int kTotal = STAGES * kStage + kEpi + 1024 /*align*/ + 256 /*barriers*/;
 };
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool kSr = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmArgs g) {
   using S = GemmSmem<BN, STAGES>;
@@ -616,7 +698,7 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             v[4 * i + 2] = __float_as_uint(f.z);
             v[4 * i + 3] = __float_as_uint(f.w);
           }
-          gemm_epilogue_chunk(g, v, m, z, n_blk * BN + ci * 32, row_ok, head_acc);
+          gemm_epilogue_chunk<kSr>(g, v, m, z, n_blk * BN + ci * 32, row_ok, head_acc);
         }
         // DPT head: N == 32 is a single chunk
         if (g.epi == EPI_HEAD && row_ok && n_blk == 0) g.out_f32[m] = fmaxf(head_acc + g.b3p[0], 0.f);

@@ -2044,14 +2044,30 @@ int vd3d_sr_upscale(vd3d_ctx* ctx, vd3d_depth* sr, int n, const uint8_t* const* 
   const bool to_target = fw != w || fh != h;
   const bool blend = p->blend_alpha >= 0.0;
   if (blend && to_target) return fail(ctx, VD3D_ERR_ARG, "blend of two different sizes (cv2.addWeighted raises)");
-  const int nst = 1 + (int)to_orig + (int)to_target + (int)blend;  // kernels after the network
+  int nst = 1 + (int)to_orig + (int)to_target + (int)blend;  // kernels after the network
+  size_t tb = (size_t)(t1w * t1h > w * h ? t1w * t1h : w * h) * 3;
+  // RRDBNet engine: postprocess_esr of the network output [ns rh, ns rw], then the reference's INTER_CUBIC resizes to
+  // (scale rw, scale rh), to (w, h) and to the target one by one, same-size ones skipped (cv2 copies)
+  const int ns = sr_net_scale(sr);
+  int chain_h[3], chain_w[3], nres = 0;
+  if (ns) {
+    int ch = ns * rh, cw = ns * rw;
+    tb = (size_t)ch * cw * 3;
+    const int want_h[3] = {p->scale * rh, h, fh}, want_w[3] = {p->scale * rw, w, fw};
+    for (int q = 0; q < 3; ++q) {
+      if (want_h[q] == ch && want_w[q] == cw) continue;
+      ch = chain_h[nres] = want_h[q];
+      cw = chain_w[nres++] = want_w[q];
+      if ((size_t)ch * cw * 3 > tb) tb = (size_t)ch * cw * 3;
+    }
+    nst = 1 + nres + (int)blend;
+  }
   CK(cudaSetDevice(ctx->device));
   cudaStream_t s = ctx->stream;
   int r;
   FitPlan fp;
   if (pct < 100.0 && (r = plan_fit(ctx, VD3D_FMT_HALF_SBS, w, h, rw, rh, fp, 1))) return r;
   const size_t fb = (size_t)h * w * 3, ob = (size_t)fh * fw * 3;
-  const size_t tb = (size_t)(t1w * t1h > w * h ? t1w * t1h : w * h) * 3;
   void *rs = nullptr, *tmp[2] = {nullptr, nullptr};
   if (pct != 100.0 && (r = sr_buffer(sr, "up.in", (size_t)rw * rh * 3, &rs))) return r;
   if (nst > 1 && (r = sr_buffer(sr, "up.0", tb, &tmp[0]))) return r;
@@ -2085,20 +2101,32 @@ int vd3d_sr_upscale(vd3d_ctx* ctx, vd3d_depth* sr, int n, const uint8_t* const* 
       x = (const uint8_t*)rs;
     }
     const float* cv;
-    if ((r = sr_network(sr, x, rh, rw, num_conv, &cv))) {
+    if ((r = ns ? rrdb_network(sr, x, rh, rw, &cv) : sr_network(sr, x, rh, rw, num_conv, &cv))) {
       ctx->err = std::string("SR engine: ") + vd3d_depth_last_error(sr);
       return r;
     }
     int k = 0;
     auto next = [&]() { return ++k == nst ? o_d : (uint8_t*)tmp[(k - 1) & 1]; };
     uint8_t* cur = next();
-    launch_sr_tail_cubic(cv, x, rh, rw, cur, t1h, t1w, s);
-    if (to_orig) {
+    if (ns) {
+      launch_rrdb_out(cv, 32, cur, (size_t)ns * rh * ns * rw, s);
+      int ch = ns * rh, cw = ns * rw;
+      for (int q = 0; q < nres; ++q) {
+        uint8_t* d = next();
+        launch_resize_cubic_u8(cur, ch, cw, 3, d, chain_h[q], chain_w[q], s);
+        cur = d;
+        ch = chain_h[q];
+        cw = chain_w[q];
+      }
+    } else {
+      launch_sr_tail_cubic(cv, x, rh, rw, cur, t1h, t1w, s);
+    }
+    if (!ns && to_orig) {
       uint8_t* d = next();
       launch_resize_cubic_u8(cur, t1h, t1w, 3, d, h, w, s);
       cur = d;
     }
-    if (to_target) {
+    if (!ns && to_target) {
       uint8_t* d = next();
       launch_resize_cubic_u8(cur, h, w, 3, d, fh, fw, s);
       cur = d;

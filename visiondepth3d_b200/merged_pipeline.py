@@ -6,9 +6,10 @@ addWeighted) as one device call, vd3d_sr_upscale.  start_merged_pipeline drives 
     core_merged_pipeline.start_merged_pipeline(settings, progress_bar, status_label)
 
 The reference loads `weights/RealESR_Gx4_fp16.onnx` through ONNXRuntime (VisionDepth3D.py:1094-1100).  ONNX files are
-not read here: the model is an upstream-format state_dict (`body.{i}.weight` ...: realesr-general-x4v3 /
-realesr-animevideov3), either handed to load_esrgan() or found as `<stem>.pth` / `<stem>.safetensors` next to the
-settings' model_path.  RIFE frame interpolation is not built: its network is not part of the reference (it loads a
+not read here: the model is an upstream-format state_dict, either handed to load_esrgan() or found as `<stem>.pth` /
+`<stem>.safetensors` next to the settings' model_path.  Two architectures are served, told apart by the keys:
+SRVGGNetCompact (`body.{i}.weight` ...: realesr-general-x4v3 / realesr-animevideov3) and RRDBNet (RealESRGAN_x4plus,
+BSRGAN x4 / x2: `conv_first`, `body.{i}.rdb{j}.conv{k}` ... or the old-ESRGAN `RRDB_trunk.{i}.RDB{j}.conv{k}` ...).  RIFE frame interpolation is not built: its network is not part of the reference (it loads a
 `RIFE_fp32.onnx` it does not ship), so rife_session stays None and run_rife returns [] -- what the reference does
 without that file.
 """
@@ -30,8 +31,100 @@ progress_bar = None
 status_label = None
 
 
+# old-ESRGAN / BSRGAN key names -> the basicsr names of the same RRDBNet tensors
+_RRDB_RENAMES = [(re.compile(r"^RRDB_trunk\.(\d+)\.RDB(\d)\.conv(\d)\."), r"body.\1.rdb\2.conv\3."),
+                 (re.compile(r"^trunk_conv\."), "conv_body."), (re.compile(r"^upconv1\."), "conv_up1."),
+                 (re.compile(r"^upconv2\."), "conv_up2."), (re.compile(r"^HRconv\."), "conv_hr.")]
+
+
+def is_rrdb_state_dict(sd):
+    """True for RRDBNet keys (either naming), False for SRVGGNetCompact's."""
+    return any(k.startswith(("conv_first.", "RRDB_trunk.")) for k in sd)
+
+
+def rrdb_layout(sd):
+    """(state dict in the basicsr naming as float32 arrays, nb, net scale) of an RRDBNet state dict in either naming;
+    ValueError unless it is exactly an RRDBNet with num_feat 64, growth 32, 3 input / output channels and one or two
+    up-convs (basicsr's pixel-unshuffle x2 / x1 variants take 12 / 48 input channels and are refused)."""
+    canon = {}
+    for k, v in sd.items():
+        for pat, new in _RRDB_RENAMES:
+            k = pat.sub(new, k)
+        canon[k] = np.asarray(v.detach().cpu().numpy() if hasattr(v, "detach") else v, dtype=np.float32)
+    w = canon.get("conv_first.weight")
+    if w is None or w.ndim != 4:
+        raise ValueError("not an RRDBNet state dict: no conv_first weight")
+    if w.shape[1] != 3:
+        raise ValueError(f"RRDBNet conv_first takes {w.shape[1]} input channels: only the 3-channel x4 / x2 models are "
+                         "served (not the pixel-unshuffle variants)")
+    nb = 0
+    while f"body.{nb}.rdb1.conv1.weight" in canon:
+        nb += 1
+    scale = 4 if "conv_up2.weight" in canon else 2
+    shapes = {"conv_first": (64, 3), "conv_body": (64, 64), "conv_up1": (64, 64), "conv_hr": (64, 64),
+              "conv_last": (3, 64)}
+    if scale == 4:
+        shapes["conv_up2"] = (64, 64)
+    for i in range(nb):
+        for j in range(1, 4):
+            for k in range(1, 6):
+                shapes[f"body.{i}.rdb{j}.conv{k}"] = (32 if k < 5 else 64, 64 + 32 * (k - 1))
+    want = {f"{n}.weight": (co, ci, 3, 3) for n, (co, ci) in shapes.items()}
+    want.update({f"{n}.bias": (co,) for n, (co, _) in shapes.items()})
+    bad = sorted(k for k in set(want) | set(canon) if k not in canon or k not in want or canon[k].shape != want[k])
+    if nb < 1 or bad:
+        raise ValueError(f"not an RRDBNet state dict (num_feat 64, growth 32): {nb} blocks, mismatched keys {bad[:4]}")
+    return canon, nb, scale
+
+
+def _pack3x3(w, cols, cin_pad, rows=None):
+    """Conv weight [Cout, Cin, 3, 3] -> f16 [rows or Cout, 9 * cin_pad], tap-major, input channel c at column cols[c]."""
+    co, ci = w.shape[:2]
+    out = np.zeros((rows or co, 9, cin_pad), dtype=np.float32)
+    out[:co, :, cols] = w.transpose(0, 2, 3, 1).reshape(co, 9, ci)
+    return out.reshape(-1, 9 * cin_pad).astype(np.float16)
+
+
+def _phase_weights(w):
+    """nearest x2 followed by a 3x3 conv (pad 1) as four 3x3 convs on the low-resolution map, one per output phase
+    (py, px): output (2y + py, 2x + px) reads upsampled row 2y + py + dy = low row y + (py + dy) // 2, so the taps that
+    land on one low-resolution pixel add up.  [4 * Cout, Cin, 3, 3], rows (py * 2 + px) * Cout + co."""
+    co = w.shape[0]
+    ph = np.zeros((2, 2) + w.shape, dtype=np.float32)
+    for py in range(2):
+        for px in range(2):
+            for dy in (-1, 0, 1):
+                for dx in (-1, 0, 1):
+                    ph[py, px, :, :, (py + dy) // 2 + 1, (px + dx) // 2 + 1] += w[:, :, dy + 1, dx + 1]
+    return ph.reshape((4 * co,) + w.shape[1:])
+
+
+def pack_rrdb(sd):
+    """(nb, net scale, {engine tensor name: array}) of an RRDBNet state dict in either naming (vd3d_sr_set_rrdb's
+    layouts: dense-block inputs with each 32-channel growth slice padded to 64 channels)."""
+    sd, nb, scale = rrdb_layout(sd)
+    f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
+    t = {"rr.first.w": _pack3x3(sd["conv_first.weight"], [0, 1, 2], 64), "rr.first.b": f32(sd["conv_first.bias"])}
+    for i in range(nb):
+        for j in range(3):
+            for k in range(1, 6):
+                cols = list(range(64)) + [64 * (s + 1) + c for s in range(k - 1) for c in range(32)]
+                n = f"body.{i}.rdb{j + 1}.conv{k}"
+                t[f"rr.{i}.{j}.{k}.w"] = _pack3x3(sd[n + ".weight"], cols, 64 * k)
+                t[f"rr.{i}.{j}.{k}.b"] = f32(sd[n + ".bias"])
+    t["rr.body.w"], t["rr.body.b"] = _pack3x3(sd["conv_body.weight"], list(range(64)), 64), f32(sd["conv_body.bias"])
+    for u in range(1, 2 if scale == 2 else 3):
+        t[f"rr.up{u}.w"] = _pack3x3(_phase_weights(sd[f"conv_up{u}.weight"]), list(range(64)), 64)
+        t[f"rr.up{u}.b"] = f32(np.tile(sd[f"conv_up{u}.bias"], 4))
+    t["rr.hr.w"], t["rr.hr.b"] = _pack3x3(sd["conv_hr.weight"], list(range(64)), 64), f32(sd["conv_hr.bias"])
+    t["rr.last.w"] = _pack3x3(sd["conv_last.weight"], list(range(64)), 64, rows=32)
+    t["rr.last.b"] = f32(np.pad(sd["conv_last.bias"], (0, 29)))
+    return nb, scale, t
+
+
 class SrEngine:
-    """SRVGGNetCompact (num_feat 64, x4) forward on the GPU: BGR u8 [h,w,3] -> BGR u8 [4h,4w,3]."""
+    """Real-ESRGAN network forward on the GPU: SRVGGNetCompact (num_feat 64, x4) or RRDBNet (x4 or x2, chosen by the
+    state dict's keys): BGR u8 [h,w,3] -> BGR u8 [s h, s w, 3], s = net_scale."""
 
     def __init__(self, state_dict, ctx=None, device=0):
         self.lib = _lib.load()
@@ -47,6 +140,14 @@ class SrEngine:
         self.lib.vd3d_depth_last_error.restype = C.c_char_p
         self.lib.vd3d_depth_destroy.argtypes = [C.c_void_p]
         self.lib.vd3d_depth_destroy.restype = None
+        self.net_scale = 4
+        if is_rrdb_state_dict(state_dict):
+            nb, self.net_scale, tensors = pack_rrdb(state_dict)
+            for name, arr in tensors.items():
+                self._set(name, arr)
+            self.check(self.lib.vd3d_sr_set_rrdb(self.h, nb, self.net_scale))
+            self.num_conv = 0  # ignored by RRDBNet engines
+            return
         n_conv_total = len([k for k in state_dict if k.endswith(".bias")])
         self.num_conv = n_conv_total - 2
         for i in range(n_conv_total):
@@ -72,7 +173,7 @@ class SrEngine:
     def upscale(self, frame_bgr):
         f = np.ascontiguousarray(frame_bgr, dtype=np.uint8)
         h, w = f.shape[:2]
-        out = np.empty((4 * h, 4 * w, 3), dtype=np.uint8)
+        out = np.empty((self.net_scale * h, self.net_scale * w, 3), dtype=np.uint8)
         self.check(self.lib.vd3d_sr_forward(self.h, f.ctypes.data, h, w, self.num_conv, out.ctypes.data, _lib.MEM_HOST))
         return out
 
@@ -122,8 +223,51 @@ def random_srvgg_state_dict(num_conv=32, seed=0, num_feat=64):
     return sd
 
 
+def random_rrdb_state_dict(nb=23, scale=4, seed=0, naming="basicsr"):
+    """Random-init RRDBNet weights (num_feat 64, growth 32) in the basicsr naming or, with naming="esrgan", the
+    old-ESRGAN / BSRGAN one, for benchmarks and tests.  He init (LeakyReLU 0.2) on conv_first and the upsampling tail;
+    the dense blocks at a tenth of it, so that the trunk stays a modest residual over conv_first's features as in a
+    trained model; conv_last small with a 0.5 bias, so that a natural frame maps to an image with spread in [0, 1] and
+    little clipping (not a constant or saturated image against which any kernel output would pass)."""
+    rng = np.random.default_rng(seed)
+    gain = 2.0 / (1.0 + 0.2 ** 2)
+    sd = {}
+
+    def conv(name, co, ci, mult, bias_std=0.01):
+        sd[name + ".weight"] = (rng.standard_normal((co, ci, 3, 3)) * mult * (gain / (9 * ci)) ** 0.5).astype(np.float32)
+        sd[name + ".bias"] = (rng.standard_normal(co) * bias_std).astype(np.float32)
+
+    conv("conv_first", 64, 3, 1.0)
+    for i in range(nb):
+        for j in range(1, 4):
+            for k in range(1, 6):
+                conv(f"body.{i}.rdb{j}.conv{k}", 32 if k < 5 else 64, 64 + 32 * (k - 1), 0.1)
+    conv("conv_body", 64, 64, 0.1)
+    for u in range(1, 2 if scale == 2 else 3):
+        conv(f"conv_up{u}", 64, 64, 1.0)
+    conv("conv_hr", 64, 64, 1.0)
+    conv("conv_last", 3, 64, 0.035)
+    sd["conv_last.bias"] = np.full(3, 0.5, np.float32)
+    if naming == "esrgan":
+        old = {"conv_body.": "trunk_conv.", "conv_up1.": "upconv1.", "conv_up2.": "upconv2.", "conv_hr.": "HRconv."}
+        out = {}
+        for k, v in sd.items():
+            m = re.match(r"body\.(\d+)\.rdb(\d)\.conv(\d)\.(.*)", k)
+            if m:
+                k = f"RRDB_trunk.{m.group(1)}.RDB{m.group(2)}.conv{m.group(3)}.{m.group(4)}"
+            for a, b in old.items():
+                if k.startswith(a):
+                    k = b + k[len(a):]
+            out[k] = v
+        sd = out
+    elif naming != "basicsr":
+        raise ValueError(f"naming must be 'basicsr' or 'esrgan', not {naming!r}")
+    return sd
+
+
 def load_esrgan(state_dict=None, num_conv=32, seed=0):
-    """Make run_esrgan serve a model: an upstream SRVGGNetCompact state_dict (tensors or arrays), or random-init."""
+    """Make run_esrgan serve a model: an upstream SRVGGNetCompact or RRDBNet state_dict (tensors or arrays), or
+    random-init SRVGGNetCompact."""
     global esrgan_session
     if state_dict is None:
         state_dict = random_srvgg_state_dict(num_conv, seed)
@@ -339,6 +483,12 @@ def _read_state_dict(path):
             sd = sd[key]
             break
     sd = {k: (v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)) for k, v in sd.items()}
+    if is_rrdb_state_dict(sd):
+        try:
+            rrdb_layout(sd)
+        except ValueError as e:
+            raise ValueError(f"{path}: {e}") from None
+        return sd
     n = len([k for k in sd if k.startswith("body.") and k.endswith(".bias")])
     ok = n >= 3
     for i in range(n if ok else 0):
@@ -360,7 +510,7 @@ def _model_files(model_path):
 def load_esrgan_from(model_path):
     """The settings' model_path: the path itself when it is a .pth / .safetensors file, else <stem>.pth or
     <stem>.safetensors next to it (the ONNX file is not read).  None, with the reference's message, when there is
-    none; a state dict that is not SRVGGNetCompact raises."""
+    none; a state dict that is neither SRVGGNetCompact nor RRDBNet raises."""
     global esrgan_session
     for f in _model_files(model_path):
         if os.path.exists(f):
