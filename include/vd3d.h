@@ -190,7 +190,7 @@ int vd3d_render_clip(vd3d_ctx* ctx, int n, const uint8_t* const* frames, const u
                      uint8_t* const* outs, int mem, vd3d_frame_info* infos);
 
 /* depth + stereo in one pipelined loop: depth of frame i is inferred on the GPU by `depth`
- * (vd3d_depth_infer_device) and handed to the DIBR loop in HBM as a 1-channel u8 map -- the
+ * (vd3d_depth_infer_batch_device) and handed to the DIBR loop in HBM as a 1-channel u8 map -- the
  * in-memory replacement of the reference's XVID depth-video round trip (SURVEY 0.5). */
 int vd3d_render_clip_depth(vd3d_ctx* ctx, vd3d_depth* depth, int n, const uint8_t* const* frames, int src_h,
                            int src_w, const vd3d_render_params* rp, uint8_t* const* outs, int mem);
@@ -284,11 +284,9 @@ int vd3d_check_config(vd3d_ctx* ctx, int src_h, int src_w, const vd3d_render_par
  * luma, contrast around 0.5, additive brightness, clamp) */
 int vd3d_color_grade(vd3d_ctx* ctx, const float* rgb, int h, int w, double saturation, double contrast,
                      double brightness, float* out, int mem);
-/* cv2.resize(u8 plane [h,w], (ow,oh), interpolation=cv2.INTER_CUBIC): the resize the depth writer applies to the u8
- * depth (core/render_depth.py:1917, 193): float32 bicubic (A = -0.75), round half to even */
-int vd3d_resize_cubic_u8(vd3d_ctx* ctx, const uint8_t* src, int h, int w, uint8_t* dst, int oh, int ow, int mem);
-/* the same on interleaved u8 [h,w,ch] (ch <= 4): run_esrgan's INTER_CUBIC chain on BGR frames
- * (core/merged_pipeline.py:262-266) */
+/* cv2.resize(u8 [h,w,ch], (ow,oh), interpolation=cv2.INTER_CUBIC), ch <= 4: float32 bicubic (A = -0.75), round half to
+ * even.  ch = 1: the resize the depth writer applies to the u8 depth (core/render_depth.py:1917, 193); ch = 3:
+ * run_esrgan's INTER_CUBIC chain on BGR frames (core/merged_pipeline.py:262-266) */
 int vd3d_resize_cubic(vd3d_ctx* ctx, const uint8_t* src, int h, int w, int ch, uint8_t* dst, int oh, int ow, int mem);
 /* cv2.addWeighted(a, alpha, b, beta, 0) on n u8 values: blend_images (core/merged_pipeline.py:233-238) */
 int vd3d_add_weighted(vd3d_ctx* ctx, const uint8_t* a, double alpha, const uint8_t* b, double beta, size_t n, uint8_t* dst,
@@ -345,18 +343,13 @@ void vd3d_depth_add_launches(vd3d_depth* e, uint64_t n); /* bookkeeping for CUDA
 int vd3d_depth_set_tensor(vd3d_depth* e, const char* name, const void* host_data, size_t bytes);
 /* pixel_values f32 [3,image_h,image_w] -> predicted_depth f32 [image_h,image_w] */
 int vd3d_depth_forward(vd3d_depth* e, const float* pixel_values, float* depth_out, int mem);
-/* the whole depth stage of the reference for one frame: DPT image processor (antialiased
- * bicubic to image_h x image_w, /255, mean/std) -> forward -> post_process_depth_estimation
- * (bicubic back to h x w) -> convert_depth_to_grayscale min-max u8 (core/render_depth.py:
- * 1113-1119, 605-611).  _device: all pointers on the GPU, enqueued without synchronising
- * (this is what vd3d_render_clip uses for the in-memory depth -> stereo handoff). */
-int vd3d_depth_infer(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, float* depth_f32, uint8_t* depth_u8,
-                     int invert);
-int vd3d_depth_infer_device(vd3d_depth* e, const uint8_t* frame_bgr_dev, int h, int w, uint8_t* depth_u8_dev,
-                            float* depth_f32_dev_or_null, int invert);
-/* The same for B (1..8) frames of one size with ONE batched forward: the token-wise GEMMs see the stacked token
- * matrix of all frames (the reference hands the whole list to the HF pipeline too, core/render_depth.py:1113-1119).
- * Arrays of B pointers; depth_f32 / depth_u8 (or single entries) may be NULL. */
+/* the whole depth stage of the reference for B (1..8) u8 BGR frames [h,w,3] of one size (h, w >= 16): DPT image
+ * processor (antialiased bicubic to image_h x image_w, /255, mean/std) -> ONE batched forward -> per frame
+ * post_process_depth_estimation (bicubic back to h x w) -> convert_depth_to_grayscale min-max u8
+ * (core/render_depth.py:1113-1119, 605-611).  The token-wise GEMMs see the stacked token matrix of all frames (the
+ * reference hands the whole list to the HF pipeline too).  Arrays of B pointers; depth_f32 / depth_u8 (or single
+ * entries) may be NULL.  _device: all pointers on the GPU, enqueued without synchronising (this is what
+ * vd3d_render_clip_depth uses for the in-memory depth -> stereo handoff). */
 int vd3d_depth_infer_batch(vd3d_depth* e, int B, const uint8_t* const* frames_bgr, int h, int w, float* const* depth_f32,
                            uint8_t* const* depth_u8, int invert);
 int vd3d_depth_infer_batch_device(vd3d_depth* e, int B, const uint8_t* const* frames_bgr_dev, int h, int w,

@@ -76,8 +76,8 @@ def test_vr_loop_vs_oracle_and_golden(R, golden_dir):
 
 
 def test_resize_cubic_u8_matches_oracle():
-    """vd3d_resize_cubic_u8 (the depth writer's cv2 INTER_CUBIC) against the cv2-pinned oracle: same float32
-    arithmetic, exact."""
+    """resize_cubic_u8 (vd3d_resize_cubic on one channel: the depth writer's cv2 INTER_CUBIC) against the cv2-pinned
+    oracle: same float32 arithmetic, exact."""
     from visiondepth3d_b200 import render_depth as RD
     rng = np.random.default_rng(9)
     for (w, h, ow, oh) in ((924, 518, 1920, 1080), (100, 70, 133, 91), (640, 360, 320, 180), (37, 23, 80, 50), (64, 48, 64, 48)):

@@ -72,8 +72,8 @@ def test_infer_images_mixed_sources_equal_single_images(weights):
 def test_infer_images_with_inference_size(weights):
     """With an inference size: Pillow resize, the engine's depth at that size, INTER_CUBIC back -- the host
     composition of hf_batch_safe_pipe + convert_depth_to_grayscale + the resize of the depth writer, from the engine's
-    own pixels.  The resize back is the project's cv2.resize restatement (vd3d_resize_cubic_u8, what the depth-video
-    pass applies), which stays within 1 LSB of the installed cv2 on < 0.2 % of the pixels."""
+    own pixels.  The resize back is the project's cv2.resize restatement (resize_cubic_u8, what the depth-video pass
+    applies), which stays within 1 LSB of the installed cv2 on < 0.2 % of the pixels."""
     import torch
     from PIL import Image
     from visiondepth3d_b200 import render_depth as RD

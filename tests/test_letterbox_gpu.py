@@ -223,6 +223,43 @@ def test_tracked_depth_frames_equal_repad_of_plain_depth(depth_model):
             assert (got[i][: b[0]] == got[i][0, 0]).all()
 
 
+class _Bars:
+    """Stand-in tracker: fixed bars after every batch; records the index of each batch's first frame."""
+
+    def __init__(self, bars):
+        self.bars, self.first = bars, []
+
+    def update_batch(self, frames, first_idx=0):
+        self.first.append(first_idx)
+        return [self.bars] * len(frames)
+
+
+@pytest.mark.parametrize("inf,bars,invert", [((224, 126), None, False), ((224, 126), (12, 10), True),
+                                             ((448, 252), None, True), ((448, 252), (12, 10), False)])
+def test_depth_frames_with_inference_size_equal_host_composition(depth_model, inf, bars, invert):
+    """process_video2 with an inference size: each frame through hf_batch_safe_pipe at that size (Pillow resize in
+    the pipe), convert_depth_to_grayscale, inversion, INTER_CUBIC back to the frame size and the re-pad to the
+    tracked bars."""
+    from PIL import Image
+    from tests.test_letterbox_cpu import _Cap
+    RD = depth_model
+    frames = L.track_frames()[:10]
+    tracker = _Bars(bars) if bars else None
+    got = list(RD.iter_depth_frames(_Cap(frames, 2), 320, 180, invert, inf, batch_size=4, tracker=tracker))
+    assert len(got) == len(frames)
+    if tracker:
+        assert tracker.first == [1, 5, 9]
+    for f, g in zip(frames, got):
+        d = RD.hf_batch_safe_pipe([Image.fromarray(f[..., ::-1].copy())], inf)[0]["predicted_depth"]
+        want = RD.convert_depth_to_grayscale(d)
+        if invert:
+            want = 255 - want
+        want = RD.resize_cubic_u8(want, 320, 180)
+        if bars:
+            want = RD.letterbox_repad(want, *bars)
+        assert np.array_equal(g, want)
+
+
 def test_depth_video_end_to_end(depth_model, tmp_path):
     import cv2
     RD = depth_model

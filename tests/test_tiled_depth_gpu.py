@@ -336,7 +336,8 @@ class _Bars:
         return [self.bars] * len(frames)
 
 
-@pytest.mark.parametrize("inf,tracker,invert", [(None, None, False), ((160, 96), None, True), (None, (8, 6), False)])
+@pytest.mark.parametrize("inf,tracker,invert", [(None, None, False), ((160, 96), None, True), (None, (8, 6), False),
+                                                ((160, 96), (8, 6), False)])
 def test_video_pass_tiled(model, inf, tracker, invert):
     from PIL import Image
     R = model

@@ -99,12 +99,12 @@ SYMBOLS = [
     "vd3d_set_exact", "vd3d_get_exact", "vd3d_graphs_active",
     "vd3d_pixel_shift", "vd3d_plan_sizes", "vd3d_render_frame", "vd3d_render_clip",
     "vd3d_sharpen", "vd3d_dof_grade", "vd3d_struct_size", "vd3d_pack", "vd3d_fit_eye", "vd3d_area_table", "vd3d_area_linear_table", "vd3d_heal",
-    "vd3d_profile", "vd3d_profile_collect", "vd3d_check_config", "vd3d_color_grade", "vd3d_resize_cubic_u8", "vd3d_resize_cubic", "vd3d_add_weighted",
+    "vd3d_profile", "vd3d_profile_collect", "vd3d_check_config", "vd3d_color_grade", "vd3d_resize_cubic", "vd3d_add_weighted",
     "vd3d_sr_create", "vd3d_sr_forward", "vd3d_sr_upscale", "vd3d_sr_set_rrdb",
     # depth forward (bound in depth_engine.py)
     "vd3d_depth_create", "vd3d_depth_destroy", "vd3d_depth_last_error", "vd3d_depth_launch_count",
     "vd3d_depth_set_tensor", "vd3d_depth_forward", "vd3d_depth_get_buffer", "vd3d_gemm_f16", "vd3d_gemm_bench", "vd3d_conv_f16",
-    "vd3d_depth_infer", "vd3d_depth_infer_device", "vd3d_depth_infer_batch", "vd3d_depth_infer_batch_device",
+    "vd3d_depth_infer_batch", "vd3d_depth_infer_batch_device",
     "vd3d_set_depth_batch", "vd3d_get_depth_batch", "vd3d_render_clip_depth", "vd3d_depth_add_launches", "vd3d_depth_clone", "vd3d_release_depth",
     "vd3d_depth_profile", "vd3d_depth_profile_collect", "vd3d_depth_profile_spans",
     "vd3d_advance_state", "vd3d_state_bytes", "vd3d_export_state", "vd3d_import_state",
@@ -223,8 +223,6 @@ def load():
     lib.vd3d_release_depth.restype = i
     lib.vd3d_check_config.argtypes = [vp, i, i, C.POINTER(RenderParams)]
     lib.vd3d_check_config.restype = i
-    lib.vd3d_resize_cubic_u8.argtypes = [vp, u8p, i, i, u8p, i, i, i]
-    lib.vd3d_resize_cubic_u8.restype = i
     lib.vd3d_resize_cubic.argtypes = [vp, u8p, i, i, i, u8p, i, i, i]
     lib.vd3d_resize_cubic.restype = i
     lib.vd3d_add_weighted.argtypes = [vp, u8p, C.c_double, u8p, C.c_double, C.c_size_t, u8p, i]

@@ -1436,46 +1436,4 @@ int vd3d_sr_forward(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, int n
   return VD3D_OK;
 }
 
-// frame (BGR u8 [h,w,3], DEVICE) -> processor -> forward -> bicubic back to (h,w) -> min-max u8 [h,w]
-// (hf pipeline + convert_depth_to_grayscale, core/render_depth.py:1113-1119,605-611,1907-1917).
-// Enqueues on the engine stream without synchronising; depth_f32_or_null receives the resized
-// float depth ("predicted_depth" of the pipe protocol).
-int vd3d_depth_infer_device(vd3d_depth* e, const uint8_t* frame_bgr_dev, int h, int w, uint8_t* depth_u8_dev,
-                            float* depth_f32_or_null, int invert) {
-  if (!e || !frame_bgr_dev || h < 16 || w < 16) return VD3D_ERR_ARG;
-  const int IH = e->cfg.image_h, IW = e->cfg.image_w;
-  cudaStream_t s = e->stream;
-  void *tmp, *rgb, *px, *up, *mm, *dd;
-  int r;
-  if ((r = get_buf(e, "pp.tmp", (size_t)h * IW * 3, &tmp)) || (r = get_buf(e, "pp.rgb", (size_t)IH * IW * 3, &rgb)) ||
-      (r = get_buf(e, "px", (size_t)3 * IH * IW * 4, &px)) || (r = get_buf(e, "depth", (size_t)IH * IW * 4, &dd)) ||
-      (r = get_buf(e, "post.up", (size_t)h * w * 4, &up)) || (r = get_buf(e, "post.mm", 64, &mm)))
-    return r;
-  launch_preprocess(frame_bgr_dev, h, w, (uint8_t*)tmp, (uint8_t*)rgb, (float*)px, IH, IW, s);
-  e->launches += 3;
-  if ((r = vd3d_depth_forward(e, (const float*)px, (float*)dd, VD3D_MEM_DEVICE))) return r;
-  float* upt = depth_f32_or_null ? depth_f32_or_null : (float*)up;
-  launch_depth_post((const float*)dd, IH, IW, upt, h, w, (unsigned*)mm, depth_u8_dev, invert, s);
-  e->launches += depth_u8_dev ? 3 : 2;
-  DCK(cudaGetLastError());
-  return VD3D_OK;
-}
-
-// host-buffer form (pipe protocol / tests): frame BGR u8 [h,w,3] -> depth f32 [h,w] and/or u8 [h,w]
-int vd3d_depth_infer(vd3d_depth* e, const uint8_t* frame_bgr, int h, int w, float* depth_f32, uint8_t* depth_u8,
-                     int invert) {
-  if (!e || !frame_bgr) return VD3D_ERR_ARG;
-  void *fd, *u8d, *f32d;
-  int r;
-  if ((r = get_buf(e, "io.frame", (size_t)h * w * 3, &fd)) || (r = get_buf(e, "io.u8", (size_t)h * w, &u8d)) ||
-      (r = get_buf(e, "io.f32", (size_t)h * w * 4, &f32d)))
-    return r;
-  DCK(cudaMemcpyAsync(fd, frame_bgr, (size_t)h * w * 3, cudaMemcpyHostToDevice, e->stream));
-  if ((r = vd3d_depth_infer_device(e, (const uint8_t*)fd, h, w, (uint8_t*)u8d, (float*)f32d, invert))) return r;
-  if (depth_f32) DCK(cudaMemcpyAsync(depth_f32, f32d, (size_t)h * w * 4, cudaMemcpyDeviceToHost, e->stream));
-  if (depth_u8) DCK(cudaMemcpyAsync(depth_u8, u8d, (size_t)h * w, cudaMemcpyDeviceToHost, e->stream));
-  DCK(cudaStreamSynchronize(e->stream));
-  return VD3D_OK;
-}
-
 }  // extern "C"

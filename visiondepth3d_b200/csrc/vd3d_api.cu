@@ -1999,9 +1999,6 @@ int vd3d_resize_cubic(vd3d_ctx* ctx, const uint8_t* src, int h, int w, int ch, u
   ctx->launches += 1;
   return stage_finish(ctx, dst, o_d, (size_t)oh * ow * ch, mem);
 }
-int vd3d_resize_cubic_u8(vd3d_ctx* ctx, const uint8_t* src, int h, int w, uint8_t* dst, int oh, int ow, int mem) {
-  return vd3d_resize_cubic(ctx, src, h, w, 1, dst, oh, ow, mem);
-}
 
 // cv2.addWeighted(a, alpha, b, 1 - alpha... any beta, 0) on n bytes (blend_images, core/merged_pipeline.py:233-238)
 int vd3d_add_weighted(vd3d_ctx* ctx, const uint8_t* a, double alpha, const uint8_t* b, double beta, size_t n, uint8_t* dst,

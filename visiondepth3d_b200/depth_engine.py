@@ -50,10 +50,6 @@ def _bind(lib):
     lib.vd3d_gemm_bench.restype = i
     lib.vd3d_conv_f16.argtypes = [vp, vp, i, i, i, vp, i, i, vp, i, vp]
     lib.vd3d_conv_f16.restype = i
-    lib.vd3d_depth_infer.argtypes = [vp, vp, i, i, vp, vp, i]
-    lib.vd3d_depth_infer.restype = i
-    lib.vd3d_depth_infer_device.argtypes = [vp, vp, i, i, vp, vp, i]
-    lib.vd3d_depth_infer_device.restype = i
     lib.vd3d_depth_infer_batch.argtypes = [vp, i, C.POINTER(vp), i, i, C.POINTER(vp), C.POINTER(vp), i]
     lib.vd3d_depth_infer_batch.restype = i
     lib.vd3d_depth_infer_batch_device.argtypes = [vp, i, C.POINTER(vp), i, i, C.POINTER(vp), C.POINTER(vp), i]
@@ -122,17 +118,9 @@ class DepthEngine:
     def infer(self, frame_bgr, invert=False, check_size=True):
         """BGR u8 [h,w,3] -> (predicted_depth f32 [h,w] resized to the frame, min-max u8 [h,w]).
         check_size: refuse frames whose DPT processed size differs from the one this engine was built for (the HF
-        processor would pick another keep-aspect /14 size, so the depth would differ from the reference's)."""
-        f = np.ascontiguousarray(frame_bgr, dtype=np.uint8)
-        h, w = f.shape[:2]
-        if check_size and processed_size(w, h) != (self.image_h, self.image_w):
-            raise ValueError(f"engine built for processed size {(self.image_h, self.image_w)}, a {w}x{h} frame needs "
-                             f"{processed_size(w, h)}")
-        d32 = np.empty((h, w), dtype=np.float32)
-        d8 = np.empty((h, w), dtype=np.uint8)
-        self.check(self.lib.vd3d_depth_infer(self.h, f.ctypes.data, h, w, d32.ctypes.data, d8.ctypes.data,
-                                             int(bool(invert))))
-        return d32, d8
+        processor would pick another keep-aspect /14 size, so the depth would differ from the reference's).
+        The one-frame case of infer_batch."""
+        return self.infer_batch([frame_bgr], invert, check_size)[0]
 
     def infer_batch(self, frames_bgr, invert=False, check_size=True):
         """List of same-shape BGR frames -> list of (predicted_depth f32, min-max u8), up to 8 frames per batched
@@ -221,14 +209,27 @@ class DepthEngine:
         return list(zip(u8, f32 if want_f32 else [None] * n))
 
     def resize_pil(self, rgb, width, height):
-        """vd3d_depth_resize_pil: Image.fromarray(rgb).resize((width, height), Image.BICUBIC) on a host RGB u8
-        [h,w,3] array, on the GPU."""
-        src = np.ascontiguousarray(rgb, dtype=np.uint8)
-        if src.ndim != 3 or src.shape[2] != 3:
-            raise ValueError("expected an RGB uint8 array [h, w, 3]")
-        out = np.empty((int(height), int(width), 3), np.uint8)
-        self.check(self.lib.vd3d_depth_resize_pil(self.h, src.ctypes.data, src.shape[0], src.shape[1], out.ctypes.data,
-                                                  int(height), int(width), _lib.MEM_HOST))
+        """vd3d_depth_resize_pil: Image.fromarray(rgb).resize((width, height), Image.BICUBIC) on an RGB u8 [h,w,3]
+        image, on the GPU.  Pillow resamples each channel on its own, so BGR works the same.  rgb: a host array, or a
+        CUDA uint8 tensor (the result is then a CUDA tensor)."""
+        import torch
+        if isinstance(rgb, torch.Tensor) and rgb.is_cuda:
+            src = rgb.contiguous()
+            if src.dtype != torch.uint8 or src.dim() != 3 or src.shape[2] != 3:
+                raise ValueError("expected a CUDA uint8 tensor [h, w, 3]")
+            out = torch.empty((int(height), int(width), 3), dtype=torch.uint8, device=src.device)
+            ptr, mem = (lambda t: t.data_ptr()), _lib.MEM_DEVICE
+            torch.cuda.current_stream().synchronize()  # the image may come from work queued on torch's stream
+        else:
+            src = np.ascontiguousarray(rgb, dtype=np.uint8)
+            if src.ndim != 3 or src.shape[2] != 3:
+                raise ValueError("expected an RGB uint8 array [h, w, 3]")
+            out = np.empty((int(height), int(width), 3), np.uint8)
+            ptr, mem = (lambda a: a.ctypes.data), _lib.MEM_HOST
+        self.check(self.lib.vd3d_depth_resize_pil(self.h, ptr(src), int(src.shape[0]), int(src.shape[1]), ptr(out),
+                                                  int(height), int(width), mem))
+        if mem == _lib.MEM_DEVICE:
+            self.ctx.check(self.lib.vd3d_sync(self.ctx.h))
         return out
 
     def get_buffer(self, name, shape, dtype):

@@ -191,15 +191,15 @@ def convert_depth_to_grayscale(depth):
 
 
 def resize_cubic_u8(plane, width, height):
-    """cv2.resize(u8 plane, (width, height), interpolation=cv2.INTER_CUBIC) on the GPU (vd3d_resize_cubic_u8): the
-    resize the reference's depth writer applies to the u8 depth (core/render_depth.py:1917, 193)."""
+    """cv2.resize(u8 plane, (width, height), interpolation=cv2.INTER_CUBIC) on the GPU (vd3d_resize_cubic, one
+    channel): the resize the reference's depth writer applies to the u8 depth (core/render_depth.py:1917, 193)."""
     from . import _lib
     ctx = _lib.default_context(0)
     src = np.ascontiguousarray(plane, dtype=np.uint8)
     assert src.ndim == 2
     out = np.empty((int(height), int(width)), dtype=np.uint8)
-    ctx.check(ctx.lib.vd3d_resize_cubic_u8(ctx.h, src.ctypes.data, src.shape[0], src.shape[1], out.ctypes.data,
-                                           int(height), int(width), _lib.MEM_HOST))
+    ctx.check(ctx.lib.vd3d_resize_cubic(ctx.h, src.ctypes.data, src.shape[0], src.shape[1], 1, out.ctypes.data,
+                                        int(height), int(width), _lib.MEM_HOST))
     return out
 
 
@@ -897,84 +897,68 @@ def _repad_device(src, top, bottom, dst):
                                            _lib.MEM_DEVICE))
 
 
-_staging = {}  # (n, H, W) -> pinned host tensor [n, H, W, 3]: the upload buffer of the tracked batch path
-
-
-def _tracked_batch_device(batch, W, H, invert, tracker):
-    """One tracked depth batch on one device copy of its frames: the tracker's statistics and the depth forward read
-    the same upload, the re-pad works on the device depth, and the written planes come back in one download."""
-    eng = _engine_for(W, H)
-    n = len(batch)
-    host = _staging.get((n, H, W))
-    if host is None:
-        host = _staging[(n, H, W)] = torch.empty((n, H, W, 3), dtype=torch.uint8).pin_memory()
-    hn = host.numpy()
-    for k, f in enumerate(batch):
-        hn[k] = f
-    dev = host.to("cuda", non_blocking=True)
-    bars = tracker.update_batch(dev)[-1]  # synchronises torch's stream before the statistics read `dev`
-    d8 = torch.empty((n, H, W), dtype=torch.uint8, device=dev.device)
-    for i0 in range(0, n, 8):
-        idx = range(i0, min(n, i0 + 8))
-        eng.infer_batch_u8_device([dev[k].data_ptr() for k in idx], H, W, [d8[k].data_ptr() for k in idx], invert)
-    if bars[0] or bars[1]:
-        out = torch.empty_like(d8)
-        for k in range(n):
-            _repad_device(d8[k], bars[0], bars[1], out[k])
-        d8 = out
-    eng.ctx.check(eng.lib.vd3d_sync(eng.ctx.h))
-    return list(d8.cpu().numpy())
+_staging = {}  # (n, H, W) -> pinned host tensor [n, H, W, 3]: the upload buffer of the depth-video pass
 
 
 def iter_depth_frames(cap, W, H, invert=False, inference_size=None, batch_size=8, max_frames=None, tracker=None,
                       status=None):
     """The u8 depth planes depth_video_from_video writes, in order, from the frames cap.read() returns.  With a
     bootstrapped `tracker` (ignore_letterbox_bars), every frame read goes through tracker.update and each frame of a
-    batch is re-padded with the bars the tracker holds after the batch's last frame, as process_video2 does."""
-    from PIL import Image
+    batch is re-padded with the bars the tracker holds after the batch's last frame, as process_video2 does.
+    Each batch goes to the GPU in one pinned upload; the tracker's statistics and the depth read that copy, the re-pad
+    works on the device depth, and the planes come back in one download."""
+    from . import _lib
     n, batch = 0, []
     tiled = USE_TILED_DEPTH
 
-    def flush_tiled():
-        # process_video2's tiled branch: _run_pipe_or_tile -> infer_depth_tile on each (PIL-resized) frame, then
-        # _normalize_to_u8 to the frame size and the re-pad, in one vd3d_depth_tiled call per batch
-        bars = tracker.update_batch(batch, n + 1)[-1] if tracker is not None else (0, 0)
-        frames = batch
-        if inference_size is not None:
-            frames = [np.ascontiguousarray(np.asarray(Image.fromarray(f[..., ::-1].copy()).resize(
-                tuple(inference_size), Image.BICUBIC))[..., ::-1]) for f in batch]
-        th, tw = frames[0].shape[:2]
-        d8s, _, ranges = depth_tiled(frames, tw, th, (W, H), invert)
-        _print_tile_log(tw, th, ranges)
-        batch.clear()
-        if bars[0] or bars[1]:
-            d8s = [letterbox_repad(d8, bars[0], bars[1]) for d8 in d8s]
-        return d8s
-
     def flush():
-        if tiled:
-            return flush_tiled()
-        if tracker is not None and inference_size is None:
-            d8s = _tracked_batch_device(batch, W, H, invert, tracker)
-            batch.clear()
-            return d8s
-        bars = (0, 0)
-        if tracker is not None:
-            bars = tracker.update_batch(batch, n + 1)[-1]
-        if inference_size is None:
-            d8s = [d8 for _, d8 in _engine_for(W, H).infer_batch(batch, invert=invert)]
-        else:
-            d8s = []
-            pil = [Image.fromarray(f[..., ::-1].copy()) for f in batch]
-            for res in hf_batch_safe_pipe(pil, inference_size):
-                d8 = convert_depth_to_grayscale(res["predicted_depth"])
-                if invert:
-                    d8 = 255 - d8
-                d8s.append(resize_cubic_u8(d8, W, H))
+        k = len(batch)
+        host = _staging.get((k, H, W))
+        if host is None:
+            host = _staging[(k, H, W)] = torch.empty((k, H, W, 3), dtype=torch.uint8).pin_memory()
+        hn = host.numpy()
+        for i, f in enumerate(batch):
+            hn[i] = f
         batch.clear()
-        if tracker is not None and (bars[0] or bars[1]):
-            d8s = [letterbox_repad(d8, bars[0], bars[1]) for d8 in d8s]
-        return d8s
+        dev = host.to("cuda", non_blocking=True)
+        torch.cuda.current_stream().synchronize()  # the library reads `dev` on its own stream
+        bars = tracker.update_batch(dev, n + 1)[-1] if tracker is not None else (0, 0)
+        if tiled:
+            # process_video2's tiled branch: _run_pipe_or_tile -> infer_depth_tile on each (Pillow-resized) frame,
+            # then _normalize_to_u8 to the frame size, in one vd3d_depth_tiled call
+            frames, tw, th = dev, W, H
+            if inference_size is not None:
+                tw, th = int(inference_size[0]), int(inference_size[1])
+                eng = _plan_for(tw, th, TILE_SIZE, TILE_PAD).engines()[0]  # the resize needs no weights: any engine
+                frames = torch.stack([eng.resize_pil(f, tw, th) for f in dev])
+            d8, _, ranges = depth_tiled(frames, tw, th, (W, H), invert)
+            _print_tile_log(tw, th, ranges)
+        elif inference_size is None:
+            eng = _engine_for(W, H)
+            d8 = torch.empty((k, H, W), dtype=torch.uint8, device=dev.device)
+            for i0 in range(0, k, 8):
+                idx = range(i0, min(k, i0 + 8))
+                eng.infer_batch_u8_device([dev[i].data_ptr() for i in idx], H, W, [d8[i].data_ptr() for i in idx],
+                                          invert)
+        else:
+            # hf_batch_safe_pipe at inference_size -> convert_depth_to_grayscale -> invert -> INTER_CUBIC back to the
+            # frame size: the composition vd3d_depth_infer_images computes for RGB images
+            eng = _engine_for(*inference_size)
+            rgb = dev.flip(-1)
+            planes = []
+            for i0 in range(0, k, 8):
+                chunk = list(rgb[i0:i0 + 8])
+                planes += [u8 for u8, _ in eng.infer_images(chunk, [inference_size] * len(chunk), invert)]
+            d8 = torch.stack(planes)
+            torch.cuda.current_stream().synchronize()  # stacked on torch's stream; the re-pad reads it on the library's
+        if bars[0] or bars[1]:
+            out = torch.empty_like(d8)
+            for i in range(k):
+                _repad_device(d8[i], bars[0], bars[1], out[i])
+            d8 = out
+        ctx = _lib.default_context(0)
+        ctx.check(ctx.lib.vd3d_sync(ctx.h))
+        return list(d8.cpu().numpy())
 
     while not cancel_requested.is_set():
         ok, frame = cap.read()
