@@ -126,7 +126,7 @@ typedef struct {
 
 /* sizeof() of the ABI structs, so bindings can verify their layout:
  * 0 vd3d_shift_params, 1 vd3d_render_params, 2 vd3d_size_plan, 3 vd3d_frame_info, 4 vd3d_upscale_params,
- * 5 vd3d_tile */
+ * 5 vd3d_tile, 6 vd3d_depth_config_ex */
 int vd3d_struct_size(int which);
 
 /* ---- lifecycle ------------------------------------------------------- */
@@ -327,6 +327,24 @@ typedef struct {
   int32_t image_h, image_w;      /* processed size, multiples of 14 (518 x 924 for 16:9) */
 } vd3d_depth_config;
 int vd3d_depth_create(const vd3d_depth_config* cfg, void* cuda_stream, vd3d_depth** out);
+/* ---- other ViT-DPT depth checkpoints: the family, patch size, LayerNorm epsilon and image processor of the model.
+ * VD3D_DEPTH_DA_V2 with patch 14, eps 1e-6, bicubic and ImageNet mean / std is what vd3d_depth_create builds.
+ * VD3D_DEPTH_DPT is DPT-Large (transformers DPTForDepthEstimation, "Intel/dpt-large"): ViT without LayerScale, taps =
+ * the raw residual stream after the base.taps layers (no final LayerNorm), the project readout GELU(Linear(cat(tok,
+ * cls))) per tap (weights "ro{i}.wt" f16 [D, D] token half, "ro{i}.wc" f16 [D, D] CLS half, "ro{i}.b" f32 [D]),
+ * and the processor's fixed image_h x image_w target (square, a multiple of 32).  The processed size of any frame is
+ * then the engine's own, so vd3d_depth_infer_images accepts every input size. */
+enum { VD3D_DEPTH_DA_V2 = 0, VD3D_DEPTH_DPT = 1 };
+typedef struct {
+  vd3d_depth_config base; /* image_h / image_w multiples of patch */
+  int32_t family;         /* VD3D_DEPTH_DA_V2 or VD3D_DEPTH_DPT */
+  int32_t patch;          /* 14 (DINOv2) or 16 (ViT-L/16) */
+  float ln_eps;           /* 1e-6 (DINOv2) or 1e-12 (DPT) */
+  int32_t resample;       /* the processor's PIL resample code: 3 bicubic or 2 bilinear */
+  float mean[3], std[3];  /* the processor's normalisation */
+} vd3d_depth_config_ex;
+/* VD3D_ERR_ARG for any other family, patch or resample, a DPT size that is not square or not a multiple of 32 */
+int vd3d_depth_create_ex(const vd3d_depth_config_ex* cfg, void* cuda_stream, vd3d_depth** out);
 void vd3d_depth_destroy(vd3d_depth* e);
 /* CUDA-event timing of the fc1 GEMM launches (k_umma_gemm<128,4>; M = tokens, N = 4*hidden, K = hidden) */
 int vd3d_depth_profile(vd3d_depth* e, int enable);

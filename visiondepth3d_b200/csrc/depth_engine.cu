@@ -51,6 +51,10 @@ struct DTensor {
 
 struct vd3d_depth {
   vd3d_depth_config cfg;
+  // model family, patch, LayerNorm epsilon and image processor (vd3d_depth_create_ex; DA-V2 defaults otherwise)
+  int family = VD3D_DEPTH_DA_V2, patch = 14;
+  float ln_eps = 1e-6f;
+  PreprocParams pre = kImagenetBicubic;
   cudaStream_t stream = nullptr;
   std::string err;
   std::map<std::string, DTensor> w;    // weights by name
@@ -231,18 +235,35 @@ int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
 extern "C" {
 
-int vd3d_depth_create(const vd3d_depth_config* cfg, void* stream, vd3d_depth** out) {
-  if (!cfg || !out) return VD3D_ERR_ARG;
+int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth** out) {
+  if (!x || !out) return VD3D_ERR_ARG;
   *out = nullptr;
   if (!load_encode()) return VD3D_ERR_CUDA;
-  if (cfg->hidden % 128 || cfg->hidden > 1024 || cfg->hidden / cfg->heads != 64 || cfg->fusion % 64 ||
-      cfg->image_h % 14 || cfg->image_w % 14)
+  const vd3d_depth_config* cfg = &x->base;
+  const bool dpt = x->family == VD3D_DEPTH_DPT;
+  if ((x->family != VD3D_DEPTH_DA_V2 && !dpt) || (x->patch != 14 && x->patch != 16) ||
+      (x->resample != 2 && x->resample != 3) || !(x->ln_eps > 0.f) || cfg->heads < 1)
     return VD3D_ERR_ARG;
+  if (cfg->hidden % 128 || cfg->hidden > 1024 || cfg->hidden / cfg->heads != 64 || cfg->fusion % 64 ||
+      cfg->image_h % x->patch || cfg->image_w % x->patch)
+    return VD3D_ERR_ARG;
+  // DPT reshapes the tokens as a square grid, and every fusion x2 must land on the next map: an even square grid
+  if (dpt && (cfg->image_h != cfg->image_w || cfg->image_h % 32)) return VD3D_ERR_ARG;
+  for (int c = 0; c < 3; ++c)
+    if (!(x->std[c] != 0.f)) return VD3D_ERR_ARG;
   vd3d_depth* e = new vd3d_depth();
   e->cfg = *cfg;
+  e->family = x->family;
+  e->patch = x->patch;
+  e->ln_eps = x->ln_eps;
+  e->pre.bilinear = x->resample == 2;
+  for (int c = 0; c < 3; ++c) {
+    e->pre.mean[c] = x->mean[c];
+    e->pre.std[c] = x->std[c];
+  }
   e->stream = (cudaStream_t)stream;
-  e->ph = cfg->image_h / 14;
-  e->pw = cfg->image_w / 14;
+  e->ph = cfg->image_h / x->patch;
+  e->pw = cfg->image_w / x->patch;
   e->ntok = e->ph * e->pw + 1;
   e->npad = round_up(e->ntok, 128);
   if (e->ntok > 3072) {
@@ -251,6 +272,22 @@ int vd3d_depth_create(const vd3d_depth_config* cfg, void* stream, vd3d_depth** o
   }
   *out = e;
   return VD3D_OK;
+}
+
+int vd3d_depth_create(const vd3d_depth_config* cfg, void* stream, vd3d_depth** out) {
+  if (!cfg || !out) return VD3D_ERR_ARG;
+  vd3d_depth_config_ex x;
+  memset(&x, 0, sizeof x);
+  x.base = *cfg;
+  x.family = VD3D_DEPTH_DA_V2;
+  x.patch = 14;
+  x.ln_eps = 1e-6f;
+  x.resample = 3;
+  for (int c = 0; c < 3; ++c) {
+    x.mean[c] = kImagenetBicubic.mean[c];
+    x.std[c] = kImagenetBicubic.std[c];
+  }
+  return vd3d_depth_create_ex(&x, stream, out);
 }
 
 // device timing of the fc1 GEMM launches (k_umma_gemm<128,4>, M=tokens, N=4D, K=D): bench.py roofline
@@ -315,6 +352,10 @@ int vd3d_depth_clone(vd3d_depth* src, void* stream, vd3d_depth** out) {
   if (!src || !out) return VD3D_ERR_ARG;
   vd3d_depth* e = new vd3d_depth();
   e->cfg = src->cfg;
+  e->family = src->family;
+  e->patch = src->patch;
+  e->ln_eps = src->ln_eps;
+  e->pre = src->pre;
   e->stream = (cudaStream_t)stream;
   e->w = src->w;
   e->owns_weights = false;
@@ -504,7 +545,9 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
   const int D = c.hidden, L = c.layers, Hh = c.heads, F = c.fusion;
   const int ph = e->ph, pw = e->pw, NT = e->ntok, NP = e->npad, NPATCH = ph * pw;
   const int IH = c.image_h, IW = c.image_w;
-  const int KPE = 592;
+  const int P = e->patch;
+  const int KPE = round_up(3 * P * P, 16);  // 592 for patch 14 (588 + zero columns), 768 for 16
+  const bool dpt = e->family == VD3D_DEPTH_DPT;
   int r;
   char nm[96];
   // ---- buffers ----
@@ -528,7 +571,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     return r;
   for (int b = 0; b < B; ++b) {
     float* xb = (float*)x + (size_t)b * NP * D;
-    launch_patch_im2col(px_dev[b], IH, IW, ph, pw, (__half*)ape, KPE, s);
+    launch_patch_im2col(px_dev[b], IH, IW, ph, pw, (__half*)ape, KPE, P, s);
     GemmArgs g = base_args(NPATCH, D, KPE, EPI_PATCH);
     g.out_f32 = xb;
     g.bias = pe_b;
@@ -561,7 +604,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
         (r = W(e, nmf("ls2"), &ls2, D)))
       return r;
     int sp_ = e->span_begin("ln", s);
-    launch_layernorm((const float*)x, MT, D, g1, b1, (__half*)xn, 0, s);
+    launch_layernorm((const float*)x, MT, D, g1, b1, (__half*)xn, 0, e->ln_eps, s);
     e->span_end(sp_, s);
     sp_ = e->span_begin("qkv", s);
     {
@@ -599,7 +642,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     }
     e->span_end(sp_, s);
     sp_ = e->span_begin("ln", s);
-    launch_layernorm((const float*)x, MT, D, g2, b2, (__half*)xn, 0, s);
+    launch_layernorm((const float*)x, MT, D, g2, b2, (__half*)xn, 0, e->ln_eps, s);
     e->span_end(sp_, s);
     sp_ = e->span_begin("fc1", s);
     {
@@ -634,7 +677,36 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     }
     e->span_end(sp_, s);
     e->launches += 2;
-    if (tap_idx < 4 && c.taps[tap_idx] == l + 1) {
+    if (tap_idx < 4 && c.taps[tap_idx] == l + 1 && dpt) {
+      // DPT: the raw residual stream (hidden_states[l + 1]), then the project readout over the patch rows of all
+      // images in one GEMM: GELU(W_t tok + (W_c cls_b + bias)), the CLS term computed once per image
+      void *tp, *cb, *ro;
+      const __half *wt, *wc;
+      const float* rb;
+      const int MR = B * NPATCH;
+      snprintf(nm, sizeof nm, "ro%d.wt", tap_idx);
+      if ((r = W(e, nm, &wt, (size_t)D * D))) return r;
+      snprintf(nm, sizeof nm, "ro%d.wc", tap_idx);
+      if ((r = W(e, nm, &wc, (size_t)D * D))) return r;
+      snprintf(nm, sizeof nm, "ro%d.b", tap_idx);
+      if ((r = W(e, nm, &rb, D))) return r;
+      snprintf(nm, sizeof nm, "tap%d", tap_idx);
+      if ((r = get_buf(e, nm, (size_t)round_up(MR, 128) * D * 2, &tp))) return r;
+      snprintf(nm, sizeof nm, "ro%d.c", tap_idx);
+      if ((r = get_buf(e, nm, (size_t)B * D * 4, &cb))) return r;
+      snprintf(nm, sizeof nm, "ro%d", tap_idx);
+      if ((r = get_buf(e, nm, (size_t)round_up(MR, 128) * D * 2, &ro))) return r;
+      launch_tap_f16((const float*)x, NP, NPATCH, D, B, (__half*)tp, s);
+      launch_readout_cls((const float*)x, NP, D, B, wc, rb, D, (float*)cb, s);
+      e->launches += 2;
+      GemmArgs g = base_args(MR, D, D, EPI_READOUT);
+      g.out_f16 = (__half*)ro;
+      g.img_bias = (const float*)cb;
+      g.npad = NPATCH;
+      g.ldc = D;
+      if ((r = gemm(e, (const __half*)tp, D, wt, D, g))) return r;
+      ++tap_idx;
+    } else if (tap_idx < 4 && c.taps[tap_idx] == l + 1) {
       // backbone output: final LayerNorm applied (apply_layernorm=True), CLS dropped by the neck
       const float *ng, *nb;
       if ((r = W(e, "norm.g", &ng, D)) || (r = W(e, "norm.b", &nb, D))) return r;
@@ -642,7 +714,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
         void* tp;
         snprintf(nm, sizeof nm, "tap%d.%d", tap_idx, b);
         if ((r = get_buf(e, nm, (size_t)round_up(NPATCH, 128) * D * 2, &tp))) return r;
-        launch_layernorm((const float*)x + (size_t)b * NP * D, NPATCH, D, ng, nb, (__half*)tp, 1, s);
+        launch_layernorm((const float*)x + (size_t)b * NP * D, NPATCH, D, ng, nb, (__half*)tp, 1, e->ln_eps, s);
         e->launches++;
       }
       ++tap_idx;
@@ -685,8 +757,14 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     if ((r = W(e, nm, &pw_, (size_t)CP * D))) return r;
     snprintf(nm, sizeof nm, "r%d.proj.b", i);
     if ((r = W(e, nm, &pb, CP))) return r;
-    snprintf(nm, sizeof nm, "tap%d.%d", i, b);
-    void *tp = e->buf[nm].p, *rp, *rs = nullptr;
+    void *tp, *rp, *rs = nullptr;
+    if (dpt) {  // image b's rows of the readout output
+      snprintf(nm, sizeof nm, "ro%d", i);
+      tp = (__half*)e->buf[nm].p + (size_t)b * NPATCH * D;
+    } else {
+      snprintf(nm, sizeof nm, "tap%d.%d", i, b);
+      tp = e->buf[nm].p;
+    }
     snprintf(nm, sizeof nm, "r%d.p", i);
     if ((r = get_buf(e, bname(nm), (size_t)round_up(NPATCH, 128) * CP * 2, &rp))) return r;
     {
@@ -1018,7 +1096,7 @@ int vd3d_depth_infer_batch_device(vd3d_depth* e, int B, const uint8_t* const* fr
     if ((r = get_buf(e, nm, (size_t)3 * IH * IW * 4, &px))) return r;
     snprintf(nm, sizeof nm, b ? "depth.%d" : "depth", b);
     if ((r = get_buf(e, nm, (size_t)IH * IW * 4, &dd))) return r;
-    launch_preprocess(frames_bgr_dev[b], h, w, (uint8_t*)tmp, (uint8_t*)rgb, (float*)px, IH, IW, s);
+    launch_preprocess(frames_bgr_dev[b], h, w, (uint8_t*)tmp, (uint8_t*)rgb, (float*)px, IH, IW, s, 1, e->pre);
     e->launches += 3;
     pxs[b] = (const float*)px;
     dds[b] = (float*)dd;
@@ -1114,8 +1192,8 @@ int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_r
   for (int b = 0; b < B; ++b) {
     const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
     if (!images_rgb[b] || !depth_u8[b] || sh < 1 || sw < 1 || ih < 16 || iw < 16) return VD3D_ERR_ARG;
-    int ph, pw;
-    processed_size(ih, iw, &ph, &pw);
+    int ph = IH, pw = IW;  // DPT's processor resizes every input to its fixed size
+    if (e->family == VD3D_DEPTH_DA_V2) processed_size(ih, iw, &ph, &pw);
     if (ph != IH || pw != IW) {
       char m[160];
       snprintf(m, sizeof m, "image %d: a %dx%d input maps to processed size %dx%d, the engine serves %dx%d", b, iw, ih,
@@ -1181,7 +1259,7 @@ int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_r
       if ((r = pil_resize(e, img, sh, sw, (uint8_t*)ptmp, (uint8_t*)rs, ih, iw))) return r;
       img = (const uint8_t*)rs;
     }
-    launch_preprocess(img, ih, iw, (uint8_t*)tmp, (uint8_t*)rgb, (float*)pxs[b], IH, IW, s, 0);
+    launch_preprocess(img, ih, iw, (uint8_t*)tmp, (uint8_t*)rgb, (float*)pxs[b], IH, IW, s, 0, e->pre);
     e->launches += 3;
   }
   if ((r = forward_core(e, B, pxs, dds))) return r;
@@ -1240,6 +1318,8 @@ namespace vd3d {
 cudaStream_t sr_stream(vd3d_depth* e) { return e->stream; }
 
 int sr_net_scale(vd3d_depth* e) { return e->rr_scale; }
+
+int depth_family(vd3d_depth* e) { return e->family; }
 
 int sr_buffer(vd3d_depth* e, const char* name, size_t bytes, void** out) { return get_buf(e, name, bytes, out); }
 

@@ -12,7 +12,7 @@
 namespace vd3d {
 
 // ---------------------------------------------------------------------------
-// LayerNorm (eps 1e-6) over the fp32 residual stream -> f16 GEMM operand.  One warp per row.
+// LayerNorm (eps 1e-6 for DINOv2, 1e-12 for DPT's ViT) over the fp32 residual stream -> f16 GEMM operand.  One warp per row.
 // row_off / out_off: skip the CLS row when producing the backbone feature maps.
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_layernorm(const float* __restrict__ x, int rows, int D,
@@ -57,17 +57,67 @@ __global__ void __launch_bounds__(256) k_layernorm(const float* __restrict__ x, 
     }
 }
 
-// patch embedding im2col: pixel_values f32 [3, IH, IW] -> A f16 [ph*pw, kpad], k = c*196 + dy*14 + dx
+// patch embedding im2col: pixel_values f32 [3, IH, IW] -> A f16 [ph*pw, kpad], k = c*P*P + dy*P + dx (P = patch)
 __global__ void __launch_bounds__(256) k_patch_im2col(const float* __restrict__ px, int IH, int IW, int ph, int pw,
-                                                      __half* __restrict__ A, int kpad) {
+                                                      __half* __restrict__ A, int kpad, int P) {
   int idx = blockIdx.x * 256 + threadIdx.x;
-  int total = ph * pw * 588;
+  const int kk = 3 * P * P;
+  int total = ph * pw * kk;
   if (idx >= total) return;
-  int k = idx % 588, t = idx / 588;
-  int c = k / 196, rr = k % 196, dy = rr / 14, dx = rr % 14;
+  int k = idx % kk, t = idx / kk;
+  int c = k / (P * P), rr = k % (P * P), dy = rr / P, dx = rr % P;
   int py = t / pw, pxx = t % pw;
-  float v = px[((size_t)c * IH + (py * 14 + dy)) * IW + (pxx * 14 + dx)];
+  float v = px[((size_t)c * IH + (py * P + dy)) * IW + (pxx * P + dx)];
   A[(size_t)t * kpad + k] = __float2half_rn(v);
+}
+
+// the un-normalised taps of DPT's ViT: patch rows of the fp32 residual stream of B images ([B * npad, D], CLS at row
+// 0 of each image) -> f16 [B * npatch, D], image after image.  Without LayerScale the residual stream of a ViT-L
+// carries channels in the hundreds; values beyond the f16 range saturate to +-65504 instead of becoming inf.
+__global__ void __launch_bounds__(256) k_tap_f16(const float* __restrict__ x, int npad, int npatch, int D, int images,
+                                                 __half* __restrict__ out) {
+  const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;  // one thread per 4 channels
+  const int d4 = D / 4;
+  if (i >= (size_t)images * npatch * d4) return;
+  const int c4 = (int)(i % d4);
+  const size_t row = i / d4;
+  const int b = (int)(row / npatch), t = (int)(row % npatch);
+  const float4 v = ((const float4*)(x + ((size_t)b * npad + 1 + t) * D))[c4];
+  const float L = 65504.f;
+  __half2 h0 = __floats2half2_rn(fminf(fmaxf(v.x, -L), L), fminf(fmaxf(v.y, -L), L));
+  __half2 h1 = __floats2half2_rn(fminf(fmaxf(v.z, -L), L), fminf(fmaxf(v.w, -L), L));
+  uint2 u;
+  u.x = *(uint32_t*)&h0;
+  u.y = *(uint32_t*)&h1;
+  ((uint2*)(out + row * D))[c4] = u;
+}
+
+// the CLS half of DPT's project readout: c[b, n] = bias[n] + sum_k Wc[n, k] * x[b * npad, k] for every image b, with
+// the fp32 CLS row of the residual stream and Wc f16 [N, D].  One warp per output column n, all images at once.
+__global__ void __launch_bounds__(256) k_readout_cls(const float* __restrict__ x, int npad, int D, int images,
+                                                     const __half* __restrict__ wc, const float* __restrict__ bias,
+                                                     int N, float* __restrict__ c) {
+  const int n = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (n >= N) return;
+  float acc[8];
+#pragma unroll
+  for (int b = 0; b < 8; ++b) acc[b] = 0.f;
+  const __half* w = wc + (size_t)n * D;
+  for (int k = lane * 2; k < D; k += 64) {
+    const float2 wf = __half22float2(*(const __half2*)(w + k));
+#pragma unroll
+    for (int b = 0; b < 8; ++b)
+      if (b < images) {
+        const float2 xv = *(const float2*)(x + (size_t)b * npad * D + k);
+        acc[b] = fmaf(wf.x, xv.x, fmaf(wf.y, xv.y, acc[b]));
+      }
+  }
+#pragma unroll
+  for (int b = 0; b < 8; ++b) {
+    float v = acc[b];
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0 && b < images) c[(size_t)b * N + n] = v + bias[n];
+  }
 }
 
 // x[0, :] = cls + pos[0, :]
@@ -143,9 +193,10 @@ __global__ void __launch_bounds__(256) k_relu_f16(const __half* __restrict__ in,
 }
 
 // ---------------------------------------------------------------------------
-// DPT image processor (transformers 5.5 image_processing_dpt.py): antialiased bicubic
-// resize of the uint8 frame (separable, width first, uint8 intermediate, like ATen's
-// _upsample_bicubic2d_aa on uint8), then rescale 1/255 and ImageNet mean/std.
+// DPT image processor (transformers 5.5 image_processing_dpt.py): antialiased bicubic (or, for a
+// checkpoint whose processor names resample 2, bilinear) resize of the uint8 frame (separable, width
+// first, uint8 intermediate, like ATen's _upsample_{bicubic,bilinear}2d_aa on uint8), then rescale 1/255
+// and mean/std (ImageNet for Depth-Anything, 0.5 for DPT).
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ float cubic_aa(float x) {  // a = -0.5 (PIL / ATen antialias filter)
   const float a = -0.5f;
@@ -156,23 +207,25 @@ __device__ __forceinline__ float cubic_aa(float x) {  // a = -0.5 (PIL / ATen an
 }
 
 // one axis of the antialiased resize on interleaved u8 [rows, in, 3] -> [rows, out, 3] (axis = x)
-// or [in, cols, 3] -> [out, cols, 3] (axis = y)
+// or [in, cols, 3] -> [out, cols, 3] (axis = y); bilinear: the triangle filter (support 1) instead of the cubic
 __global__ void __launch_bounds__(256) k_resize_aa_u8(const uint8_t* __restrict__ src, int IH, int IW,
                                                       uint8_t* __restrict__ dst, int OH, int OW, int axis_y,
-                                                      int bgr_to_rgb) {
+                                                      int bgr_to_rgb, int bilinear) {
   int ox = blockIdx.x * 32 + (threadIdx.x & 31);
   int oy = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (ox >= OW || oy >= OH) return;
   const int in_sz = axis_y ? IH : IW, out_sz = axis_y ? OH : OW, o = axis_y ? oy : ox;
   float scale = (float)in_sz / (float)out_sz;
-  float support = (scale >= 1.0f) ? 2.0f * scale : 2.0f;
+  const float base = bilinear ? 1.0f : 2.0f;
+  float support = (scale >= 1.0f) ? base * scale : base;
   float invscale = (scale >= 1.0f) ? 1.0f / scale : 1.0f;
   float center = scale * ((float)o + 0.5f);
   int xmin = max(0, (int)(center - support + 0.5f));
   int xmax = min(in_sz, (int)(center + support + 0.5f));
   float wsum = 0.f, acc[3] = {0.f, 0.f, 0.f};
   for (int j = xmin; j < xmax; ++j) {
-    float w = cubic_aa(((float)j - center + 0.5f) * invscale);
+    const float t = ((float)j - center + 0.5f) * invscale;
+    float w = bilinear ? fmaxf(0.f, 1.0f - fabsf(t)) : cubic_aa(t);
     wsum += w;
     const uint8_t* q = axis_y ? src + ((size_t)j * IW + ox) * 3 : src + ((size_t)oy * IW + j) * 3;
     acc[0] += w * (float)q[0];
@@ -219,14 +272,13 @@ __global__ void __launch_bounds__(256) k_resize_pil_u8(const uint8_t* __restrict
 
 // u8 RGB interleaved [H, W, 3] -> f32 CHW normalised pixel_values
 __global__ void __launch_bounds__(256) k_normalize_px(const uint8_t* __restrict__ rgb, int H, int W,
-                                                      float* __restrict__ px) {
+                                                      float* __restrict__ px, PreprocParams pp) {
   int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= H * W) return;
-  const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     float v = (float)rgb[(size_t)i * 3 + c] * (1.0f / 255.0f);
-    px[(size_t)c * H * W + i] = (v - mean[c]) / stdv[c];
+    px[(size_t)c * H * W + i] = (v - pp.mean[c]) / pp.std[c];
   }
 }
 
@@ -346,11 +398,11 @@ __global__ void __launch_bounds__(256) k_add_relu_f16(const __half* __restrict__
 // launchers
 // ---------------------------------------------------------------------------
 void launch_preprocess(const uint8_t* frame_bgr, int H, int W, uint8_t* tmp_u8, uint8_t* rgb_u8, float* px, int OH,
-                       int OW, cudaStream_t s, int swap_rb) {
+                       int OW, cudaStream_t s, int swap_rb, const PreprocParams& pp) {
   dim3 g1((OW + 31) / 32, (H + 7) / 8), g2((OW + 31) / 32, (OH + 7) / 8);
-  k_resize_aa_u8<<<g1, 256, 0, s>>>(frame_bgr, H, W, tmp_u8, H, OW, 0, 0);       // width pass
-  k_resize_aa_u8<<<g2, 256, 0, s>>>(tmp_u8, H, OW, rgb_u8, OH, OW, 1, swap_rb);  // height pass (+BGR->RGB)
-  k_normalize_px<<<(OH * OW + 255) / 256, 256, 0, s>>>(rgb_u8, OH, OW, px);
+  k_resize_aa_u8<<<g1, 256, 0, s>>>(frame_bgr, H, W, tmp_u8, H, OW, 0, 0, pp.bilinear);       // width pass
+  k_resize_aa_u8<<<g2, 256, 0, s>>>(tmp_u8, H, OW, rgb_u8, OH, OW, 1, swap_rb, pp.bilinear);  // height pass (+BGR->RGB)
+  k_normalize_px<<<(OH * OW + 255) / 256, 256, 0, s>>>(rgb_u8, OH, OW, px, pp);
 }
 void launch_resize_pil_u8(const uint8_t* src, int IH, int IW, uint8_t* dst, int OH, int OW, const int* tab, int ksize,
                           int axis_y, cudaStream_t s) {
@@ -369,12 +421,21 @@ void launch_add_relu_f16(const __half* a, const __half* b, __half* sum, __half* 
   k_add_relu_f16<<<(unsigned)((n8 + 255) / 256), 256, 0, s>>>(a, b, sum, sum_relu, n8);
 }
 void launch_layernorm(const float* x, int rows, int D, const float* g, const float* b, __half* out, int row_off,
-                      cudaStream_t s) {
-  k_layernorm<<<(rows + 7) / 8, 256, 0, s>>>(x, rows, D, g, b, out, row_off, 1e-6f);
+                      float eps, cudaStream_t s) {
+  k_layernorm<<<(rows + 7) / 8, 256, 0, s>>>(x, rows, D, g, b, out, row_off, eps);
 }
-void launch_patch_im2col(const float* px, int IH, int IW, int ph, int pw, __half* A, int kpad, cudaStream_t s) {
-  int total = ph * pw * 588;
-  k_patch_im2col<<<(total + 255) / 256, 256, 0, s>>>(px, IH, IW, ph, pw, A, kpad);
+void launch_patch_im2col(const float* px, int IH, int IW, int ph, int pw, __half* A, int kpad, int patch,
+                         cudaStream_t s) {
+  int total = ph * pw * 3 * patch * patch;
+  k_patch_im2col<<<(total + 255) / 256, 256, 0, s>>>(px, IH, IW, ph, pw, A, kpad, patch);
+}
+void launch_tap_f16(const float* x, int npad, int npatch, int D, int images, __half* out, cudaStream_t s) {
+  const size_t total = (size_t)images * npatch * (D / 4);
+  k_tap_f16<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(x, npad, npatch, D, images, out);
+}
+void launch_readout_cls(const float* x, int npad, int D, int images, const __half* wc, const float* bias, int N,
+                        float* c, cudaStream_t s) {
+  k_readout_cls<<<(N + 7) / 8, 256, 0, s>>>(x, npad, D, images, wc, bias, N, c);
 }
 void launch_set_cls(float* x, const float* cls, const float* pos, int D, cudaStream_t s) {
   k_set_cls<<<(D + 255) / 256, 256, 0, s>>>(x, cls, pos, D);

@@ -7,15 +7,28 @@
 
 namespace vd3d {
 struct GemmArgs;
+// the image processor's filter and normalisation (Depth-Anything-V2: bicubic, ImageNet mean / std)
+struct PreprocParams {
+  int bilinear;  // 0: bicubic (PIL resample 3), 1: bilinear (2)
+  float mean[3], std[3];
+};
+constexpr PreprocParams kImagenetBicubic = {0, {0.485f, 0.456f, 0.406f}, {0.229f, 0.224f, 0.225f}};
 void launch_layernorm(const float* x, int rows, int D, const float* g, const float* b, __half* out, int row_off,
-                      cudaStream_t s);
-void launch_patch_im2col(const float* px, int IH, int IW, int ph, int pw, __half* A, int kpad, cudaStream_t s);
+                      float eps, cudaStream_t s);
+// patch embedding im2col for patch x patch patches: A f16 [ph*pw, kpad], K = 3*patch*patch
+void launch_patch_im2col(const float* px, int IH, int IW, int ph, int pw, __half* A, int kpad, int patch,
+                         cudaStream_t s);
+// DPT: the patch rows of B images' fp32 residual stream -> f16 [B*npatch, D] (saturating), and the per-image CLS half
+// of the project readout c [B, N] = Wc . cls_b + bias
+void launch_tap_f16(const float* x, int npad, int npatch, int D, int images, __half* out, cudaStream_t s);
+void launch_readout_cls(const float* x, int npad, int D, int images, const __half* wc, const float* bias, int N,
+                        float* c, cudaStream_t s);
 void launch_set_cls(float* x, const float* cls, const float* pos, int D, cudaStream_t s);
 void launch_im2col_s2(const __half* in, int H, int W, int C, int ldc, __half* out, int OH, int OW, cudaStream_t s);
 void launch_upsample_ac(const __half* in, int H, int W, int C, __half* out, int OH, int OW, cudaStream_t s);
 // DPT image processor: BGR u8 [H,W,3] -> pixel_values f32 [3,OH,OW] (3 launches); swap_rb = 0 takes RGB input
 void launch_preprocess(const uint8_t* frame_bgr, int H, int W, uint8_t* tmp_u8, uint8_t* rgb_u8, float* px, int OH,
-                       int OW, cudaStream_t s, int swap_rb = 1);
+                       int OW, cudaStream_t s, int swap_rb = 1, const PreprocParams& pp = kImagenetBicubic);
 // one pass of Pillow's 8-bit bicubic resize on u8 [IH,IW,3] (axis_y = 0: width, 1: height) with a host-built table
 void launch_resize_pil_u8(const uint8_t* src, int IH, int IW, uint8_t* dst, int OH, int OW, const int* tab, int ksize,
                           int axis_y, cudaStream_t s);

@@ -35,6 +35,7 @@ enum Epi : int {
   EPI_CONVT = 5,      // ConvTranspose2d(k=s): pixel-shuffle scatter into NHWC f16
   EPI_HEAD = 6,       // depth[m] = relu(sum_n relu(acc+bias)[n] * w3[n] + b3)
   EPI_SR = 7,         // RRDBNet convs (k_umma_gemm<.., .., true> only): see sr_epilogue_chunk
+  EPI_READOUT = 8,    // out_f16[m, n] = GELU(acc + img_bias[m / npad, n])  (DPT project readout, per-image CLS term)
 };
 
 struct GemmArgs {
@@ -75,6 +76,8 @@ struct GemmArgs {
   // EPI_SR: second scaled residual and the two residual scales (act 4 = LeakyReLU(0.2) there)
   const __half* res2_f16;
   float rs, rs2;
+  // EPI_READOUT: [images, N] f32, the image of row m is m / npad (npad = patch rows per image)
+  const float* img_bias;
 };
 
 namespace umma {
@@ -547,6 +550,25 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmArgs& g, const uin
 #pragma unroll
       for (int j = 0; j < 32; ++j)
         if (j < nvalid) head_acc += fmaxf(a[j], 0.f) * __ldg(g.w3 + n0 + j);
+    } break;
+    case EPI_READOUT: {
+      // the token half of Linear(cat(tok, cls)) is this GEMM; the CLS half plus the bias arrives per image
+      const float* cb = g.img_bias + (size_t)(m / g.npad) * g.N + n0;
+      const size_t o = (size_t)m * g.ldc + n0;
+#pragma unroll
+      for (int j = 0; j < 32; ++j)
+        if (j < nvalid) a[j] = umma::gelu_erf(a[j] + __ldg(cb + j));
+      if (full && ((o & 15) == 0)) {
+        uint32_t u[8];
+        umma::pack16(a, 0, false, u);
+        umma::stg_v8(g.out_f16 + o, u);
+        umma::pack16(a, 16, false, u);
+        umma::stg_v8(g.out_f16 + o + 16, u);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 32; ++j)
+          if (j < nvalid) g.out_f16[o + j] = __float2half_rn(a[j]);
+      }
     } break;
   }
 }

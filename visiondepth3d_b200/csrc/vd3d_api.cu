@@ -879,6 +879,7 @@ int vd3d_struct_size(int which) {
     case 3: return (int)sizeof(vd3d_frame_info);
     case 4: return (int)sizeof(vd3d_upscale_params);
     case 5: return (int)sizeof(vd3d_tile);
+    case 6: return (int)sizeof(vd3d_depth_config_ex);
     default: return -1;
   }
 }
@@ -1766,6 +1767,8 @@ int vd3d_render_clip(vd3d_ctx* ctx, int n, const uint8_t* const* frames, const u
 int vd3d_render_clip_depth(vd3d_ctx* ctx, vd3d_depth* depth, int n, const uint8_t* const* frames, int src_h,
                            int src_w, const vd3d_render_params* rp, uint8_t* const* outs, int mem) {
   if (!ctx || !depth || !frames || !rp || !outs || n < 0) return fail(ctx, VD3D_ERR_ARG, "null argument");
+  if (depth_family(depth) != VD3D_DEPTH_DA_V2)
+    return fail(ctx, VD3D_ERR_UNSUPPORTED, "the joined depth -> stereo path serves Depth-Anything-V2 engines only");
   CK(cudaSetDevice(ctx->device));
   vd3d_size_plan pl;
   int r = vd3d_plan_sizes(src_w, src_h, rp, &pl);
@@ -2713,6 +2716,8 @@ int vd3d_depth_tiled(vd3d_ctx* ctx, vd3d_depth* const* engines, int n_classes, i
     return fail(ctx, VD3D_ERR_ARG, "bad argument");
   for (int c = 0; c < n_classes; ++c) {
     if (!engines[c]) return fail(ctx, VD3D_ERR_ARG, "missing engine");
+    if (depth_family(engines[c]) != VD3D_DEPTH_DA_V2)
+      return fail(ctx, VD3D_ERR_UNSUPPORTED, "tiled depth serves Depth-Anything-V2 engines only");
     // the gather and the blend run on ctx->stream: an engine on another stream would race them
     if (sr_stream(engines[c]) != ctx->stream)
       return fail(ctx, VD3D_ERR_ARG, "the depth engines must be created on vd3d_stream(ctx)");

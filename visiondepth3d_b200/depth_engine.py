@@ -5,7 +5,7 @@ import sys as _sys
 import numpy as np
 
 from . import _lib
-from .depth_weights import CONFIGS, prepare
+from .depth_weights import CONFIGS, DPT_CONFIGS, DPT_PROCESSOR, dpt_processed_size, prepare, prepare_dpt
 
 
 def processed_size(width, height, target=518, multiple=14):
@@ -26,12 +26,25 @@ class DepthConfig(C.Structure):
                 ("neck", C.c_int32 * 4), ("fusion", C.c_int32), ("image_h", C.c_int32), ("image_w", C.c_int32)]
 
 
+class DepthConfigEx(C.Structure):
+    """vd3d_depth_config_ex: the model family, patch, LayerNorm epsilon and image processor."""
+    _fields_ = [("base", DepthConfig), ("family", C.c_int32), ("patch", C.c_int32), ("ln_eps", C.c_float),
+                ("resample", C.c_int32), ("mean", C.c_float * 3), ("std", C.c_float * 3)]
+
+
+FAMILY_DA_V2, FAMILY_DPT = "da-v2", "dpt"
+
+
 def _bind(lib):
     if getattr(lib, "_depth_bound", False):
         return
     vp, i = C.c_void_p, C.c_int
     lib.vd3d_depth_create.argtypes = [C.POINTER(DepthConfig), vp, C.POINTER(vp)]
     lib.vd3d_depth_create.restype = i
+    lib.vd3d_depth_create_ex.argtypes = [C.POINTER(DepthConfigEx), vp, C.POINTER(vp)]
+    lib.vd3d_depth_create_ex.restype = i
+    if lib.vd3d_struct_size(6) != C.sizeof(DepthConfigEx):
+        raise OSError(f"libvd3d ABI mismatch for DepthConfigEx: {lib.vd3d_struct_size(6)} != {C.sizeof(DepthConfigEx)}")
     lib.vd3d_depth_destroy.argtypes = [vp]
     lib.vd3d_depth_destroy.restype = None
     lib.vd3d_depth_last_error.argtypes = [vp]
@@ -71,29 +84,59 @@ def _bind(lib):
 
 
 class DepthEngine:
-    """Depth-Anything-V2 forward on wgmma tensor cores.  `cfg` is a key of CONFIGS or a dict."""
+    """Depth forward on wgmma tensor cores.  family "da-v2" (default): Depth-Anything-V2, `cfg` a key of CONFIGS or a
+    dict.  family "dpt": DPT-Large (ViT-L/16, project readout), `cfg` a key of DPT_CONFIGS or a dict, `processor` the
+    image processor's settings (depth_weights.DPT_PROCESSOR, or dpt_processor_from_json of a checkpoint's
+    preprocessor_config.json); the processed size is the processor's, image_h / image_w default to it."""
 
-    def __init__(self, cfg="vits", image_h=518, image_w=924, ctx=None, device=0):
+    def __init__(self, cfg="vits", image_h=None, image_w=None, ctx=None, device=0, family=FAMILY_DA_V2,
+                 processor=None):
         self.lib = _lib.load()
         _bind(self.lib)
         self.ctx = ctx or _lib.default_context(device)
-        self.cfg = dict(CONFIGS[cfg]) if isinstance(cfg, str) else dict(cfg)
-        self.image_h, self.image_w = int(image_h), int(image_w)
+        if family not in (FAMILY_DA_V2, FAMILY_DPT):
+            raise ValueError(f"unknown depth model family {family!r}")
+        self.family = family
+        table = DPT_CONFIGS if family == FAMILY_DPT else CONFIGS
+        self.cfg = dict(table[cfg]) if isinstance(cfg, str) else dict(cfg)
         c = self.cfg
+        if family == FAMILY_DPT:
+            self.processor = dict(processor or DPT_PROCESSOR)
+            ph, pw = dpt_processed_size(self.processor)
+            image_h, image_w = image_h or ph, image_w or pw
+        else:
+            self.processor = None
+            image_h, image_w = image_h or 518, image_w or 924
+        self.image_h, self.image_w = int(image_h), int(image_w)
         dc = DepthConfig(c["hidden"], c["layers"], c["heads"], (C.c_int32 * 4)(*c["taps"]),
                          (C.c_int32 * 4)(*c["neck"]), c["fusion"], self.image_h, self.image_w)
         h = C.c_void_p()
-        rc = self.lib.vd3d_depth_create(C.byref(dc), self.lib.vd3d_stream(self.ctx.h), C.byref(h))
+        stream = self.lib.vd3d_stream(self.ctx.h)
+        if family == FAMILY_DPT:
+            p = self.processor
+            dx = DepthConfigEx(dc, 1, c["patch"], c["ln_eps"], p["resample"], (C.c_float * 3)(*p["mean"]),
+                               (C.c_float * 3)(*p["std"]))
+            rc = self.lib.vd3d_depth_create_ex(C.byref(dx), stream, C.byref(h))
+        else:
+            rc = self.lib.vd3d_depth_create(C.byref(dc), stream, C.byref(h))
         if rc != 0:
             raise _lib.Vd3dError(f"vd3d_depth_create failed ({rc})")
         self.h = h
+
+    def processed_size(self, width, height):
+        """(h, w) the model's image processor resizes a (width, height) image to: Depth-Anything's keep-aspect
+        multiple-of-14 size, DPT's fixed size."""
+        if self.family == FAMILY_DPT:
+            return dpt_processed_size(self.processor)
+        return processed_size(width, height)
 
     def check(self, rc):
         if rc != 0:
             raise _lib.Vd3dError(f"libvd3d depth error {rc}: {self.lib.vd3d_depth_last_error(self.h).decode()}")
 
     def load_state_dict(self, sd):
-        for name, arr in prepare(sd, self.cfg, self.image_h, self.image_w).items():
+        prep = prepare_dpt if self.family == FAMILY_DPT else prepare
+        for name, arr in prep(sd, self.cfg, self.image_h, self.image_w).items():
             arr = np.ascontiguousarray(arr)
             self.check(self.lib.vd3d_depth_set_tensor(self.h, name.encode(), arr.ctypes.data, arr.nbytes))
 
@@ -131,9 +174,9 @@ class DepthEngine:
         h, w = frames[0].shape[:2]
         if any(f.shape[:2] != (h, w) for f in frames):
             raise ValueError("infer_batch needs frames of one shape")
-        if check_size and processed_size(w, h) != (self.image_h, self.image_w):
+        if check_size and self.processed_size(w, h) != (self.image_h, self.image_w):
             raise ValueError(f"engine built for processed size {(self.image_h, self.image_w)}, a {w}x{h} frame needs "
-                             f"{processed_size(w, h)}")
+                             f"{self.processed_size(w, h)}")
         out = []
         for i0 in range(0, len(frames), 8):
             chunk = frames[i0:i0 + 8]
@@ -153,9 +196,9 @@ class DepthEngine:
         n = len(frame_ptrs)
         if not 1 <= n <= 8 or len(u8_ptrs) != n:
             raise ValueError("infer_batch_u8_device takes 1..8 frames and one output per frame")
-        if processed_size(w, h) != (self.image_h, self.image_w):
+        if self.processed_size(w, h) != (self.image_h, self.image_w):
             raise ValueError(f"engine built for processed size {(self.image_h, self.image_w)}, a {w}x{h} frame needs "
-                             f"{processed_size(w, h)}")
+                             f"{self.processed_size(w, h)}")
         fp = (C.c_void_p * n)(*frame_ptrs)
         p8 = (C.c_void_p * n)(*u8_ptrs)
         self.check(self.lib.vd3d_depth_infer_batch_device(self.h, n, fp, h, w, p8, None, int(bool(invert))))
@@ -185,9 +228,9 @@ class DepthEngine:
         for k, (img, ins) in enumerate(zip(imgs, input_sizes)):
             sh, sw = int(img.shape[0]), int(img.shape[1])
             iw, ih = (sw, sh) if ins is None else (int(ins[0]), int(ins[1]))
-            if processed_size(iw, ih) != (self.image_h, self.image_w):
+            if self.processed_size(iw, ih) != (self.image_h, self.image_w):
                 raise ValueError(f"engine built for processed size {(self.image_h, self.image_w)}, a {iw}x{ih} input "
-                                 f"needs {processed_size(iw, ih)}")
+                                 f"needs {self.processed_size(iw, ih)}")
             sizes[k] = sh, sw, ih, iw
         if device:
             dev = imgs[0].device

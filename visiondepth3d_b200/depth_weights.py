@@ -54,7 +54,7 @@ def _pad_vec(b, n):
 
 def prepare(sd, cfg, image_h, image_w):
     """state_dict -> {name: np.ndarray} in the layouts depth_engine.cu expects."""
-    D, L, Fz = cfg["hidden"], cfg["layers"], cfg["fusion"]
+    D, L = cfg["hidden"], cfg["layers"]
     ph, pw = image_h // 14, image_w // 14
     out = {}
     e = "backbone.embeddings."
@@ -90,6 +90,16 @@ def prepare(sd, cfg, image_h, image_w):
         out[f"l{i}.ls2"] = _f32(sd[p + "layer_scale2.lambda1"])
     out["norm.g"] = _f32(sd["backbone.layernorm.weight"])
     out["norm.b"] = _f32(sd["backbone.layernorm.bias"])
+    out.update(_prepare_tail(sd, cfg))
+    return out
+
+
+def _prepare_tail(sd, cfg):
+    """The reassemble layers, neck convs, fusion stage and head (HF names of DepthAnythingForDepthEstimation) in the
+    engine's layouts: shared by Depth-Anything and DPT.  Fusion layer 0 never runs its residual_layer1; it is packed
+    when the state dict has it."""
+    D, Fz = cfg["hidden"], cfg["fusion"]
+    out = {}
     for i, C in enumerate(cfg["neck"]):
         CP = _up(C, 64)
         r = f"neck.reassemble_stage.layers.{i}."
@@ -113,6 +123,8 @@ def prepare(sd, cfg, image_h, image_w):
     for j in range(4):
         f = f"neck.fusion_stage.layers.{j}."
         for unit, hf in (("rl1", "residual_layer1"), ("rl2", "residual_layer2")):
+            if f + hf + ".convolution1.weight" not in sd and j == 0 and unit == "rl1":
+                continue
             for c, hc in (("c1", "convolution1"), ("c2", "convolution2")):
                 out[f"f{j}.{unit}.{c}.w"] = _conv3(sd[f + hf + "." + hc + ".weight"], Fz)
                 out[f"f{j}.{unit}.{c}.b"] = _f32(sd[f + hf + "." + hc + ".bias"])
@@ -125,4 +137,197 @@ def prepare(sd, cfg, image_h, image_w):
     out["h.c2.b"] = _f32(sd["head.conv2.bias"])
     out["h.c3.w"] = _f32(sd["head.conv3.weight"].reshape(-1))
     out["h.c3.b"] = _f32(sd["head.conv3.bias"].reshape(-1))
+    return out
+
+
+# ---------------------------------------------------------------------------
+# DPT-Large (Intel/dpt-large; transformers 5.5 DPTForDepthEstimation): ViT-L/16 without LayerScale, LayerNorm eps
+# 1e-12, taps = the raw residual stream after layers 6 / 12 / 18 / 24 (backbone_out_indices [5, 11, 17, 23] over
+# hidden_states[1:]), project readout GELU(Linear_{2D -> D}(cat(tok, cls))) per tap, then the neck and head of
+# Depth-Anything with the head's upsample x2 (= patch x grid).
+# ---------------------------------------------------------------------------
+DPT_CONFIGS = {
+    "dpt-large": dict(hidden=1024, layers=24, heads=16, taps=[6, 12, 18, 24], neck=[256, 512, 1024, 1024], fusion=256,
+                      patch=16, ln_eps=1e-12, image_size=384),
+}
+
+# DPTImageProcessor's class defaults, which Intel/dpt-large's preprocessor_config.json repeats: a fixed 384 x 384
+# target without keeping the aspect ratio, bicubic, mean = std = 0.5
+DPT_PROCESSOR = dict(size=(384, 384), resample=3, mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5))
+
+
+def hf_dpt_config(name="dpt-large", **cfg):
+    """transformers DPTConfig equal to the checkpoint's (Intel/dpt-large's config.json); `cfg` overrides entries of
+    DPT_CONFIGS[name] (a smaller ViT for tests)."""
+    from transformers import DPTConfig
+    c = dict(DPT_CONFIGS[name], **cfg)
+    return DPTConfig(hidden_size=c["hidden"], num_hidden_layers=c["layers"], num_attention_heads=c["heads"],
+                     intermediate_size=4 * c["hidden"], hidden_act="gelu", layer_norm_eps=c["ln_eps"],
+                     image_size=c["image_size"], patch_size=c["patch"], num_channels=3, qkv_bias=True,
+                     is_hybrid=False, backbone_out_indices=[t - 1 for t in c["taps"]], readout_type="project",
+                     reassemble_factors=[4, 2, 1, 0.5], neck_hidden_sizes=c["neck"], fusion_hidden_size=c["fusion"],
+                     head_in_index=-1, use_batch_norm_in_fusion_residual=False, use_bias_in_fusion_residual=None,
+                     add_projection=False)
+
+
+def dpt_config_from_json(cj):
+    """The engine configuration of a DPT config.json (dict), or ValueError naming what this engine does not serve."""
+    def bad(what):
+        raise ValueError(f"config.json: {what} is not served (DPT with a ViT backbone and project readout only)")
+    if cj.get("is_hybrid") or cj.get("backbone_config"):
+        bad("a hybrid / external backbone")
+    if cj.get("readout_type", "project") != "project":
+        bad(f"readout_type {cj.get('readout_type')!r}")
+    if cj.get("add_projection") or cj.get("use_batch_norm_in_fusion_residual"):
+        bad("a head projection or batch-norm fusion units")
+    if list(cj.get("reassemble_factors", [4, 2, 1, 0.5])) != [4, 2, 1, 0.5]:
+        bad(f"reassemble_factors {cj.get('reassemble_factors')}")
+    if cj.get("hidden_act", "gelu") != "gelu" or cj.get("use_bias_in_fusion_residual") is False:
+        bad("another activation or bias-free fusion units")
+    hidden = int(cj.get("hidden_size", 768))
+    heads = int(cj.get("num_attention_heads", 12))
+    if int(cj.get("intermediate_size", 4 * hidden)) != 4 * hidden or hidden != 64 * heads:
+        bad("an MLP width other than 4 x hidden or a head size other than 64")
+    return dict(hidden=hidden, layers=int(cj.get("num_hidden_layers", 12)), heads=heads,
+                taps=[int(t) + 1 for t in cj.get("backbone_out_indices", [2, 5, 8, 11])],
+                neck=[int(v) for v in cj.get("neck_hidden_sizes", [96, 192, 384, 768])],
+                fusion=int(cj.get("fusion_hidden_size", 256)), patch=int(cj.get("patch_size", 16)),
+                ln_eps=float(cj.get("layer_norm_eps", 1e-12)), image_size=int(cj.get("image_size", 384)))
+
+
+def dpt_processor_from_json(pj):
+    """DPT_PROCESSOR updated from a preprocessor_config.json (dict); ValueError for what the engine's processor does
+    not do (keep_aspect_ratio, ensure_multiple_of > 1, padding, a resample other than bicubic / bilinear)."""
+    p = dict(DPT_PROCESSOR)
+    if pj.get("keep_aspect_ratio") or int(pj.get("ensure_multiple_of", 1)) != 1 or pj.get("do_pad"):
+        raise ValueError("preprocessor_config.json: keep_aspect_ratio / ensure_multiple_of / do_pad are not served")
+    if pj.get("do_resize", True) is False or pj.get("do_rescale", True) is False or pj.get("do_normalize", True) is False:
+        raise ValueError("preprocessor_config.json: the processor must resize, rescale and normalise")
+    if abs(float(pj.get("rescale_factor", 1 / 255)) - 1 / 255) > 1e-9:
+        raise ValueError("preprocessor_config.json: rescale_factor must be 1/255")
+    size = pj.get("size", {"height": 384, "width": 384})
+    if isinstance(size, int):
+        size = {"height": size, "width": size}
+    if "height" not in size or "width" not in size:
+        raise ValueError(f"preprocessor_config.json: size {size} is not a height / width pair")
+    p["size"] = (int(size["height"]), int(size["width"]))
+    p["resample"] = int(pj.get("resample", 3))
+    if p["resample"] not in (2, 3):
+        raise ValueError(f"preprocessor_config.json: resample {p['resample']} is not served (2 bilinear, 3 bicubic)")
+    for k, key in (("mean", "image_mean"), ("std", "image_std")):
+        if key in pj:
+            v = pj[key]
+            p[k] = tuple(float(x) for x in (v if isinstance(v, (list, tuple)) else [v] * 3))
+    return p
+
+
+def dpt_processed_size(processor=None):
+    """(h, w) DPTImageProcessor resizes every image to (keep_aspect_ratio False, ensure_multiple_of 1): the fixed
+    size, whatever the frame.  ValueError unless it is square with a side that is a multiple of 32: DPT reshapes the
+    tokens as a square grid, and an even grid makes each fusion x2 land on the next map."""
+    h, w = (processor or DPT_PROCESSOR)["size"]
+    if h != w or h % 32 or h < 32:
+        raise ValueError(f"DPT processed size {w}x{h} is not served: it must be square with a side that is a "
+                         "multiple of 32")
+    return h, w
+
+
+def dpt_keys(cfg):
+    """Every state_dict key (and its shape) the DPT depth forward reads."""
+    D, L, P = cfg["hidden"], cfg["layers"], cfg["patch"]
+    g = cfg["image_size"] // P
+    k = {"dpt.embeddings.cls_token": (1, 1, D), "dpt.embeddings.position_embeddings": (1, g * g + 1, D),
+         "dpt.embeddings.patch_embeddings.projection.weight": (D, 3, P, P),
+         "dpt.embeddings.patch_embeddings.projection.bias": (D,)}
+    for i in range(L):
+        p = f"dpt.encoder.layer.{i}."
+        for n in ("layernorm_before", "layernorm_after"):
+            k[p + n + ".weight"] = k[p + n + ".bias"] = (D,)
+        for n in ("query", "key", "value"):
+            k[p + "attention.attention." + n + ".weight"] = (D, D)
+            k[p + "attention.attention." + n + ".bias"] = (D,)
+        k[p + "attention.output.dense.weight"], k[p + "attention.output.dense.bias"] = (D, D), (D,)
+        k[p + "intermediate.dense.weight"], k[p + "intermediate.dense.bias"] = (4 * D, D), (4 * D,)
+        k[p + "output.dense.weight"], k[p + "output.dense.bias"] = (D, 4 * D), (D,)
+    Fz = cfg["fusion"]
+    for i, C in enumerate(cfg["neck"]):
+        r = f"neck.reassemble_stage."
+        k[r + f"readout_projects.{i}.0.weight"], k[r + f"readout_projects.{i}.0.bias"] = (D, 2 * D), (D,)
+        r += f"layers.{i}."
+        k[r + "projection.weight"], k[r + "projection.bias"] = (C, D, 1, 1), (C,)
+        if i < 2:
+            f = 4 if i == 0 else 2
+            k[r + "resize.weight"], k[r + "resize.bias"] = (C, C, f, f), (C,)
+        elif i == 3:
+            k[r + "resize.weight"], k[r + "resize.bias"] = (C, C, 3, 3), (C,)
+        k[f"neck.convs.{i}.weight"] = (Fz, C, 3, 3)
+    for j in range(4):
+        f = f"neck.fusion_stage.layers.{j}."
+        for u in ("residual_layer1", "residual_layer2") if j else ("residual_layer2",):
+            for c in ("convolution1", "convolution2"):
+                k[f + u + "." + c + ".weight"], k[f + u + "." + c + ".bias"] = (Fz, Fz, 3, 3), (Fz,)
+        k[f + "projection.weight"], k[f + "projection.bias"] = (Fz, Fz, 1, 1), (Fz,)
+    k["head.head.0.weight"], k["head.head.0.bias"] = (Fz // 2, Fz, 3, 3), (Fz // 2,)
+    k["head.head.2.weight"], k["head.head.2.bias"] = (32, Fz // 2, 3, 3), (32,)
+    k["head.head.4.weight"], k["head.head.4.bias"] = (1, 32, 1, 1), (1,)
+    return k
+
+
+def check_dpt_state_dict(sd, cfg):
+    """ValueError naming the first missing or mis-shaped key the DPT forward reads.  Other keys (the final
+    dpt.layernorm, a pooler, fusion layer 0's unused residual_layer1) are ignored."""
+    for name, shape in dpt_keys(cfg).items():
+        if name not in sd:
+            raise ValueError(f"DPT state dict: missing key {name}")
+        if tuple(sd[name].shape) != shape:
+            raise ValueError(f"DPT state dict: {name} has shape {tuple(sd[name].shape)}, expected {shape}")
+
+
+def prepare_dpt(sd, cfg, image_h, image_w):
+    """DPT state_dict -> {name: np.ndarray} in the layouts depth_engine.cu expects (the tensor names of `prepare`
+    where the op is shared; LayerScale as vectors of ones, exact in EPI_RESID_LS; the readout split into its token
+    and CLS halves "ro{i}.wt" / "ro{i}.wc")."""
+    check_dpt_state_dict(sd, cfg)
+    D, P = cfg["hidden"], cfg["patch"]
+    ph, pw = image_h // P, image_w // P
+    e = "dpt.embeddings."
+    out = {"pe.w": _f16(sd[e + "patch_embeddings.projection.weight"].float().reshape(D, 3 * P * P)),
+           "pe.b": _f32(sd[e + "patch_embeddings.projection.bias"]),
+           "cls": _f32(sd[e + "cls_token"].reshape(D))}
+    pos = sd[e + "position_embeddings"].float()
+    g = int(round((pos.shape[1] - 1) ** 0.5))
+    pp = pos[:, 1:].reshape(1, g, g, D).permute(0, 3, 1, 2)
+    pp = F.interpolate(pp, size=(ph, pw), mode="bilinear")  # DPTViTEmbeddings._resize_pos_embed (identity at g x g)
+    out["pos"] = _f32(torch.cat((pos[:, :1], pp.permute(0, 2, 3, 1).reshape(1, -1, D)), dim=1).reshape(-1, D))
+    ones = np.ones(D, np.float32)
+    for i in range(cfg["layers"]):
+        p = f"dpt.encoder.layer.{i}."
+        a = p + "attention.attention."
+        out[f"l{i}.ln1.g"] = _f32(sd[p + "layernorm_before.weight"])
+        out[f"l{i}.ln1.b"] = _f32(sd[p + "layernorm_before.bias"])
+        out[f"l{i}.qkv.w"] = _f16(torch.cat([sd[a + "query.weight"], sd[a + "key.weight"], sd[a + "value.weight"]], 0))
+        out[f"l{i}.qkv.b"] = _f32(torch.cat([sd[a + "query.bias"], sd[a + "key.bias"], sd[a + "value.bias"]], 0))
+        out[f"l{i}.proj.w"] = _f16(sd[p + "attention.output.dense.weight"])
+        out[f"l{i}.proj.b"] = _f32(sd[p + "attention.output.dense.bias"])
+        out[f"l{i}.ls1"] = ones
+        out[f"l{i}.ln2.g"] = _f32(sd[p + "layernorm_after.weight"])
+        out[f"l{i}.ln2.b"] = _f32(sd[p + "layernorm_after.bias"])
+        out[f"l{i}.fc1.w"] = _f16(sd[p + "intermediate.dense.weight"])
+        out[f"l{i}.fc1.b"] = _f32(sd[p + "intermediate.dense.bias"])
+        out[f"l{i}.fc2.w"] = _f16(sd[p + "output.dense.weight"])
+        out[f"l{i}.fc2.b"] = _f32(sd[p + "output.dense.bias"])
+        out[f"l{i}.ls2"] = ones
+    for i in range(4):
+        r = f"neck.reassemble_stage.readout_projects.{i}.0."
+        w = sd[r + "weight"].float()
+        out[f"ro{i}.wt"] = _f16(w[:, :D])
+        out[f"ro{i}.wc"] = _f16(w[:, D:])
+        out[f"ro{i}.b"] = _f32(sd[r + "bias"])
+    # the neck, fusion and head share Depth-Anything's layouts: rename the head and reuse `prepare`'s code for them
+    shared = {k: v for k, v in sd.items() if k.startswith("neck.reassemble_stage.layers.") or k.startswith("neck.convs.")
+              or k.startswith("neck.fusion_stage.")}
+    for j, n in ((0, "conv1"), (2, "conv2"), (4, "conv3")):
+        shared[f"head.{n}.weight"] = sd[f"head.head.{j}.weight"]
+        shared[f"head.{n}.bias"] = sd[f"head.head.{j}.bias"]
+    out.update(_prepare_tail(shared, cfg))
     return out

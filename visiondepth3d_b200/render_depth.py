@@ -17,8 +17,9 @@ from ctypes import c_void_p as C_void_p
 
 import numpy as np
 
-from .depth_engine import DepthEngine, processed_size as _processed_size
-from .depth_weights import CONFIGS, hf_config
+from .depth_engine import FAMILY_DA_V2, FAMILY_DPT, DepthEngine, processed_size as _processed_size
+from .depth_weights import (CONFIGS, DPT_CONFIGS, DPT_PROCESSOR, dpt_config_from_json, dpt_processed_size,
+                            dpt_processor_from_json, hf_config, hf_dpt_config)
 from .render_3d import _dialog, _val
 
 try:
@@ -32,18 +33,39 @@ pipe = None
 pipe_type = None
 _engine = None
 
-# the three checkpoints of the hot path (core/render_depth.py:695-697)
+# the checkpoints of the hot path (core/render_depth.py:689-712): the three Depth-Anything-V2 sizes and DPT-Large
 supported_models = {
     "Depth Anything V2 Small": ("depth-anything/Depth-Anything-V2-Small-hf", "vits"),
     "Depth Anything V2 Base": ("depth-anything/Depth-Anything-V2-Base-hf", "vitb"),
     "Depth Anything V2 Large": ("depth-anything/Depth-Anything-V2-Large-hf", "vitl"),
+    "DPT-Large": ("Intel/dpt-large", "dpt-large"),
+    "Manojb - DPT-Large": ("Manojb/dpt-large", "dpt-large"),
 }
+
+
+def _family_of(arch):
+    return FAMILY_DPT if arch in DPT_CONFIGS else FAMILY_DA_V2
+
+
+def _load_dpt_checkpoint(sd, cfg_path):
+    """arch of a DPT state dict (dpt.* keys): DPT-Large when its shapes (and config.json, when present) say so."""
+    import json
+    c = DPT_CONFIGS["dpt-large"]
+    if os.path.exists(cfg_path):
+        with open(cfg_path) as f:
+            got = dpt_config_from_json(json.load(f))
+        if got != c:
+            raise ValueError(f"config.json {got} does not match the built-in dpt-large configuration {c}")
+    hidden = sd["dpt.embeddings.cls_token"].shape[-1]
+    layers = len({k.split(".")[3] for k in sd if k.startswith("dpt.encoder.layer.")})
+    return "dpt-large" if (hidden, layers) == (c["hidden"], c["layers"]) else None
 
 
 def load_checkpoint(path):
     """HF-format checkpoint (model.safetensors / pytorch_model.bin of
-    depth-anything/Depth-Anything-V2-{Small,Base,Large}-hf) -> state_dict.  If a config.json sits next
-    to it, the architecture is cross-checked against depth_weights.CONFIGS."""
+    depth-anything/Depth-Anything-V2-{Small,Base,Large}-hf or Intel/dpt-large) -> (arch, state_dict), arch None for
+    another model.  If a config.json sits next to it, the architecture is cross-checked against
+    depth_weights.CONFIGS / DPT_CONFIGS."""
     import json
     import os
     if path.endswith(".safetensors"):
@@ -51,6 +73,10 @@ def load_checkpoint(path):
         sd = load_file(path)
     else:
         sd = torch.load(path, map_location="cpu")
+    if "dpt.embeddings.cls_token" in sd:
+        return _load_dpt_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
+    if "backbone.embeddings.cls_token" not in sd:
+        return None, sd
     arch = None
     hidden = sd["backbone.embeddings.cls_token"].shape[-1]
     for name, c in CONFIGS.items():
@@ -71,6 +97,7 @@ def load_checkpoint(path):
 
 _state_dict = None      # weights of the loaded model (HF naming): engines for other processed sizes are built from it
 _arch = None
+_processor = None       # DPT: the image processor's settings (depth_weights.DPT_PROCESSOR or preprocessor_config.json)
 _engines = {}           # (processed_h, processed_w) -> DepthEngine, all sharing _state_dict
 cancel_requested = threading.Event()   # core/render_depth.py:38 (the GUI's cancel flag for depth jobs)
 
@@ -83,40 +110,66 @@ def _weights_dir():
 local_model_dir = _weights_dir()
 
 
+def model_processed_size(width, height):
+    """(h, w) the loaded model's image processor resizes a (width, height) image to: Depth-Anything-V2 keeps the
+    aspect at multiples of 14 near 518, DPT-Large resizes every image to its processor's fixed size."""
+    if _family_of(_arch) == FAMILY_DPT:
+        return dpt_processed_size(_processor)
+    return _processed_size(width, height)
+
+
+def _check_tiled_supported():
+    if USE_TILED_DEPTH and _family_of(_arch) == FAMILY_DPT:
+        raise ValueError("USE_TILED_DEPTH is served for Depth-Anything-V2 models only, not for DPT-Large")
+
+
 def _engine_for(width, height):
-    """The engine whose DPT processed size fits a (width, height) image; built on first use from the loaded weights
-    (the HF processor picks a keep-aspect multiple-of-14 size per image, so one model serves every aspect)."""
+    """The engine whose processed size fits a (width, height) image; built on first use from the loaded weights
+    (the DA processor picks a keep-aspect multiple-of-14 size per image, so one model serves every aspect)."""
     global _engine
     if _state_dict is None:
         raise RuntimeError("no depth model loaded: call load_depth_model() / update_pipeline() first")
-    key = _processed_size(width, height)
+    key = model_processed_size(width, height)
     eng = _engines.get(key)
     if eng is None:
-        eng = DepthEngine(_arch, key[0], key[1])
+        eng = DepthEngine(_arch, key[0], key[1], family=_family_of(_arch), processor=_processor)
         eng.load_state_dict(_state_dict)
         _engines[key] = eng
     _engine = eng
     return eng
 
 
-def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed=0):
-    """Make `pipe` serve a Depth-Anything-V2 model.  `state_dict` uses HF DepthAnythingForDepthEstimation naming
-    (e.g. from a local safetensors checkpoint); without one a random-init model (torch.manual_seed(seed)) is used --
-    there is no network here and the reference ships no weights.  (width, height) only pre-builds the engine for that
-    frame shape; other shapes get their own engine on first use."""
-    global pipe, pipe_type, _state_dict, _arch
+def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed=0, processor=None):
+    """Make `pipe` serve a Depth-Anything-V2 model ("vits" / "vitb" / "vitl") or DPT-Large ("dpt-large").
+    `state_dict` uses HF DepthAnythingForDepthEstimation / DPTForDepthEstimation naming (e.g. from a local
+    safetensors checkpoint); without one a random-init model (torch.manual_seed(seed)) is used -- there is no network
+    here and the reference ships no weights.  processor (DPT only): the image processor's settings
+    (dpt_processor_from_json of the checkpoint's preprocessor_config.json; default DPTImageProcessor's).  (width,
+    height) only pre-builds the engine for that frame shape; other shapes get their own engine on first use."""
+    global pipe, pipe_type, _state_dict, _arch, _processor
+    dpt = _family_of(arch) == FAMILY_DPT
+    if not dpt and arch not in CONFIGS:
+        raise ValueError(f"unknown depth model {arch!r}")
+    if dpt:
+        processor = dict(processor or DPT_PROCESSOR)
+        dpt_processed_size(processor)  # refuse an unserved processor before anything is built
     if state_dict is None:
-        from transformers import DepthAnythingForDepthEstimation
         torch.manual_seed(seed)
-        state_dict = DepthAnythingForDepthEstimation(hf_config(arch)).eval().state_dict()
+        if dpt:
+            from transformers import DPTForDepthEstimation
+            state_dict = DPTForDepthEstimation(hf_dpt_config(arch)).eval().state_dict()
+        else:
+            from transformers import DepthAnythingForDepthEstimation
+            state_dict = DepthAnythingForDepthEstimation(hf_config(arch)).eval().state_dict()
     for e in _engines.values():
         e.close()
     _engines.clear()
-    _state_dict, _arch = state_dict, arch
+    _state_dict, _arch, _processor = state_dict, arch, (processor if dpt else None)
     eng = _engine_for(width, height)
     pipe = hf_batch_safe_pipe
     pipe_type = "hf"
-    return pipe, {"arch": arch, "processed_size": (eng.image_h, eng.image_w), "config": CONFIGS[arch]}
+    return pipe, {"arch": arch, "processed_size": (eng.image_h, eng.image_w),
+                  "config": (DPT_CONFIGS if dpt else CONFIGS)[arch]}
 
 
 def hf_batch_safe_pipe(images, inference_size=None):
@@ -343,6 +396,7 @@ def depth_tiled(frames, width, height, out_size, invert=False, tile=None, pad=No
     by _normalize_to_u8 to out_size = (W, H).  frames: a list of host frames or a CUDA uint8 tensor [n, h, w, 3] (the
     results are then CUDA tensors).  Returns (u8 planes, float32 depth planes or None, [(min, max)] per frame)."""
     from . import _lib
+    _check_tiled_supported()
     tile = TILE_SIZE if tile is None else int(tile)
     pad = TILE_PAD if pad is None else int(pad)
     ctx = _lib.default_context(0)
@@ -433,6 +487,7 @@ def _run_pipe_or_tile(images_pil, inference_size):
     """core/render_depth.py:201-268 for the HF pipe: with USE_TILED_DEPTH each image goes through infer_depth_tile
     (one "[tile] range" line per image), otherwise the whole list through pipe."""
     if USE_TILED_DEPTH:
+        _check_tiled_supported()
         preds = []
         for img in images_pil:
             rgb = np.array(img.convert("RGB"))
@@ -489,9 +544,23 @@ def ensure_model_downloaded(checkpoint):
         print(f"❌ Failed to load {path}: {e}")
         return None, None
     if arch is None:
-        print(f"❌ {path} is not a Depth-Anything-V2 Small / Base / Large checkpoint")
+        print(f"❌ {path} is not a Depth-Anything-V2 Small / Base / Large or DPT-Large checkpoint")
         return None, None
-    return sd, {"arch": arch, "is_b200": True, "path": path}
+    meta = {"arch": arch, "is_b200": True, "path": path}
+    if _family_of(arch) == FAMILY_DPT:
+        import json
+        pp = os.path.join(os.path.dirname(path), "preprocessor_config.json")
+        try:
+            if os.path.exists(pp):
+                with open(pp) as f:
+                    meta["processor"] = dpt_processor_from_json(json.load(f))
+            else:
+                meta["processor"] = dict(DPT_PROCESSOR)
+            dpt_processed_size(meta["processor"])
+        except ValueError as e:
+            print(f"❌ {pp}: {e}")
+            return None, None
+    return sd, meta
 
 
 def _notify(widget, text):
@@ -523,7 +592,7 @@ def update_pipeline(selected_model_var, status_label_widget, inference_res_var, 
                 _notify(status_label_widget, f"❌ Failed to load model: {name}")
                 return
             _notify(status_label_widget, "🔄 Warming up H100 depth engine...")
-            load_depth_model(meta["arch"], sd, 384, 384)
+            load_depth_model(meta["arch"], sd, 384, 384, processor=meta.get("processor"))
             from PIL import Image
             pipe([Image.new("RGB", (384, 384), (127, 127, 127))])
             _notify(status_label_widget, f"✅ Depth model loaded: {name} (libvd3d, sm_90a)")
@@ -908,6 +977,7 @@ def iter_depth_frames(cap, W, H, invert=False, inference_size=None, batch_size=8
     Each batch goes to the GPU in one pinned upload; the tracker's statistics and the depth read that copy, the re-pad
     works on the device depth, and the planes come back in one download."""
     from . import _lib
+    _check_tiled_supported()
     n, batch = 0, []
     tiled = USE_TILED_DEPTH
 
@@ -988,6 +1058,7 @@ def depth_video_from_video(input_path, output_path, invert=False, inference_size
     bootstrap on the first int(fps * 3) frames decides the sidecar's bars, every frame updates the tracker, and each
     depth frame is re-padded to the tracked bars (iter_depth_frames)."""
     import cv2
+    _check_tiled_supported()
     cap = cv2.VideoCapture(input_path)
     if not cap.isOpened():
         print(f"❌ Cannot open {input_path}")
@@ -1065,7 +1136,7 @@ def depth_images(images, inference_size=None, invert=False):
     groups = {}
     for k, a in enumerate(rgbs):
         iw, ih = inference_size if inference_size is not None else (a.shape[1], a.shape[0])
-        groups.setdefault(_processed_size(int(iw), int(ih)), []).append(k)
+        groups.setdefault(model_processed_size(int(iw), int(ih)), []).append(k)
     out = [None] * len(rgbs)
     for (ph, pw), idxs in groups.items():
         iw, ih = inference_size if inference_size is not None else (rgbs[idxs[0]].shape[1], rgbs[idxs[0]].shape[0])
@@ -1118,6 +1189,7 @@ def process_images_in_folder(folder_path, batch_size_widget, output_dir_var, inf
     (u8 grayscale, the image's size) in the output directory, in chunks of the batch size.  GUI variables may be Tk
     variables or plain values; status text goes to status_label (or stdout), root is not used.  With USE_TILED_DEPTH
     each image goes through infer_depth_tile and _normalize_to_u8, otherwise through depth_images."""
+    _check_tiled_supported()
     output_dir = str(_val(output_dir_var) or "").strip()
     if not _ensure_output_dir(output_dir, status_label):
         return
@@ -1178,6 +1250,7 @@ def process_image(file_path, colormap_var, invert_var, output_dir_var, inference
     driver writes for it.  The Tk previews (input_label / output_label thumbnails) are not produced; colour maps fall
     back to grayscale."""
     from PIL import Image
+    _check_tiled_supported()
     image = Image.open(file_path).convert("RGB")
     inference_size = parse_inference_resolution(_val(inference_res_var))
     print("📏 Using inference size:", inference_size)
