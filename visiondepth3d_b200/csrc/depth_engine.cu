@@ -623,7 +623,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     sp_ = e->span_begin("attn", s);
     {  // fused wgmma attention: scores and probabilities stay in registers
       CUtensorMap mq, mk, mv;
-      if ((r = make_map(e, &mq, q, 64, NT, B * Hh, 64, (uint64_t)NP * 64, 128, 1))) return r;
+      if ((r = make_map(e, &mq, q, 64, NT, B * Hh, 64, (uint64_t)NP * 64, kAttnRows, 1))) return r;
       if ((r = make_map(e, &mk, k, 64, NT, B * Hh, 64, (uint64_t)NP * 64, 128, 1))) return r;
       if ((r = make_map(e, &mv, vt, NT, 64, B * Hh, NP, (uint64_t)64 * NP, 64, 1))) return r;
       cudaError_t ce = launch_attention(mq, mk, mv, NT, D, (__half*)attn, Hh, B, NP, s);

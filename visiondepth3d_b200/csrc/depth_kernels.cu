@@ -527,7 +527,7 @@ cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const C
   a.out = out;
   a.heads = heads;
   a.npad = npad;
-  dim3 grid((ntok + 127) / 128, heads * images);
+  dim3 grid((ntok + kAttnRows - 1) / kAttnRows, heads * images);
   k_umma_attention<<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a);
   return cudaGetLastError();
 }

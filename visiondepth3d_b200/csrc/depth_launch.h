@@ -40,7 +40,9 @@ void launch_relu_f16(const __half* in, __half* out, size_t n, cudaStream_t s);
 // Real-ESRGAN stage: BGR u8 -> 64-channel f16 NHWC (RGB/255 in channels 0..2); pixel-shuffle + base + clip + u8 BGR
 void launch_sr_in(const uint8_t* bgr, __half* x, int npix, cudaStream_t s);
 void launch_sr_out(const float* conv, int ldc, const uint8_t* bgr, uint8_t* out, int h, int w, cudaStream_t s);
-// fused attention: q,k [image][h][npad][64] (q pre-scaled), vT [image][h][64][npad] -> out [images * npad, dmodel]
+// fused attention: q,k [image][h][npad][64] (q pre-scaled), vT [image][h][64][npad] -> out [images * npad, dmodel].
+// One CTA per kAttnRows queries of one head; the q map's box is 64 x kAttnRows (the k map's 64 x 128, v's 64 x 64).
+constexpr int kAttnRows = 192;
 cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, int ntok, int dmodel,
                              __half* out, int heads, int images, int npad, cudaStream_t s);
 // bn in {32, 64, 128}; grid = (ceil(N/bn), m_tiles, batch)
