@@ -298,8 +298,8 @@ int vd3d_sharpen(vd3d_ctx* ctx, const uint8_t* src, int h, int w, double factor,
 int vd3d_heal(vd3d_ctx* ctx, const float* warped, const float* original, const float* edge_mask_or_null, int h, int w,
               double heal_strength, float* out, int mem);
 /* eye fit on one u8 BGR image [h,w,3] -> [target_h,target_w,3]: keep_aspect != 0 = pad_to_aspect_ratio (101-131, black
- * canvas), 0 = cv2.resize(..., INTER_AREA) as in the Half-SBS branch (1413-1414).  Shrinking only: identity, integer
- * factors, or cv2's general (fractional) area tables; enlarging returns VD3D_ERR_UNSUPPORTED */
+ * canvas), 0 = cv2.resize(..., INTER_AREA) as in the Half-SBS branch (1413-1414).  Identity, integer factors, cv2's
+ * general (fractional) area tables, or its fixed-point bilinear emulation when an axis is enlarged */
 int vd3d_fit_eye(vd3d_ctx* ctx, const uint8_t* src, int h, int w, int target_w, int target_h, int keep_aspect,
                  uint8_t* dst, int mem);
 /* host-only test hook (no GPU needed): the cv2 area-resize tables vd3d_fit_eye / the frame path build for a
@@ -435,12 +435,6 @@ int vd3d_sr_upscale(vd3d_ctx* ctx, vd3d_depth* sr, int n, const uint8_t* const* 
 int vd3d_depth_get_buffer(vd3d_depth* e, const char* name, void* host_out, size_t bytes);
 /* unit-test hooks for the tensor-core kernels */
 int vd3d_gemm_f16(vd3d_depth* e, const void* A_f16, const void* B_f16, int M, int N, int K, float* C_host, int bn);
-/* tuning hook: average launch time (ms) of one M x N x K GEMM on device-resident operands, on the 128 x 128 tile
-   kernel with an operand ring of 4 (variant 0, the default), 3 (variant 1) or 2 (variant 2) stages; other variants
-   return VD3D_ERR_ARG.  dbg (low 3 bits): 0 normal, 2 no TMA loads (MMA rate), 3 prologue + teardown only, 4 no
-   epilogue (the epilogue warpgroup only releases the staging tile), other values VD3D_ERR_ARG; bit 3: poll barriers with test_wait.  act: 0 none, 1 GELU; 0x100 selects the
-   residual (proj / fc2) epilogue */
-int vd3d_gemm_bench(vd3d_depth* e, int M, int N, int K, int variant, int dbg, int act, int iters, float* ms_out);
 int vd3d_conv_f16(vd3d_depth* e, const void* in_nhwc_f16, int H, int W, int cin, const void* w_f16, int cout,
                   int k3, const float* bias, int relu, float* out_host);
 

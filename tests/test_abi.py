@@ -98,7 +98,7 @@ def test_area_tables_match_cv2_restatement(lib):
             assert [e[0] for e in ent] == list(range(ofs[dx], ofs[dx] + cnt[dx]))  # consecutive sources
             assert np.array_equal(al[dx, :cnt[dx]], np.array([e[1] for e in ent], np.float32)), (ss, ds, dx)
     assert lib.vd3d_area_table(10, 20, None, None, None, 4) < 0  # enlarging is not an area shrink
-    # enlarging axes: cv2's fixed-point bilinear emulation (opt-in CUDA branch, VD3D_FIT_ENLARGE=1)
+    # enlarging axes: cv2's fixed-point bilinear emulation
     from oracle.dibr import _area_linear_tab
     for ss, ds in ((1280, 1920), (720, 1080), (160, 1440), (100, 133), (70, 140), (64, 65), (31, 200), (100, 80)):
         ofs = np.zeros(ds, np.int32)

@@ -47,11 +47,11 @@ def _tol(mode, kind="noise"):
     """(scalar abs tol, shift abs tol, eye bytes that may differ by one LSB, packed-frame bytes that may differ at all,
     packed-frame bytes that may differ by more than one, max LSB on packed frames).
 
-    Every u8 eye is gated at <= 1 LSB (north_star).  How MANY bytes sit on the other side of a truncation boundary is
-    a property of the content: the warped value of locally flat / ramp content lands exactly on k/255, where a 1e-7
-    change of any float intermediate flips the LSB (tools/diag_fast2.py: the fp32 pow accounts for 0.14 % of the bytes
-    of the natural set, the separable box sum for 0.2 %; the oracle itself is 0.05 % / 2-3 % away from the real
-    reference for the same reason, tests/test_oracle_golden.py).  Downstream, the reference's lossy identity colour
+    Every u8 eye is gated at <= 1 LSB (north_star).  How MANY bytes sit on the other side of a truncation boundary is a
+    property of the content: the warped value of locally flat / ramp content lands exactly on k/255, where a 1e-7 change
+    of any float intermediate flips the LSB (tools/diag_fast2.py of commit 79e8bd4: the fp32 pow accounts for 0.14 % of
+    the bytes of the natural set, the separable box sum for 0.2 %; the oracle itself is 0.05 % / 2-3 % away from the
+    real reference for the same reason, tests/test_oracle_golden.py).  Downstream, the reference's lossy identity colour
     grade can turn a one-LSB flip into two and apply_sharpening (centre 4.33, neighbours -0.83) spreads it over five
     pixels with up to 2 x 7.7 LSB at the centre -- hence the packed-frame budgets."""
     if mode == "exact":

@@ -103,7 +103,7 @@ SYMBOLS = [
     "vd3d_sr_create", "vd3d_sr_forward", "vd3d_sr_upscale", "vd3d_sr_set_rrdb",
     # depth forward (bound in depth_engine.py)
     "vd3d_depth_create", "vd3d_depth_create_ex", "vd3d_depth_destroy", "vd3d_depth_last_error", "vd3d_depth_launch_count",
-    "vd3d_depth_set_tensor", "vd3d_depth_forward", "vd3d_depth_get_buffer", "vd3d_gemm_f16", "vd3d_gemm_bench", "vd3d_conv_f16",
+    "vd3d_depth_set_tensor", "vd3d_depth_forward", "vd3d_depth_get_buffer", "vd3d_gemm_f16", "vd3d_conv_f16",
     "vd3d_depth_infer_batch", "vd3d_depth_infer_batch_device",
     "vd3d_set_depth_batch", "vd3d_get_depth_batch", "vd3d_render_clip_depth", "vd3d_depth_add_launches", "vd3d_depth_clone", "vd3d_release_depth",
     "vd3d_depth_profile", "vd3d_depth_profile_collect", "vd3d_depth_profile_spans",

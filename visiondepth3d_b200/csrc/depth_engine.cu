@@ -445,59 +445,6 @@ int vd3d_gemm_f16(vd3d_depth* e, const void* A, const void* B, int M, int N, int
   return VD3D_OK;
 }
 
-// tuning hook: time one GEMM shape (EPI_F16 epilogue, optional GELU) on device-resident operands with an explicit
-// kernel variant (launch_gemm_variant) and debug mode (GemmArgs::dbg); returns the average launch time in ms
-int vd3d_gemm_bench(vd3d_depth* e, int M, int N, int K, int variant, int dbg, int act, int iters, float* ms_out) {
-  if (!e || !ms_out || (K % 8) || iters < 1) return VD3D_ERR_ARG;
-  if (variant < 0 || variant > 2 || (dbg & 7) == 1 || (dbg & 7) > 4) return VD3D_ERR_ARG;
-  void *da, *db, *dc;
-  int r;
-  if ((r = get_buf(e, "t.ba", (size_t)M * K * 2, &da))) return r;
-  if ((r = get_buf(e, "t.bb", (size_t)N * K * 2, &db))) return r;
-  if ((r = get_buf(e, "t.bc", (size_t)M * N * 2, &dc))) return r;
-  DCK(cudaMemsetAsync(da, 0x2c, (size_t)M * K * 2, e->stream));  // 0x2c2c = 0.0652 in f16
-  DCK(cudaMemsetAsync(db, 0x2c, (size_t)N * K * 2, e->stream));
-  GemmArgs g = base_args(M, N, K, EPI_F16);
-  g.out_f16 = (__half*)dc;
-  g.act = act & 0xff;
-  g.dbg = dbg;
-  if (act & 0x100) {  // the proj / fc2 epilogue: fp32 residual stream read-modify-write with bias and LayerScale
-    void *dx, *dv;
-    if ((r = get_buf(e, "t.bx", (size_t)M * N * 4, &dx))) return r;
-    if ((r = get_buf(e, "t.bv", (size_t)N * 4, &dv))) return r;  // zeros: bias = ls = 0 keeps x finite over the iterations
-    g.epi = EPI_RESID_LS;
-    g.act = 0;
-    g.out_f32 = (float*)dx;
-    g.bias = (const float*)dv;
-    g.ls = (const float*)dv;
-    g.ldc = N;
-  }
-  CUtensorMap ma, mb;
-  if ((r = make_map(e, &ma, da, K, M, 1, K, (uint64_t)K * M, 128, 1))) return r;
-  if ((r = make_map(e, &mb, db, K, N, 1, K, (uint64_t)K * N, 128, 1))) return r;
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  auto done = [&](int rc) {
-    if (e0) cudaEventDestroy(e0);
-    if (e1) cudaEventDestroy(e1);
-    return rc;
-  };
-  if (cudaEventCreate(&e0) != cudaSuccess || cudaEventCreate(&e1) != cudaSuccess)
-    return done(dfail(e, VD3D_ERR_CUDA, "gemm bench: event creation failed"));
-  cudaError_t ce = cudaSuccess;
-  for (int i = 0; i < 3 + iters && ce == cudaSuccess; ++i) {
-    if (i == 3) ce = cudaEventRecord(e0, e->stream);
-    if (ce == cudaSuccess) ce = launch_gemm_variant(variant, ma, mb, g, (M + 127) / 128, 1, e->stream);
-  }
-  if (ce == cudaSuccess) ce = cudaEventRecord(e1, e->stream);
-  if (ce == cudaSuccess) ce = cudaEventSynchronize(e1);
-  float ms = 0.f;
-  if (ce == cudaSuccess) ce = cudaEventElapsedTime(&ms, e0, e1);
-  if (ce != cudaSuccess) return done(dfail(e, VD3D_ERR_CUDA, std::string("gemm bench: ") + cudaGetErrorString(ce)));
-  done(0);
-  *ms_out = ms / iters;
-  return VD3D_OK;
-}
-
 // unit-test hook: 3x3 (or 1x1) conv on an NHWC f16 map through the implicit-GEMM path
 int vd3d_conv_f16(vd3d_depth* e, const void* in_nhwc, int H, int W, int cin, const void* wt, int cout, int k3,
                   const float* bias, int relu, float* out_host) {

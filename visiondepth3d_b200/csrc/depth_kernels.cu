@@ -542,24 +542,6 @@ static int sm_count() {
   return sms;
 }
 
-// tuning hook (vd3d_gemm_bench): pick the ring depth of the 128 x 128 kernel explicitly.
-//   0: 4 stages (the default)   1: 3 stages   2: 2 stages
-cudaError_t launch_gemm_variant(int variant, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g_in,
-                                int m_tiles, int batch, cudaStream_t s) {
-  GemmArgs g = g_in;
-  g.nt = (g.N + 127) / 128;
-  g.mt = m_tiles;
-  g.nz = batch;
-  const int total = g.nt * g.mt * g.nz, sms = sm_count();
-  dim3 grid(total < sms ? total : sms, 1, 1);
-  switch (variant) {
-    case 0: return launch_gemm_t<128, 4>(a, b, g, grid, s);
-    case 1: return launch_gemm_t<128, 3>(a, b, g, grid, s);
-    case 2: return launch_gemm_t<128, 2>(a, b, g, grid, s);
-    default: return cudaErrorInvalidValue;
-  }
-}
-
 // bn: 32 / 64 / 128 = 128 x bn tiles; the B tensor map's box has bn rows
 cudaError_t launch_gemm(int bn, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g_in, int m_tiles,
                         int batch, cudaStream_t s) {

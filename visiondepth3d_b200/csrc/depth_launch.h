@@ -48,8 +48,6 @@ cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const C
 // bn in {32, 64, 128}; grid = (ceil(N/bn), m_tiles, batch)
 cudaError_t launch_gemm(int bn, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, int m_tiles,
                         int batch, cudaStream_t s);
-cudaError_t launch_gemm_variant(int variant, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, int m_tiles,
-                        int batch, cudaStream_t s);
 // launch_gemm for the RRDBNet convs (epilogue EPI_SR), batch 1
 cudaError_t launch_gemm_sr(int bn, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, int m_tiles,
                            cudaStream_t s);

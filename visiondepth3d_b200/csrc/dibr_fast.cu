@@ -685,7 +685,6 @@ __global__ void __launch_bounds__(NT, 1) k_stats(StatsArgs a) {
         float ax = fabsf(xr);
         // |x|^gamma = 2^(gamma*log2|x|) on the SFU: <= ~3e-7 relative (exact path: fp64 pow, one rounding)
         float pw = (ax > 0.f) ? exp2f(gamma * __log2f(ax)) : (gamma == 0.f ? 1.f : 0.f);
-        if (a.dbg & 1) pw = (float)pow((double)ax, (double)gamma);
         float sg = (xr > 0.f) ? 1.f : ((xr < 0.f) ? -1.f : 0.f);
         float o = clamp01((sg * pw) + mid);
         if (inb) a.d[idx] = o;

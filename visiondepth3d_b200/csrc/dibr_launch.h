@@ -219,7 +219,6 @@ struct StatsArgs {
   DevState* st;
   FrameScalars* fs;  // zeroed by the host before the launch (the centre / motion sums accumulate into it)
   unsigned* bar;     // grid barrier counter, zeroed by the host before the launch
-  int dbg;           // triage bits (env VD3D_FAST_DEBUG): 1 = correctly rounded pow in the shaping phase
 };
 
 struct RenderArgs {

@@ -69,10 +69,6 @@ struct GemmArgs {
   // EPI_HEAD
   const float* w3;
   const float* b3p;
-  // tuning hook (vd3d_gemm_bench), low 3 bits: 0 = normal, 2 = skip the TMA loads (MMA rate), 3 = prologue +
-  // teardown only, 4 = no epilogue (the epilogue warpgroup only releases the staging tile); bit 3 (8): poll barriers
-  // with test_wait instead of try_wait
-  int dbg;
   // EPI_SR: second scaled residual and the two residual scales (act 4 = LeakyReLU(0.2) there)
   const __half* res2_f16;
   float rs, rs2;
@@ -105,26 +101,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "}\n" ::"r"(bar),
       "r"(parity)
       : "memory");
-}
-// non-suspending variant (tuning hook): polls with test_wait instead of the potentially-suspending try_wait
-__device__ __forceinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred P1;\n"
-      "LAB_WAIT:\n"
-      "mbarrier.test_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-      "@P1 bra DONE;\n"
-      "bra LAB_WAIT;\n"
-      "DONE:\n"
-      "}\n" ::"r"(bar),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_wait_dbg(uint32_t bar, uint32_t parity, int spin) {
-  if (spin)
-    mbar_wait_spin(bar, parity);
-  else
-    mbar_wait(bar, parity);
 }
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -619,7 +595,6 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   // persistent: this CTA walks tiles blockIdx.x, +gridDim.x, ...; n fastest so co-resident CTAs share A in L2
   const int total_tiles = g.nt * g.mt * g.nz;
   const int nkb = (g.K + kBK - 1) / kBK;
-  const int dmode = g.dbg & 7, spin = g.dbg & 8;
 
   if (warp == 0 && lane == 0) {
     umma::prefetch_tmap(&tmA);
@@ -647,9 +622,7 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     }
   };
 
-  if (dmode == 3) {
-    // tuning: prologue + teardown only
-  } else if (warp < 4) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));  // registers go to the consumers
     if (warp == 0 && lane == 0) {
@@ -660,12 +633,8 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         for (int kb = 0; kb < nkb; ++kb, ++kit) {
           const int s = kit % STAGES;
           const uint32_t ph = (kit / STAGES) & 1;
-          umma::mbar_wait_dbg(umma::smem_u32(&empty[s]), ph ^ 1, spin);
+          umma::mbar_wait(umma::smem_u32(&empty[s]), ph ^ 1);
           const uint32_t fb = umma::smem_u32(&full[s]);
-          if (dmode == 2) {
-            umma::mbar_arrive(fb);
-            continue;
-          }
           umma::mbar_expect_tx(fb, S::kStage);
           const uint32_t sa = umma::smem_u32(smem + s * S::kStage);
           const uint32_t sb = sa + S::kABytes;
@@ -704,27 +673,25 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         m = m_blk * 128 + r;
         row_ok = m < g.M;
       }
-      umma::mbar_wait_dbg(umma::smem_u32(epi_full), j & 1, spin);
-      if (dmode != 4) {
-        // the fused epilogue on the row's BN / 32 chunks of 32 consecutive columns, in column order
-        float head_acc = 0.f;
+      umma::mbar_wait(umma::smem_u32(epi_full), j & 1);
+      // the fused epilogue on the row's BN / 32 chunks of 32 consecutive columns, in column order
+      float head_acc = 0.f;
 #pragma unroll 1
-        for (int ci = 0; ci < BN / 32; ++ci) {
-          uint32_t v[32];
-          const float4* src = (const float4*)(epi_buf + r * S::kPitch + ci * 32);
+      for (int ci = 0; ci < BN / 32; ++ci) {
+        uint32_t v[32];
+        const float4* src = (const float4*)(epi_buf + r * S::kPitch + ci * 32);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 f = src[i];
-            v[4 * i] = __float_as_uint(f.x);
-            v[4 * i + 1] = __float_as_uint(f.y);
-            v[4 * i + 2] = __float_as_uint(f.z);
-            v[4 * i + 3] = __float_as_uint(f.w);
-          }
-          gemm_epilogue_chunk<kSr>(g, v, m, z, n_blk * BN + ci * 32, row_ok, head_acc);
+        for (int i = 0; i < 8; ++i) {
+          const float4 f = src[i];
+          v[4 * i] = __float_as_uint(f.x);
+          v[4 * i + 1] = __float_as_uint(f.y);
+          v[4 * i + 2] = __float_as_uint(f.z);
+          v[4 * i + 3] = __float_as_uint(f.w);
         }
-        // DPT head: N == 32 is a single chunk
-        if (g.epi == EPI_HEAD && row_ok && n_blk == 0) g.out_f32[m] = fmaxf(head_acc + g.b3p[0], 0.f);
+        gemm_epilogue_chunk<kSr>(g, v, m, z, n_blk * BN + ci * 32, row_ok, head_acc);
       }
+      // DPT head: N == 32 is a single chunk
+      if (g.epi == EPI_HEAD && row_ok && n_blk == 0) g.out_f32[m] = fmaxf(head_acc + g.b3p[0], 0.f);
       umma::mbar_arrive(umma::smem_u32(epi_empty));
     }
   } else {
@@ -752,7 +719,7 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         for (int kb = kb0; kb < kend; ++kb, ++kit) {
           const int s = kit % STAGES;
           const uint32_t ph = (kit / STAGES) & 1;
-          umma::mbar_wait_dbg(umma::smem_u32(&full[s]), ph, spin);
+          umma::mbar_wait(umma::smem_u32(&full[s]), ph);
           const uint32_t sa = umma::smem_u32(smem + s * S::kStage) + (uint32_t)(wg * 64 * 128);
           const uint32_t sb = umma::smem_u32(smem + s * S::kStage) + S::kABytes;
           const uint64_t da = umma::make_desc(sa), db = umma::make_desc(sb);
@@ -773,7 +740,7 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       if (prev >= 0 && t == 0) umma::mbar_arrive(umma::smem_u32(&empty[prev]));
 
       // ---- hand-off: once the epilogue warpgroup has read the previous tile, stage this one ----
-      umma::mbar_wait_dbg(umma::smem_u32(epi_empty), (j & 1) ^ 1, spin);
+      umma::mbar_wait(umma::smem_u32(epi_empty), (j & 1) ^ 1);
       // fragment of m64nN: tot[4 i + q] is row 16 wq + lane/4 + 8 (q >> 1), column 8 i + 2 (lane & 3) + (q & 1)
 #pragma unroll
       for (int i = 0; i < BN / 8; ++i) {

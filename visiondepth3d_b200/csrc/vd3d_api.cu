@@ -49,7 +49,6 @@ struct vd3d_ctx {
   // bumped whenever a device resource that captured graphs bake in moves or changes content (ensure() reallocations,
   // linspace axes, INTER_AREA tables, DOF kernel bank); run_frame_slot drops stale graphs
   uint64_t res_epoch = 0, fg_epoch = 0;
-  int fast_dbg = 0;           // env VD3D_FAST_DEBUG: triage bits of the fast path (1 exact pow, 2 exact k_shift)
   int prof_depth_frames = 0;  // frames covered by the stage-2 (depth) samples since the last collect
   uint64_t dclone_wver = 0;
   unsigned* bar = nullptr;  // grid barrier counter of k_stats (inside jobwords: zeroed by begin_frame)
@@ -443,14 +442,10 @@ int run_core_fast(vd3d_ctx* ctx, const CoreIn& in, const FastLoop* lp, const Fas
   sa.st = ctx->st;
   sa.fs = ctx->fs;
   sa.bar = ctx->bar;
-  sa.dbg = ctx->fast_dbg;
   CK(launch_stats(sa, ctx->stats_blocks, s));
   ctx->launches += 1;
   if (ctx->stats_only) return VD3D_OK;
-  if (ctx->fast_dbg & 2)
-    launch_shift(d, shift, H, W, ctx->fs, in.p.enable_edge_masking ? 1 : 0, (float)in.p.feather_strength, s);
-  else
-    launch_shift_fast(d, shift, H, W, ctx->fs, in.p.enable_edge_masking ? 1 : 0, (float)in.p.feather_strength, s);
+  launch_shift_fast(d, shift, H, W, ctx->fs, in.p.enable_edge_masking ? 1 : 0, (float)in.p.feather_strength, s);
   ctx->launches += 1;
 
   RenderArgs ra;
@@ -577,7 +572,7 @@ struct FitPlan {
   const int *xofs = nullptr, *xcnt = nullptr, *yofs = nullptr, *ycnt = nullptr;
   const float *xal = nullptr, *yal = nullptr;
   int area_t = 0;
-  int lin = 0;  // enlarged axis: cv2's fixed-point bilinear emulation of INTER_AREA (opt-in, see plan_fit)
+  int lin = 0;  // enlarged axis: cv2's fixed-point bilinear emulation of INTER_AREA (see plan_fit)
 };
 
 // cv2's computeResizeAreaTab (imgproc/src/resize.cpp, opencv 4.13 as installed with the reference): geometry in double,
@@ -726,13 +721,7 @@ int plan_fit(vd3d_ctx* ctx, int fmt, int W, int H, int pw, int ph, FitPlan& f, i
   }
   if (nw > W || nh > H) {
     // cv2 switches INTER_AREA to a fixed-point bilinear scheme as soon as one axis grows (e.g. the hard-coded
-    // 1920x1080 Full-SBS eyes for sources below 1080p, core/render_3d.py:1121).  VD3D_FIT_ENLARGE=0 rejects these.
-    static int enlarge = -1;
-    if (enlarge < 0) {
-      const char* v = getenv("VD3D_FIT_ENLARGE");
-      enlarge = v ? atoi(v) : 1;
-    }
-    if (!enlarge) return fail(ctx, VD3D_ERR_UNSUPPORTED, "eye fit would enlarge the eye (INTER_AREA upscaling)");
+    // 1920x1080 Full-SBS eyes for sources below 1080p, core/render_3d.py:1121).
     f.sx = f.sy = 0;
     // the key of the cached tables does not encode the mode: W x H -> nw x nh is either a shrink or an enlargement
     return ensure_area_tabs(ctx, tab_slot, W, H, nw, nh, f, true);
@@ -940,15 +929,10 @@ int vd3d_create(int device, vd3d_ctx** out) {
   if ((e = cudaMallocHost(&ctx->st_pinned, sizeof(DevState))) != cudaSuccess) return bail("cudaMallocHost", e);
   if ((e = init_kernel_attributes()) != cudaSuccess) return bail("cudaFuncSetAttribute", e);
   if ((e = stats_grid(device, &ctx->stats_blocks)) != cudaSuccess) return bail("k_stats occupancy", e);
-  if (const char* v = getenv("VD3D_STATS_BLOCKS")) {  // tuning: fewer CTAs leave SMs to the depth kernels of the next batch
-    int n = atoi(v);
-    if (n >= 8 && n < ctx->stats_blocks) ctx->stats_blocks = n;
-  }
   {
     const char* v = getenv("VD3D_EXACT");
     ctx->exact = (v && atoi(v)) ? 1 : 0;
     if ((v = getenv("VD3D_DEPTH_BATCH"))) ctx->depth_batch = atoi(v);
-    if ((v = getenv("VD3D_FAST_DEBUG"))) ctx->fast_dbg = atoi(v);
     if (ctx->depth_batch < 1) ctx->depth_batch = 1;
     if (ctx->depth_batch > kMaxDepthBatch) ctx->depth_batch = kMaxDepthBatch;
   }

@@ -59,8 +59,6 @@ def _bind(lib):
     lib.vd3d_depth_get_buffer.restype = i
     lib.vd3d_gemm_f16.argtypes = [vp, vp, vp, i, i, i, vp, i]
     lib.vd3d_gemm_f16.restype = i
-    lib.vd3d_gemm_bench.argtypes = [vp, i, i, i, i, i, i, i, C.POINTER(C.c_float)]
-    lib.vd3d_gemm_bench.restype = i
     lib.vd3d_conv_f16.argtypes = [vp, vp, i, i, i, vp, i, i, vp, i, vp]
     lib.vd3d_conv_f16.restype = i
     lib.vd3d_depth_infer_batch.argtypes = [vp, i, C.POINTER(vp), i, i, C.POINTER(vp), C.POINTER(vp), i]
@@ -288,12 +286,6 @@ class DepthEngine:
         Cc = np.empty((M, N), dtype=np.float32)
         self.check(self.lib.vd3d_gemm_f16(self.h, A.ctypes.data, B.ctypes.data, M, N, K, Cc.ctypes.data, bn))
         return Cc
-
-    def gemm_bench(self, M, N, K, variant=0, dbg=0, act=0, iters=20):
-        """Average launch time (ms) of one GEMM shape on device operands (tuning hook, see include/vd3d.h)."""
-        ms = C.c_float(0)
-        self.check(self.lib.vd3d_gemm_bench(self.h, M, N, K, variant, dbg, act, iters, C.byref(ms)))
-        return ms.value
 
     def conv(self, x_nhwc, w, bias=None, k3=True, relu=False):
         x = np.ascontiguousarray(x_nhwc, dtype=np.float16)
