@@ -8,10 +8,10 @@
 //   wgmma.mma_async m64nBNk16 (A and B read from shared memory through matrix descriptors),
 //   accumulating in registers; a ring slot is released once the wgmmas reading it retired;
 // * the finished accumulator is staged through shared memory and handed (mbarriers) to a
-//   dedicated epilogue warpgroup, one thread per tile row, which runs the fused epilogue
-//   (bias, GELU, LayerScale+residual, QKV head split with V transposed, pixel-shuffle for
-//   ConvTranspose, ReLU / residual for convs, DPT head) on 32-column chunks of its row while
-//   the consumers already run the next tile's mainloop.
+//   dedicated epilogue warpgroup, which runs the fused epilogue (bias, GELU, LayerScale+residual,
+//   QKV head split with V transposed, pixel-shuffle for ConvTranspose, ReLU / residual for convs,
+//   DPT head) while the consumers already run the next tile's mainloop: a warp per tile row
+//   (coalesced) for the token GEMMs, one thread per tile row otherwise.
 // * A can also be an NHWC activation read through a 3-D tensor map (C, W, H): the K loop
 //   then walks the 3x3 taps and channel blocks (implicit GEMM); out-of-image taps are
 //   zero-filled by TMA, so no im2col buffer and no padding copies exist.
@@ -337,6 +337,15 @@ __device__ __forceinline__ void sr_epilogue_chunk(const GemmArgs& g, float (&a)[
   }
 }
 
+// EPI_QKV, V columns: 32 values of head dimension d0 .. d0 + 31 of token tok into vT [image][head][64][npad] (zh =
+// image * heads + head); transposed, so the lanes of a warp (consecutive rows) write consecutive tokens
+__device__ __forceinline__ void qkv_store_vt(const GemmArgs& g, const float (&a)[32], const size_t zh, const int d0,
+                                             const int tok) {
+  __half* dst = g.vt + (zh * 64 + d0) * g.npad + tok;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) dst[(size_t)j * g.npad] = __float2half_rn(a[j]);
+}
+
 // Fused epilogue of one 32-column chunk of one accumulator row (thread == row): v = raw fp32 accumulator bits,
 // m = logical output row, n0 = first output column.  Every
 // register array is indexed with compile-time constants only so the chunk stays in registers.  kSr: the RRDBNet
@@ -489,9 +498,7 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmArgs& g, const uin
         umma::pack16(a, 16, false, u);
         umma::stg_v8(dst + 16, u);
       } else {
-        __half* dst = g.vt + (zh * 64 + d0) * g.npad + tok;  // transposed: lanes -> consecutive tokens
-#pragma unroll
-        for (int j = 0; j < 32; ++j) dst[(size_t)j * g.npad] = __float2half_rn(a[j]);
+        qkv_store_vt(g, a, zh, d0, tok);
       }
     } break;
     case EPI_PATCH: {
@@ -549,9 +556,207 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmArgs& g, const uin
   }
 }
 
+// The row-per-warp epilogue (gemm_epilogue_rows) serves the plain-GEMM epilogues whose global accesses become
+// contiguous when a warp walks a row: EPI_RESID_LS, EPI_F16, EPI_QKV and EPI_READOUT.  It is decided per launch:
+// 128-column tiles that all lie inside N (N a multiple of 128), no conv row mapping, and every pointer and row pitch
+// aligned for the 4-column vectors of a lane.  Every other launch keeps the thread-per-row epilogue.
+template <int BN, bool kSr>
+__device__ __forceinline__ bool gemm_launch_by_rows(const GemmArgs& g) {
+  if constexpr (BN != 128 || kSr) {
+    return false;
+  } else {
+    auto al = [](const void* p, int bytes) { return ((uintptr_t)p & (uintptr_t)(bytes - 1)) == 0; };
+    if (g.conv || (g.N & 127) || !al(g.bias, 16)) return false;
+    switch (g.epi) {
+      case EPI_RESID_LS: return (g.ldc & 3) == 0 && al(g.out_f32, 16) && al(g.ls, 16);
+      case EPI_F16:
+        return (g.ldc & 3) == 0 && (g.out_batch_stride & 3) == 0 && al(g.out_f16, 8) && al(g.out2_f16, 8) &&
+               al(g.res_f16, 8) && (g.act != 3 || al(g.ls, 16));
+      case EPI_QKV: return (g.dmodel & 127) == 0 && al(g.q, 8) && al(g.k, 8);
+      case EPI_READOUT: return (g.ldc & 3) == 0 && al(g.out_f16, 8) && al(g.img_bias, 16);
+      default: return false;
+    }
+  }
+}
+
+// rows per warp in flight: their global loads all issue before the first store (8 do not fit the 120 registers)
+constexpr int kEpiRows = 4;
+
+namespace umma {
+// 4 fp32 -> 4 f16 (8 bytes), each element rounded on its own as in pack16
+__device__ __forceinline__ uint2 pack4(const float4 a) {
+  __half2 lo = __floats2half2_rn(a.x, a.y), hi = __floats2half2_rn(a.z, a.w);
+  return make_uint2(*(uint32_t*)&lo, *(uint32_t*)&hi);
+}
+__device__ __forceinline__ float4 lds_f4(const uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ float4 relu4(const float4 a) {
+  return make_float4(fmaxf(a.x, 0.f), fmaxf(a.y, 0.f), fmaxf(a.z, 0.f), fmaxf(a.w, 0.f));
+}
+}  // namespace umma
+
+// Row-per-warp fused epilogue of one 128 x 128 tile of a plain GEMM, every column inside N: warp w of the epilogue
+// warpgroup takes tile rows w, w + 4, ..., w + 124, lane l columns 4 l .. 4 l + 3.  A staging read is one contiguous
+// 512-byte row (conflict-free at pitch 132), the bias / LayerScale of the lane's columns are loaded once per tile, and a
+// warp's global access is one contiguous piece of an output row: 512 bytes of the fp32 residual, 256 bytes of an f16
+// output, two 128-byte head rows of q or k (where a thread per row touched 32 rows per instruction).  Rows come in
+// groups of kEpiRows whose global loads are issued before the group's first store.  The arithmetic per element is that
+// of gemm_epilogue_chunk (same operations, same order, same roundings), so both paths write the same bits.
+__device__ __forceinline__ void gemm_epilogue_rows(const GemmArgs& g, const float* tile, const int pitch,
+                                                   const int m_blk, const int n_blk, const int z) {
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int n = n_blk * 128 + 4 * lane;
+  const int nrows = min(128, g.M - m_blk * 128);  // rows of the tile inside M
+  const size_t row0 = (size_t)m_blk * 128;
+  const uint32_t srow = umma::smem_u32(tile) + 16 * lane;
+  const float4 b4 = g.bias ? __ldg((const float4*)(g.bias + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
+  // acc (+ bias) of the lane's 4 columns of tile row r; without a bias the accumulator is taken as it is
+  auto row_acc = [&](const int r) {
+    float4 a = umma::lds_f4(srow + r * pitch * 4);
+    if (g.bias) {
+      a.x += b4.x;
+      a.y += b4.y;
+      a.z += b4.z;
+      a.w += b4.w;
+    }
+    return a;
+  };
+  switch (g.epi) {
+    case EPI_RESID_LS: {
+      const float4 l4 = __ldg((const float4*)(g.ls + n));
+      float* const x0 = g.out_f32 + n;
+#pragma unroll 1
+      for (int r0 = w; r0 < nrows; r0 += 4 * kEpiRows) {
+        float4 x[kEpiRows];
+#pragma unroll
+        for (int i = 0; i < kEpiRows; ++i)
+          if (r0 + 4 * i < nrows) x[i] = *(const float4*)(x0 + (row0 + r0 + 4 * i) * g.ldc);
+#pragma unroll
+        for (int i = 0; i < kEpiRows; ++i) {
+          if (r0 + 4 * i >= nrows) break;
+          const float4 a = row_acc(r0 + 4 * i);
+          x[i].x = fmaf(l4.x, a.x, x[i].x);
+          x[i].y = fmaf(l4.y, a.y, x[i].y);
+          x[i].z = fmaf(l4.z, a.z, x[i].z);
+          x[i].w = fmaf(l4.w, a.w, x[i].w);
+          *(float4*)(x0 + (row0 + r0 + 4 * i) * g.ldc) = x[i];
+        }
+      }
+    } break;
+    case EPI_F16: {
+      const float4 s4 = g.act == 3 ? __ldg((const float4*)(g.ls + n)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const size_t o0 = (size_t)z * g.out_batch_stride + n;
+#pragma unroll 1
+      for (int r0 = w; r0 < nrows; r0 += 4 * kEpiRows) {
+        uint2 rv[kEpiRows];
+        if (g.res_f16) {
+#pragma unroll
+          for (int i = 0; i < kEpiRows; ++i)
+            if (r0 + 4 * i < nrows) rv[i] = __ldg((const uint2*)(g.res_f16 + o0 + (row0 + r0 + 4 * i) * g.ldc));
+        }
+#pragma unroll
+        for (int i = 0; i < kEpiRows; ++i) {
+          if (r0 + 4 * i >= nrows) break;
+          const size_t o = o0 + (row0 + r0 + 4 * i) * g.ldc;
+          float4 a = row_acc(r0 + 4 * i);
+          if (g.res_f16) {
+            const float2 f0 = __half22float2(*(const __half2*)&rv[i].x), f1 = __half22float2(*(const __half2*)&rv[i].y);
+            a.x += f0.x;
+            a.y += f0.y;
+            a.z += f1.x;
+            a.w += f1.y;
+          }
+          if (g.act == 1) {
+            a = make_float4(umma::gelu_erf(a.x), umma::gelu_erf(a.y), umma::gelu_erf(a.z), umma::gelu_erf(a.w));
+          } else if (g.act == 2) {
+            a = umma::relu4(a);
+          } else if (g.act == 3) {
+            a.x = a.x > 0.f ? a.x : a.x * s4.x;
+            a.y = a.y > 0.f ? a.y : a.y * s4.y;
+            a.z = a.z > 0.f ? a.z : a.z * s4.z;
+            a.w = a.w > 0.f ? a.w : a.w * s4.w;
+          }
+          *(uint2*)(g.out_f16 + o) = umma::pack4(a);
+          if (g.out2_f16) *(uint2*)(g.out2_f16 + o) = umma::pack4(umma::relu4(a));
+        }
+      }
+    } break;
+    case EPI_QKV: {
+      const int which = n_blk * 128 / g.dmodel;
+      if (which == 2) {
+        // V: thread t keeps tile row t, whose transposed stores are already coalesced across the lanes
+        const int r = threadIdx.x & 127;
+        if (r >= nrows) break;
+        const int m = m_blk * 128 + r, img = m / g.npad, tok = m - img * g.npad;
+#pragma unroll 1
+        for (int ci = 0; ci < 4; ++ci) {
+          const int n0 = n_blk * 128 + 32 * ci;
+          float a[32];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            float4 f = umma::lds_f4(umma::smem_u32(tile + r * pitch + 32 * ci + 4 * i));
+            if (g.bias) {
+              const float4 bb = __ldg((const float4*)(g.bias + n0) + i);
+              f.x += bb.x;
+              f.y += bb.y;
+              f.z += bb.z;
+              f.w += bb.w;
+            }
+            a[4 * i] = f.x;
+            a[4 * i + 1] = f.y;
+            a[4 * i + 2] = f.z;
+            a[4 * i + 3] = f.w;
+          }
+          const int rem = n0 - 2 * g.dmodel;
+          qkv_store_vt(g, a, (size_t)img * g.heads + (rem >> 6), rem & 63, tok);
+        }
+        break;
+      }
+      // q or k: the tile's 128 columns are heads h0 and h0 + 1, lanes 0-15 write 128 contiguous bytes of a row of head
+      // h0, lanes 16-31 of head h0 + 1
+      const int h = (n_blk * 128 - which * g.dmodel + 4 * lane) >> 6, d0 = (4 * lane) & 63;
+      __half* const base = which == 0 ? g.q : g.k;
+      const float sc = which == 0 ? g.qscale : 1.0f;
+#pragma unroll 4
+      for (int r = w; r < nrows; r += 4) {
+        const int m = m_blk * 128 + r;
+        const int img = m / g.npad, tok = m - img * g.npad;
+        float4 a = row_acc(r);
+        a.x *= sc;
+        a.y *= sc;
+        a.z *= sc;
+        a.w *= sc;
+        *(uint2*)(base + (((size_t)img * g.heads + h) * g.npad + tok) * 64 + d0) = umma::pack4(a);
+      }
+    } break;
+    case EPI_READOUT: {
+#pragma unroll 1
+      for (int r0 = w; r0 < nrows; r0 += 4 * kEpiRows) {
+        float4 cb[kEpiRows];
+#pragma unroll
+        for (int i = 0; i < kEpiRows; ++i)
+          if (r0 + 4 * i < nrows)
+            cb[i] = __ldg((const float4*)(g.img_bias + (size_t)((m_blk * 128 + r0 + 4 * i) / g.npad) * g.N + n));
+#pragma unroll
+        for (int i = 0; i < kEpiRows; ++i) {
+          if (r0 + 4 * i >= nrows) break;
+          const float4 a = row_acc(r0 + 4 * i);
+          const float4 y = make_float4(umma::gelu_erf(a.x + cb[i].x), umma::gelu_erf(a.y + cb[i].y),
+                                       umma::gelu_erf(a.z + cb[i].z), umma::gelu_erf(a.w + cb[i].w));
+          *(uint2*)(g.out_f16 + (row0 + r0 + 4 * i) * g.ldc + n) = umma::pack4(y);
+        }
+      }
+    } break;
+  }
+}
+
 // Four warpgroups:
 //   WG0 (warps 0-3)   TMA producer; warp 0 issues, warps 1-3 only make the other warpgroups whole and aligned;
-//   WG1 (warps 4-7)   epilogue: thread t owns row t of the 128 x BN tile;
+//   WG1 (warps 4-7)   epilogue: warp w walks rows w, w + 4, ... of the 128 x BN tile (gemm_epilogue_rows), or thread
+//                     t owns row t (every launch gemm_launch_by_rows turns down);
 //   WG2-3 (warps 8-15) MMA consumers, 64 accumulator rows each.
 // The consumers hand each finished tile to the epilogue warpgroup through the fp32 staging tile and go straight on to
 // the next tile's mainloop, so the tensor cores stay busy while the epilogue of the previous tile runs.
@@ -657,6 +862,19 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   } else if (warp < 8) {
     // ===================== epilogue warpgroup =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kEpilogueRegs));
+    // One tile loop per epilogue mapping (decided for the whole launch), so that neither constrains the other's
+    // registers under the 120 of this warpgroup
+    if (gemm_launch_by_rows<BN, kSr>(g)) {
+      int j = 0;  // staging round (tiles of this CTA)
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++j) {
+        int n_blk, m_blk, z, px0, py0;
+        decode(tile, n_blk, m_blk, z, px0, py0);
+        umma::mbar_wait(umma::smem_u32(epi_full), j & 1);
+        gemm_epilogue_rows(g, epi_buf, S::kPitch, m_blk, n_blk, z);
+        umma::mbar_arrive(umma::smem_u32(epi_empty));
+      }
+      return;
+    }
     const int r = threadIdx.x & 127;  // accumulator row inside the tile
     int j = 0;                        // staging round (tiles of this CTA)
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++j) {
