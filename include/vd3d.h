@@ -333,8 +333,12 @@ int vd3d_depth_create(const vd3d_depth_config* cfg, void* cuda_stream, vd3d_dept
  * the raw residual stream after the base.taps layers (no final LayerNorm), the project readout GELU(Linear(cat(tok,
  * cls))) per tap (weights "ro{i}.wt" f16 [D, D] token half, "ro{i}.wc" f16 [D, D] CLS half, "ro{i}.b" f32 [D]),
  * and the processor's fixed image_h x image_w target (square, a multiple of 32).  The processed size of any frame is
- * then the engine's own, so vd3d_depth_infer_images accepts every input size. */
+ * then the engine's own, so vd3d_depth_infer_images accepts every input size.
+ * VD3D_DEPTH_DA_V2 also serves the other DepthAnythingForDepthEstimation checkpoints: Depth Anything V1 (base.taps the
+ * last four layers), Distill-Any-Depth, and the V2 metric models, whose head ends in max_depth * sigmoid instead of
+ * ReLU (head = VD3D_HEAD_METRIC). */
 enum { VD3D_DEPTH_DA_V2 = 0, VD3D_DEPTH_DPT = 1 };
+enum { VD3D_HEAD_RELATIVE = 0, VD3D_HEAD_METRIC = 1 };
 typedef struct {
   vd3d_depth_config base; /* image_h / image_w multiples of patch */
   int32_t family;         /* VD3D_DEPTH_DA_V2 or VD3D_DEPTH_DPT */
@@ -342,8 +346,11 @@ typedef struct {
   float ln_eps;           /* 1e-6 (DINOv2) or 1e-12 (DPT) */
   int32_t resample;       /* the processor's PIL resample code: 3 bicubic or 2 bilinear */
   float mean[3], std[3];  /* the processor's normalisation */
+  int32_t head;           /* VD3D_HEAD_RELATIVE: depth = ReLU(conv3); VD3D_HEAD_METRIC: max_depth * sigmoid(conv3) */
+  float max_depth;        /* > 0 and finite; the metric head's scale (20 indoor, 80 outdoor); 1 for a relative head */
 } vd3d_depth_config_ex;
-/* VD3D_ERR_ARG for any other family, patch or resample, a DPT size that is not square or not a multiple of 32 */
+/* VD3D_ERR_ARG for any other family, patch, resample or head kind, a max_depth that is not finite and positive, a
+ * metric head on VD3D_DEPTH_DPT, a DPT size that is not square or not a multiple of 32 */
 int vd3d_depth_create_ex(const vd3d_depth_config_ex* cfg, void* cuda_stream, vd3d_depth** out);
 void vd3d_depth_destroy(vd3d_depth* e);
 /* CUDA-event timing of the fc1 GEMM launches (k_umma_gemm<128,4>; M = tokens, N = 4*hidden, K = hidden) */

@@ -55,6 +55,9 @@ struct vd3d_depth {
   int family = VD3D_DEPTH_DA_V2, patch = 14;
   float ln_eps = 1e-6f;
   PreprocParams pre = kImagenetBicubic;
+  // the head's last activation (VD3D_HEAD_RELATIVE / _METRIC) and the metric head's scale; every EPI_HEAD reads them
+  int head = VD3D_HEAD_RELATIVE;
+  float max_depth = 1.f;
   cudaStream_t stream = nullptr;
   std::string err;
   std::map<std::string, DTensor> w;    // weights by name
@@ -244,6 +247,9 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
   if ((x->family != VD3D_DEPTH_DA_V2 && !dpt) || (x->patch != 14 && x->patch != 16) ||
       (x->resample != 2 && x->resample != 3) || !(x->ln_eps > 0.f) || cfg->heads < 1)
     return VD3D_ERR_ARG;
+  if ((x->head != VD3D_HEAD_RELATIVE && x->head != VD3D_HEAD_METRIC) || !(x->max_depth > 0.f) ||
+      !isfinite(x->max_depth) || (dpt && x->head == VD3D_HEAD_METRIC))
+    return VD3D_ERR_ARG;
   if (cfg->hidden % 128 || cfg->hidden > 1024 || cfg->hidden / cfg->heads != 64 || cfg->fusion % 64 ||
       cfg->image_h % x->patch || cfg->image_w % x->patch)
     return VD3D_ERR_ARG;
@@ -256,6 +262,8 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
   e->family = x->family;
   e->patch = x->patch;
   e->ln_eps = x->ln_eps;
+  e->head = x->head;
+  e->max_depth = x->max_depth;
   e->pre.bilinear = x->resample == 2;
   for (int c = 0; c < 3; ++c) {
     e->pre.mean[c] = x->mean[c];
@@ -283,6 +291,8 @@ int vd3d_depth_create(const vd3d_depth_config* cfg, void* stream, vd3d_depth** o
   x.patch = 14;
   x.ln_eps = 1e-6f;
   x.resample = 3;
+  x.head = VD3D_HEAD_RELATIVE;
+  x.max_depth = 1.f;
   for (int c = 0; c < 3; ++c) {
     x.mean[c] = kImagenetBicubic.mean[c];
     x.std[c] = kImagenetBicubic.std[c];
@@ -355,6 +365,8 @@ int vd3d_depth_clone(vd3d_depth* src, void* stream, vd3d_depth** out) {
   e->family = src->family;
   e->patch = src->patch;
   e->ln_eps = src->ln_eps;
+  e->head = src->head;
+  e->max_depth = src->max_depth;
   e->pre = src->pre;
   e->stream = (cudaStream_t)stream;
   e->w = src->w;
@@ -884,6 +896,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     g2.bias = b2h;
     g2.w3 = w3;
     g2.b3p = b3;
+    g2.head_max = e->head == VD3D_HEAD_METRIC ? e->max_depth : 0.f;
     if ((r = conv(e, (const __half*)h1u, IH, IW, F2, w2, true, g2, 32))) return r;
   }
   if (fork) DCK(cudaEventRecord(e->ev_join[b], s));

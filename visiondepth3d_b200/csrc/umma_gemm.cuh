@@ -33,7 +33,7 @@ enum Epi : int {
   EPI_QKV = 3,        // split heads: q (x scale), k -> [h][m][64]; v -> vT [h][64][m]
   EPI_PATCH = 4,      // x_f32[m+1, n] = acc + bias[n] + pos[m+1, n]       (patch embedding)
   EPI_CONVT = 5,      // ConvTranspose2d(k=s): pixel-shuffle scatter into NHWC f16
-  EPI_HEAD = 6,       // depth[m] = relu(sum_n relu(acc+bias)[n] * w3[n] + b3)
+  EPI_HEAD = 6,       // depth[m] = relu(s) or head_max * sigmoid(s), s = sum_n relu(acc+bias)[n] * w3[n] + b3
   EPI_SR = 7,         // RRDBNet convs (k_umma_gemm<.., .., true> only): see sr_epilogue_chunk
   EPI_READOUT = 8,    // out_f16[m, n] = GELU(acc + img_bias[m / npad, n])  (DPT project readout, per-image CLS term)
 };
@@ -69,6 +69,7 @@ struct GemmArgs {
   // EPI_HEAD
   const float* w3;
   const float* b3p;
+  float head_max;  // 0: relative head (ReLU); > 0: metric head, max_depth * sigmoid in fp32 with an accurate expf
   // EPI_SR: second scaled residual and the two residual scales (act 4 = LeakyReLU(0.2) there)
   const __half* res2_f16;
   float rs, rs2;
@@ -909,7 +910,10 @@ k_umma_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         gemm_epilogue_chunk<kSr>(g, v, m, z, n_blk * BN + ci * 32, row_ok, head_acc);
       }
       // DPT head: N == 32 is a single chunk
-      if (g.epi == EPI_HEAD && row_ok && n_blk == 0) g.out_f32[m] = fmaxf(head_acc + g.b3p[0], 0.f);
+      if (g.epi == EPI_HEAD && row_ok && n_blk == 0) {
+        const float s = head_acc + g.b3p[0];
+        g.out_f32[m] = g.head_max > 0.f ? g.head_max * (1.f / (1.f + expf(-s))) : fmaxf(s, 0.f);
+      }
       umma::mbar_arrive(umma::smem_u32(epi_empty));
     }
   } else {

@@ -5,7 +5,8 @@ import sys as _sys
 import numpy as np
 
 from . import _lib
-from .depth_weights import CONFIGS, DPT_CONFIGS, DPT_PROCESSOR, dpt_processed_size, prepare, prepare_dpt
+from .depth_weights import (DA_PROCESSOR, DPT_CONFIGS, DPT_PROCESSOR, da_spec, dpt_processed_size, is_plain_v2, prepare,
+                            prepare_dpt)
 
 
 def processed_size(width, height, target=518, multiple=14):
@@ -27,9 +28,13 @@ class DepthConfig(C.Structure):
 
 
 class DepthConfigEx(C.Structure):
-    """vd3d_depth_config_ex: the model family, patch, LayerNorm epsilon and image processor."""
+    """vd3d_depth_config_ex: the model family, patch, LayerNorm epsilon, image processor and depth head."""
     _fields_ = [("base", DepthConfig), ("family", C.c_int32), ("patch", C.c_int32), ("ln_eps", C.c_float),
-                ("resample", C.c_int32), ("mean", C.c_float * 3), ("std", C.c_float * 3)]
+                ("resample", C.c_int32), ("mean", C.c_float * 3), ("std", C.c_float * 3), ("head", C.c_int32),
+                ("max_depth", C.c_float)]
+
+
+HEAD_KINDS = {"relative": 0, "metric": 1}  # VD3D_HEAD_RELATIVE / VD3D_HEAD_METRIC
 
 
 FAMILY_DA_V2, FAMILY_DPT = "da-v2", "dpt"
@@ -82,8 +87,8 @@ def _bind(lib):
 
 
 class DepthEngine:
-    """Depth forward on wgmma tensor cores.  family "da-v2" (default): Depth-Anything-V2, `cfg` a key of CONFIGS or a
-    dict.  family "dpt": DPT-Large (ViT-L/16, project readout), `cfg` a key of DPT_CONFIGS or a dict, `processor` the
+    """Depth forward on wgmma tensor cores.  family "da-v2" (default): Depth-Anything, `cfg` a key of CONFIGS or a
+    spec dict (depth_weights.da_spec / da_config_from_json: the V2 sizes, V1's taps, a metric head).  family "dpt": DPT-Large (ViT-L/16, project readout), `cfg` a key of DPT_CONFIGS or a dict, `processor` the
     image processor's settings (depth_weights.DPT_PROCESSOR, or dpt_processor_from_json of a checkpoint's
     preprocessor_config.json); the processed size is the processor's, image_h / image_w default to it."""
 
@@ -95,8 +100,10 @@ class DepthEngine:
         if family not in (FAMILY_DA_V2, FAMILY_DPT):
             raise ValueError(f"unknown depth model family {family!r}")
         self.family = family
-        table = DPT_CONFIGS if family == FAMILY_DPT else CONFIGS
-        self.cfg = dict(table[cfg]) if isinstance(cfg, str) else dict(cfg)
+        if family == FAMILY_DPT:
+            self.cfg = dict(DPT_CONFIGS[cfg]) if isinstance(cfg, str) else dict(cfg)
+        else:
+            self.cfg = da_spec(cfg)  # taps, head and max_depth of the spec; V2's relative head by default
         c = self.cfg
         if family == FAMILY_DPT:
             self.processor = dict(processor or DPT_PROCESSOR)
@@ -113,7 +120,12 @@ class DepthEngine:
         if family == FAMILY_DPT:
             p = self.processor
             dx = DepthConfigEx(dc, 1, c["patch"], c["ln_eps"], p["resample"], (C.c_float * 3)(*p["mean"]),
-                               (C.c_float * 3)(*p["std"]))
+                               (C.c_float * 3)(*p["std"]), HEAD_KINDS["relative"], 1.0)
+            rc = self.lib.vd3d_depth_create_ex(C.byref(dx), stream, C.byref(h))
+        elif not is_plain_v2(c):  # Depth Anything V1, Distill-Any-Depth, the V2 metric models
+            p = DA_PROCESSOR
+            dx = DepthConfigEx(dc, 0, 14, 1e-6, p["resample"], (C.c_float * 3)(*p["mean"]), (C.c_float * 3)(*p["std"]),
+                               HEAD_KINDS[c["head"]], c["max_depth"])
             rc = self.lib.vd3d_depth_create_ex(C.byref(dx), stream, C.byref(h))
         else:
             rc = self.lib.vd3d_depth_create(C.byref(dc), stream, C.byref(h))

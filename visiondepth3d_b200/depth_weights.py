@@ -13,16 +13,156 @@ CONFIGS = {  # SURVEY section 8(c); verify against config.json when real checkpo
 }
 
 
+# Depth Anything V1 (LiheYoung/depth-anything-{small,base,large}-hf) taps the last four layers of the backbone
+V1_TAPS = {"vits": [9, 10, 11, 12], "vitb": [9, 10, 11, 12], "vitl": [21, 22, 23, 24]}
+HEADS = ("relative", "metric")
+
+
+def da_spec(cfg, taps=None, head=None, max_depth=None):
+    """The full engine spec of a Depth-Anything model: `cfg` (a key of CONFIGS or a dict) with the head kind and
+    max_depth filled in (relative, 1.0 by default) and any of taps / head / max_depth overridden."""
+    c = dict(CONFIGS[cfg]) if isinstance(cfg, str) else dict(cfg)
+    c["taps"] = [int(t) for t in (taps if taps is not None else c["taps"])]
+    c["head"] = head if head is not None else c.get("head", "relative")
+    c["max_depth"] = float(max_depth if max_depth is not None else c.get("max_depth", 1.0))
+    if c["head"] not in HEADS:
+        raise ValueError(f"unknown depth head {c['head']!r}")
+    return c
+
+
+def da_arch(cfg):
+    """The CONFIGS key of a Depth-Anything spec's backbone size ("vits" / "vitb" / "vitl"), or None."""
+    for name, c in CONFIGS.items():
+        if (c["hidden"], c["layers"], c["heads"]) == (cfg["hidden"], cfg["layers"], cfg["heads"]):
+            return name
+    return None
+
+
+def is_plain_v2(cfg):
+    """True when a spec is exactly one of the three Depth-Anything-V2 sizes with the relative head."""
+    arch = da_arch(cfg)
+    s = da_spec(cfg)
+    return arch is not None and s == da_spec(arch)
+
+
 def hf_config(name):
-    """transformers config objects equivalent to depth-anything/Depth-Anything-V2-{Small,Base,Large}-hf."""
+    """transformers config objects equivalent to depth-anything/Depth-Anything-V2-{Small,Base,Large}-hf; `name` may
+    also be a spec dict (da_spec / da_config_from_json): V1 taps, a metric head with its max_depth."""
     from transformers import DepthAnythingConfig, Dinov2Config
-    c = CONFIGS[name]
+    c = da_spec(name)
     bc = Dinov2Config(hidden_size=c["hidden"], num_hidden_layers=c["layers"], num_attention_heads=c["heads"],
                       image_size=518, patch_size=14, out_indices=c["taps"], apply_layernorm=True,
                       reshape_hidden_states=False)
     return DepthAnythingConfig(backbone_config=bc, reassemble_hidden_size=c["hidden"],
                                neck_hidden_sizes=c["neck"], fusion_hidden_size=c["fusion"], head_hidden_size=32,
-                               patch_size=14, reassemble_factors=[4, 2, 1, 0.5])
+                               patch_size=14, reassemble_factors=[4, 2, 1, 0.5], depth_estimation_type=c["head"],
+                               max_depth=int(c["max_depth"]) if c["max_depth"].is_integer() else c["max_depth"])
+
+
+def da_config_from_json(cj):
+    """The engine spec (hidden, layers, heads, taps, neck, fusion, head, max_depth) of a DepthAnythingForDepthEstimation
+    config.json (dict), or ValueError naming the field this engine does not serve.  Missing fields take transformers'
+    defaults (DepthAnythingConfig: the V1-Small model; Dinov2Config for the backbone's own fields)."""
+    import math
+
+    def bad(field, value):
+        raise ValueError(f"config.json: {field} = {value!r} is not served (Depth-Anything on a DINOv2 ViT-S/B/L "
+                         "backbone with the DPT neck and head)")
+    if cj.get("model_type", "depth_anything") != "depth_anything":
+        bad("model_type", cj.get("model_type"))
+    bj = cj.get("backbone_config")
+    if bj is None:
+        bj = dict(model_type="dinov2", hidden_size=384, num_hidden_layers=12, num_attention_heads=6,
+                  reshape_hidden_states=False, out_indices=[9, 10, 11, 12])
+    if not isinstance(bj, dict):
+        bad("backbone_config", bj)
+    if bj.get("model_type") != "dinov2":
+        bad("backbone_config.model_type", bj.get("model_type"))
+    for field, want in (("patch_size", 14), ("mlp_ratio", 4), ("num_channels", 3)):
+        if bj.get(field, want) != want:
+            bad(f"backbone_config.{field}", bj.get(field))
+    if cj.get("patch_size", 14) != 14:
+        bad("patch_size", cj.get("patch_size"))
+    hidden, layers, heads = (int(bj.get("hidden_size", 768)), int(bj.get("num_hidden_layers", 12)),
+                             int(bj.get("num_attention_heads", 12)))
+    arch = da_arch(dict(hidden=hidden, layers=layers, heads=heads))
+    if arch is None:
+        bad("backbone_config.hidden_size / num_hidden_layers / num_attention_heads", (hidden, layers, heads))
+    if bj.get("use_swiglu_ffn", False):
+        bad("backbone_config.use_swiglu_ffn", bj.get("use_swiglu_ffn"))
+    eps = bj.get("layer_norm_eps", 1e-6)
+    if not isinstance(eps, (int, float)) or abs(float(eps) - 1e-6) > 1e-12:
+        bad("backbone_config.layer_norm_eps", eps)
+    if bj.get("hidden_act", "gelu") != "gelu":
+        bad("backbone_config.hidden_act", bj.get("hidden_act"))
+    if bj.get("qkv_bias", True) is not True:
+        bad("backbone_config.qkv_bias", bj.get("qkv_bias"))
+    if bj.get("apply_layernorm", True) is not True:
+        bad("backbone_config.apply_layernorm", bj.get("apply_layernorm"))
+    if bj.get("reshape_hidden_states", True) is not False:
+        bad("backbone_config.reshape_hidden_states", bj.get("reshape_hidden_states", True))
+    taps = bj.get("out_indices")
+    if (not isinstance(taps, (list, tuple)) or len(taps) != 4 or any(type(t) is not int for t in taps)
+            or not 1 <= taps[0] < taps[1] < taps[2] < taps[3] <= layers):
+        bad("backbone_config.out_indices", taps)
+    if cj.get("reassemble_hidden_size", 384) != hidden:
+        bad("reassemble_hidden_size", cj.get("reassemble_hidden_size", 384))
+    if [float(f) for f in cj.get("reassemble_factors", [4, 2, 1, 0.5])] != [4.0, 2.0, 1.0, 0.5]:
+        bad("reassemble_factors", cj.get("reassemble_factors"))
+    neck = cj.get("neck_hidden_sizes", [48, 96, 192, 384])
+    if not isinstance(neck, (list, tuple)) or len(neck) != 4 or any(type(v) is not int or v < 1 for v in neck):
+        bad("neck_hidden_sizes", neck)
+    fusion = cj.get("fusion_hidden_size", 64)
+    if type(fusion) is not int or fusion < 64 or fusion % 64:
+        bad("fusion_hidden_size", fusion)
+    if cj.get("head_hidden_size", 32) != 32:
+        bad("head_hidden_size", cj.get("head_hidden_size"))
+    if cj.get("head_in_index", -1) != -1:
+        bad("head_in_index", cj.get("head_in_index"))
+    head = cj.get("depth_estimation_type", "relative")
+    if head not in HEADS:
+        bad("depth_estimation_type", head)
+    md = cj.get("max_depth") or 1  # DepthAnythingConfig: max_depth if max_depth else 1
+    if not isinstance(md, (int, float)) or not math.isfinite(md) or md <= 0 or (head == "relative" and md != 1):
+        bad("max_depth", cj.get("max_depth"))
+    return dict(hidden=hidden, layers=layers, heads=heads, taps=list(taps), neck=list(neck), fusion=fusion,
+                head=head, max_depth=float(md))
+
+
+# DPTImageProcessor as Depth-Anything's checkpoints configure it: keep the aspect ratio, sides multiples of 14 near
+# 518, bicubic, ImageNet mean / std, no padding
+DA_PROCESSOR = dict(size=(518, 518), resample=3, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225))
+
+
+def da_processor_from_json(pj):
+    """DA_PROCESSOR when a preprocessor_config.json (dict) is Depth-Anything's processor, else ValueError naming the
+    field that differs: the engine's processor does exactly that resize and normalisation."""
+    def bad(field, value):
+        raise ValueError(f"preprocessor_config.json: {field} = {value!r} is not served (Depth-Anything's processor: "
+                         "keep_aspect_ratio, ensure_multiple_of 14, 518 x 518, bicubic, 1/255, ImageNet mean / std)")
+    for field in ("do_resize", "do_rescale", "do_normalize", "keep_aspect_ratio"):
+        if pj.get(field, True) is not True:
+            bad(field, pj.get(field))
+    if "keep_aspect_ratio" not in pj:
+        bad("keep_aspect_ratio", None)
+    if pj.get("ensure_multiple_of") != 14:
+        bad("ensure_multiple_of", pj.get("ensure_multiple_of"))
+    size = pj.get("size")
+    if size != {"height": 518, "width": 518}:
+        bad("size", size)
+    if pj.get("resample", 3) != 3:
+        bad("resample", pj.get("resample"))
+    rf = pj.get("rescale_factor", 1 / 255)
+    if not isinstance(rf, (int, float)) or abs(rf - 1 / 255) > 1e-9:
+        bad("rescale_factor", rf)
+    for field, want in (("image_mean", DA_PROCESSOR["mean"]), ("image_std", DA_PROCESSOR["std"])):
+        v = pj.get(field)
+        if (not isinstance(v, (list, tuple)) or len(v) != 3
+                or any(not isinstance(x, (int, float)) or abs(x - w) > 1e-6 for x, w in zip(v, want))):
+            bad(field, v)
+    if pj.get("do_pad", False):
+        bad("do_pad", pj.get("do_pad"))
+    return dict(DA_PROCESSOR)
 
 
 def _up(v, m):

@@ -18,8 +18,9 @@ from ctypes import c_void_p as C_void_p
 import numpy as np
 
 from .depth_engine import FAMILY_DA_V2, FAMILY_DPT, DepthEngine, processed_size as _processed_size
-from .depth_weights import (CONFIGS, DPT_CONFIGS, DPT_PROCESSOR, dpt_config_from_json, dpt_processed_size,
-                            dpt_processor_from_json, hf_config, hf_dpt_config)
+from .depth_weights import (CONFIGS, DPT_CONFIGS, DPT_PROCESSOR, da_arch, da_config_from_json, da_processor_from_json,
+                            da_spec, dpt_config_from_json, dpt_processed_size, dpt_processor_from_json, hf_config,
+                            hf_dpt_config, is_plain_v2)
 from .render_3d import _dialog, _val
 
 try:
@@ -33,14 +34,28 @@ pipe = None
 pipe_type = None
 _engine = None
 
-# the checkpoints of the hot path (core/render_depth.py:689-712): the three Depth-Anything-V2 sizes and DPT-Large
+# the checkpoints of the hot path (core/render_depth.py:689-712): the Depth-Anything family (V2, V1, Distill-Any-Depth,
+# the V2 metric models) and DPT-Large.  label -> (checkpoint id, backbone size)
 supported_models = {
-    "Depth Anything V2 Small": ("depth-anything/Depth-Anything-V2-Small-hf", "vits"),
-    "Depth Anything V2 Base": ("depth-anything/Depth-Anything-V2-Base-hf", "vitb"),
+    "Distil-Any-Depth-Large": ("xingyang1/Distill-Any-Depth-Large-hf", "vitl"),
+    "Distil-Any-Depth-Small": ("xingyang1/Distill-Any-Depth-Small-hf", "vits"),
+    "keetrap-Distil-Any-Depth-Large": ("keetrap/Distil-Any-Depth-Large-hf", "vitl"),
+    "keetrap-Distil-Any-Depth-Small": ("keetrap/Distill-Any-Depth-Small-hf", "vits"),
     "Depth Anything V2 Large": ("depth-anything/Depth-Anything-V2-Large-hf", "vitl"),
+    "Depth Anything V2 Base": ("depth-anything/Depth-Anything-V2-Base-hf", "vitb"),
+    "Depth Anything V2 Small": ("depth-anything/Depth-Anything-V2-Small-hf", "vits"),
+    "Depth Anything V1 Large": ("LiheYoung/depth-anything-large-hf", "vitl"),
+    "Depth Anything V1 Base": ("LiheYoung/depth-anything-base-hf", "vitb"),
+    "Depth Anything V1 Small": ("LiheYoung/depth-anything-small-hf", "vits"),
+    "V2-Metric-Indoor-Large": ("depth-anything/Depth-Anything-V2-Metric-Indoor-Large-hf", "vitl"),
+    "V2-Metric-Outdoor-Large": ("depth-anything/Depth-Anything-V2-Metric-Outdoor-Large-hf", "vitl"),
     "DPT-Large": ("Intel/dpt-large", "dpt-large"),
     "Manojb - DPT-Large": ("Manojb/dpt-large", "dpt-large"),
 }
+# the Depth-Anything checkpoints other than V2's: their taps and head are only in config.json (the tensors have V2's
+# shapes), so they load only with it, and with Depth-Anything's preprocessor_config.json when one is present
+DA_CONFIG_REQUIRED = frozenset(v[0] for k, v in supported_models.items()
+                               if v[1] != "dpt-large" and not k.startswith("Depth Anything V2"))
 
 
 def _family_of(arch):
@@ -61,11 +76,23 @@ def _load_dpt_checkpoint(sd, cfg_path):
     return "dpt-large" if (hidden, layers) == (c["hidden"], c["layers"]) else None
 
 
+def _check_da_state_dict(sd, spec):
+    """ValueError when a Depth-Anything state dict does not have the shapes of `spec` (config.json)."""
+    got = dict(hidden=sd["backbone.embeddings.cls_token"].shape[-1],
+               layers=len({k.split(".")[3] for k in sd if k.startswith("backbone.encoder.layer.")}),
+               neck=[sd[f"neck.reassemble_stage.layers.{i}.projection.weight"].shape[0] for i in range(4)],
+               fusion=sd["neck.convs.0.weight"].shape[0])
+    want = {k: spec[k] for k in got}
+    if got != want:
+        raise ValueError(f"state dict {got} does not match its config.json {want}")
+
+
 def load_checkpoint(path):
-    """HF-format checkpoint (model.safetensors / pytorch_model.bin of
-    depth-anything/Depth-Anything-V2-{Small,Base,Large}-hf or Intel/dpt-large) -> (arch, state_dict), arch None for
-    another model.  If a config.json sits next to it, the architecture is cross-checked against
-    depth_weights.CONFIGS / DPT_CONFIGS."""
+    """HF-format checkpoint (model.safetensors / pytorch_model.bin of a DepthAnythingForDepthEstimation or
+    Intel/dpt-large model) -> (arch, state_dict), arch None for another model.  Depth-Anything: with a config.json next
+    to it, the model is what da_config_from_json reads there (ValueError for what the engine does not serve): arch is
+    the size key of depth_weights.CONFIGS for a plain V2 model, else the spec dict (V1 taps, a metric head); without
+    one, the V2 size of the hidden width.  DPT: cross-checked against DPT_CONFIGS."""
     import json
     import os
     if path.endswith(".safetensors"):
@@ -77,26 +104,23 @@ def load_checkpoint(path):
         return _load_dpt_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
     if "backbone.embeddings.cls_token" not in sd:
         return None, sd
+    cfg_path = os.path.join(os.path.dirname(path), "config.json")
+    if os.path.exists(cfg_path):
+        with open(cfg_path) as f:
+            spec = da_config_from_json(json.load(f))
+        _check_da_state_dict(sd, spec)
+        return (da_arch(spec) if is_plain_v2(spec) else spec), sd
     arch = None
     hidden = sd["backbone.embeddings.cls_token"].shape[-1]
     for name, c in CONFIGS.items():
         if c["hidden"] == hidden:
             arch = name
-    cfg_path = os.path.join(os.path.dirname(path), "config.json")
-    if arch and os.path.exists(cfg_path):
-        cj = json.load(open(cfg_path))
-        c = CONFIGS[arch]
-        got = (cj.get("neck_hidden_sizes"), cj.get("fusion_hidden_size"),
-               cj.get("backbone_config", {}).get("out_indices"))
-        want = (c["neck"], c["fusion"], c["taps"])
-        if any(g is not None and list(g) != list(w) if isinstance(w, list) else (g is not None and g != w)
-               for g, w in zip(got, want)):
-            raise ValueError(f"config.json {got} does not match the built-in {arch} configuration {want}")
     return arch, sd
 
 
 _state_dict = None      # weights of the loaded model (HF naming): engines for other processed sizes are built from it
-_arch = None
+_arch = None            # "vits" / "vitb" / "vitl" (the Depth-Anything backbone size) or "dpt-large"
+_spec = None            # Depth-Anything: the spec (taps, head, max_depth; depth_weights.da_spec) every engine is built with
 _processor = None       # DPT: the image processor's settings (depth_weights.DPT_PROCESSOR or preprocessor_config.json)
 _engines = {}           # (processed_h, processed_w) -> DepthEngine, all sharing _state_dict
 cancel_requested = threading.Event()   # core/render_depth.py:38 (the GUI's cancel flag for depth jobs)
@@ -132,7 +156,8 @@ def _engine_for(width, height):
     key = model_processed_size(width, height)
     eng = _engines.get(key)
     if eng is None:
-        eng = DepthEngine(_arch, key[0], key[1], family=_family_of(_arch), processor=_processor)
+        dpt = _family_of(_arch) == FAMILY_DPT
+        eng = DepthEngine(_arch if dpt else _spec, key[0], key[1], family=_family_of(_arch), processor=_processor)
         eng.load_state_dict(_state_dict)
         _engines[key] = eng
     _engine = eng
@@ -140,16 +165,26 @@ def _engine_for(width, height):
 
 
 def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed=0, processor=None):
-    """Make `pipe` serve a Depth-Anything-V2 model ("vits" / "vitb" / "vitl") or DPT-Large ("dpt-large").
+    """Make `pipe` serve a Depth-Anything model or DPT-Large ("dpt-large").  arch: a Depth-Anything-V2 size ("vits" /
+    "vitb" / "vitl") or a Depth-Anything spec dict (depth_weights.da_spec / da_config_from_json: V1's taps, a metric
+    head with its max_depth), which every engine built from these weights then carries.
     `state_dict` uses HF DepthAnythingForDepthEstimation / DPTForDepthEstimation naming (e.g. from a local
     safetensors checkpoint); without one a random-init model (torch.manual_seed(seed)) is used -- there is no network
     here and the reference ships no weights.  processor (DPT only): the image processor's settings
     (dpt_processor_from_json of the checkpoint's preprocessor_config.json; default DPTImageProcessor's).  (width,
     height) only pre-builds the engine for that frame shape; other shapes get their own engine on first use."""
-    global pipe, pipe_type, _state_dict, _arch, _processor
+    global pipe, pipe_type, _state_dict, _arch, _spec, _processor
+    spec = None
+    if isinstance(arch, dict):
+        spec = da_spec(arch)
+        arch = da_arch(spec)
+        if arch is None:
+            raise ValueError(f"unknown depth model {spec!r}")
     dpt = _family_of(arch) == FAMILY_DPT
     if not dpt and arch not in CONFIGS:
         raise ValueError(f"unknown depth model {arch!r}")
+    if not dpt and spec is None:
+        spec = da_spec(arch)
     if dpt:
         processor = dict(processor or DPT_PROCESSOR)
         dpt_processed_size(processor)  # refuse an unserved processor before anything is built
@@ -160,16 +195,16 @@ def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed
             state_dict = DPTForDepthEstimation(hf_dpt_config(arch)).eval().state_dict()
         else:
             from transformers import DepthAnythingForDepthEstimation
-            state_dict = DepthAnythingForDepthEstimation(hf_config(arch)).eval().state_dict()
+            state_dict = DepthAnythingForDepthEstimation(hf_config(spec)).eval().state_dict()
     for e in _engines.values():
         e.close()
     _engines.clear()
-    _state_dict, _arch, _processor = state_dict, arch, (processor if dpt else None)
+    _state_dict, _arch, _spec, _processor = state_dict, arch, spec, (processor if dpt else None)
     eng = _engine_for(width, height)
     pipe = hf_batch_safe_pipe
     pipe_type = "hf"
     return pipe, {"arch": arch, "processed_size": (eng.image_h, eng.image_w),
-                  "config": (DPT_CONFIGS if dpt else CONFIGS)[arch]}
+                  "config": DPT_CONFIGS[arch] if dpt else dict(spec)}
 
 
 def hf_batch_safe_pipe(images, inference_size=None):
@@ -515,7 +550,7 @@ def _run_pipe_or_tile(images_pil, inference_size):
 
 
 # ---------------------------------------------------------------------------
-# model loading entry points (core/render_depth.py:728-829, 973-1140) for the three DA-V2 checkpoints of the hot path
+# model loading entry points (core/render_depth.py:728-829, 973-1140) for the Depth-Anything and DPT checkpoints of the hot path
 # ---------------------------------------------------------------------------
 def _find_checkpoint_file(folder):
     for root, _dirs, files in os.walk(folder):
@@ -538,18 +573,38 @@ def ensure_model_downloaded(checkpoint):
     if path is None:
         print(f"❌ No local weights for {checkpoint} under {folder} (no network: place model.safetensors there)")
         return None, None
+    import json
+    ckdir = os.path.dirname(path)
+    needs_config = checkpoint in DA_CONFIG_REQUIRED
+    if needs_config and not os.path.exists(os.path.join(ckdir, "config.json")):
+        print(f"❌ {checkpoint}: no config.json next to {path} (its taps and head are only there)")
+        return None, None
     try:
         arch, sd = load_checkpoint(path)
     except Exception as e:
         print(f"❌ Failed to load {path}: {e}")
         return None, None
     if arch is None:
-        print(f"❌ {path} is not a Depth-Anything-V2 Small / Base / Large or DPT-Large checkpoint")
+        print(f"❌ {path} is not a Depth-Anything (V2, V1, Distill-Any-Depth, V2-Metric) or DPT-Large checkpoint")
         return None, None
+    spec = None
+    if isinstance(arch, dict):
+        spec, arch = arch, da_arch(arch)
+    elif _family_of(arch) == FAMILY_DA_V2:
+        spec = da_spec(arch)
     meta = {"arch": arch, "is_b200": True, "path": path}
+    if spec is not None:
+        meta["spec"] = spec
+        pp = os.path.join(ckdir, "preprocessor_config.json")
+        if (needs_config or not is_plain_v2(spec)) and os.path.exists(pp):
+            try:
+                with open(pp) as f:
+                    da_processor_from_json(json.load(f))
+            except ValueError as e:
+                print(f"❌ {pp}: {e}")
+                return None, None
     if _family_of(arch) == FAMILY_DPT:
-        import json
-        pp = os.path.join(os.path.dirname(path), "preprocessor_config.json")
+        pp = os.path.join(ckdir, "preprocessor_config.json")
         try:
             if os.path.exists(pp):
                 with open(pp) as f:
@@ -592,7 +647,7 @@ def update_pipeline(selected_model_var, status_label_widget, inference_res_var, 
                 _notify(status_label_widget, f"❌ Failed to load model: {name}")
                 return
             _notify(status_label_widget, "🔄 Warming up H100 depth engine...")
-            load_depth_model(meta["arch"], sd, 384, 384, processor=meta.get("processor"))
+            load_depth_model(meta.get("spec") or meta["arch"], sd, 384, 384, processor=meta.get("processor"))
             from PIL import Image
             pipe([Image.new("RGB", (384, 384), (127, 127, 127))])
             _notify(status_label_widget, f"✅ Depth model loaded: {name} (libvd3d, sm_90a)")
