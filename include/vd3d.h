@@ -158,6 +158,13 @@ int vd3d_set_exact(vd3d_ctx* ctx, int enable);
 int vd3d_get_exact(vd3d_ctx* ctx);
 /* 1 while CUDA-graph replay is on; 0 after vd3d_set_graphs(ctx, 0) or after a failed capture fell back to eager launches */
 int vd3d_graphs_active(vd3d_ctx* ctx);
+/* test hook: synchronise ctx's stream and copy `bytes` of a DIBR buffer to host memory, for checking one kernel of the
+ * last frame against a recomputation from the inputs the device stored for it.  Planes: "xs", "ys" (linspace axes),
+ * "tdf", "dn0", "dn1", "dn" (normalised depth of the last frame), "dn_prev" (the one it read as the previous frame's),
+ * "rgb_s", "frameB", "d", "shift", "eyeL", "eyeR".  Records: "fs" (FrameScalars), "st" (DevState), "render" (int[3]:
+ * K, SRC, FUSE of the last k_render instance enqueued on the fast path; -1 before any).  Adds no work to a frame.
+ * VD3D_ERR_ARG for an unknown name or more bytes than the buffer holds. */
+int vd3d_get_buffer(vd3d_ctx* ctx, const char* name, void* host_out, size_t bytes);
 
 /* ---- DIBR ------------------------------------------------------------ */
 /* pixel_shift_cuda (core/render_3d.py:561-712).

@@ -96,7 +96,7 @@ class Tile(C.Structure):
 SYMBOLS = [
     "vd3d_create", "vd3d_destroy", "vd3d_last_error", "vd3d_reset_state", "vd3d_host_alloc",
     "vd3d_host_free", "vd3d_stream", "vd3d_sync", "vd3d_launch_count", "vd3d_set_graphs",
-    "vd3d_set_exact", "vd3d_get_exact", "vd3d_graphs_active",
+    "vd3d_set_exact", "vd3d_get_exact", "vd3d_graphs_active", "vd3d_get_buffer",
     "vd3d_pixel_shift", "vd3d_plan_sizes", "vd3d_render_frame", "vd3d_render_clip",
     "vd3d_sharpen", "vd3d_dof_grade", "vd3d_struct_size", "vd3d_pack", "vd3d_fit_eye", "vd3d_area_table", "vd3d_area_linear_table", "vd3d_heal",
     "vd3d_profile", "vd3d_profile_collect", "vd3d_check_config", "vd3d_color_grade", "vd3d_resize_cubic", "vd3d_add_weighted",
@@ -168,6 +168,8 @@ def load():
     lib.vd3d_get_exact.restype = i
     lib.vd3d_graphs_active.argtypes = [vp]
     lib.vd3d_graphs_active.restype = i
+    lib.vd3d_get_buffer.argtypes = [vp, C.c_char_p, vp, C.c_size_t]
+    lib.vd3d_get_buffer.restype = i
     lib.vd3d_pixel_shift.argtypes = [vp, fp, fp, i, i, i, i, C.POINTER(ShiftParams), u8p, u8p, fp, i,
                                      C.POINTER(FrameInfo)]
     lib.vd3d_pixel_shift.restype = i

@@ -756,7 +756,9 @@ __global__ void __launch_bounds__(256) k_shift_fast(const float* __restrict__ d,
         float g = sqrt_approx((dx * dx) + (dy * dy));
         float t = __expf(-((g - 0.02f) * f5));   // 1 - 1/(1+t) = t/(1+t)
         m = __fdividef(t, 1.0f + t);
-        if (!(t < 3.0e38f)) m = 1.0f;             // exp overflow: sigmoid -> 0, mask -> 1
+        // __fdividef returns 0 for a divisor above 2^126 (CUDA C++ Programming Guide, intrinsic functions); from there
+        // on t/(1+t) rounds to 1 in fp32, and an exp overflow (t = inf) means sigmoid -> 0, mask -> 1 as well
+        if (!(t < 0x1p126f)) m = 1.0f;
       }
       sm[ty][tx] = m;
     }
@@ -1092,7 +1094,7 @@ __global__ void __launch_bounds__(RT) k_render(RenderArgs a) {
 }
 
 template <int K, int SRC, int FUSE>
-cudaError_t render_launch(const RenderArgs& a, cudaStream_t s) {
+cudaError_t render_launch(const RenderArgs& a, cudaStream_t s, int* inst) {
   using G = RenderGeom<K, FUSE>;
   static bool attr_done = false;
   if (!attr_done) {
@@ -1102,23 +1104,26 @@ cudaError_t render_launch(const RenderArgs& a, cudaStream_t s) {
   }
   dim3 g((a.c.W + TX - 1) / TX, (a.c.H + TY - 1) / TY);
   k_render<K, SRC, FUSE><<<g, RT, G::SMEM, s>>>(a);
+  inst[0] = K;
+  inst[1] = SRC;
+  inst[2] = FUSE;
   return cudaGetLastError();
 }
 
 template <int K, int SRC>
-cudaError_t render_fuse(const RenderArgs& a, cudaStream_t s) {
+cudaError_t render_fuse(const RenderArgs& a, cudaStream_t s, int* inst) {
   switch (a.fuse) {
-    case 0: return render_launch<K, SRC, 0>(a, s);
-    case 1: return render_launch<K, SRC, 1>(a, s);
-    default: return render_launch<K, SRC, 2>(a, s);
+    case 0: return render_launch<K, SRC, 0>(a, s, inst);
+    case 1: return render_launch<K, SRC, 1>(a, s, inst);
+    default: return render_launch<K, SRC, 2>(a, s, inst);
   }
 }
 
 template <int K>
-cudaError_t render_src(const RenderArgs& a, cudaStream_t s) {
-  if (a.c.src_u8) return render_fuse<K, 0>(a, s);
-  if (a.src_rgbx) return render_fuse<K, 1>(a, s);
-  return render_fuse<K, 2>(a, s);
+cudaError_t render_src(const RenderArgs& a, cudaStream_t s, int* inst) {
+  if (a.c.src_u8) return render_fuse<K, 0>(a, s, inst);
+  if (a.src_rgbx) return render_fuse<K, 1>(a, s, inst);
+  return render_fuse<K, 2>(a, s, inst);
 }
 
 }  // namespace
@@ -1131,15 +1136,15 @@ void launch_shift_fast(const float* d, float* shift, int H, int W, const FrameSc
 
 bool render_supports(int feather, int k) { return !feather || (k >= 1 && k <= 9 && (k & 1)); }
 
-cudaError_t launch_render(const RenderArgs& a, cudaStream_t s) {
+cudaError_t launch_render(const RenderArgs& a, cudaStream_t s, int inst[3]) {
   const int k = a.c.feather ? a.c.k : 0;
   switch (k) {
-    case 0: return render_src<0>(a, s);
-    case 1: return render_src<1>(a, s);
-    case 3: return render_src<3>(a, s);
-    case 5: return render_src<5>(a, s);
-    case 7: return render_src<7>(a, s);
-    case 9: return render_src<9>(a, s);
+    case 0: return render_src<0>(a, s, inst);
+    case 1: return render_src<1>(a, s, inst);
+    case 3: return render_src<3>(a, s, inst);
+    case 5: return render_src<5>(a, s, inst);
+    case 7: return render_src<7>(a, s, inst);
+    case 9: return render_src<9>(a, s, inst);
     default: return cudaErrorInvalidValue;
   }
 }

@@ -235,7 +235,8 @@ struct RenderArgs {
 };
 
 bool render_supports(int feather, int k);
-cudaError_t launch_render(const RenderArgs& a, cudaStream_t s);
+// inst: set to the (K, SRC, FUSE) of the k_render instance launched
+cudaError_t launch_render(const RenderArgs& a, cudaStream_t s, int inst[3]);
 cudaError_t stats_grid(int device, int* blocks);
 cudaError_t launch_stats(const StatsArgs& a, int blocks, cudaStream_t s);
 void launch_shift_fast(const float* d, float* shift, int H, int W, const FrameScalars* fs, int edge_mask, float feather,

@@ -92,6 +92,7 @@ struct vd3d_ctx {
   int at_t[2] = {0, 0};
   int tdf_w = 0, tdf_h = 0;
   int frame_parity = 0;
+  int last_render[3] = {-1, -1, -1};  // (K, SRC, FUSE) of the last k_render enqueued (vd3d_get_buffer "render")
   cudaEvent_t ev_h2d[kSlots] = {}, ev_done[kSlots] = {}, ev_d2h[kSlots] = {};
   // optional per-stage device timing (bench.py roofline): event pairs on ctx->stream
   int prof = 0;
@@ -464,7 +465,7 @@ int run_core_fast(vd3d_ctx* ctx, const CoreIn& in, const FastLoop* lp, const Fas
   ra.per_eye_w = post.per_eye_w;
   {
     ProfScope ps(ctx, 1);
-    CK(launch_render(ra, s));
+    CK(launch_render(ra, s, ctx->last_render));
   }
   ctx->launches += 1;
   CK(cudaGetLastError());
@@ -1077,6 +1078,48 @@ int vd3d_set_exact(vd3d_ctx* ctx, int enable) {
 int vd3d_get_exact(vd3d_ctx* ctx) { return ctx ? ctx->exact : -1; }
 // 1 while frame graphs are enabled (0 after vd3d_set_graphs(0) or after a failed capture fell back to eager launches)
 int vd3d_graphs_active(vd3d_ctx* ctx) { return ctx ? ctx->use_graphs : -1; }
+
+// test hook: a DIBR buffer of the last frame, copied to the host after the stream drains (no work is added to a frame)
+int vd3d_get_buffer(vd3d_ctx* ctx, const char* name, void* host_out, size_t bytes) {
+  if (!ctx || !name || !host_out) return VD3D_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  CK(cudaStreamSynchronize(ctx->stream));
+  const std::string n(name);
+  if (n == "render") {
+    if (bytes > sizeof ctx->last_render) return fail(ctx, VD3D_ERR_ARG, "buffer smaller than requested");
+    memcpy(host_out, ctx->last_render, bytes);
+    return VD3D_OK;
+  }
+  const void* p = nullptr;
+  size_t cap = 0;
+  if (n == "fs") {
+    p = ctx->fs;
+    cap = sizeof(FrameScalars);
+  } else if (n == "st") {
+    p = ctx->st;
+    cap = sizeof(DevState);
+  } else {
+    // the frame that just ran wrote the plane its parity selected, then flipped the parity
+    const Buf* dn_last = ctx->frame_parity ? &ctx->dn0 : &ctx->dn1;
+    const Buf* dn_read = ctx->frame_parity ? &ctx->dn1 : &ctx->dn0;
+    const struct {
+      const char* name;
+      const Buf* b;
+    } planes[] = {{"xs", &ctx->xs},         {"ys", &ctx->ys},       {"tdf", &ctx->tdf},   {"dn0", &ctx->dn0},
+                  {"dn1", &ctx->dn1},       {"dn", dn_last},        {"dn_prev", dn_read}, {"rgb_s", &ctx->rgb_s},
+                  {"frameB", &ctx->frameB}, {"d", &ctx->d},         {"shift", &ctx->shift}, {"eyeL", &ctx->eyeL},
+                  {"eyeR", &ctx->eyeR}};
+    for (const auto& e : planes)
+      if (n == e.name) {
+        p = e.b->p;
+        cap = e.b->cap;
+      }
+    if (!p) return fail(ctx, VD3D_ERR_ARG, (std::string("no such buffer: ") + n).c_str());
+  }
+  if (bytes > cap) return fail(ctx, VD3D_ERR_ARG, "buffer smaller than requested");
+  CK(cudaMemcpy(host_out, p, bytes, cudaMemcpyDeviceToHost));
+  return VD3D_OK;
+}
 int vd3d_set_graphs(vd3d_ctx* ctx, int enable) {
   if (!ctx) return VD3D_ERR_ARG;
   ctx->use_graphs = enable;
