@@ -343,12 +343,16 @@ int vd3d_depth_create(const vd3d_depth_config* cfg, void* cuda_stream, vd3d_dept
  * then the engine's own, so vd3d_depth_infer_images accepts every input size.
  * VD3D_DEPTH_DA_V2 also serves the other DepthAnythingForDepthEstimation checkpoints: Depth Anything V1 (base.taps the
  * last four layers), Distill-Any-Depth, and the V2 metric models, whose head ends in max_depth * sigmoid instead of
- * ReLU (head = VD3D_HEAD_METRIC). */
-enum { VD3D_DEPTH_DA_V2 = 0, VD3D_DEPTH_DPT = 1 };
+ * ReLU (head = VD3D_HEAD_METRIC).
+ * VD3D_DEPTH_DPT_HYBRID is MiDaS 3.0 ("Intel/dpt-hybrid-midas"): DPT with a BiT ResNet-50 front end (stem and stages
+ * 1-3, weight-standardised convs, GroupNorm(32)) in place of the patch embedding.  The stage-1 and stage-2 maps are
+ * neck inputs 0 and 1 as they are (base.neck[0..1] must be 256 and 512); the last two base.taps feed the readout
+ * ("ro2", "ro3") and reassemble layers 2 and 3.  Patch 16, relative head, square size a multiple of 32, as DPT. */
+enum { VD3D_DEPTH_DA_V2 = 0, VD3D_DEPTH_DPT = 1, VD3D_DEPTH_DPT_HYBRID = 2 };
 enum { VD3D_HEAD_RELATIVE = 0, VD3D_HEAD_METRIC = 1 };
 typedef struct {
   vd3d_depth_config base; /* image_h / image_w multiples of patch */
-  int32_t family;         /* VD3D_DEPTH_DA_V2 or VD3D_DEPTH_DPT */
+  int32_t family;         /* VD3D_DEPTH_DA_V2, VD3D_DEPTH_DPT or VD3D_DEPTH_DPT_HYBRID */
   int32_t patch;          /* 14 (DINOv2) or 16 (ViT-L/16) */
   float ln_eps;           /* 1e-6 (DINOv2) or 1e-12 (DPT) */
   int32_t resample;       /* the processor's PIL resample code: 3 bicubic or 2 bilinear */
@@ -357,7 +361,8 @@ typedef struct {
   float max_depth;        /* > 0 and finite; the metric head's scale (20 indoor, 80 outdoor); 1 for a relative head */
 } vd3d_depth_config_ex;
 /* VD3D_ERR_ARG for any other family, patch, resample or head kind, a max_depth that is not finite and positive, a
- * metric head on VD3D_DEPTH_DPT, a DPT size that is not square or not a multiple of 32 */
+ * metric head on VD3D_DEPTH_DPT / _DPT_HYBRID, a DPT size that is not square or not a multiple of 32, a hybrid with a
+ * patch other than 16 or base.neck[0..1] other than 256 / 512 */
 int vd3d_depth_create_ex(const vd3d_depth_config_ex* cfg, void* cuda_stream, vd3d_depth** out);
 void vd3d_depth_destroy(vd3d_depth* e);
 /* CUDA-event timing of the fc1 GEMM launches (k_umma_gemm<128,4>; M = tokens, N = 4*hidden, K = hidden) */
@@ -451,6 +456,14 @@ int vd3d_depth_get_buffer(vd3d_depth* e, const char* name, void* host_out, size_
 int vd3d_gemm_f16(vd3d_depth* e, const void* A_f16, const void* B_f16, int M, int N, int K, float* C_host, int bn);
 int vd3d_conv_f16(vd3d_depth* e, const void* in_nhwc_f16, int H, int W, int cin, const void* w_f16, int cout,
                   int k3, const float* bias, int relu, float* out_host);
+/* unit-test hook for the BiT kernels of VD3D_DEPTH_DPT_HYBRID: one launch sequence on tensors uploaded with
+ * vd3d_depth_set_tensor ("t.in", "t.in2", "t.res", "t.w", "t.g", "t.b", "t.g2", "t.b2") into the buffer "t.out", read
+ * back with vd3d_depth_get_buffer (the GroupNorm's chunk partials in "t.part" / "t.part2").  Synchronises.
+ *   op 0 stem conv (dims H, W): t.in f32 [3, H, W], t.w f32 [64, 147] -> f32 [H/2 * W/2, 64]
+ *   op 1 GroupNorm (dims rows, C, flags: 1 ReLU, 2 + GN(t.in2; t.g2, t.b2), 4 + t.res f16): t.in f32 [rows, C] -> f16
+ *   op 2 max-pool (dims H, W, C): t.in f16 [H, W, C] -> f16 [H/2, W/2, C]
+ *   op 3 SAME im2col (dims H, W, C, k, pb): t.in f16 [H, W, C] -> f16 [H/2 * W/2, k * k * C] */
+int vd3d_bit_kernel(vd3d_depth* e, int op, const int32_t* dims);
 
 #ifdef __cplusplus
 }

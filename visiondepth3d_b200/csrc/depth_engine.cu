@@ -243,7 +243,8 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
   *out = nullptr;
   if (!load_encode()) return VD3D_ERR_CUDA;
   const vd3d_depth_config* cfg = &x->base;
-  const bool dpt = x->family == VD3D_DEPTH_DPT;
+  const bool hybrid = x->family == VD3D_DEPTH_DPT_HYBRID;
+  const bool dpt = x->family == VD3D_DEPTH_DPT || hybrid;
   if ((x->family != VD3D_DEPTH_DA_V2 && !dpt) || (x->patch != 14 && x->patch != 16) ||
       (x->resample != 2 && x->resample != 3) || !(x->ln_eps > 0.f) || cfg->heads < 1)
     return VD3D_ERR_ARG;
@@ -255,6 +256,8 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
     return VD3D_ERR_ARG;
   // DPT reshapes the tokens as a square grid, and every fusion x2 must land on the next map: an even square grid
   if (dpt && (cfg->image_h != cfg->image_w || cfg->image_h % 32)) return VD3D_ERR_ARG;
+  // the hybrid's fixed BiT front end: patch 16 (stage 3 is the S/16 token grid), stage maps of 256 / 512 channels
+  if (hybrid && (x->patch != 16 || cfg->neck[0] != 256 || cfg->neck[1] != 512)) return VD3D_ERR_ARG;
   for (int c = 0; c < 3; ++c)
     if (!(x->std[c] != 0.f)) return VD3D_ERR_ARG;
   vd3d_depth* e = new vd3d_depth();
@@ -485,11 +488,224 @@ int vd3d_conv_f16(vd3d_depth* e, const void* in_nhwc, int H, int W, int cin, con
   return VD3D_OK;
 }
 
+int vd3d_bit_kernel(vd3d_depth* e, int op, const int32_t* d) {
+  if (!e || !d || op < 0 || op > 3) return VD3D_ERR_ARG;
+  cudaStream_t s = e->stream;
+  int r;
+  void* out;
+  if (op == 0) {
+    const int H = d[0], Wd = d[1];
+    if (H < 2 || Wd < 2 || (H | Wd) & 1) return VD3D_ERR_ARG;
+    const float *in, *w;
+    if ((r = W(e, "t.in", &in, (size_t)3 * H * Wd)) || (r = W(e, "t.w", &w, 64 * 147))) return r;
+    if ((r = get_buf(e, "t.out", (size_t)(H / 2) * (Wd / 2) * 64 * 4, &out))) return r;
+    launch_bit_stem(in, H, Wd, w, (float*)out, s);
+  } else if (op == 1) {
+    const int rows = d[0], C = d[1], flags = d[2];
+    if (rows < 1 || C < 64 || C > 1024 || (C & (C - 1))) return VD3D_ERR_ARG;
+    GnInput a, b;
+    memset(&b, 0, sizeof b);
+    const __half* res = nullptr;
+    void *p0, *p1;
+    if ((r = W(e, "t.in", &a.y, (size_t)rows * C)) || (r = W(e, "t.g", &a.gamma, C)) || (r = W(e, "t.b", &a.beta, C)))
+      return r;
+    if ((flags & 2) && ((r = W(e, "t.in2", &b.y, (size_t)rows * C)) || (r = W(e, "t.g2", &b.gamma, C)) ||
+                        (r = W(e, "t.b2", &b.beta, C))))
+      return r;
+    if ((flags & 4) && (r = W(e, "t.res", &res, (size_t)rows * C))) return r;
+    if ((r = get_buf(e, "t.out", (size_t)rows * C * 2, &out)) ||
+        (r = get_buf(e, "t.part", (size_t)kGnMaxChunks * 32 * sizeof(float2), &p0)) ||
+        (r = get_buf(e, "t.part2", (size_t)kGnMaxChunks * 32 * sizeof(float2), &p1)))
+      return r;
+    a.part = (const float2*)p0;
+    b.part = (const float2*)p1;
+    launch_gn_stats(a.y, rows, C, (float2*)p0, s);
+    if (b.y) launch_gn_stats(b.y, rows, C, (float2*)p1, s);
+    launch_gn_apply(a, b, res, flags & 1, rows, C, (__half*)out, s);
+  } else {
+    const int H = d[0], Wd = d[1], C = d[2], k = op == 3 ? d[3] : 3, pb = op == 3 ? d[4] : 0;
+    if (H < 2 || Wd < 2 || (H | Wd) & 1 || C < 8 || C % 8 || (k != 1 && k != 3) || pb < 0 || pb >= k) return VD3D_ERR_ARG;
+    const __half* in;
+    if ((r = W(e, "t.in", &in, (size_t)H * Wd * C))) return r;
+    if ((r = get_buf(e, "t.out", (size_t)(H / 2) * (Wd / 2) * (op == 3 ? k * k : 1) * C * 2, &out))) return r;
+    if (op == 2)
+      launch_maxpool_same(in, H, Wd, C, (__half*)out, s);
+    else
+      launch_im2col_same(in, H, Wd, C, k, pb, (__half*)out, s);
+  }
+  DCK(cudaGetLastError());
+  DCK(cudaStreamSynchronize(s));
+  return VD3D_OK;
+}
+
 }  // extern "C"
 
 namespace {
 
 constexpr int kMaxBatch = 8;
+
+// ---- DPT-Hybrid (MiDaS 3.0): the BiT ResNet-50 front end, stem + stages 1-3 (depths 3 / 4 / 9, widths 256 / 512 /
+// 1024, bottleneck mids a quarter of that, 32 groups), on one image of side S = IH = IW (a multiple of 32).
+// transformers 5.5 BitEmbeddings / BitBottleneckLayer / BitDownsampleConv with global_padding "SAME":
+//   stem  = maxpool3x3s2_SAME(relu(GN(conv7x7s2_SAME(px))))                                        -> [S/4]^2 x 64
+//   block = relu(GN3(conv1x1(relu(GN2(conv3x3_s(relu(GN1(conv1x1(x)))))))) + shortcut)
+//   shortcut = GN(conv1x1_s(x)) on the first block of a stage (stride 1, 2, 2), x on the others.
+// Every conv is weight-standardised at load time (depth_weights.prepare_dpt_hybrid) and has no bias.  The stem conv runs
+// in f32 on the CUDA cores; the others on k_umma_gemm (f16 operands, f32 output for the GroupNorm): 1x1 convs as plain
+// GEMMs on the NHWC row matrix, stride-1 3x3 convs on the implicit-GEMM conv, and the stride-2 3x3 conv (SAME: 0 before,
+// 1 after) and stride-2 1x1 shortcut on k_im2col_same's rows.  Block outputs are f16 NHWC.
+// Weights: "bit.stem.w" f32 [64, 147], "bit.s{st}.b{k}.c{1,2,3}.w" f16 ([mid, cin], [mid, 9 mid] tap-major, [out, mid]),
+// ".n{1,2,3}.g/.b" f32, first blocks ".ds.w" f16 [out, cin] and ".ds.g/.b"; "bit.stem.g/.b".
+// Outputs: stage1 f16 [(S/4)^2, 256] and stage2 f16 [(S/8)^2, 512] in the per-image buffers "bit.stage1.{b}" /
+// "bit.stage2.{b}" (neck inputs 0 and 1), stage3 f16 [(S/16)^2, 1024] in *stage3.  The image's launches run in order on
+// the engine stream with shared scratch buffers: "bit.y" / "bit.y2" (f32 conv outputs), "bit.t1" / "bit.t2" (f16 mids),
+// "bit.xa" / "bit.xb" (f16 block outputs), "bit.col" (im2col), "bit.gn0" / "bit.gn1" (GroupNorm partials).
+constexpr int kBitDepths[3] = {3, 4, 9}, kBitWidths[3] = {256, 512, 1024};
+
+int bit_backbone(vd3d_depth* e, int b, const float* px, const __half** stage3) {
+  cudaStream_t s = e->stream;
+  const int S = e->cfg.image_h, S2 = S / 2, S4 = S / 4;
+  const size_t big = (size_t)S2 * S2 * 64;  // the largest map: stem output = stage-1 output = stage-2 block 0's conv1
+  int r;
+  char nm[64];
+  void *y, *y2, *t1, *t2, *xa, *xb, *col, *p0, *p1, *st1, *st2;
+  // im2col rows of the stride-2 3x3 convs (stages 2 and 3), rounded up to the GEMM's 128-row tiles
+  const size_t col_el = std::max((size_t)round_up((S / 8) * (S / 8), 128) * 9 * 128,
+                                 (size_t)round_up((S / 16) * (S / 16), 128) * 9 * 256);
+  if ((r = get_buf(e, "bit.y", big * 4, &y)) || (r = get_buf(e, "bit.y2", big * 4, &y2)) ||
+      (r = get_buf(e, "bit.t1", big * 2, &t1)) || (r = get_buf(e, "bit.t2", big * 2, &t2)) ||
+      (r = get_buf(e, "bit.xa", big * 2, &xa)) || (r = get_buf(e, "bit.xb", big * 2, &xb)) ||
+      (r = get_buf(e, "bit.col", col_el * 2, &col)) ||
+      (r = get_buf(e, "bit.gn0", (size_t)kGnMaxChunks * 32 * sizeof(float2), &p0)) ||
+      (r = get_buf(e, "bit.gn1", (size_t)kGnMaxChunks * 32 * sizeof(float2), &p1)))
+    return r;
+  snprintf(nm, sizeof nm, "bit.stage1.%d", b);
+  if ((r = get_buf(e, nm, (size_t)S4 * S4 * 256 * 2, &st1))) return r;
+  snprintf(nm, sizeof nm, "bit.stage2.%d", b);
+  if ((r = get_buf(e, nm, (size_t)(S / 8) * (S / 8) * 512 * 2, &st2))) return r;
+  auto gn_in = [&](const char* base, const float* map, const void* part, GnInput* out) -> int {
+    int rr;
+    snprintf(nm, sizeof nm, "%s.g", base);
+    if ((rr = W(e, nm, &out->gamma))) return rr;
+    snprintf(nm, sizeof nm, "%s.b", base);
+    if ((rr = W(e, nm, &out->beta))) return rr;
+    out->y = map;
+    out->part = (const float2*)part;
+    return VD3D_OK;
+  };
+  // GroupNorm of one f32 map (and optionally of a second, added) + residual / ReLU -> f16
+  auto groupnorm = [&](const char* na, const float* ya, const char* nb, const float* yb, const __half* res, int relu,
+                       int rows, int C, __half* out) -> int {
+    GnInput ga, gb;
+    memset(&gb, 0, sizeof gb);
+    int rr;
+    if ((rr = gn_in(na, ya, p0, &ga))) return rr;
+    if (nb && (rr = gn_in(nb, yb, p1, &gb))) return rr;
+    const int sp = e->span_begin("bit.gn", s);
+    launch_gn_stats(ya, rows, C, (float2*)p0, s);
+    if (nb) launch_gn_stats(yb, rows, C, (float2*)p1, s);
+    launch_gn_apply(ga, gb, res, relu, rows, C, out, s);
+    e->span_end(sp, s);
+    e->launches += nb ? 3 : 2;
+    return VD3D_OK;
+  };
+  // 1x1 conv as a GEMM: A [rows, cin] f16 -> f32 [rows, cout]
+  auto conv1 = [&](const char* wname, const __half* in, int rows, int cin, int cout, float* out) -> int {
+    const __half* w;
+    int rr;
+    if ((rr = W(e, wname, &w, (size_t)cout * cin))) return rr;
+    GemmArgs g = base_args(rows, cout, cin, EPI_F32);
+    g.out_f32 = out;
+    const int sp = e->span_begin("bit.conv", s);
+    rr = gemm(e, in, cin, w, cin, g);
+    e->span_end(sp, s);
+    return rr;
+  };
+
+  // ---- stem ----
+  {
+    const float* w;
+    if ((r = W(e, "bit.stem.w", &w, 64 * 147))) return r;
+    int sp = e->span_begin("bit.stem", s);
+    launch_bit_stem(px, S, S, w, (float*)y, s);
+    e->span_end(sp, s);
+    e->launches++;
+    if ((r = groupnorm("bit.stem", (const float*)y, nullptr, nullptr, nullptr, 1, S2 * S2, 64, (__half*)t1))) return r;
+    sp = e->span_begin("bit.pool", s);
+    launch_maxpool_same((const __half*)t1, S2, S2, 64, (__half*)xa, s);
+    e->span_end(sp, s);
+    e->launches++;
+  }
+  // ---- stages ----
+  const __half* x = (const __half*)xa;
+  int H = S4, cin = 64;
+  for (int st = 0; st < 3; ++st) {
+    const int out_c = kBitWidths[st], mid = out_c / 4;
+    for (int k = 0; k < kBitDepths[st]; ++k) {
+      const bool first = k == 0, s2 = first && st > 0;
+      const int Ho = s2 ? H / 2 : H, rows_in = H * H, rows = Ho * Ho;
+      char pfx[32];
+      snprintf(pfx, sizeof pfx, "bit.s%d.b%d", st, k);
+      auto wn = [&](const char* suffix) {
+        snprintf(nm, sizeof nm, "%s.%s", pfx, suffix);
+        return std::string(nm);
+      };
+      // conv1 (1x1) + GN1 + ReLU at the input resolution
+      if ((r = conv1(wn("c1.w").c_str(), x, rows_in, cin, mid, (float*)y))) return r;
+      if ((r = groupnorm(wn("n1").c_str(), (const float*)y, nullptr, nullptr, nullptr, 1, rows_in, mid, (__half*)t1)))
+        return r;
+      // conv2 (3x3, stride 1 or 2) + GN2 + ReLU
+      {
+        const __half* w;
+        if ((r = W(e, wn("c2.w"), &w, (size_t)mid * 9 * mid))) return r;
+        GemmArgs g = base_args(rows, mid, 9 * mid, EPI_F32);
+        g.out_f32 = (float*)y;
+        g.ldc = mid;
+        if (s2) {
+          int sp = e->span_begin("bit.im2col", s);
+          launch_im2col_same((const __half*)t1, H, H, mid, 3, 0, (__half*)col, s);
+          e->span_end(sp, s);
+          e->launches++;
+          sp = e->span_begin("bit.conv", s);
+          r = gemm(e, (const __half*)col, 9 * mid, w, 9 * mid, g);
+          e->span_end(sp, s);
+        } else {
+          const int sp = e->span_begin("bit.conv", s);
+          r = conv(e, (const __half*)t1, H, H, mid, w, true, g);
+          e->span_end(sp, s);
+        }
+        if (r) return r;
+      }
+      if ((r = groupnorm(wn("n2").c_str(), (const float*)y, nullptr, nullptr, nullptr, 1, rows, mid, (__half*)t2)))
+        return r;
+      // conv3 (1x1) -> y; the first block's shortcut conv -> y2
+      if ((r = conv1(wn("c3.w").c_str(), (const __half*)t2, rows, mid, out_c, (float*)y))) return r;
+      __half* out = (k == kBitDepths[st] - 1 && st < 2) ? (__half*)(st == 0 ? st1 : st2)
+                                                        : (__half*)(x == (const __half*)xa ? xb : xa);
+      if (first) {
+        const __half* xs = x;
+        if (s2) {  // stride-2 1x1: the even pixels
+          const int sp = e->span_begin("bit.im2col", s);
+          launch_im2col_same(x, H, H, cin, 1, 0, (__half*)col, s);
+          e->span_end(sp, s);
+          e->launches++;
+          xs = (const __half*)col;
+        }
+        if ((r = conv1(wn("ds.w").c_str(), xs, rows, cin, out_c, (float*)y2))) return r;
+        if ((r = groupnorm(wn("n3").c_str(), (const float*)y, wn("ds").c_str(), (const float*)y2, nullptr, 1, rows,
+                           out_c, out)))
+          return r;
+      } else {
+        if ((r = groupnorm(wn("n3").c_str(), (const float*)y, nullptr, nullptr, x, 1, rows, out_c, out))) return r;
+      }
+      x = out;
+      H = Ho;
+      cin = out_c;
+    }
+  }
+  *stage3 = x;
+  return VD3D_OK;
+}
 
 // B images through the network in one pass.  The token-wise stages (LayerNorm, QKV / proj / fc1 / fc2 GEMMs) see one
 // matrix of (B-1)*NP + NT rows -- image b owns rows [b*NP, b*NP + NT), NP = NT rounded up to the 128-row tile -- so the
@@ -506,7 +722,8 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
   const int IH = c.image_h, IW = c.image_w;
   const int P = e->patch;
   const int KPE = round_up(3 * P * P, 16);  // 592 for patch 14 (588 + zero columns), 768 for 16
-  const bool dpt = e->family == VD3D_DEPTH_DPT;
+  const bool hybrid = e->family == VD3D_DEPTH_DPT_HYBRID;
+  const bool dpt = e->family == VD3D_DEPTH_DPT || hybrid;  // ViT without LayerScale, raw taps, project readout
   int r;
   char nm[96];
   // ---- buffers ----
@@ -519,26 +736,36 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
   if ((r = get_buf(e, "vt", (size_t)B * Hh * 64 * NP * 2, &vt))) return r;
   if ((r = get_buf(e, "attn", (size_t)B * NP * D * 2, &attn))) return r;
   if ((r = get_buf(e, "h", (size_t)B * NP * 4 * D * 2, &hb))) return r;
-  if ((r = get_buf(e, "ape", (size_t)NPATCH * KPE * 2, &ape))) return r;
+  if (!hybrid && (r = get_buf(e, "ape", (size_t)NPATCH * KPE * 2, &ape))) return r;
 
   // ---- patch embedding + CLS + position embeddings ----
-  const int sp_embed = e->span_begin("embed", s);
+  const int sp_embed = hybrid ? -1 : e->span_begin("embed", s);  // the hybrid's backbone has spans of its own
+  // DPT-Hybrid: the BiT stage-3 map [NPATCH, 1024] takes the place of the patch matrix (a 1x1 projection with bias)
+  const int KE = hybrid ? 1024 : KPE;
   const __half* pe_w;
   const float *pe_b, *cls, *pos;
-  if ((r = W(e, "pe.w", &pe_w, (size_t)D * KPE)) || (r = W(e, "pe.b", &pe_b, D)) || (r = W(e, "cls", &cls, D)) ||
+  if ((r = W(e, "pe.w", &pe_w, (size_t)D * KE)) || (r = W(e, "pe.b", &pe_b, D)) || (r = W(e, "cls", &cls, D)) ||
       (r = W(e, "pos", &pos, (size_t)NT * D)))
     return r;
   for (int b = 0; b < B; ++b) {
     float* xb = (float*)x + (size_t)b * NP * D;
-    launch_patch_im2col(px_dev[b], IH, IW, ph, pw, (__half*)ape, KPE, P, s);
-    GemmArgs g = base_args(NPATCH, D, KPE, EPI_PATCH);
+    const __half* a_emb = (const __half*)ape;
+    if (hybrid) {
+      if ((r = bit_backbone(e, b, px_dev[b], &a_emb))) return r;
+    } else {
+      launch_patch_im2col(px_dev[b], IH, IW, ph, pw, (__half*)ape, KPE, P, s);
+      e->launches++;
+    }
+    const int sp_proj = hybrid ? e->span_begin("bit.proj", s) : -1;
+    GemmArgs g = base_args(NPATCH, D, KE, EPI_PATCH);
     g.out_f32 = xb;
     g.bias = pe_b;
     g.pos = pos;
     g.ldc = D;
-    if ((r = gemm(e, (const __half*)ape, KPE, pe_w, KPE, g))) return r;
+    if ((r = gemm(e, a_emb, KE, pe_w, KE, g))) return r;
     launch_set_cls(xb, cls, pos, D, s);
-    e->launches += 2;
+    e->launches++;
+    e->span_end(sp_proj, s);
     // rows [NT, NP) of every image but the last take part in the stacked GEMMs: keep them at zero so that they stay
     // finite from frame to frame (they are never read as keys / values: the attention tensor maps end at NT)
     if (b + 1 < B) DCK(cudaMemsetAsync(xb + (size_t)NT * D, 0, (size_t)(NP - NT) * D * 4, s));
@@ -546,7 +773,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
 
   e->span_end(sp_embed, s);
   // ---- transformer blocks ----
-  int tap_idx = 0;
+  int tap_idx = hybrid ? 2 : 0;  // the hybrid's neck inputs 0 and 1 are BiT stages, not ViT taps
   for (int l = 0; l < L; ++l) {
     const float *g1, *b1, *g2, *b2, *bqkv, *bo, *ls1, *bf1, *bf2, *ls2;
     const __half *wqkv, *wo, *wf1, *wf2;
@@ -712,6 +939,21 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     const int C = c.neck[i], CP = round_up(C, 64);
     const __half *pw_, *cw;
     const float* pb;
+    if (hybrid && i < 2) {  // the BiT stage-1 / stage-2 map (NHWC f16, C channels) is the neck input as it is
+      fh[i] = ph * (4 >> i);
+      fw[i] = pw * (4 >> i);
+      snprintf(nm, sizeof nm, "n%d.conv.w", i);
+      if ((r = W(e, nm, &cw, (size_t)F * 9 * CP))) return r;
+      snprintf(nm, sizeof nm, "bit.stage%d.%d", i + 1, b);
+      const void* stage = e->buf[nm].p;
+      snprintf(nm, sizeof nm, "f%d", i);
+      if ((r = get_buf(e, bname(nm), (size_t)fh[i] * fw[i] * F * 2, &feat[i]))) return r;
+      GemmArgs g = base_args(0, F, 0, EPI_F16);
+      g.out_f16 = (__half*)feat[i];
+      g.ldc = F;
+      if ((r = conv(e, (const __half*)stage, fh[i], fw[i], CP, cw, true, g))) return r;
+      continue;
+    }
     snprintf(nm, sizeof nm, "r%d.proj.w", i);
     if ((r = W(e, nm, &pw_, (size_t)CP * D))) return r;
     snprintf(nm, sizeof nm, "r%d.proj.b", i);

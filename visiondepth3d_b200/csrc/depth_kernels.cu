@@ -395,6 +395,255 @@ __global__ void __launch_bounds__(256) k_add_relu_f16(const __half* __restrict__
 }
 
 // ---------------------------------------------------------------------------
+// BiT ResNet front end of DPT-Hybrid (transformers 5.5 models/bit/modeling_bit.py: BitEmbeddings and
+// BitBottleneckLayer with global_padding "SAME").  The convolutions run on k_umma_gemm; these are the stem conv, the
+// GroupNorm, the max-pool and the stride-2 im2col with TF SAME (asymmetric) padding.
+// ---------------------------------------------------------------------------
+
+// 7x7 stride-2 conv 3 -> 64 without bias, TF SAME padding (2 before, 3 after), in f32 on the CUDA cores: pixel_values
+// [3, H, W] -> y NHWC f32 [OH * OW, 64].  w: the weight-standardised kernel f32 [64, 3 * 49] (c, ky, kx order).  Each
+// output sums its taps in (c, ky, kx) order with fmaf, skipping the padding.  A warp owns 32 pixels and 16 channels,
+// so every weight read is a shared-memory broadcast.
+__global__ void __launch_bounds__(256) k_bit_stem(const float* __restrict__ px, int H, int W,
+                                                  const float* __restrict__ w, float* __restrict__ y, int OH, int OW) {
+  __shared__ float ws[64 * 147];
+  for (int i = threadIdx.x; i < 64 * 147; i += 256) ws[i] = w[i];
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int cg = warp & 3, sub = warp >> 2;
+  const int npix = OH * OW;
+  for (int p0 = blockIdx.x * 64; p0 < npix; p0 += gridDim.x * 64) {
+    const int p = p0 + sub * 32 + lane;
+    if (p >= npix) continue;
+    const int oy = p / OW, ox = p % OW;
+    const int iy0 = 2 * oy - 2, ix0 = 2 * ox - 2;
+    float acc[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) acc[j] = 0.f;
+    for (int c = 0; c < 3; ++c)
+      for (int ky = 0; ky < 7; ++ky) {
+        const int iy = iy0 + ky;
+        if (iy < 0 || iy >= H) continue;
+        const float* row = px + ((size_t)c * H + iy) * W;
+        const float* wr = ws + (cg * 16) * 147 + c * 49 + ky * 7;
+#pragma unroll
+        for (int kx = 0; kx < 7; ++kx) {
+          const int ix = ix0 + kx;
+          if (ix < 0 || ix >= W) continue;
+          const float v = __ldg(row + ix);
+#pragma unroll
+          for (int j = 0; j < 16; ++j) acc[j] = fmaf(wr[j * 147 + kx], v, acc[j]);
+        }
+      }
+    float4* dst = (float4*)(y + (size_t)p * 64 + cg * 16);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) dst[j] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
+  }
+}
+
+// GroupNorm(32) statistics of an NHWC f32 map [rows, C] (C a power of two, 64 .. 1024), one CTA per chunk of `chunk`
+// rows (gn_chunk): the chunk's mean of every group, then the sum of squared deviations from it (two passes; no E[x^2]
+// - E[x]^2), both summed in a fixed order -> part [chunk index][32] = (mean, M2).  A thread owns 4 channels of every
+// (256 / (C / 4))-th row; each group then gathers exactly 32 thread values, one per lane of a warp.
+__global__ void __launch_bounds__(256) k_gn_stats(const float* __restrict__ y, int rows, int C, int chunk,
+                                                  float2* __restrict__ part) {
+  __shared__ float red[256 * 4];
+  __shared__ float gmean[32];
+  const int t = threadIdx.x, c4n = C >> 2, R = 256 / c4n, cpg = C >> 5;
+  const int c4 = t % c4n, rl = t / c4n;
+  const int r0 = blockIdx.x * chunk, r1 = min(rows, r0 + chunk);
+  const int warp = t >> 5, lane = t & 31;
+  const float n = (float)((r1 - r0) * cpg);
+  auto group_sum = [&](int g) {  // the 32 values of group g: row lane lane / cpg, channel g * cpg + lane % cpg
+    const int ch = g * cpg + lane % cpg;
+    float v = red[((lane / cpg) * c4n + (ch >> 2)) * 4 + (ch & 3)];
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+  };
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int r = r0 + rl; r < r1; r += R) {
+    const float4 v = __ldg((const float4*)(y + (size_t)r * C) + c4);
+    s.x += v.x;
+    s.y += v.y;
+    s.z += v.z;
+    s.w += v.w;
+  }
+  *(float4*)(red + 4 * t) = s;
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float v = group_sum(warp + 8 * i);
+    if (lane == 0) gmean[warp + 8 * i] = v / n;
+  }
+  __syncthreads();
+  const float m0 = gmean[(4 * c4) / cpg], m1 = gmean[(4 * c4 + 1) / cpg], m2 = gmean[(4 * c4 + 2) / cpg],
+              m3 = gmean[(4 * c4 + 3) / cpg];
+  float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int r = r0 + rl; r < r1; r += R) {
+    const float4 v = __ldg((const float4*)(y + (size_t)r * C) + c4);
+    const float a = v.x - m0, b = v.y - m1, c = v.z - m2, d = v.w - m3;
+    q.x = fmaf(a, a, q.x);
+    q.y = fmaf(b, b, q.y);
+    q.z = fmaf(c, c, q.z);
+    q.w = fmaf(d, d, q.w);
+  }
+  *(float4*)(red + 4 * t) = q;
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int g = warp + 8 * i;
+    const float v = group_sum(g);
+    if (lane == 0) part[(size_t)blockIdx.x * 32 + g] = make_float2(gmean[g], v);
+  }
+}
+
+// Chan et al.'s pairwise update: (n, mean, M2) of the union of two disjoint sets
+__device__ __forceinline__ void chan_merge(float& n, float& m, float& M2, float nb, float mb, float Mb) {
+  if (nb == 0.f) return;
+  if (n == 0.f) {
+    n = nb;
+    m = mb;
+    M2 = Mb;
+    return;
+  }
+  const float nn = n + nb, d = mb - m;
+  m = fmaf(d, nb / nn, m);
+  M2 = M2 + Mb + d * d * (n * nb / nn);
+  n = nn;
+}
+
+// mean and 1 / sqrt(var + eps) of group g from the chunk partials of k_gn_stats, by one warp: lane l merges chunks l,
+// l + 32, ... in order, then lanes merge down a fixed tree into lane 0, which stores them to st[0][g] / st[1][g].  The
+// same order in every CTA and every launch.
+__device__ __forceinline__ void gn_group_stats(const float2* __restrict__ part, int rows, int chunk, int cpg, int g,
+                                               float eps, int lane, float (*st)[32]) {
+  const int nch = (rows + chunk - 1) / chunk;
+  float n = 0.f, m = 0.f, M2 = 0.f;
+  for (int k = lane; k < nch; k += 32) {
+    const float2 p = part[(size_t)k * 32 + g];
+    chan_merge(n, m, M2, (float)((min(rows, (k + 1) * chunk) - k * chunk) * cpg), p.x, p.y);
+  }
+  for (int o = 16; o; o >>= 1) {
+    const float nb = __shfl_down_sync(0xffffffffu, n, o), mb = __shfl_down_sync(0xffffffffu, m, o),
+                Mb = __shfl_down_sync(0xffffffffu, M2, o);
+    if (lane < o) chan_merge(n, m, M2, nb, mb, Mb);
+  }
+  if (lane == 0) {
+    st[0][g] = m;
+    st[1][g] = rsqrtf(M2 / n + eps);
+  }
+}
+
+// v[j] (+)= (y - mean) rstd gamma + beta for the 8 channels c0 .. c0 + 7 of the f32 element offset o
+__device__ __forceinline__ void gn_norm8(const GnInput& in, const float (*st)[32], size_t o, int c0, int cpg, bool add,
+                                         float* v) {
+  float y[8], gm[8], bt[8];
+  *(float4*)y = __ldg((const float4*)(in.y + o));
+  *(float4*)(y + 4) = __ldg((const float4*)(in.y + o) + 1);
+  *(float4*)gm = __ldg((const float4*)(in.gamma + c0));
+  *(float4*)(gm + 4) = __ldg((const float4*)(in.gamma + c0) + 1);
+  *(float4*)bt = __ldg((const float4*)(in.beta + c0));
+  *(float4*)(bt + 4) = __ldg((const float4*)(in.beta + c0) + 1);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int grp = (c0 + j) / cpg;
+    const float r = (y[j] - st[0][grp]) * st[1][grp] * gm[j] + bt[j];
+    v[j] = add ? v[j] + r : r;
+  }
+}
+
+// GroupNorm apply on NHWC f32 [rows, C] -> f16: out = [relu]( (y - mean) rstd gamma + beta  [+ the same of y2 with its
+// own statistics and affine]  [+ res] ).  8 channels per thread: two 16-byte loads per f32 input, one 16-byte store.
+__global__ void __launch_bounds__(256) k_gn_apply(GnInput a, GnInput b, const __half* __restrict__ res, int relu,
+                                                  int rows, int C, int chunk, float eps, __half* __restrict__ out) {
+  __shared__ float st[2][2][32];  // [input][mean, rstd][group]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, cpg = C >> 5;
+#pragma unroll 1
+  for (int i = 0; i < 4; ++i) {
+    gn_group_stats(a.part, rows, chunk, cpg, warp + 8 * i, eps, lane, st[0]);
+    if (b.y) gn_group_stats(b.part, rows, chunk, cpg, warp + 8 * i, eps, lane, st[1]);
+  }
+  __syncthreads();
+  const size_t idx = (size_t)blockIdx.x * 256 + threadIdx.x;
+  const int c8n = C >> 3;
+  if (idx >= (size_t)rows * c8n) return;
+  const int c0 = (int)(idx % c8n) * 8;
+  const size_t o = idx * 8;
+  __align__(16) float v[8];
+  gn_norm8(a, st[0], o, c0, cpg, false, v);
+  if (b.y) gn_norm8(b, st[1], o, c0, cpg, true, v);
+  if (res) {
+    const uint4 rv = __ldg((const uint4*)(res + o));
+    const __half2* h = (const __half2*)&rv;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = __half22float2(h[j]);
+      v[2 * j] += f.x;
+      v[2 * j + 1] += f.y;
+    }
+  }
+  uint4 u;
+  __half2* hu = (__half2*)&u;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float x0 = v[2 * j], x1 = v[2 * j + 1];
+    if (relu) {
+      x0 = fmaxf(x0, 0.f);
+      x1 = fmaxf(x1, 0.f);
+    }
+    hu[j] = __floats2half2_rn(x0, x1);
+  }
+  *(uint4*)(out + o) = u;
+}
+
+// 3x3 stride-2 max-pool with TF SAME padding (0 before, 1 after, pad value 0: BitMaxPool2d with dynamic padding) on
+// NHWC f16 [H, W, C] -> [OH, OW, C], 8 channels per thread
+__global__ void __launch_bounds__(256) k_maxpool_same(const __half* __restrict__ in, int H, int W, int C,
+                                                      __half* __restrict__ out, int OH, int OW) {
+  const size_t idx = (size_t)blockIdx.x * 256 + threadIdx.x;
+  const int c8n = C >> 3;
+  if (idx >= (size_t)OH * OW * c8n) return;
+  const int c8 = (int)(idx % c8n);
+  const size_t o = idx / c8n;
+  const int ox = (int)(o % OW), oy = (int)(o / OW);
+  const bool padded = 2 * oy + 2 >= H || 2 * ox + 2 >= W;
+  const __half2 init = padded ? __floats2half2_rn(0.f, 0.f) : __half2half2(__ushort_as_half(0xFC00u));  // 0 or -inf
+  __half2 m[4] = {init, init, init, init};
+  for (int dy = 0; dy < 3; ++dy) {
+    const int iy = 2 * oy + dy;
+    if (iy >= H) break;
+    for (int dx = 0; dx < 3; ++dx) {
+      const int ix = 2 * ox + dx;
+      if (ix >= W) break;
+      const uint4 v = __ldg((const uint4*)(in + ((size_t)iy * W + ix) * C) + c8);
+      const __half2* h = (const __half2*)&v;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) m[j] = __hmax2(m[j], h[j]);
+    }
+  }
+  ((uint4*)(out + o * C))[c8] = *(const uint4*)m;
+}
+
+// stride-2 im2col of a k x k conv (k = 1 or 3) with TF SAME padding: `pb` zero rows / columns before, the rest after,
+// on NHWC f16 [H, W, C] -> [OH * OW, k * k * C], column tap * C + c.  k = 1, pb = 0 is the subsample of the even pixels.
+// 8 channels per thread.
+__global__ void __launch_bounds__(256) k_im2col_same(const __half* __restrict__ in, int H, int W, int C, int k, int pb,
+                                                     __half* __restrict__ out, int OH, int OW) {
+  const size_t idx = (size_t)blockIdx.x * 256 + threadIdx.x;
+  const int c8n = C >> 3, kk = k * k;
+  if (idx >= (size_t)OH * OW * kk * c8n) return;
+  const int c8 = (int)(idx % c8n);
+  const size_t r = idx / c8n;
+  const int tap = (int)(r % kk);
+  const size_t o = r / kk;
+  const int ox = (int)(o % OW), oy = (int)(o / OW);
+  const int iy = 2 * oy - pb + tap / k, ix = 2 * ox - pb + tap % k;
+  uint4 v = make_uint4(0u, 0u, 0u, 0u);
+  if (iy >= 0 && iy < H && ix >= 0 && ix < W) v = __ldg((const uint4*)(in + ((size_t)iy * W + ix) * C) + c8);
+  ((uint4*)out)[idx] = v;
+}
+
+// ---------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------
 void launch_preprocess(const uint8_t* frame_bgr, int H, int W, uint8_t* tmp_u8, uint8_t* rgb_u8, float* px, int OH,
@@ -576,6 +825,33 @@ cudaError_t launch_gemm_sr(int bn, const CUtensorMap& a, const CUtensorMap& b, c
     case 32: return launch_gemm_t<32, 6, true>(a, b, g, grid, s);
     default: return cudaErrorInvalidValue;
   }
+}
+
+// BiT front end of DPT-Hybrid
+void launch_bit_stem(const float* px, int H, int W, const float* w, float* y, cudaStream_t s) {
+  const int OH = H / 2, OW = W / 2;
+  const int blocks = (OH * OW + 63) / 64, cap = 4 * sm_count();  // 37.6 KB of weights per CTA: a few CTAs per SM
+  k_bit_stem<<<blocks < cap ? blocks : cap, 256, 0, s>>>(px, H, W, w, y, OH, OW);
+}
+int gn_chunk(int rows) { return (rows + kGnMaxChunks - 1) / kGnMaxChunks; }
+void launch_gn_stats(const float* y, int rows, int C, float2* part, cudaStream_t s) {
+  const int chunk = gn_chunk(rows);
+  k_gn_stats<<<(rows + chunk - 1) / chunk, 256, 0, s>>>(y, rows, C, chunk, part);
+}
+void launch_gn_apply(const GnInput& a, const GnInput& b, const __half* res, int relu, int rows, int C, __half* out,
+                     cudaStream_t s) {
+  const size_t total = (size_t)rows * (C / 8);
+  k_gn_apply<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(a, b, res, relu, rows, C, gn_chunk(rows), kGnEps, out);
+}
+void launch_maxpool_same(const __half* in, int H, int W, int C, __half* out, cudaStream_t s) {
+  const int OH = H / 2, OW = W / 2;
+  const size_t total = (size_t)OH * OW * (C / 8);
+  k_maxpool_same<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, H, W, C, out, OH, OW);
+}
+void launch_im2col_same(const __half* in, int H, int W, int C, int k, int pb, __half* out, cudaStream_t s) {
+  const int OH = H / 2, OW = W / 2;
+  const size_t total = (size_t)OH * OW * k * k * (C / 8);
+  k_im2col_same<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(in, H, W, C, k, pb, out, OH, OW);
 }
 
 }  // namespace vd3d

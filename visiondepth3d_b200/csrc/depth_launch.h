@@ -48,6 +48,29 @@ cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const C
 // bn in {32, 64, 128}; grid = (ceil(N/bn), m_tiles, batch)
 cudaError_t launch_gemm(int bn, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, int m_tiles,
                         int batch, cudaStream_t s);
+// ---- BiT front end of DPT-Hybrid (even H, W; the output of every stride-2 op is H/2 x W/2) ----
+// 7x7 stride-2 stem conv 3 -> 64 in f32 (SAME: pad 2 before, 3 after): px [3, H, W], w f32 [64, 147] -> y f32 NHWC
+void launch_bit_stem(const float* px, int H, int W, const float* w, float* y, cudaStream_t s);
+// GroupNorm(32, eps 1e-5) on NHWC f32 [rows, C], C a power of two in 64..1024.  Statistics: chunk partials (mean, M2)
+// float2 [ceil(rows / gn_chunk(rows))][32] (at most kGnMaxChunks chunks), merged in a fixed order by the apply kernel.
+constexpr int kGnMaxChunks = 128;
+constexpr float kGnEps = 1e-5f;
+int gn_chunk(int rows);
+void launch_gn_stats(const float* y, int rows, int C, float2* part, cudaStream_t s);
+// one GroupNorm'd input: the map, its partials and its affine (f32 [C])
+struct GnInput {
+  const float* y;
+  const float2* part;
+  const float *gamma, *beta;
+};
+// out f16 [rows, C] = [relu](GN_a(a.y) [+ GN_b(b.y) when b.y] [+ res f16 [rows, C]])
+void launch_gn_apply(const GnInput& a, const GnInput& b, const __half* res, int relu, int rows, int C, __half* out,
+                     cudaStream_t s);
+// 3x3 stride-2 max-pool, SAME padding 0 before / 1 after with pad value 0: f16 NHWC [H, W, C] -> [H/2, W/2, C]
+void launch_maxpool_same(const __half* in, int H, int W, int C, __half* out, cudaStream_t s);
+// stride-2 im2col of a k x k conv (k 1 or 3) with `pb` zero pixels before and the rest after: f16 NHWC [H, W, C] ->
+// [(H/2) * (W/2), k * k * C] (tap-major); k = 1, pb = 0: the even pixels.  C a multiple of 8.
+void launch_im2col_same(const __half* in, int H, int W, int C, int k, int pb, __half* out, cudaStream_t s);
 // launch_gemm for the RRDBNet convs (epilogue EPI_SR), batch 1
 cudaError_t launch_gemm_sr(int bn, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, int m_tiles,
                            cudaStream_t s);

@@ -5,8 +5,8 @@ import sys as _sys
 import numpy as np
 
 from . import _lib
-from .depth_weights import (DA_PROCESSOR, DPT_CONFIGS, DPT_PROCESSOR, da_spec, dpt_processed_size, is_plain_v2, prepare,
-                            prepare_dpt)
+from .depth_weights import (DA_PROCESSOR, DPT_CONFIGS, DPT_HYBRID_CONFIGS, DPT_PROCESSOR, da_spec, dpt_processed_size,
+                            is_plain_v2, prepare, prepare_dpt, prepare_dpt_hybrid)
 
 
 def processed_size(width, height, target=518, multiple=14):
@@ -37,7 +37,9 @@ class DepthConfigEx(C.Structure):
 HEAD_KINDS = {"relative": 0, "metric": 1}  # VD3D_HEAD_RELATIVE / VD3D_HEAD_METRIC
 
 
-FAMILY_DA_V2, FAMILY_DPT = "da-v2", "dpt"
+FAMILY_DA_V2, FAMILY_DPT, FAMILY_DPT_HYBRID = "da-v2", "dpt", "dpt-hybrid"
+_FAMILY_CODES = {FAMILY_DA_V2: 0, FAMILY_DPT: 1, FAMILY_DPT_HYBRID: 2}  # VD3D_DEPTH_DA_V2 / _DPT / _DPT_HYBRID
+_DPT_LIKE = (FAMILY_DPT, FAMILY_DPT_HYBRID)  # the fixed-size DPT image processor
 
 
 def _bind(lib):
@@ -66,6 +68,8 @@ def _bind(lib):
     lib.vd3d_gemm_f16.restype = i
     lib.vd3d_conv_f16.argtypes = [vp, vp, i, i, i, vp, i, i, vp, i, vp]
     lib.vd3d_conv_f16.restype = i
+    lib.vd3d_bit_kernel.argtypes = [vp, i, C.POINTER(C.c_int32)]
+    lib.vd3d_bit_kernel.restype = i
     lib.vd3d_depth_infer_batch.argtypes = [vp, i, C.POINTER(vp), i, i, C.POINTER(vp), C.POINTER(vp), i]
     lib.vd3d_depth_infer_batch.restype = i
     lib.vd3d_depth_infer_batch_device.argtypes = [vp, i, C.POINTER(vp), i, i, C.POINTER(vp), C.POINTER(vp), i]
@@ -88,8 +92,9 @@ def _bind(lib):
 
 class DepthEngine:
     """Depth forward on wgmma tensor cores.  family "da-v2" (default): Depth-Anything, `cfg` a key of CONFIGS or a
-    spec dict (depth_weights.da_spec / da_config_from_json: the V2 sizes, V1's taps, a metric head).  family "dpt": DPT-Large (ViT-L/16, project readout), `cfg` a key of DPT_CONFIGS or a dict, `processor` the
-    image processor's settings (depth_weights.DPT_PROCESSOR, or dpt_processor_from_json of a checkpoint's
+    spec dict (depth_weights.da_spec / da_config_from_json: the V2 sizes, V1's taps, a metric head).  family "dpt": DPT-Large (ViT-L/16, project readout), `cfg` a key of DPT_CONFIGS or a dict; family
+    "dpt-hybrid": MiDaS 3.0 (BiT ResNet-50 front end + ViT-B/16), `cfg` a key of DPT_HYBRID_CONFIGS or a dict.  For
+    both DPT families `processor` is the image processor's settings (depth_weights.DPT_PROCESSOR, or dpt_processor_from_json of a checkpoint's
     preprocessor_config.json); the processed size is the processor's, image_h / image_w default to it."""
 
     def __init__(self, cfg="vits", image_h=None, image_w=None, ctx=None, device=0, family=FAMILY_DA_V2,
@@ -97,15 +102,17 @@ class DepthEngine:
         self.lib = _lib.load()
         _bind(self.lib)
         self.ctx = ctx or _lib.default_context(device)
-        if family not in (FAMILY_DA_V2, FAMILY_DPT):
+        if family not in _FAMILY_CODES:
             raise ValueError(f"unknown depth model family {family!r}")
         self.family = family
         if family == FAMILY_DPT:
             self.cfg = dict(DPT_CONFIGS[cfg]) if isinstance(cfg, str) else dict(cfg)
+        elif family == FAMILY_DPT_HYBRID:
+            self.cfg = dict(DPT_HYBRID_CONFIGS[cfg]) if isinstance(cfg, str) else dict(cfg)
         else:
             self.cfg = da_spec(cfg)  # taps, head and max_depth of the spec; V2's relative head by default
         c = self.cfg
-        if family == FAMILY_DPT:
+        if family in _DPT_LIKE:
             self.processor = dict(processor or DPT_PROCESSOR)
             ph, pw = dpt_processed_size(self.processor)
             image_h, image_w = image_h or ph, image_w or pw
@@ -117,9 +124,9 @@ class DepthEngine:
                          (C.c_int32 * 4)(*c["neck"]), c["fusion"], self.image_h, self.image_w)
         h = C.c_void_p()
         stream = self.lib.vd3d_stream(self.ctx.h)
-        if family == FAMILY_DPT:
+        if family in _DPT_LIKE:
             p = self.processor
-            dx = DepthConfigEx(dc, 1, c["patch"], c["ln_eps"], p["resample"], (C.c_float * 3)(*p["mean"]),
+            dx = DepthConfigEx(dc, _FAMILY_CODES[family], c["patch"], c["ln_eps"], p["resample"], (C.c_float * 3)(*p["mean"]),
                                (C.c_float * 3)(*p["std"]), HEAD_KINDS["relative"], 1.0)
             rc = self.lib.vd3d_depth_create_ex(C.byref(dx), stream, C.byref(h))
         elif not is_plain_v2(c):  # Depth Anything V1, Distill-Any-Depth, the V2 metric models
@@ -136,7 +143,7 @@ class DepthEngine:
     def processed_size(self, width, height):
         """(h, w) the model's image processor resizes a (width, height) image to: Depth-Anything's keep-aspect
         multiple-of-14 size, DPT's fixed size."""
-        if self.family == FAMILY_DPT:
+        if self.family in _DPT_LIKE:
             return dpt_processed_size(self.processor)
         return processed_size(width, height)
 
@@ -145,7 +152,7 @@ class DepthEngine:
             raise _lib.Vd3dError(f"libvd3d depth error {rc}: {self.lib.vd3d_depth_last_error(self.h).decode()}")
 
     def load_state_dict(self, sd):
-        prep = prepare_dpt if self.family == FAMILY_DPT else prepare
+        prep = {FAMILY_DPT: prepare_dpt, FAMILY_DPT_HYBRID: prepare_dpt_hybrid}.get(self.family, prepare)
         for name, arr in prep(sd, self.cfg, self.image_h, self.image_w).items():
             arr = np.ascontiguousarray(arr)
             self.check(self.lib.vd3d_depth_set_tensor(self.h, name.encode(), arr.ctypes.data, arr.nbytes))
@@ -309,6 +316,15 @@ class DepthEngine:
         self.check(self.lib.vd3d_conv_f16(self.h, x.ctypes.data, H, W_, cin, w.ctypes.data, cout, int(k3),
                                           b.ctypes.data if b is not None else None, int(relu), out.ctypes.data))
         return out
+
+    def bit_kernel(self, op, dims, tensors, out_shape, out_dtype):
+        """vd3d_bit_kernel: upload `tensors` ({"t.in": array, ...}) and run one BiT kernel op on them -> "t.out"."""
+        for name, arr in tensors.items():
+            arr = np.ascontiguousarray(arr)
+            self.check(self.lib.vd3d_depth_set_tensor(self.h, name.encode(), arr.ctypes.data, arr.nbytes))
+        d = (C.c_int32 * 5)(*(list(dims) + [0] * (5 - len(dims))))
+        self.check(self.lib.vd3d_bit_kernel(self.h, int(op), d))
+        return self.get_buffer("t.out", out_shape, out_dtype)
 
     @property
     def launches(self):

@@ -234,14 +234,17 @@ def prepare(sd, cfg, image_h, image_w):
     return out
 
 
-def _prepare_tail(sd, cfg):
+def _prepare_tail(sd, cfg, direct=()):
     """The reassemble layers, neck convs, fusion stage and head (HF names of DepthAnythingForDepthEstimation) in the
     engine's layouts: shared by Depth-Anything and DPT.  Fusion layer 0 never runs its residual_layer1; it is packed
-    when the state dict has it."""
+    when the state dict has it.  direct: neck inputs without a reassemble layer (DPT-Hybrid's BiT stages 1 and 2)."""
     D, Fz = cfg["hidden"], cfg["fusion"]
     out = {}
     for i, C in enumerate(cfg["neck"]):
         CP = _up(C, 64)
+        if i in direct:
+            out[f"n{i}.conv.w"] = _conv3(sd[f"neck.convs.{i}.weight"], CP)
+            continue
         r = f"neck.reassemble_stage.layers.{i}."
         pw_ = torch.zeros(CP, D)
         pw_[:C] = sd[r + "projection.weight"].float().reshape(C, D)
@@ -429,11 +432,20 @@ def prepare_dpt(sd, cfg, image_h, image_w):
     and CLS halves "ro{i}.wt" / "ro{i}.wc")."""
     check_dpt_state_dict(sd, cfg)
     D, P = cfg["hidden"], cfg["patch"]
-    ph, pw = image_h // P, image_w // P
     e = "dpt.embeddings."
     out = {"pe.w": _f16(sd[e + "patch_embeddings.projection.weight"].float().reshape(D, 3 * P * P)),
-           "pe.b": _f32(sd[e + "patch_embeddings.projection.bias"]),
-           "cls": _f32(sd[e + "cls_token"].reshape(D))}
+           "pe.b": _f32(sd[e + "patch_embeddings.projection.bias"])}
+    out.update(_prepare_dpt_vit(sd, cfg, image_h, image_w, range(4)))
+    return out
+
+
+def _prepare_dpt_vit(sd, cfg, image_h, image_w, readouts, direct=()):
+    """DPT's CLS token, position embeddings, ViT layers, the project readouts `readouts` and the neck, fusion and head
+    (shared by DPT-Large and DPT-Hybrid)."""
+    D, P = cfg["hidden"], cfg["patch"]
+    ph, pw = image_h // P, image_w // P
+    e = "dpt.embeddings."
+    out = {"cls": _f32(sd[e + "cls_token"].reshape(D))}
     pos = sd[e + "position_embeddings"].float()
     g = int(round((pos.shape[1] - 1) ** 0.5))
     pp = pos[:, 1:].reshape(1, g, g, D).permute(0, 3, 1, 2)
@@ -457,7 +469,7 @@ def prepare_dpt(sd, cfg, image_h, image_w):
         out[f"l{i}.fc2.w"] = _f16(sd[p + "output.dense.weight"])
         out[f"l{i}.fc2.b"] = _f32(sd[p + "output.dense.bias"])
         out[f"l{i}.ls2"] = ones
-    for i in range(4):
+    for i in readouts:
         r = f"neck.reassemble_stage.readout_projects.{i}.0."
         w = sd[r + "weight"].float()
         out[f"ro{i}.wt"] = _f16(w[:, :D])
@@ -469,5 +481,193 @@ def prepare_dpt(sd, cfg, image_h, image_w):
     for j, n in ((0, "conv1"), (2, "conv2"), (4, "conv3")):
         shared[f"head.{n}.weight"] = sd[f"head.head.{j}.weight"]
         shared[f"head.{n}.bias"] = sd[f"head.head.{j}.bias"]
-    out.update(_prepare_tail(shared, cfg))
+    out.update(_prepare_tail(shared, cfg, direct))
+    return out
+
+
+# ---------------------------------------------------------------------------
+# DPT-Hybrid / MiDaS 3.0 (Intel/dpt-hybrid-midas; transformers 5.5 DPTForDepthEstimation with is_hybrid=True): a BiT
+# ResNet-50 front end (BitConfig layer_type "bottleneck", global_padding "SAME", depths [3, 4, 9], 32 groups) whose
+# stage-3 map, projected 1024 -> hidden by a 1x1 conv, is the ViT-B/16's token grid; the stage-1 and stage-2 maps are
+# neck inputs 0 and 1 as they are; the residual stream after layers 9 and 12 (backbone_out_indices[2:]) feeds readouts
+# 2 and 3.  From the ViT on it is DPT-Large's path.
+# ---------------------------------------------------------------------------
+DPT_HYBRID_CONFIGS = {
+    "dpt-hybrid-midas": dict(hidden=768, layers=12, heads=12, taps=[3, 6, 9, 12], neck=[256, 512, 768, 768],
+                             fusion=256, patch=16, ln_eps=1e-12, image_size=384),
+}
+BIT_DEPTHS, BIT_WIDTHS, BIT_GROUPS = (3, 4, 9), (256, 512, 1024), 32
+
+
+def hf_dpt_hybrid_config(name="dpt-hybrid-midas", **cfg):
+    """transformers DPTConfig of the hybrid checkpoint (Intel/dpt-hybrid-midas's config.json as far as the engine reads
+    it); `cfg` overrides entries of DPT_HYBRID_CONFIGS[name] (a smaller ViT and image for tests)."""
+    from transformers import DPTConfig
+    c = dict(DPT_HYBRID_CONFIGS[name], **cfg)
+    g = c["image_size"] // c["patch"]
+    return DPTConfig(hidden_size=c["hidden"], num_hidden_layers=c["layers"], num_attention_heads=c["heads"],
+                     intermediate_size=4 * c["hidden"], hidden_act="gelu", layer_norm_eps=c["ln_eps"],
+                     image_size=c["image_size"], patch_size=c["patch"], num_channels=3, qkv_bias=True,
+                     is_hybrid=True, backbone_out_indices=[t - 1 for t in c["taps"]], readout_type="project",
+                     reassemble_factors=[1, 1, 1, 0.5], neck_hidden_sizes=c["neck"], fusion_hidden_size=c["fusion"],
+                     head_in_index=-1, use_batch_norm_in_fusion_residual=False, use_bias_in_fusion_residual=None,
+                     add_projection=False, backbone_featmap_shape=[1, 1024, g, g],
+                     backbone_config=dict(model_type="bit", layer_type="bottleneck", global_padding="same",
+                                          embedding_dynamic_padding=True, depths=list(BIT_DEPTHS),
+                                          hidden_sizes=[256, 512, 1024, 2048], embedding_size=64,
+                                          num_groups=BIT_GROUPS, hidden_act="relu",
+                                          out_features=["stage1", "stage2", "stage3"]))
+
+
+def dpt_hybrid_config_from_json(cj):
+    """The engine configuration of a DPT-Hybrid config.json (dict), or ValueError naming the field the engine does not
+    serve: the backbone must be BiT's bottleneck ResNet with SAME padding, depths [3, 4, 9], widths 256 / 512 / 1024 and
+    32 groups; readout "project", reassemble_factors [1, 1, 1, 0.5], neck_hidden_sizes[:2] [256, 512], no head
+    projection or batch-norm fusion units."""
+    def bad(field, value):
+        raise ValueError(f"config.json: {field} = {value!r} is not served (DPT-Hybrid: BiT ResNet-50 stages 1-3 and a "
+                         "ViT with project readout)")
+    if cj.get("model_type", "dpt") != "dpt":
+        bad("model_type", cj.get("model_type"))
+    if cj.get("is_hybrid") is not True:
+        bad("is_hybrid", cj.get("is_hybrid"))
+    bj = cj.get("backbone_config")
+    if not isinstance(bj, dict):
+        bad("backbone_config", bj)
+    if bj.get("model_type", "bit") != "bit":
+        bad("backbone_config.model_type", bj.get("model_type"))
+    if bj.get("layer_type") != "bottleneck":
+        bad("backbone_config.layer_type", bj.get("layer_type"))
+    if str(bj.get("global_padding", "")).upper() != "SAME":
+        bad("backbone_config.global_padding", bj.get("global_padding"))
+    if bj.get("embedding_dynamic_padding") is not True:
+        bad("backbone_config.embedding_dynamic_padding", bj.get("embedding_dynamic_padding"))
+    if list(bj.get("depths", [])) != list(BIT_DEPTHS):
+        bad("backbone_config.depths", bj.get("depths"))
+    hs = bj.get("hidden_sizes", [])
+    if list(hs)[:3] != list(BIT_WIDTHS):
+        bad("backbone_config.hidden_sizes", hs)
+    for field, want in (("num_groups", BIT_GROUPS), ("embedding_size", 64), ("num_channels", 3),
+                        ("hidden_act", "relu"), ("width_factor", 1), ("output_stride", 32)):
+        if bj.get(field, want) != want:
+            bad(f"backbone_config.{field}", bj.get(field))
+    if list(bj.get("out_features", ["stage1", "stage2", "stage3"])) != ["stage1", "stage2", "stage3"]:
+        bad("backbone_config.out_features", bj.get("out_features"))
+    if cj.get("readout_type", "project") != "project":
+        bad("readout_type", cj.get("readout_type"))
+    if [float(f) for f in cj.get("reassemble_factors", [4, 2, 1, 0.5])] != [1.0, 1.0, 1.0, 0.5]:
+        bad("reassemble_factors", cj.get("reassemble_factors"))
+    neck = cj.get("neck_hidden_sizes", [96, 192, 384, 768])
+    if not isinstance(neck, (list, tuple)) or len(neck) != 4 or list(neck[:2]) != [256, 512]:
+        bad("neck_hidden_sizes", neck)
+    if cj.get("add_projection"):
+        bad("add_projection", cj.get("add_projection"))
+    if cj.get("use_batch_norm_in_fusion_residual"):
+        bad("use_batch_norm_in_fusion_residual", cj.get("use_batch_norm_in_fusion_residual"))
+    if cj.get("use_bias_in_fusion_residual") is False:
+        bad("use_bias_in_fusion_residual", False)
+    if cj.get("hidden_act", "gelu") != "gelu":
+        bad("hidden_act", cj.get("hidden_act"))
+    if cj.get("head_in_index", -1) != -1:
+        bad("head_in_index", cj.get("head_in_index"))
+    hidden = int(cj.get("hidden_size", 768))
+    heads = int(cj.get("num_attention_heads", 12))
+    if int(cj.get("intermediate_size", 4 * hidden)) != 4 * hidden:
+        bad("intermediate_size", cj.get("intermediate_size"))
+    if hidden != 64 * heads:
+        bad("hidden_size / num_attention_heads", (hidden, heads))
+    if int(cj.get("patch_size", 16)) != 16:
+        bad("patch_size", cj.get("patch_size"))
+    layers = int(cj.get("num_hidden_layers", 12))
+    taps = cj.get("backbone_out_indices", [2, 5, 8, 11])
+    if (not isinstance(taps, (list, tuple)) or len(taps) != 4 or any(type(t) is not int for t in taps)
+            or not 0 <= taps[0] < taps[1] < taps[2] < taps[3] < layers):
+        bad("backbone_out_indices", taps)
+    size = cj.get("image_size", 384)
+    fmap = cj.get("backbone_featmap_shape", [1, 1024, size // 16, size // 16])
+    if list(fmap)[1:] != [1024, size // 16, size // 16]:
+        bad("backbone_featmap_shape", fmap)
+    return dict(hidden=hidden, layers=layers, heads=heads, taps=[int(t) + 1 for t in taps],
+                neck=[int(v) for v in neck], fusion=int(cj.get("fusion_hidden_size", 256)), patch=16,
+                ln_eps=float(cj.get("layer_norm_eps", 1e-12)), image_size=int(size))
+
+
+_BIT = "dpt.embeddings.backbone.bit."
+
+
+def dpt_hybrid_keys(cfg):
+    """Every state_dict key (and its shape) the DPT-Hybrid depth forward reads: DPT's keys without the patch embedding,
+    readouts 0 / 1 and reassemble layers 0 / 1, plus the BiT stem and stages and the 1x1 projection."""
+    k = {n: v for n, v in dpt_keys(cfg).items() if not n.startswith("dpt.embeddings.patch_embeddings.")
+         and not any(n.startswith(f"neck.reassemble_stage.{m}.{i}.") for m in ("readout_projects", "layers")
+                     for i in (0, 1))}
+    k[_BIT + "embedder.convolution.weight"] = (64, 3, 7, 7)
+    k[_BIT + "embedder.norm.weight"] = k[_BIT + "embedder.norm.bias"] = (64,)
+    cin = 64
+    for st, (depth, out_c) in enumerate(zip(BIT_DEPTHS, BIT_WIDTHS)):
+        mid = out_c // 4
+        for b in range(depth):
+            p = f"{_BIT}encoder.stages.{st}.layers.{b}."
+            if b == 0:
+                k[p + "downsample.conv.weight"] = (out_c, cin, 1, 1)
+                k[p + "downsample.norm.weight"] = k[p + "downsample.norm.bias"] = (out_c,)
+            k[p + "conv1.weight"] = (mid, cin if b == 0 else out_c, 1, 1)
+            k[p + "conv2.weight"] = (mid, mid, 3, 3)
+            k[p + "conv3.weight"] = (out_c, mid, 1, 1)
+            for n, c in (("norm1", mid), ("norm2", mid), ("norm3", out_c)):
+                k[p + n + ".weight"] = k[p + n + ".bias"] = (c,)
+        cin = out_c
+    k["dpt.embeddings.projection.weight"] = (cfg["hidden"], 1024, 1, 1)
+    k["dpt.embeddings.projection.bias"] = (cfg["hidden"],)
+    return k
+
+
+def check_dpt_hybrid_state_dict(sd, cfg):
+    """ValueError naming the first missing or mis-shaped key the DPT-Hybrid forward reads."""
+    for name, shape in dpt_hybrid_keys(cfg).items():
+        if name not in sd:
+            raise ValueError(f"DPT-Hybrid state dict: missing key {name}")
+        if tuple(sd[name].shape) != shape:
+            raise ValueError(f"DPT-Hybrid state dict: {name} has shape {tuple(sd[name].shape)}, expected {shape}")
+
+
+def standardize_weight(w, eps=1e-8):
+    """BiT's weight standardisation (WeightStandardizedConv2d: batch_norm over each output channel's weights, biased
+    variance, eps 1e-8) in float64: (w - mean) / sqrt(var + eps)."""
+    w = w.detach().double()
+    flat = w.reshape(w.shape[0], -1)
+    m = flat.mean(dim=1, keepdim=True)
+    v = ((flat - m) ** 2).mean(dim=1, keepdim=True)
+    return ((flat - m) / torch.sqrt(v + eps)).reshape(w.shape)
+
+
+def prepare_dpt_hybrid(sd, cfg, image_h, image_w):
+    """DPT-Hybrid state_dict -> {name: np.ndarray} in the layouts depth_engine.cu expects: the BiT convs weight-
+    standardised in float64 at load time, then f16 ("bit.s{st}.b{k}.c{1,2,3}.w", ".ds.w"; 3x3 kernels tap-major) or
+    f32 for the stem conv, which runs in f32 ("bit.stem.w" [64, 147]); GroupNorm affines f32; the 1x1 projection as
+    "pe.w" / "pe.b"; the ViT, readouts 2 / 3, neck, fusion and head as for DPT-Large."""
+    check_dpt_hybrid_state_dict(sd, cfg)
+    D = cfg["hidden"]
+    out = {"bit.stem.w": _f32(standardize_weight(sd[_BIT + "embedder.convolution.weight"]).reshape(64, 147)),
+           "bit.stem.g": _f32(sd[_BIT + "embedder.norm.weight"]), "bit.stem.b": _f32(sd[_BIT + "embedder.norm.bias"])}
+    for st, depth in enumerate(BIT_DEPTHS):
+        for b in range(depth):
+            p = f"{_BIT}encoder.stages.{st}.layers.{b}."
+            q = f"bit.s{st}.b{b}."
+            w1 = standardize_weight(sd[p + "conv1.weight"])
+            out[q + "c1.w"] = _f16(w1.reshape(w1.shape[0], -1))
+            out[q + "c2.w"] = _conv3(standardize_weight(sd[p + "conv2.weight"]), sd[p + "conv2.weight"].shape[1])
+            w3 = standardize_weight(sd[p + "conv3.weight"])
+            out[q + "c3.w"] = _f16(w3.reshape(w3.shape[0], -1))
+            for i in (1, 2, 3):
+                out[q + f"n{i}.g"] = _f32(sd[p + f"norm{i}.weight"])
+                out[q + f"n{i}.b"] = _f32(sd[p + f"norm{i}.bias"])
+            if b == 0:
+                wd = standardize_weight(sd[p + "downsample.conv.weight"])
+                out[q + "ds.w"] = _f16(wd.reshape(wd.shape[0], -1))
+                out[q + "ds.g"] = _f32(sd[p + "downsample.norm.weight"])
+                out[q + "ds.b"] = _f32(sd[p + "downsample.norm.bias"])
+    out["pe.w"] = _f16(sd["dpt.embeddings.projection.weight"].float().reshape(D, 1024))
+    out["pe.b"] = _f32(sd["dpt.embeddings.projection.bias"])
+    out.update(_prepare_dpt_vit(sd, cfg, image_h, image_w, (2, 3), direct=(0, 1)))
     return out

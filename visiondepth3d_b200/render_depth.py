@@ -17,10 +17,11 @@ from ctypes import c_void_p as C_void_p
 
 import numpy as np
 
-from .depth_engine import FAMILY_DA_V2, FAMILY_DPT, DepthEngine, processed_size as _processed_size
-from .depth_weights import (CONFIGS, DPT_CONFIGS, DPT_PROCESSOR, da_arch, da_config_from_json, da_processor_from_json,
-                            da_spec, dpt_config_from_json, dpt_processed_size, dpt_processor_from_json, hf_config,
-                            hf_dpt_config, is_plain_v2)
+from .depth_engine import FAMILY_DA_V2, FAMILY_DPT, FAMILY_DPT_HYBRID, DepthEngine, processed_size as _processed_size
+from .depth_weights import (CONFIGS, DPT_CONFIGS, DPT_HYBRID_CONFIGS, DPT_PROCESSOR, da_arch, da_config_from_json,
+                            da_processor_from_json, da_spec, dpt_config_from_json, dpt_hybrid_config_from_json,
+                            dpt_processed_size, dpt_processor_from_json, hf_config, hf_dpt_config,
+                            hf_dpt_hybrid_config, is_plain_v2)
 from .render_3d import _dialog, _val
 
 try:
@@ -35,7 +36,7 @@ pipe_type = None
 _engine = None
 
 # the checkpoints of the hot path (core/render_depth.py:689-712): the Depth-Anything family (V2, V1, Distill-Any-Depth,
-# the V2 metric models) and DPT-Large.  label -> (checkpoint id, backbone size)
+# the V2 metric models), DPT-Large and MiDaS 3.0 (DPT-Hybrid).  label -> (checkpoint id, backbone size)
 supported_models = {
     "Distil-Any-Depth-Large": ("xingyang1/Distill-Any-Depth-Large-hf", "vitl"),
     "Distil-Any-Depth-Small": ("xingyang1/Distill-Any-Depth-Small-hf", "vits"),
@@ -51,15 +52,44 @@ supported_models = {
     "V2-Metric-Outdoor-Large": ("depth-anything/Depth-Anything-V2-Metric-Outdoor-Large-hf", "vitl"),
     "DPT-Large": ("Intel/dpt-large", "dpt-large"),
     "Manojb - DPT-Large": ("Manojb/dpt-large", "dpt-large"),
+    "MiDaS 3.0": ("Intel/dpt-hybrid-midas", "dpt-hybrid-midas"),
 }
 # the Depth-Anything checkpoints other than V2's: their taps and head are only in config.json (the tensors have V2's
 # shapes), so they load only with it, and with Depth-Anything's preprocessor_config.json when one is present
 DA_CONFIG_REQUIRED = frozenset(v[0] for k, v in supported_models.items()
-                               if v[1] != "dpt-large" and not k.startswith("Depth Anything V2"))
+                               if v[1] in CONFIGS and not k.startswith("Depth Anything V2"))
+# DPT-Hybrid's BiT backbone is described only in config.json, so its checkpoints load only with one
+DPT_HYBRID_CONFIG_REQUIRED = frozenset(v[0] for v in supported_models.values() if v[1] in DPT_HYBRID_CONFIGS)
+_SERVED = "Depth-Anything (V2, V1, Distill-Any-Depth, V2-Metric), DPT-Large or MiDaS 3.0 (DPT-Hybrid)"
 
 
 def _family_of(arch):
+    if arch in DPT_HYBRID_CONFIGS:
+        return FAMILY_DPT_HYBRID
     return FAMILY_DPT if arch in DPT_CONFIGS else FAMILY_DA_V2
+
+
+def _dpt_like(arch):
+    """DPT-Large and DPT-Hybrid: the fixed-size DPT processor, no tiled depth."""
+    return _family_of(arch) in (FAMILY_DPT, FAMILY_DPT_HYBRID)
+
+
+def _dpt_configs(arch):
+    return DPT_HYBRID_CONFIGS[arch] if _family_of(arch) == FAMILY_DPT_HYBRID else DPT_CONFIGS[arch]
+
+
+def _load_dpt_hybrid_checkpoint(sd, cfg_path):
+    """arch of a DPT-Hybrid state dict (dpt.embeddings.backbone.bit.* keys): "dpt-hybrid-midas" when config.json
+    (required: the backbone is described only there) is served and matches the built-in configuration."""
+    import json
+    if not os.path.exists(cfg_path):
+        raise ValueError(f"a DPT-Hybrid checkpoint needs its config.json (not found: {cfg_path})")
+    with open(cfg_path) as f:
+        got = dpt_hybrid_config_from_json(json.load(f))
+    c = DPT_HYBRID_CONFIGS["dpt-hybrid-midas"]
+    if got != c:
+        raise ValueError(f"config.json {got} does not match the built-in dpt-hybrid-midas configuration {c}")
+    return "dpt-hybrid-midas"
 
 
 def _load_dpt_checkpoint(sd, cfg_path):
@@ -89,10 +119,11 @@ def _check_da_state_dict(sd, spec):
 
 def load_checkpoint(path):
     """HF-format checkpoint (model.safetensors / pytorch_model.bin of a DepthAnythingForDepthEstimation or
-    Intel/dpt-large model) -> (arch, state_dict), arch None for another model.  Depth-Anything: with a config.json next
+    Intel/dpt-large or Intel/dpt-hybrid-midas model) -> (arch, state_dict), arch None for another model.  Depth-Anything: with a config.json next
     to it, the model is what da_config_from_json reads there (ValueError for what the engine does not serve): arch is
     the size key of depth_weights.CONFIGS for a plain V2 model, else the spec dict (V1 taps, a metric head); without
-    one, the V2 size of the hidden width.  DPT: cross-checked against DPT_CONFIGS."""
+    one, the V2 size of the hidden width.  DPT: cross-checked against DPT_CONFIGS.  DPT-Hybrid (BiT backbone keys):
+    config.json is required and must be the one DPT_HYBRID_CONFIGS serves."""
     import json
     import os
     if path.endswith(".safetensors"):
@@ -100,6 +131,8 @@ def load_checkpoint(path):
         sd = load_file(path)
     else:
         sd = torch.load(path, map_location="cpu")
+    if any(k.startswith("dpt.embeddings.backbone.bit.") for k in sd):
+        return _load_dpt_hybrid_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
     if "dpt.embeddings.cls_token" in sd:
         return _load_dpt_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
     if "backbone.embeddings.cls_token" not in sd:
@@ -119,7 +152,7 @@ def load_checkpoint(path):
 
 
 _state_dict = None      # weights of the loaded model (HF naming): engines for other processed sizes are built from it
-_arch = None            # "vits" / "vitb" / "vitl" (the Depth-Anything backbone size) or "dpt-large"
+_arch = None            # "vits" / "vitb" / "vitl" (the Depth-Anything backbone size), "dpt-large" or "dpt-hybrid-midas"
 _spec = None            # Depth-Anything: the spec (taps, head, max_depth; depth_weights.da_spec) every engine is built with
 _processor = None       # DPT: the image processor's settings (depth_weights.DPT_PROCESSOR or preprocessor_config.json)
 _engines = {}           # (processed_h, processed_w) -> DepthEngine, all sharing _state_dict
@@ -136,15 +169,15 @@ local_model_dir = _weights_dir()
 
 def model_processed_size(width, height):
     """(h, w) the loaded model's image processor resizes a (width, height) image to: Depth-Anything-V2 keeps the
-    aspect at multiples of 14 near 518, DPT-Large resizes every image to its processor's fixed size."""
-    if _family_of(_arch) == FAMILY_DPT:
+    aspect at multiples of 14 near 518, DPT-Large and MiDaS 3.0 resize every image to their processor's fixed size."""
+    if _dpt_like(_arch):
         return dpt_processed_size(_processor)
     return _processed_size(width, height)
 
 
 def _check_tiled_supported():
-    if USE_TILED_DEPTH and _family_of(_arch) == FAMILY_DPT:
-        raise ValueError("USE_TILED_DEPTH is served for Depth-Anything-V2 models only, not for DPT-Large")
+    if USE_TILED_DEPTH and _dpt_like(_arch):
+        raise ValueError("USE_TILED_DEPTH is served for Depth-Anything-V2 models only, not for DPT-Large or MiDaS 3.0")
 
 
 def _engine_for(width, height):
@@ -156,7 +189,7 @@ def _engine_for(width, height):
     key = model_processed_size(width, height)
     eng = _engines.get(key)
     if eng is None:
-        dpt = _family_of(_arch) == FAMILY_DPT
+        dpt = _dpt_like(_arch)
         eng = DepthEngine(_arch if dpt else _spec, key[0], key[1], family=_family_of(_arch), processor=_processor)
         eng.load_state_dict(_state_dict)
         _engines[key] = eng
@@ -165,7 +198,7 @@ def _engine_for(width, height):
 
 
 def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed=0, processor=None):
-    """Make `pipe` serve a Depth-Anything model or DPT-Large ("dpt-large").  arch: a Depth-Anything-V2 size ("vits" /
+    """Make `pipe` serve a Depth-Anything model, DPT-Large ("dpt-large") or MiDaS 3.0 ("dpt-hybrid-midas").  arch: a Depth-Anything-V2 size ("vits" /
     "vitb" / "vitl") or a Depth-Anything spec dict (depth_weights.da_spec / da_config_from_json: V1's taps, a metric
     head with its max_depth), which every engine built from these weights then carries.
     `state_dict` uses HF DepthAnythingForDepthEstimation / DPTForDepthEstimation naming (e.g. from a local
@@ -180,7 +213,7 @@ def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed
         arch = da_arch(spec)
         if arch is None:
             raise ValueError(f"unknown depth model {spec!r}")
-    dpt = _family_of(arch) == FAMILY_DPT
+    dpt = _dpt_like(arch)
     if not dpt and arch not in CONFIGS:
         raise ValueError(f"unknown depth model {arch!r}")
     if not dpt and spec is None:
@@ -192,7 +225,8 @@ def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed
         torch.manual_seed(seed)
         if dpt:
             from transformers import DPTForDepthEstimation
-            state_dict = DPTForDepthEstimation(hf_dpt_config(arch)).eval().state_dict()
+            hf = hf_dpt_hybrid_config(arch) if _family_of(arch) == FAMILY_DPT_HYBRID else hf_dpt_config(arch)
+            state_dict = DPTForDepthEstimation(hf).eval().state_dict()
         else:
             from transformers import DepthAnythingForDepthEstimation
             state_dict = DepthAnythingForDepthEstimation(hf_config(spec)).eval().state_dict()
@@ -204,7 +238,7 @@ def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed
     pipe = hf_batch_safe_pipe
     pipe_type = "hf"
     return pipe, {"arch": arch, "processed_size": (eng.image_h, eng.image_w),
-                  "config": DPT_CONFIGS[arch] if dpt else dict(spec)}
+                  "config": _dpt_configs(arch) if dpt else dict(spec)}
 
 
 def hf_batch_safe_pipe(images, inference_size=None):
@@ -579,13 +613,16 @@ def ensure_model_downloaded(checkpoint):
     if needs_config and not os.path.exists(os.path.join(ckdir, "config.json")):
         print(f"❌ {checkpoint}: no config.json next to {path} (its taps and head are only there)")
         return None, None
+    if checkpoint in DPT_HYBRID_CONFIG_REQUIRED and not os.path.exists(os.path.join(ckdir, "config.json")):
+        print(f"❌ {checkpoint}: no config.json next to {path} (its BiT backbone is described only there)")
+        return None, None
     try:
         arch, sd = load_checkpoint(path)
     except Exception as e:
         print(f"❌ Failed to load {path}: {e}")
         return None, None
     if arch is None:
-        print(f"❌ {path} is not a Depth-Anything (V2, V1, Distill-Any-Depth, V2-Metric) or DPT-Large checkpoint")
+        print(f"❌ {path} is not a {_SERVED} checkpoint")
         return None, None
     spec = None
     if isinstance(arch, dict):
@@ -603,7 +640,7 @@ def ensure_model_downloaded(checkpoint):
             except ValueError as e:
                 print(f"❌ {pp}: {e}")
                 return None, None
-    if _family_of(arch) == FAMILY_DPT:
+    if _dpt_like(arch):
         pp = os.path.join(ckdir, "preprocessor_config.json")
         try:
             if os.path.exists(pp):
