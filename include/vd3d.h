@@ -347,12 +347,19 @@ int vd3d_depth_create(const vd3d_depth_config* cfg, void* cuda_stream, vd3d_dept
  * VD3D_DEPTH_DPT_HYBRID is MiDaS 3.0 ("Intel/dpt-hybrid-midas"): DPT with a BiT ResNet-50 front end (stem and stages
  * 1-3, weight-standardised convs, GroupNorm(32)) in place of the patch embedding.  The stage-1 and stage-2 maps are
  * neck inputs 0 and 1 as they are (base.neck[0..1] must be 256 and 512); the last two base.taps feed the readout
- * ("ro2", "ro3") and reassemble layers 2 and 3.  Patch 16, relative head, square size a multiple of 32, as DPT. */
-enum { VD3D_DEPTH_DA_V2 = 0, VD3D_DEPTH_DPT = 1, VD3D_DEPTH_DPT_HYBRID = 2 };
+ * ("ro2", "ro3") and reassemble layers 2 and 3.  Patch 16, relative head, square size a multiple of 32, as DPT.
+ * VD3D_DEPTH_DPT_BEIT is MiDaS v3.1 BEiT-L 512 ("Intel/dpt-beit-large-512"): DPT-Large's launch sequence on a BEiT
+ * backbone.  Each layer adds its relative position bias table "l{i}.rpb" (f32 [heads][(2 ph - 1)(2 pw - 1) + 3],
+ * resampled to the ph x pw token grid) to the attention scores; "ls1" / "ls2" are the LayerScale lambdas; the key
+ * third of "qkv.b" and "pos" are zero.  Patch 16, relative head; image_h and image_w multiples of 32 (rectangular
+ * grids allowed).  The table, one int per key column and the attention's 91 KB must fit the 227 KB of shared memory of
+ * one block: every grid inside the engine's 3072-token limit does (at most ~152 KB).  The processor resizes every
+ * image to image_h x image_w, or keeps the aspect ratio after vd3d_depth_set_fit. */
+enum { VD3D_DEPTH_DA_V2 = 0, VD3D_DEPTH_DPT = 1, VD3D_DEPTH_DPT_HYBRID = 2, VD3D_DEPTH_DPT_BEIT = 3 };
 enum { VD3D_HEAD_RELATIVE = 0, VD3D_HEAD_METRIC = 1 };
 typedef struct {
   vd3d_depth_config base; /* image_h / image_w multiples of patch */
-  int32_t family;         /* VD3D_DEPTH_DA_V2, VD3D_DEPTH_DPT or VD3D_DEPTH_DPT_HYBRID */
+  int32_t family;         /* VD3D_DEPTH_DA_V2, VD3D_DEPTH_DPT, VD3D_DEPTH_DPT_HYBRID or VD3D_DEPTH_DPT_BEIT */
   int32_t patch;          /* 14 (DINOv2) or 16 (ViT-L/16) */
   float ln_eps;           /* 1e-6 (DINOv2) or 1e-12 (DPT) */
   int32_t resample;       /* the processor's PIL resample code: 3 bicubic or 2 bilinear */
@@ -361,9 +368,15 @@ typedef struct {
   float max_depth;        /* > 0 and finite; the metric head's scale (20 indoor, 80 outdoor); 1 for a relative head */
 } vd3d_depth_config_ex;
 /* VD3D_ERR_ARG for any other family, patch, resample or head kind, a max_depth that is not finite and positive, a
- * metric head on VD3D_DEPTH_DPT / _DPT_HYBRID, a DPT size that is not square or not a multiple of 32, a hybrid with a
- * patch other than 16 or base.neck[0..1] other than 256 / 512 */
+ * metric head on a DPT family, a DPT-Large / hybrid size that is not square or not a multiple of 32, a hybrid with a
+ * patch other than 16 or base.neck[0..1] other than 256 / 512, a BEiT size whose sides are not multiples of 32 or
+ * whose bias table does not fit the attention's shared memory */
 int vd3d_depth_create_ex(const vd3d_depth_config_ex* cfg, void* cuda_stream, vd3d_depth** out);
+/* VD3D_DEPTH_DPT_BEIT: the image processor keeps the aspect ratio (DPTImageProcessor with keep_aspect_ratio and
+ * ensure_multiple_of): scale the side whose scale to fit_h x fit_w is closer to 1, round both sides to multiples of
+ * `multiple` (32); vd3d_depth_infer_images then serves the inputs that map to image_h x image_w.  multiple 0: back to
+ * the fixed size.  VD3D_ERR_ARG for another family, a multiple other than 0 / 32 or a target side below 32. */
+int vd3d_depth_set_fit(vd3d_depth* e, int fit_h, int fit_w, int multiple);
 void vd3d_depth_destroy(vd3d_depth* e);
 /* CUDA-event timing of the fc1 GEMM launches (k_umma_gemm<128,4>; M = tokens, N = 4*hidden, K = hidden) */
 int vd3d_depth_profile(vd3d_depth* e, int enable);
@@ -403,7 +416,8 @@ int vd3d_depth_resize_pil(vd3d_depth* e, const uint8_t* src, int h, int w, uint8
 int vd3d_pil_bicubic_table(int in_size, int out_size, int32_t* bounds, int32_t* kk, int cap);
 /* B (1..8) u8 RGB images, each of its own size, through ONE batched forward.  sizes [B][4] = src_h, src_w, in_h, in_w:
  * the image's size and its input size (the inference size, or the source size again).  Every input size must map to the
- * engine's processed size (the DPT processor's keep-aspect multiple-of-14 size), else VD3D_ERR_ARG.  Per image: the
+ * engine's processed size (the model processor's: Depth-Anything's keep-aspect multiple-of-14 size near 518, BEiT's
+ * keep-aspect size of vd3d_depth_set_fit, the fixed size of the others), else VD3D_ERR_ARG.  Per image: the
  * Pillow resize to the input size when it differs, the DPT processor into the image's slot of the batch; then the
  * forward on the stacked token matrix (as vd3d_depth_infer_batch); then per image bicubic back to the input size, min-max
  * u8 (255 - u8 when invert) and cv2 INTER_CUBIC to the source size when it differs -> depth_u8[b] [src_h,src_w].

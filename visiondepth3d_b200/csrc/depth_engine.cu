@@ -55,6 +55,8 @@ struct vd3d_depth {
   int family = VD3D_DEPTH_DA_V2, patch = 14;
   float ln_eps = 1e-6f;
   PreprocParams pre = kImagenetBicubic;
+  // BEiT's keep-aspect processor (vd3d_depth_set_fit): target and multiple; fit_multiple 0: a fixed size
+  int fit_h = 0, fit_w = 0, fit_multiple = 0;
   // the head's last activation (VD3D_HEAD_RELATIVE / _METRIC) and the metric head's scale; every EPI_HEAD reads them
   int head = VD3D_HEAD_RELATIVE;
   float max_depth = 1.f;
@@ -243,8 +245,8 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
   *out = nullptr;
   if (!load_encode()) return VD3D_ERR_CUDA;
   const vd3d_depth_config* cfg = &x->base;
-  const bool hybrid = x->family == VD3D_DEPTH_DPT_HYBRID;
-  const bool dpt = x->family == VD3D_DEPTH_DPT || hybrid;
+  const bool hybrid = x->family == VD3D_DEPTH_DPT_HYBRID, beit = x->family == VD3D_DEPTH_DPT_BEIT;
+  const bool dpt = x->family == VD3D_DEPTH_DPT || hybrid || beit;
   if ((x->family != VD3D_DEPTH_DA_V2 && !dpt) || (x->patch != 14 && x->patch != 16) ||
       (x->resample != 2 && x->resample != 3) || !(x->ln_eps > 0.f) || cfg->heads < 1)
     return VD3D_ERR_ARG;
@@ -254,10 +256,14 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
   if (cfg->hidden % 128 || cfg->hidden > 1024 || cfg->hidden / cfg->heads != 64 || cfg->fusion % 64 ||
       cfg->image_h % x->patch || cfg->image_w % x->patch)
     return VD3D_ERR_ARG;
-  // DPT reshapes the tokens as a square grid, and every fusion x2 must land on the next map: an even square grid
-  if (dpt && (cfg->image_h != cfg->image_w || cfg->image_h % 32)) return VD3D_ERR_ARG;
+  // every fusion x2 must land on the next map: sides that are multiples of 32.  DPT-Large and the hybrid reshape the
+  // tokens as a square grid; BEiT takes the grid of the input (patch_height x patch_width), rectangular included
+  if (dpt && (cfg->image_h % 32 || cfg->image_w % 32 || (!beit && cfg->image_h != cfg->image_w))) return VD3D_ERR_ARG;
   // the hybrid's fixed BiT front end: patch 16 (stage 3 is the S/16 token grid), stage maps of 256 / 512 channels
   if (hybrid && (x->patch != 16 || cfg->neck[0] != 256 || cfg->neck[1] != 512)) return VD3D_ERR_ARG;
+  // BEiT: the relative position bias table of the grid is staged in the attention's shared memory
+  if (beit && (x->patch != 16 || attention_bias_smem(cfg->image_h / 16, cfg->image_w / 16) > (size_t)kAttnSmemMax))
+    return VD3D_ERR_ARG;
   for (int c = 0; c < 3; ++c)
     if (!(x->std[c] != 0.f)) return VD3D_ERR_ARG;
   vd3d_depth* e = new vd3d_depth();
@@ -282,6 +288,15 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
     return VD3D_ERR_UNSUPPORTED;
   }
   *out = e;
+  return VD3D_OK;
+}
+
+int vd3d_depth_set_fit(vd3d_depth* e, int fit_h, int fit_w, int multiple) {
+  if (!e || e->family != VD3D_DEPTH_DPT_BEIT || (multiple != 0 && multiple != 32) || (multiple && (fit_h < 32 || fit_w < 32)))
+    return VD3D_ERR_ARG;
+  e->fit_h = multiple ? fit_h : 0;
+  e->fit_w = multiple ? fit_w : 0;
+  e->fit_multiple = multiple;
   return VD3D_OK;
 }
 
@@ -371,6 +386,9 @@ int vd3d_depth_clone(vd3d_depth* src, void* stream, vd3d_depth** out) {
   e->head = src->head;
   e->max_depth = src->max_depth;
   e->pre = src->pre;
+  e->fit_h = src->fit_h;
+  e->fit_w = src->fit_w;
+  e->fit_multiple = src->fit_multiple;
   e->stream = (cudaStream_t)stream;
   e->w = src->w;
   e->owns_weights = false;
@@ -722,8 +740,9 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
   const int IH = c.image_h, IW = c.image_w;
   const int P = e->patch;
   const int KPE = round_up(3 * P * P, 16);  // 592 for patch 14 (588 + zero columns), 768 for 16
-  const bool hybrid = e->family == VD3D_DEPTH_DPT_HYBRID;
-  const bool dpt = e->family == VD3D_DEPTH_DPT || hybrid;  // ViT without LayerScale, raw taps, project readout
+  const bool hybrid = e->family == VD3D_DEPTH_DPT_HYBRID, beit = e->family == VD3D_DEPTH_DPT_BEIT;
+  // raw taps and the project readout (DPT-Large and the hybrid without LayerScale: ls1 / ls2 of ones)
+  const bool dpt = e->family == VD3D_DEPTH_DPT || hybrid || beit;
   int r;
   char nm[96];
   // ---- buffers ----
@@ -789,6 +808,9 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
         (r = W(e, nmf("fc2.w"), &wf2, (size_t)4 * D * D)) || (r = W(e, nmf("fc2.b"), &bf2, D)) ||
         (r = W(e, nmf("ls2"), &ls2, D)))
       return r;
+    // BEiT: the layer's relative position bias, one table per head for this grid
+    const float* rpb = nullptr;
+    if (beit && (r = W(e, nmf("rpb"), &rpb, (size_t)Hh * ((2 * ph - 1) * (2 * pw - 1) + 3)))) return r;
     int sp_ = e->span_begin("ln", s);
     launch_layernorm((const float*)x, MT, D, g1, b1, (__half*)xn, 0, e->ln_eps, s);
     e->span_end(sp_, s);
@@ -812,7 +834,7 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
       if ((r = make_map(e, &mq, q, 64, NT, B * Hh, 64, (uint64_t)NP * 64, kAttnRows, 1))) return r;
       if ((r = make_map(e, &mk, k, 64, NT, B * Hh, 64, (uint64_t)NP * 64, 128, 1))) return r;
       if ((r = make_map(e, &mv, vt, NT, 64, B * Hh, NP, (uint64_t)64 * NP, 64, 1))) return r;
-      cudaError_t ce = launch_attention(mq, mk, mv, NT, D, (__half*)attn, Hh, B, NP, s);
+      cudaError_t ce = launch_attention(mq, mk, mv, NT, D, (__half*)attn, Hh, B, NP, s, rpb, pw);
       if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("attention launch: ") + cudaGetErrorString(ce));
       e->launches++;
     }
@@ -1238,15 +1260,16 @@ int pil_resize(vd3d_depth* e, const uint8_t* src, int h, int w, uint8_t* tmp, ui
   return VD3D_OK;
 }
 
-// (h, w) the DPT image processor resizes an image to (depth_engine.py processed_size): keep the aspect ratio, scale the
-// side closer to 518, round to multiples of 14 (Python's round: half to even)
-void processed_size(int h, int w, int* ph, int* pw) {
-  double sh = 518.0 / h, sw = 518.0 / w;
+// (h, w) DPTImageProcessor resizes an image to with keep_aspect_ratio (depth_engine.py processed_size): scale the side
+// whose scale to the target (th, tw) is closer to 1 for both, round each to a multiple of `mult` (Python's round: half to
+// even), at least `mult`.  Depth-Anything: 518 x 518 and 14; BEiT: the processor's target and 32.
+void processed_size(int h, int w, int th, int tw, int mult, int* ph, int* pw) {
+  double sh = (double)th / h, sw = (double)tw / w;
   if (fabs(1 - sw) < fabs(1 - sh))
     sh = sw;
   else
     sw = sh;
-  auto rnd = [](double v) { int r = (int)nearbyint(v / 14) * 14; return r < 14 ? 14 : r; };
+  auto rnd = [mult](double v) { int r = (int)nearbyint(v / mult) * mult; return r < mult ? mult : r; };
   *ph = rnd(sh * h);
   *pw = rnd(sw * w);
 }
@@ -1395,7 +1418,10 @@ int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_r
     const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
     if (!images_rgb[b] || !depth_u8[b] || sh < 1 || sw < 1 || ih < 16 || iw < 16) return VD3D_ERR_ARG;
     int ph = IH, pw = IW;  // DPT's processor resizes every input to its fixed size
-    if (e->family == VD3D_DEPTH_DA_V2) processed_size(ih, iw, &ph, &pw);
+    if (e->family == VD3D_DEPTH_DA_V2)
+      processed_size(ih, iw, 518, 518, 14, &ph, &pw);
+    else if (e->fit_multiple)
+      processed_size(ih, iw, e->fit_h, e->fit_w, e->fit_multiple, &ph, &pw);
     if (ph != IH || pw != IW) {
       char m[160];
       snprintf(m, sizeof m, "image %d: a %dx%d input maps to processed size %dx%d, the engine serves %dx%d", b, iw, ih,

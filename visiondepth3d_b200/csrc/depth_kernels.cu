@@ -762,11 +762,16 @@ static cudaError_t launch_gemm_t(const CUtensorMap& a, const CUtensorMap& b, con
   return cudaGetLastError();
 }
 
+size_t attention_bias_smem(int ph, int pw) {
+  const size_t num = (size_t)(2 * ph - 1) * (2 * pw - 1) + 3;
+  return kAttnSmem + (num + 3) / 4 * 16 + (size_t)((ph * pw + 1 + 127) / 128) * 128 * 4;
+}
+
 cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, int ntok, int dmodel,
-                             __half* out, int heads, int images, int npad, cudaStream_t s) {
-  static bool attr_set = false;
+                             __half* out, int heads, int images, int npad, cudaStream_t s, const float* rpb, int gw) {
+  static bool attr_set = false, attr_bias_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(k_umma_attention, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
+    cudaError_t e = cudaFuncSetAttribute(k_umma_attention<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
@@ -776,8 +781,22 @@ cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const C
   a.out = out;
   a.heads = heads;
   a.npad = npad;
+  a.rpb = rpb;
+  a.gw = gw;
   dim3 grid((ntok + kAttnRows - 1) / kAttnRows, heads * images);
-  k_umma_attention<<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a);
+  if (!rpb) {
+    k_umma_attention<false><<<grid, kAttnThreads, kAttnSmem, s>>>(q, k, v, a);
+    return cudaGetLastError();
+  }
+  if (gw < 1 || (ntok - 1) % gw) return cudaErrorInvalidValue;
+  const size_t smem = attention_bias_smem((ntok - 1) / gw, gw);
+  if (smem > (size_t)kAttnSmemMax) return cudaErrorInvalidValue;
+  if (!attr_bias_set) {
+    cudaError_t e = cudaFuncSetAttribute(k_umma_attention<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemMax);
+    if (e != cudaSuccess) return e;
+    attr_bias_set = true;
+  }
+  k_umma_attention<true><<<grid, kAttnThreads, smem, s>>>(q, k, v, a);
   return cudaGetLastError();
 }
 

@@ -42,9 +42,17 @@ void launch_sr_in(const uint8_t* bgr, __half* x, int npix, cudaStream_t s);
 void launch_sr_out(const float* conv, int ldc, const uint8_t* bgr, uint8_t* out, int h, int w, cudaStream_t s);
 // fused attention: q,k [image][h][npad][64] (q pre-scaled), vT [image][h][64][npad] -> out [images * npad, dmodel].
 // One CTA per kAttnRows queries of one head; the q map's box is 64 x kAttnRows (the k map's 64 x 128, v's 64 x 64).
+// rpb (BEiT): the layer's relative position bias tables f32 [heads][(2 ph - 1)(2 pw - 1) + 3] of the ph x gw token grid
+// (ntok = ph * gw + 1), added to the scores in k_umma_attention<true>; null: the bias-free kernel.
 constexpr int kAttnRows = 192;
 cudaError_t launch_attention(const CUtensorMap& q, const CUtensorMap& k, const CUtensorMap& v, int ntok, int dmodel,
-                             __half* out, int heads, int images, int npad, cudaStream_t s);
+                             __half* out, int heads, int images, int npad, cudaStream_t s, const float* rpb = nullptr,
+                             int gw = 0);
+// dynamic shared memory of k_umma_attention<true> on a ph x pw grid: the bias-free kernel's, one head's table (rounded to
+// 16 bytes) and one int per key column of its 128-key tiles.  It must stay within kAttnSmemMax, the opt-in limit of an
+// sm_90 block (227 KB).
+constexpr int kAttnSmemMax = 227 * 1024;
+size_t attention_bias_smem(int ph, int pw);
 // bn in {32, 64, 128}; grid = (ceil(N/bn), m_tiles, batch)
 cudaError_t launch_gemm(int bn, const CUtensorMap& a, const CUtensorMap& b, const GemmArgs& g, int m_tiles,
                         int batch, cudaStream_t s);

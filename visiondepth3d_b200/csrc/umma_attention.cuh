@@ -20,6 +20,18 @@
 // output does not depend on it.  192-row blocks also cut the query padding at the model's token counts (2443 tokens:
 // 13 blocks, 2.2 % padding, against 20 blocks and 4.8 % at 128).
 //
+// Relative position bias (k_umma_attention<true>, BEiT: transformers 5.5 models/beit/modeling_beit.py
+// BeitSelfAttention + BeitRelativePositionBias): S[m, n] += table[h][idx(m, n)] before the running maximum.  In token
+// order (CLS at 0, patch p = token - 1 at grid row p / pw, column p % pw) the patch-to-patch index
+//   (qy - ky + ph - 1) (2 pw - 1) + (qx - kx + pw - 1) = A(m) - B(n),   B(n) = p + (p / pw) (pw - 1),  A(m) = B(m) + Bmax
+// with Bmax = (ph - 1)(2 pw - 1) + pw - 1, so every index lies in [0, 2 Bmax] = [0, num - 4].  Each CTA stages its head's
+// table (f32, num = (2 ph - 1)(2 pw - 1) + 3 entries) and 4 B (bytes) of every key column in shared memory once; a thread
+// holds &table[A] for its two rows, and each score element costs one subtract, one shared load and one FMA (an index in
+// elements would cost a fourth instruction, the address, per element).  Key columns past ntok take
+// B(ntok - 1), a valid index (they are masked to -inf after).  CLS column n = 0 takes entry num - 2; the CLS row takes
+// num - 3 on every key and num - 1 on the CLS key, which, since a softmax row is unchanged by a constant added to all of
+// it, the kernel applies as 0 on every key and (num - 1) - (num - 3) on the CLS key (the row's weight on A - B is 0).
+//
 // Replaces Dinov2SelfAttention (transformers 5.5 models/dinov2/modeling_dinov2.py) inside the depth
 // forward called from core/render_depth.py:1106-1119.
 #pragma once
@@ -34,6 +46,8 @@ struct AttnArgs {
   __half* out;  // [images * npad, dmodel], head h of image i writes rows i*npad + token, columns [64h, 64h+64)
   int heads;    // blockIdx.y = image * heads + head (the tensor maps' third coordinate)
   int npad;     // rows per image in `out`
+  const float* rpb;  // k_umma_attention<true>: the layer's relative position bias tables, f32 [heads][num]
+  int gw;            // k_umma_attention<true>: the token grid's width pw (ntok = ph * pw + 1)
 };
 
 static_assert(kAttnRows % 64 == 0 && kAttnRows <= 256, "64-row warpgroup slices; a TMA box spans at most 256 rows");
@@ -45,6 +59,8 @@ constexpr int kAttnSmem = kAttnQBytes + kAttnKS * (16384 /*K*/ + 16384 /*V^T*/) 
 constexpr int kAttnProducerRegs = 24;
 constexpr int kAttnConsumerRegs = 160;
 static_assert(128 * kAttnProducerRegs + 128 * kAttnConsumers * kAttnConsumerRegs <= 65536, "register file overcommitted");
+// the bias variant's staging area starts 256 bytes past the barriers, inside kAttnSmem's 256-byte barrier allowance
+constexpr int kAttnBiasOffset = kAttnQBytes + kAttnKS * 32768 + 256;
 
 namespace umma {
 // reductions over the four threads of a quad: one fragment row
@@ -62,6 +78,7 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 }
 }  // namespace umma
 
+template <bool kBias>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 k_umma_attention(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                  const __grid_constant__ CUtensorMap tmV, const AttnArgs g) {
@@ -118,6 +135,33 @@ k_umma_attention(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 
+  // relative position bias: the head's table and B of every key column of the T tiles, staged by the consumers
+  const int* sB = nullptr;
+  const char* arow[2] = {nullptr, nullptr};  // &table[A(row)]: the element's entry is arow - 4 B(n) bytes
+  float wrow[2] = {0.f, 0.f}, ccol[2] = {0.f, 0.f};
+  if constexpr (kBias) {
+    float* tab = (float*)(smem_raw + (sm - umma::smem_u32(smem_raw)) + kAttnBiasOffset);
+    const int pw = g.gw, ph = (g.ntok - 1) / pw, wd = 2 * pw - 1;
+    const int num = (2 * ph - 1) * wd + 3, bmax = (ph - 1) * wd + pw - 1;
+    int* boff = (int*)(tab + ((num + 3) & ~3));
+    const float* src = g.rpb + (size_t)h * num;
+    for (int i = threadIdx.x - 128; i < num; i += 128 * kAttnConsumers) tab[i] = src[i];
+    for (int n = threadIdx.x - 128; n < T * 128; n += 128 * kAttnConsumers) {
+      const int p = min(n, g.ntok - 1) - 1;  // the CLS key (p = -1) takes its own entry below; 0 keeps it in range
+      boff[n] = 4 * (p < 0 ? 0 : p + (p / pw) * (pw - 1));  // in bytes
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(128 * kAttnConsumers) : "memory");  // the consumer warpgroups only
+    const int r0 = qblk * kAttnRows + wg * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const int p = min(r0 + 8 * rr, g.ntok - 1) - 1;  // query rows past ntok are never written: any valid index
+      arow[rr] = (const char*)(tab + (p < 0 ? bmax : p + (p / pw) * (pw - 1) + bmax));
+      wrow[rr] = p < 0 ? 0.f : 1.f;
+      ccol[rr] = p < 0 ? tab[num - 1] - tab[num - 3] : tab[num - 2];
+    }
+    sB = boff;
+  }
+
   umma::mbar_wait(q_full, 0);
   const uint64_t dq = umma::make_desc(sQ + (uint32_t)(wg * 64 * 128));
   for (int t = 0; t < T; ++t) {
@@ -136,12 +180,21 @@ k_umma_attention(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     const int nvalid = g.ntok - t * 128;  // keys of this tile that exist
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-    for (int j = 0; j < 16; ++j)
+    for (int j = 0; j < 16; ++j) {
+      int2 bk = make_int2(0, 0);
+      if constexpr (kBias) bk = *(const int2*)(sB + t * 128 + 8 * j + cq);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
+        if constexpr (kBias) {
+          const float v = s[4 * j + i];
+          const float b = fmaf(*(const float*)(arow[i >> 1] - ((i & 1) ? bk.y : bk.x)), wrow[i >> 1], v);
+          const bool cls_key = j == 0 && !(i & 1) && t == 0 && cq == 0;  // column 8 j + cq + (i & 1) of tile t is 0
+          s[4 * j + i] = cls_key ? v + ccol[i >> 1] : b;
+        }
         if (nvalid < 128 && 8 * j + cq + (i & 1) >= nvalid) s[4 * j + i] = -INFINITY;
         mx[i >> 1] = fmaxf(mx[i >> 1], s[4 * j + i]);
       }
+    }
     float scale[2], mref[2];
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {

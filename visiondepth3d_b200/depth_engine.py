@@ -5,8 +5,9 @@ import sys as _sys
 import numpy as np
 
 from . import _lib
-from .depth_weights import (DA_PROCESSOR, DPT_CONFIGS, DPT_HYBRID_CONFIGS, DPT_PROCESSOR, da_spec, dpt_processed_size,
-                            is_plain_v2, prepare, prepare_dpt, prepare_dpt_hybrid)
+from .depth_weights import (DA_PROCESSOR, DPT_BEIT_CONFIGS, DPT_BEIT_PROCESSOR, DPT_CONFIGS, DPT_HYBRID_CONFIGS,
+                            DPT_PROCESSOR, da_spec, dpt_beit_processed_size, dpt_processed_size, is_plain_v2, prepare,
+                            prepare_dpt, prepare_dpt_beit, prepare_dpt_hybrid)
 
 
 def processed_size(width, height, target=518, multiple=14):
@@ -37,9 +38,11 @@ class DepthConfigEx(C.Structure):
 HEAD_KINDS = {"relative": 0, "metric": 1}  # VD3D_HEAD_RELATIVE / VD3D_HEAD_METRIC
 
 
-FAMILY_DA_V2, FAMILY_DPT, FAMILY_DPT_HYBRID = "da-v2", "dpt", "dpt-hybrid"
-_FAMILY_CODES = {FAMILY_DA_V2: 0, FAMILY_DPT: 1, FAMILY_DPT_HYBRID: 2}  # VD3D_DEPTH_DA_V2 / _DPT / _DPT_HYBRID
-_DPT_LIKE = (FAMILY_DPT, FAMILY_DPT_HYBRID)  # the fixed-size DPT image processor
+FAMILY_DA_V2, FAMILY_DPT, FAMILY_DPT_HYBRID, FAMILY_DPT_BEIT = "da-v2", "dpt", "dpt-hybrid", "dpt-beit"
+# VD3D_DEPTH_DA_V2 / _DPT / _DPT_HYBRID / _DPT_BEIT
+_FAMILY_CODES = {FAMILY_DA_V2: 0, FAMILY_DPT: 1, FAMILY_DPT_HYBRID: 2, FAMILY_DPT_BEIT: 3}
+_DPT_LIKE = (FAMILY_DPT, FAMILY_DPT_HYBRID, FAMILY_DPT_BEIT)  # DPTForDepthEstimation: DPT's processor settings
+_DPT_CONFIG_SETS = {FAMILY_DPT: DPT_CONFIGS, FAMILY_DPT_HYBRID: DPT_HYBRID_CONFIGS, FAMILY_DPT_BEIT: DPT_BEIT_CONFIGS}
 
 
 def _bind(lib):
@@ -52,6 +55,8 @@ def _bind(lib):
     lib.vd3d_depth_create_ex.restype = i
     if lib.vd3d_struct_size(6) != C.sizeof(DepthConfigEx):
         raise OSError(f"libvd3d ABI mismatch for DepthConfigEx: {lib.vd3d_struct_size(6)} != {C.sizeof(DepthConfigEx)}")
+    lib.vd3d_depth_set_fit.argtypes = [vp, i, i, i]
+    lib.vd3d_depth_set_fit.restype = i
     lib.vd3d_depth_destroy.argtypes = [vp]
     lib.vd3d_depth_destroy.restype = None
     lib.vd3d_depth_last_error.argtypes = [vp]
@@ -95,7 +100,10 @@ class DepthEngine:
     spec dict (depth_weights.da_spec / da_config_from_json: the V2 sizes, V1's taps, a metric head).  family "dpt": DPT-Large (ViT-L/16, project readout), `cfg` a key of DPT_CONFIGS or a dict; family
     "dpt-hybrid": MiDaS 3.0 (BiT ResNet-50 front end + ViT-B/16), `cfg` a key of DPT_HYBRID_CONFIGS or a dict.  For
     both DPT families `processor` is the image processor's settings (depth_weights.DPT_PROCESSOR, or dpt_processor_from_json of a checkpoint's
-    preprocessor_config.json); the processed size is the processor's, image_h / image_w default to it."""
+    preprocessor_config.json); the processed size is the processor's, image_h / image_w default to it.  family
+    "dpt-beit": MiDaS v3.1 BEiT-L 512, `cfg` a key of DPT_BEIT_CONFIGS or a dict, `processor` DPT_BEIT_PROCESSOR or
+    dpt_beit_processor_from_json's; with a keep-aspect processor the engine serves the frames whose processed size is
+    (image_h, image_w) (default: the processor's target, a square frame's)."""
 
     def __init__(self, cfg="vits", image_h=None, image_w=None, ctx=None, device=0, family=FAMILY_DA_V2,
                  processor=None):
@@ -105,14 +113,15 @@ class DepthEngine:
         if family not in _FAMILY_CODES:
             raise ValueError(f"unknown depth model family {family!r}")
         self.family = family
-        if family == FAMILY_DPT:
-            self.cfg = dict(DPT_CONFIGS[cfg]) if isinstance(cfg, str) else dict(cfg)
-        elif family == FAMILY_DPT_HYBRID:
-            self.cfg = dict(DPT_HYBRID_CONFIGS[cfg]) if isinstance(cfg, str) else dict(cfg)
+        if family in _DPT_LIKE:
+            self.cfg = dict(_DPT_CONFIG_SETS[family][cfg]) if isinstance(cfg, str) else dict(cfg)
         else:
             self.cfg = da_spec(cfg)  # taps, head and max_depth of the spec; V2's relative head by default
         c = self.cfg
-        if family in _DPT_LIKE:
+        if family == FAMILY_DPT_BEIT:
+            self.processor = dict(processor or DPT_BEIT_PROCESSOR)
+            image_h, image_w = image_h or self.processor["size"][0], image_w or self.processor["size"][1]
+        elif family in _DPT_LIKE:
             self.processor = dict(processor or DPT_PROCESSOR)
             ph, pw = dpt_processed_size(self.processor)
             image_h, image_w = image_h or ph, image_w or pw
@@ -129,6 +138,10 @@ class DepthEngine:
             dx = DepthConfigEx(dc, _FAMILY_CODES[family], c["patch"], c["ln_eps"], p["resample"], (C.c_float * 3)(*p["mean"]),
                                (C.c_float * 3)(*p["std"]), HEAD_KINDS["relative"], 1.0)
             rc = self.lib.vd3d_depth_create_ex(C.byref(dx), stream, C.byref(h))
+            if rc == 0 and p.get("keep_aspect"):
+                rc = self.lib.vd3d_depth_set_fit(h, p["size"][0], p["size"][1], p["multiple"])
+                if rc != 0:
+                    self.lib.vd3d_depth_destroy(h)
         elif not is_plain_v2(c):  # Depth Anything V1, Distill-Any-Depth, the V2 metric models
             p = DA_PROCESSOR
             dx = DepthConfigEx(dc, 0, 14, 1e-6, p["resample"], (C.c_float * 3)(*p["mean"]), (C.c_float * 3)(*p["std"]),
@@ -142,7 +155,9 @@ class DepthEngine:
 
     def processed_size(self, width, height):
         """(h, w) the model's image processor resizes a (width, height) image to: Depth-Anything's keep-aspect
-        multiple-of-14 size, DPT's fixed size."""
+        multiple-of-14 size, DPT's fixed size, DPT-BEiT's processor's (keep-aspect multiples of 32 or fixed)."""
+        if self.family == FAMILY_DPT_BEIT:
+            return dpt_beit_processed_size(width, height, self.processor)
         if self.family in _DPT_LIKE:
             return dpt_processed_size(self.processor)
         return processed_size(width, height)
@@ -152,7 +167,8 @@ class DepthEngine:
             raise _lib.Vd3dError(f"libvd3d depth error {rc}: {self.lib.vd3d_depth_last_error(self.h).decode()}")
 
     def load_state_dict(self, sd):
-        prep = {FAMILY_DPT: prepare_dpt, FAMILY_DPT_HYBRID: prepare_dpt_hybrid}.get(self.family, prepare)
+        prep = {FAMILY_DPT: prepare_dpt, FAMILY_DPT_HYBRID: prepare_dpt_hybrid,
+                FAMILY_DPT_BEIT: prepare_dpt_beit}.get(self.family, prepare)
         for name, arr in prep(sd, self.cfg, self.image_h, self.image_w).items():
             arr = np.ascontiguousarray(arr)
             self.check(self.lib.vd3d_depth_set_tensor(self.h, name.encode(), arr.ctypes.data, arr.nbytes))

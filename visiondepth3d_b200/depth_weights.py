@@ -451,24 +451,42 @@ def _prepare_dpt_vit(sd, cfg, image_h, image_w, readouts, direct=()):
     pp = pos[:, 1:].reshape(1, g, g, D).permute(0, 3, 1, 2)
     pp = F.interpolate(pp, size=(ph, pw), mode="bilinear")  # DPTViTEmbeddings._resize_pos_embed (identity at g x g)
     out["pos"] = _f32(torch.cat((pos[:, :1], pp.permute(0, 2, 3, 1).reshape(1, -1, D)), dim=1).reshape(-1, D))
-    ones = np.ones(D, np.float32)
+    out.update(_prepare_dpt_layers(sd, cfg, "dpt.encoder.layer."))
+    out.update(_prepare_dpt_neck(sd, cfg, readouts, direct))
+    return out
+
+
+def _prepare_dpt_layers(sd, cfg, prefix):
+    """The ViT layers of DPT (transformers' DPTViTLayer and BeitLayer share these names) under `prefix`: a missing key
+    bias (BEiT's key projection has none) is zero; LayerScale is the lambdas when cfg["layer_scale"], else ones (exact in
+    EPI_RESID_LS)."""
+    D = cfg["hidden"]
+    ones, out = np.ones(D, np.float32), {}
     for i in range(cfg["layers"]):
-        p = f"dpt.encoder.layer.{i}."
+        p = f"{prefix}{i}."
         a = p + "attention.attention."
+        kb = sd[a + "key.bias"] if a + "key.bias" in sd else torch.zeros(D)
         out[f"l{i}.ln1.g"] = _f32(sd[p + "layernorm_before.weight"])
         out[f"l{i}.ln1.b"] = _f32(sd[p + "layernorm_before.bias"])
         out[f"l{i}.qkv.w"] = _f16(torch.cat([sd[a + "query.weight"], sd[a + "key.weight"], sd[a + "value.weight"]], 0))
-        out[f"l{i}.qkv.b"] = _f32(torch.cat([sd[a + "query.bias"], sd[a + "key.bias"], sd[a + "value.bias"]], 0))
+        out[f"l{i}.qkv.b"] = _f32(torch.cat([sd[a + "query.bias"], kb, sd[a + "value.bias"]], 0))
         out[f"l{i}.proj.w"] = _f16(sd[p + "attention.output.dense.weight"])
         out[f"l{i}.proj.b"] = _f32(sd[p + "attention.output.dense.bias"])
-        out[f"l{i}.ls1"] = ones
+        out[f"l{i}.ls1"] = _f32(sd[p + "lambda_1"]) if cfg.get("layer_scale") else ones
         out[f"l{i}.ln2.g"] = _f32(sd[p + "layernorm_after.weight"])
         out[f"l{i}.ln2.b"] = _f32(sd[p + "layernorm_after.bias"])
         out[f"l{i}.fc1.w"] = _f16(sd[p + "intermediate.dense.weight"])
         out[f"l{i}.fc1.b"] = _f32(sd[p + "intermediate.dense.bias"])
         out[f"l{i}.fc2.w"] = _f16(sd[p + "output.dense.weight"])
         out[f"l{i}.fc2.b"] = _f32(sd[p + "output.dense.bias"])
-        out[f"l{i}.ls2"] = ones
+        out[f"l{i}.ls2"] = _f32(sd[p + "lambda_2"]) if cfg.get("layer_scale") else ones
+    return out
+
+
+def _prepare_dpt_neck(sd, cfg, readouts, direct=()):
+    """DPT's project readouts `readouts` (split into their token and CLS halves) and the neck, fusion and head."""
+    D = cfg["hidden"]
+    out = {}
     for i in readouts:
         r = f"neck.reassemble_stage.readout_projects.{i}.0."
         w = sd[r + "weight"].float()
@@ -670,4 +688,232 @@ def prepare_dpt_hybrid(sd, cfg, image_h, image_w):
     out["pe.w"] = _f16(sd["dpt.embeddings.projection.weight"].float().reshape(D, 1024))
     out["pe.b"] = _f32(sd["dpt.embeddings.projection.bias"])
     out.update(_prepare_dpt_vit(sd, cfg, image_h, image_w, (2, 3), direct=(0, 1)))
+    return out
+
+
+# ---------------------------------------------------------------------------
+# DPT-BEiT (Intel/dpt-beit-large-512, MiDaS v3.1 BEiT-L 512; transformers 5.5 DPTForDepthEstimation whose backbone is
+# BeitBackbone, built by load_backbone, state dict prefix "backbone."): a BEiT-L/16 with LayerScale, no absolute
+# position embedding, and a relative position bias per layer (BeitRelativePositionBias: a [(2 W - 1)^2 + 3, heads] table
+# for the pretrained W x W window, resampled bilinearly to the input's grid); its key projection has no bias.  Taps =
+# the raw hidden states (CLS included) after the out_indices layers; from there on DPT-Large's path.
+# ---------------------------------------------------------------------------
+DPT_BEIT_CONFIGS = {
+    "dpt-beit-large-512": dict(hidden=1024, layers=24, heads=16, taps=[6, 12, 18, 24], neck=[256, 512, 1024, 1024],
+                               fusion=256, patch=16, ln_eps=1e-12, image_size=512, layer_scale=True),
+}
+
+# DPTImageProcessor as MiDaS v3.1's BEiT checkpoints are expected to configure it: keep the aspect ratio, sides
+# multiples of 32 near 512, bicubic, mean = std = 0.5.  The checkpoint's preprocessor_config.json is what the drivers read.
+DPT_BEIT_PROCESSOR = dict(size=(512, 512), resample=3, mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5), keep_aspect=True,
+                          multiple=32)
+
+
+def hf_dpt_beit_config(name="dpt-beit-large-512", **cfg):
+    """transformers DPTConfig with a BeitConfig backbone equal to the checkpoint's as far as the engine reads it; `cfg`
+    overrides entries of DPT_BEIT_CONFIGS[name] (a smaller BEiT for tests; layer_scale False: no lambdas)."""
+    from transformers import BeitConfig, DPTConfig
+    c = dict(DPT_BEIT_CONFIGS[name], **cfg)
+    bc = BeitConfig(image_size=c["image_size"], patch_size=c["patch"], num_channels=3, hidden_size=c["hidden"],
+                    num_hidden_layers=c["layers"], num_attention_heads=c["heads"], intermediate_size=4 * c["hidden"],
+                    hidden_act="gelu", layer_norm_eps=c["ln_eps"], use_mask_token=False,
+                    use_absolute_position_embeddings=False, use_relative_position_bias=True,
+                    use_shared_relative_position_bias=False, layer_scale_init_value=0.1 if c["layer_scale"] else 0.0,
+                    out_indices=list(c["taps"]), reshape_hidden_states=False, add_fpn=False)
+    return DPTConfig(backbone_config=bc, hidden_size=c["hidden"], is_hybrid=False, readout_type="project",
+                     reassemble_factors=[4, 2, 1, 0.5], neck_hidden_sizes=c["neck"], fusion_hidden_size=c["fusion"],
+                     head_in_index=-1, use_batch_norm_in_fusion_residual=False, use_bias_in_fusion_residual=None,
+                     add_projection=False)
+
+
+def dpt_beit_config_from_json(cj):
+    """The engine configuration of a DPT config.json (dict) with a BEiT backbone, or ValueError naming every field the
+    engine does not compute: absolute position embeddings, a shared relative bias, no relative bias, reshaped hidden
+    states, an FPN, a patch other than 16, a head size other than 64, an activation other than GELU, taps that are not
+    four increasing layers, a readout other than "project", and the neck / fusion / head options DPT-Large does not
+    serve.  layer_scale_init_value 0 means no LayerScale (ones)."""
+    bad = []
+    if cj.get("model_type", "dpt") != "dpt":
+        bad.append(("model_type", cj.get("model_type")))
+    if cj.get("is_hybrid"):
+        bad.append(("is_hybrid", cj.get("is_hybrid")))
+    bj = cj.get("backbone_config")
+    if not isinstance(bj, dict) or bj.get("model_type") != "beit":
+        raise ValueError(f"config.json: backbone_config = {bj!r} is not a BEiT backbone")
+    for field, want in (("use_absolute_position_embeddings", False), ("use_shared_relative_position_bias", False),
+                        ("use_relative_position_bias", True), ("reshape_hidden_states", False), ("add_fpn", False)):
+        default = {"use_relative_position_bias": False, "reshape_hidden_states": True}.get(field, False)
+        if bool(bj.get(field, default)) is not want:
+            bad.append((f"backbone_config.{field}", bj.get(field, default)))
+    if bj.get("patch_size", 16) != 16:
+        bad.append(("backbone_config.patch_size", bj.get("patch_size")))
+    if bj.get("num_channels", 3) != 3:
+        bad.append(("backbone_config.num_channels", bj.get("num_channels")))
+    hidden, layers, heads = (int(bj.get("hidden_size", 768)), int(bj.get("num_hidden_layers", 12)),
+                             int(bj.get("num_attention_heads", 12)))
+    if hidden != 64 * heads or hidden % 128 or hidden > 1024:
+        bad.append(("backbone_config.hidden_size / num_attention_heads", (hidden, heads)))
+    if int(bj.get("intermediate_size", 3072)) != 4 * hidden:
+        bad.append(("backbone_config.intermediate_size", bj.get("intermediate_size", 3072)))
+    if bj.get("hidden_act", "gelu") != "gelu":
+        bad.append(("backbone_config.hidden_act", bj.get("hidden_act")))
+    taps = bj.get("out_indices")
+    if taps is None and isinstance(bj.get("out_features"), (list, tuple)):
+        taps = [int(f[5:]) if isinstance(f, str) and f.startswith("stage") and f[5:].isdigit() else f
+                for f in bj["out_features"]]
+    if (not isinstance(taps, (list, tuple)) or len(taps) != 4 or any(type(t) is not int for t in taps)
+            or not 1 <= taps[0] < taps[1] < taps[2] < taps[3] <= layers):
+        bad.append(("backbone_config.out_indices", taps))
+    if cj.get("readout_type", "project") != "project":
+        bad.append(("readout_type", cj.get("readout_type")))
+    if [float(f) for f in cj.get("reassemble_factors", [4, 2, 1, 0.5])] != [4.0, 2.0, 1.0, 0.5]:
+        bad.append(("reassemble_factors", cj.get("reassemble_factors")))
+    neck = cj.get("neck_hidden_sizes", [96, 192, 384, 768])
+    if not isinstance(neck, (list, tuple)) or len(neck) != 4 or any(type(v) is not int or v < 1 for v in neck):
+        bad.append(("neck_hidden_sizes", neck))
+    fusion = cj.get("fusion_hidden_size", 256)
+    if type(fusion) is not int or fusion < 64 or fusion % 64:
+        bad.append(("fusion_hidden_size", fusion))
+    for field, default in (("add_projection", False), ("use_batch_norm_in_fusion_residual", False)):
+        if cj.get(field, default):
+            bad.append((field, cj.get(field)))
+    if cj.get("use_bias_in_fusion_residual") is False:
+        bad.append(("use_bias_in_fusion_residual", False))
+    if cj.get("head_in_index", -1) != -1:
+        bad.append(("head_in_index", cj.get("head_in_index")))
+    if bad:
+        raise ValueError("config.json: " + ", ".join(f"{f} = {v!r}" for f, v in bad) + " not served (DPT on a BEiT "
+                         "backbone with its own relative position bias per layer and the project readout)")
+    ls = bj.get("layer_scale_init_value", 0.1)
+    return dict(hidden=hidden, layers=layers, heads=heads, taps=list(taps), neck=list(neck), fusion=fusion, patch=16,
+                ln_eps=float(bj.get("layer_norm_eps", 1e-12)), image_size=int(bj.get("image_size", 224)),
+                layer_scale=bool(ls > 0))
+
+
+def dpt_beit_processor_from_json(pj):
+    """DPT_BEIT_PROCESSOR updated from a preprocessor_config.json (dict), or ValueError: keep_aspect_ratio with
+    ensure_multiple_of 32, or a fixed size whose sides are multiples of 32; bicubic or bilinear; 1/255; no padding."""
+    def bad(field, value):
+        raise ValueError(f"preprocessor_config.json: {field} = {value!r} is not served (DPT processor: keep_aspect_ratio "
+                         "with ensure_multiple_of 32, or a fixed size of multiples of 32)")
+    for field in ("do_resize", "do_rescale", "do_normalize"):
+        if pj.get(field, True) is not True:
+            bad(field, pj.get(field))
+    if pj.get("do_pad"):
+        bad("do_pad", pj.get("do_pad"))
+    rf = pj.get("rescale_factor", 1 / 255)
+    if not isinstance(rf, (int, float)) or abs(rf - 1 / 255) > 1e-9:
+        bad("rescale_factor", rf)
+    size = pj.get("size", {"height": 384, "width": 384})
+    if isinstance(size, int):
+        size = {"height": size, "width": size}
+    if not isinstance(size, dict) or type(size.get("height")) is not int or type(size.get("width")) is not int:
+        bad("size", size)
+    h, w = size["height"], size["width"]
+    keep, mult = bool(pj.get("keep_aspect_ratio", False)), pj.get("ensure_multiple_of", 1)
+    if keep and mult != 32:
+        bad("ensure_multiple_of", mult)
+    if not keep and (mult not in (1, 32) or h % 32 or w % 32):
+        bad("size / ensure_multiple_of", (size, mult))
+    if h < 32 or w < 32:
+        bad("size", size)
+    p = dict(DPT_BEIT_PROCESSOR, size=(h, w), keep_aspect=keep, multiple=32 if keep else 0)
+    p["resample"] = pj.get("resample", 3)
+    if p["resample"] not in (2, 3):
+        bad("resample", p["resample"])
+    for k, key in (("mean", "image_mean"), ("std", "image_std")):
+        if key in pj:
+            v = pj[key]
+            v = v if isinstance(v, (list, tuple)) else [v] * 3
+            if len(v) != 3 or any(not isinstance(x, (int, float)) for x in v):
+                bad(key, pj[key])
+            p[k] = tuple(float(x) for x in v)
+    return p
+
+
+def dpt_beit_processed_size(width, height, processor=None):
+    """(h, w) a DPT-BEiT processor resizes a (width, height) image to: DPTImageProcessor's keep-aspect size (the side
+    whose scale to the target is closer to 1 sets both, each rounded to a multiple of 32) or its fixed size."""
+    p = processor or DPT_BEIT_PROCESSOR
+    th, tw = p["size"]
+    if not p["keep_aspect"]:
+        return th, tw
+    sh, sw = th / height, tw / width
+    if abs(1 - sw) < abs(1 - sh):
+        sh = sw
+    else:
+        sw = sh
+    m = p["multiple"]
+    rnd = lambda v: max(m, int(round(v / m) * m))  # noqa: E731
+    return rnd(sh * height), rnd(sw * width)
+
+
+_BEIT = "backbone."
+
+
+def dpt_beit_keys(cfg):
+    """Every state_dict key (and its shape) the DPT-BEiT depth forward reads."""
+    D, L, P, H = cfg["hidden"], cfg["layers"], cfg["patch"], cfg["heads"]
+    W = cfg["image_size"] // P
+    k = {_BEIT + "embeddings.cls_token": (1, 1, D), _BEIT + "embeddings.patch_embeddings.projection.weight": (D, 3, P, P),
+         _BEIT + "embeddings.patch_embeddings.projection.bias": (D,)}
+    for i in range(L):
+        p = f"{_BEIT}encoder.layer.{i}."
+        a = p + "attention.attention."
+        for n in ("layernorm_before", "layernorm_after"):
+            k[p + n + ".weight"] = k[p + n + ".bias"] = (D,)
+        for n in ("query", "key", "value"):
+            k[a + n + ".weight"] = (D, D)
+        k[a + "query.bias"] = k[a + "value.bias"] = (D,)
+        k[a + "relative_position_bias.relative_position_bias_table"] = ((2 * W - 1) ** 2 + 3, H)
+        if cfg.get("layer_scale"):
+            k[p + "lambda_1"] = k[p + "lambda_2"] = (D,)
+        k[p + "attention.output.dense.weight"], k[p + "attention.output.dense.bias"] = (D, D), (D,)
+        k[p + "intermediate.dense.weight"], k[p + "intermediate.dense.bias"] = (4 * D, D), (4 * D,)
+        k[p + "output.dense.weight"], k[p + "output.dense.bias"] = (D, 4 * D), (D,)
+    k.update({n: v for n, v in dpt_keys(cfg).items() if not n.startswith("dpt.")})
+    return k
+
+
+def check_dpt_beit_state_dict(sd, cfg):
+    """ValueError naming the first missing or mis-shaped key the DPT-BEiT forward reads.  Other keys (the
+    relative_position_index buffers, a mask_token, a key bias, which a softmax row does not see) are ignored."""
+    for name, shape in dpt_beit_keys(cfg).items():
+        if name not in sd:
+            raise ValueError(f"DPT-BEiT state dict: missing key {name}")
+        if tuple(sd[name].shape) != shape:
+            raise ValueError(f"DPT-BEiT state dict: {name} has shape {tuple(sd[name].shape)}, expected {shape}")
+
+
+def beit_bias_table(table, window, grid):
+    """BeitRelativePositionBias.forward's table for a token grid (ph, pw) from the pretrained window's [(2 Wh - 1)
+    (2 Ww - 1) + 3, heads] table, with the same torch ops in fp32 on the CPU: the (2 Wh - 1) x (2 Ww - 1) part resampled
+    bilinearly (align_corners False) to (2 ph - 1) x (2 pw - 1), the three CLS entries appended as they are."""
+    t = table.detach().to(device="cpu", dtype=torch.float32)
+    old_h, old_w = 2 * window[0] - 1, 2 * window[1] - 1
+    new_h, new_w = 2 * grid[0] - 1, 2 * grid[1] - 1
+    n_old = old_h * old_w
+    sub = t[:n_old].reshape(1, old_w, old_h, -1).permute(0, 3, 1, 2)
+    sub = F.interpolate(sub, size=(new_h, new_w), mode="bilinear")
+    sub = sub.permute(0, 2, 3, 1).reshape(new_h * new_w, -1)
+    return torch.cat([sub, t[n_old:]])
+
+
+def prepare_dpt_beit(sd, cfg, image_h, image_w):
+    """DPT-BEiT state_dict -> {name: np.ndarray} in the layouts depth_engine.cu expects: DPT-Large's with the lambdas as
+    LayerScale, a zero key bias, a zero "pos" (BEiT has no absolute position embedding: EPI_PATCH adds 0, exactly), and
+    "l{i}.rpb" f32 [heads, (2 ph - 1)(2 pw - 1) + 3], each layer's table resampled to the image_h x image_w grid."""
+    check_dpt_beit_state_dict(sd, cfg)
+    D, P = cfg["hidden"], cfg["patch"]
+    ph, pw = image_h // P, image_w // P
+    W = cfg["image_size"] // P
+    e = _BEIT + "embeddings."
+    out = {"pe.w": _f16(sd[e + "patch_embeddings.projection.weight"].float().reshape(D, 3 * P * P)),
+           "pe.b": _f32(sd[e + "patch_embeddings.projection.bias"]),
+           "cls": _f32(sd[e + "cls_token"].reshape(D)), "pos": np.zeros((ph * pw + 1, D), np.float32)}
+    out.update(_prepare_dpt_layers(sd, cfg, _BEIT + "encoder.layer."))
+    for i in range(cfg["layers"]):
+        t = sd[f"{_BEIT}encoder.layer.{i}.attention.attention.relative_position_bias.relative_position_bias_table"]
+        out[f"l{i}.rpb"] = _f32(beit_bias_table(t, (W, W), (ph, pw)).t())
+    out.update(_prepare_dpt_neck(sd, cfg, range(4)))
     return out

@@ -17,11 +17,13 @@ from ctypes import c_void_p as C_void_p
 
 import numpy as np
 
-from .depth_engine import FAMILY_DA_V2, FAMILY_DPT, FAMILY_DPT_HYBRID, DepthEngine, processed_size as _processed_size
-from .depth_weights import (CONFIGS, DPT_CONFIGS, DPT_HYBRID_CONFIGS, DPT_PROCESSOR, da_arch, da_config_from_json,
-                            da_processor_from_json, da_spec, dpt_config_from_json, dpt_hybrid_config_from_json,
-                            dpt_processed_size, dpt_processor_from_json, hf_config, hf_dpt_config,
-                            hf_dpt_hybrid_config, is_plain_v2)
+from .depth_engine import (FAMILY_DA_V2, FAMILY_DPT, FAMILY_DPT_BEIT, FAMILY_DPT_HYBRID, DepthEngine,
+                           processed_size as _processed_size)
+from .depth_weights import (CONFIGS, DPT_BEIT_CONFIGS, DPT_BEIT_PROCESSOR, DPT_CONFIGS, DPT_HYBRID_CONFIGS, DPT_PROCESSOR, da_arch,
+                            da_config_from_json, da_processor_from_json, da_spec, dpt_beit_config_from_json,
+                            dpt_beit_processed_size, dpt_beit_processor_from_json, dpt_config_from_json,
+                            dpt_hybrid_config_from_json, dpt_processed_size, dpt_processor_from_json, hf_config,
+                            hf_dpt_beit_config, hf_dpt_config, hf_dpt_hybrid_config, is_plain_v2)
 from .render_3d import _dialog, _val
 
 try:
@@ -36,7 +38,8 @@ pipe_type = None
 _engine = None
 
 # the checkpoints of the hot path (core/render_depth.py:689-712): the Depth-Anything family (V2, V1, Distill-Any-Depth,
-# the V2 metric models), DPT-Large and MiDaS 3.0 (DPT-Hybrid).  label -> (checkpoint id, backbone size)
+# the V2 metric models), DPT-Large, MiDaS 3.0 (DPT-Hybrid) and MiDaS v3.1 BEiT-L 512.  label -> (checkpoint id,
+# backbone size)
 supported_models = {
     "Distil-Any-Depth-Large": ("xingyang1/Distill-Any-Depth-Large-hf", "vitl"),
     "Distil-Any-Depth-Small": ("xingyang1/Distill-Any-Depth-Small-hf", "vits"),
@@ -53,6 +56,7 @@ supported_models = {
     "DPT-Large": ("Intel/dpt-large", "dpt-large"),
     "Manojb - DPT-Large": ("Manojb/dpt-large", "dpt-large"),
     "MiDaS 3.0": ("Intel/dpt-hybrid-midas", "dpt-hybrid-midas"),
+    "dpt-beit-large-512": ("Intel/dpt-beit-large-512", "dpt-beit-large-512"),
 }
 # the Depth-Anything checkpoints other than V2's: their taps and head are only in config.json (the tensors have V2's
 # shapes), so they load only with it, and with Depth-Anything's preprocessor_config.json when one is present
@@ -60,22 +64,43 @@ DA_CONFIG_REQUIRED = frozenset(v[0] for k, v in supported_models.items()
                                if v[1] in CONFIGS and not k.startswith("Depth Anything V2"))
 # DPT-Hybrid's BiT backbone is described only in config.json, so its checkpoints load only with one
 DPT_HYBRID_CONFIG_REQUIRED = frozenset(v[0] for v in supported_models.values() if v[1] in DPT_HYBRID_CONFIGS)
-_SERVED = "Depth-Anything (V2, V1, Distill-Any-Depth, V2-Metric), DPT-Large or MiDaS 3.0 (DPT-Hybrid)"
+# DPT-BEiT's out-indices, LayerScale and processed size live only in config.json and preprocessor_config.json: guessing
+# them would silently change the depth, so its checkpoints load only with both
+DPT_BEIT_FILES_REQUIRED = frozenset(v[0] for v in supported_models.values() if v[1] in DPT_BEIT_CONFIGS)
+_SERVED = ("Depth-Anything (V2, V1, Distill-Any-Depth, V2-Metric), DPT-Large, MiDaS 3.0 (DPT-Hybrid) or "
+           "dpt-beit-large-512 (MiDaS v3.1 BEiT-L)")
 
 
 def _family_of(arch):
     if arch in DPT_HYBRID_CONFIGS:
         return FAMILY_DPT_HYBRID
+    if arch in DPT_BEIT_CONFIGS:
+        return FAMILY_DPT_BEIT
     return FAMILY_DPT if arch in DPT_CONFIGS else FAMILY_DA_V2
 
 
 def _dpt_like(arch):
-    """DPT-Large and DPT-Hybrid: the fixed-size DPT processor, no tiled depth."""
-    return _family_of(arch) in (FAMILY_DPT, FAMILY_DPT_HYBRID)
+    """DPT-Large, DPT-Hybrid and DPT-BEiT: DPT's processor settings, no tiled depth."""
+    return _family_of(arch) in (FAMILY_DPT, FAMILY_DPT_HYBRID, FAMILY_DPT_BEIT)
 
 
 def _dpt_configs(arch):
-    return DPT_HYBRID_CONFIGS[arch] if _family_of(arch) == FAMILY_DPT_HYBRID else DPT_CONFIGS[arch]
+    return {FAMILY_DPT_HYBRID: DPT_HYBRID_CONFIGS, FAMILY_DPT_BEIT: DPT_BEIT_CONFIGS}.get(_family_of(arch),
+                                                                                     DPT_CONFIGS)[arch]
+
+
+def _load_dpt_beit_checkpoint(sd, cfg_path):
+    """arch of a DPT-BEiT state dict (relative_position_bias_table keys): "dpt-beit-large-512" when config.json
+    (required: the taps and LayerScale are described only there) is served and matches the built-in configuration."""
+    import json
+    if not os.path.exists(cfg_path):
+        raise ValueError(f"a DPT-BEiT checkpoint needs its config.json (not found: {cfg_path})")
+    with open(cfg_path) as f:
+        got = dpt_beit_config_from_json(json.load(f))
+    c = DPT_BEIT_CONFIGS["dpt-beit-large-512"]
+    if got != c:
+        raise ValueError(f"config.json {got} does not match the built-in dpt-beit-large-512 configuration {c}")
+    return "dpt-beit-large-512"
 
 
 def _load_dpt_hybrid_checkpoint(sd, cfg_path):
@@ -123,7 +148,8 @@ def load_checkpoint(path):
     to it, the model is what da_config_from_json reads there (ValueError for what the engine does not serve): arch is
     the size key of depth_weights.CONFIGS for a plain V2 model, else the spec dict (V1 taps, a metric head); without
     one, the V2 size of the hidden width.  DPT: cross-checked against DPT_CONFIGS.  DPT-Hybrid (BiT backbone keys):
-    config.json is required and must be the one DPT_HYBRID_CONFIGS serves."""
+    config.json is required and must be the one DPT_HYBRID_CONFIGS serves.  DPT-BEiT (relative_position_bias_table keys,
+    routed before the backbone.embeddings.cls_token test that Depth-Anything shares): likewise with DPT_BEIT_CONFIGS."""
     import json
     import os
     if path.endswith(".safetensors"):
@@ -135,6 +161,8 @@ def load_checkpoint(path):
         return _load_dpt_hybrid_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
     if "dpt.embeddings.cls_token" in sd:
         return _load_dpt_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
+    if any(k.endswith("relative_position_bias_table") for k in sd):
+        return _load_dpt_beit_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
     if "backbone.embeddings.cls_token" not in sd:
         return None, sd
     cfg_path = os.path.join(os.path.dirname(path), "config.json")
@@ -169,7 +197,10 @@ local_model_dir = _weights_dir()
 
 def model_processed_size(width, height):
     """(h, w) the loaded model's image processor resizes a (width, height) image to: Depth-Anything-V2 keeps the
-    aspect at multiples of 14 near 518, DPT-Large and MiDaS 3.0 resize every image to their processor's fixed size."""
+    aspect at multiples of 14 near 518, DPT-Large and MiDaS 3.0 resize every image to their processor's fixed size,
+    dpt-beit-large-512 keeps the aspect at multiples of 32 near 512 (or its processor's fixed size)."""
+    if _family_of(_arch) == FAMILY_DPT_BEIT:
+        return dpt_beit_processed_size(width, height, _processor)
     if _dpt_like(_arch):
         return dpt_processed_size(_processor)
     return _processed_size(width, height)
@@ -177,7 +208,8 @@ def model_processed_size(width, height):
 
 def _check_tiled_supported():
     if USE_TILED_DEPTH and _dpt_like(_arch):
-        raise ValueError("USE_TILED_DEPTH is served for Depth-Anything-V2 models only, not for DPT-Large or MiDaS 3.0")
+        raise ValueError("USE_TILED_DEPTH is served for Depth-Anything-V2 models only, not for DPT-Large, MiDaS 3.0 or "
+                         "dpt-beit-large-512")
 
 
 def _engine_for(width, height):
@@ -198,13 +230,15 @@ def _engine_for(width, height):
 
 
 def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed=0, processor=None):
-    """Make `pipe` serve a Depth-Anything model, DPT-Large ("dpt-large") or MiDaS 3.0 ("dpt-hybrid-midas").  arch: a Depth-Anything-V2 size ("vits" /
+    """Make `pipe` serve a Depth-Anything model, DPT-Large ("dpt-large"), MiDaS 3.0 ("dpt-hybrid-midas") or MiDaS v3.1
+    BEiT-L 512 ("dpt-beit-large-512").  arch: a Depth-Anything-V2 size ("vits" /
     "vitb" / "vitl") or a Depth-Anything spec dict (depth_weights.da_spec / da_config_from_json: V1's taps, a metric
     head with its max_depth), which every engine built from these weights then carries.
     `state_dict` uses HF DepthAnythingForDepthEstimation / DPTForDepthEstimation naming (e.g. from a local
     safetensors checkpoint); without one a random-init model (torch.manual_seed(seed)) is used -- there is no network
     here and the reference ships no weights.  processor (DPT only): the image processor's settings
-    (dpt_processor_from_json of the checkpoint's preprocessor_config.json; default DPTImageProcessor's).  (width,
+    (dpt_processor_from_json of the checkpoint's preprocessor_config.json, dpt_beit_processor_from_json for BEiT;
+    default DPTImageProcessor's, DPT_BEIT_PROCESSOR for BEiT).  (width,
     height) only pre-builds the engine for that frame shape; other shapes get their own engine on first use."""
     global pipe, pipe_type, _state_dict, _arch, _spec, _processor
     spec = None
@@ -218,14 +252,18 @@ def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed
         raise ValueError(f"unknown depth model {arch!r}")
     if not dpt and spec is None:
         spec = da_spec(arch)
-    if dpt:
+    beit = _family_of(arch) == FAMILY_DPT_BEIT
+    if beit:
+        processor = dict(processor or DPT_BEIT_PROCESSOR)
+    elif dpt:
         processor = dict(processor or DPT_PROCESSOR)
         dpt_processed_size(processor)  # refuse an unserved processor before anything is built
     if state_dict is None:
         torch.manual_seed(seed)
         if dpt:
             from transformers import DPTForDepthEstimation
-            hf = hf_dpt_hybrid_config(arch) if _family_of(arch) == FAMILY_DPT_HYBRID else hf_dpt_config(arch)
+            hf = {FAMILY_DPT_HYBRID: hf_dpt_hybrid_config, FAMILY_DPT_BEIT: hf_dpt_beit_config}.get(
+                _family_of(arch), hf_dpt_config)(arch)
             state_dict = DPTForDepthEstimation(hf).eval().state_dict()
         else:
             from transformers import DepthAnythingForDepthEstimation
@@ -616,6 +654,12 @@ def ensure_model_downloaded(checkpoint):
     if checkpoint in DPT_HYBRID_CONFIG_REQUIRED and not os.path.exists(os.path.join(ckdir, "config.json")):
         print(f"❌ {checkpoint}: no config.json next to {path} (its BiT backbone is described only there)")
         return None, None
+    if checkpoint in DPT_BEIT_FILES_REQUIRED:
+        for name in ("config.json", "preprocessor_config.json"):
+            if not os.path.exists(os.path.join(ckdir, name)):
+                print(f"❌ {checkpoint}: no {name} next to {path} (its out-indices, LayerScale and processed size are "
+                      "only in config.json and preprocessor_config.json)")
+                return None, None
     try:
         arch, sd = load_checkpoint(path)
     except Exception as e:
@@ -640,7 +684,15 @@ def ensure_model_downloaded(checkpoint):
             except ValueError as e:
                 print(f"❌ {pp}: {e}")
                 return None, None
-    if _dpt_like(arch):
+    if _family_of(arch) == FAMILY_DPT_BEIT:
+        pp = os.path.join(ckdir, "preprocessor_config.json")
+        try:
+            with open(pp) as f:
+                meta["processor"] = dpt_beit_processor_from_json(json.load(f))
+        except (OSError, ValueError) as e:
+            print(f"❌ {pp}: {e}")
+            return None, None
+    elif _dpt_like(arch):
         pp = os.path.join(ckdir, "preprocessor_config.json")
         try:
             if os.path.exists(pp):
