@@ -354,12 +354,18 @@ int vd3d_depth_create(const vd3d_depth_config* cfg, void* cuda_stream, vd3d_dept
  * third of "qkv.b" and "pos" are zero.  Patch 16, relative head; image_h and image_w multiples of 32 (rectangular
  * grids allowed).  The table, one int per key column and the attention's 91 KB must fit the 227 KB of shared memory of
  * one block: every grid inside the engine's 3072-token limit does (at most ~152 KB).  The processor resizes every
- * image to image_h x image_w, or keeps the aspect ratio after vd3d_depth_set_fit. */
-enum { VD3D_DEPTH_DA_V2 = 0, VD3D_DEPTH_DPT = 1, VD3D_DEPTH_DPT_HYBRID = 2, VD3D_DEPTH_DPT_BEIT = 3 };
+ * image to image_h x image_w, or keeps the aspect ratio after vd3d_depth_set_fit.
+ * VD3D_DEPTH_ZOEDEPTH is ZoeDepth ("Intel/zoedepth-nyu-kitti" and the single-configuration checkpoints): the trunk, neck
+ * and fusion of VD3D_DEPTH_DPT_BEIT (same arguments and tensors, the tables resampled from ZoeDepth's 24 x 24 window), the
+ * relative head's conv2 + ReLU activation, and the metric-bins head ("z.*" tensors, depth_weights.prepare_zoedepth) set
+ * up by vd3d_depth_set_zoe.  The two-configuration head routes each image on its own (the router's argmax is a device
+ * int, so a batch equals its single forwards).  Outputs metric depth at the processed size. */
+enum { VD3D_DEPTH_DA_V2 = 0, VD3D_DEPTH_DPT = 1, VD3D_DEPTH_DPT_HYBRID = 2, VD3D_DEPTH_DPT_BEIT = 3,
+       VD3D_DEPTH_ZOEDEPTH = 4 };
 enum { VD3D_HEAD_RELATIVE = 0, VD3D_HEAD_METRIC = 1 };
 typedef struct {
   vd3d_depth_config base; /* image_h / image_w multiples of patch */
-  int32_t family;         /* VD3D_DEPTH_DA_V2, VD3D_DEPTH_DPT, VD3D_DEPTH_DPT_HYBRID or VD3D_DEPTH_DPT_BEIT */
+  int32_t family;         /* VD3D_DEPTH_DA_V2, _DPT, _DPT_HYBRID, _DPT_BEIT or _ZOEDEPTH */
   int32_t patch;          /* 14 (DINOv2) or 16 (ViT-L/16) */
   float ln_eps;           /* 1e-6 (DINOv2) or 1e-12 (DPT) */
   int32_t resample;       /* the processor's PIL resample code: 3 bicubic or 2 bilinear */
@@ -375,8 +381,20 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* cfg, void* cuda_stream, vd3
 /* VD3D_DEPTH_DPT_BEIT: the image processor keeps the aspect ratio (DPTImageProcessor with keep_aspect_ratio and
  * ensure_multiple_of): scale the side whose scale to fit_h x fit_w is closer to 1, round both sides to multiples of
  * `multiple` (32); vd3d_depth_infer_images then serves the inputs that map to image_h x image_w.  multiple 0: back to
- * the fixed size.  VD3D_ERR_ARG for another family, a multiple other than 0 / 32 or a target side below 32. */
+ * the fixed size.  VD3D_ERR_ARG for a family other than _DPT_BEIT / _ZOEDEPTH, a multiple other than 0 / 32 or a target
+ * side below 32. */
 int vd3d_depth_set_fit(vd3d_depth* e, int fit_h, int fit_w, int multiple);
+/* VD3D_DEPTH_ZOEDEPTH's processor is ZoeDepthImageProcessor: every image is reflect-padded by int(sqrt(h / 2) * 3) rows
+ * and int(sqrt(w / 2) * 3) columns, the padded size is fitted as above (vd3d_depth_set_fit: keep-aspect multiples of 32;
+ * or the fixed size), and the resize is bilinear with align_corners on the rescaled float image.  The post-process
+ * resizes (bicubic) to the padded source size and crops the padding off.
+ * The metric head's scalars: n_conf bin configurations (1 or 2; 2 routes each image), n_bins (64), min_depth /
+ * max_depth [n_conf] (checked; the softplus bins are unbounded, so the forward does not read them), the log-binomial
+ * temperature range, attractors[4] per attractor layer (1..16; the count of each
+ * layer's conv2, 16 for every layer of the two-configuration head), cat_relative 1 when the relative depth is the
+ * log-binomial's 33rd input (the single-configuration head).  VD3D_ERR_ARG for another family or any value not served. */
+int vd3d_depth_set_zoe(vd3d_depth* e, int n_conf, int n_bins, const float* min_depth, const float* max_depth,
+                       float min_temp, float max_temp, const int32_t* attractors, int cat_relative);
 void vd3d_depth_destroy(vd3d_depth* e);
 /* CUDA-event timing of the fc1 GEMM launches (k_umma_gemm<128,4>; M = tokens, N = 4*hidden, K = hidden) */
 int vd3d_depth_profile(vd3d_depth* e, int enable);
@@ -478,6 +496,14 @@ int vd3d_conv_f16(vd3d_depth* e, const void* in_nhwc_f16, int H, int W, int cin,
  *   op 2 max-pool (dims H, W, C): t.in f16 [H, W, C] -> f16 [H/2, W/2, C]
  *   op 3 SAME im2col (dims H, W, C, k, pb): t.in f16 [H, W, C] -> f16 [H/2 * W/2, k * k * C] */
 int vd3d_bit_kernel(vd3d_depth* e, int op, const int32_t* dims);
+/* unit-test hook for the ZoeDepth kernels, in the style of vd3d_bit_kernel (output "t.out"; the route in "t.route").
+ *   op 0 preprocess (h, w, OH, OW, swap_rb): t.img u8 [h, w, 3] -> f32 [3, OH, OW] with the engine's mean / std
+ *   op 1 router (n, F): t.x f32 [n, F], t.w packed router, t.pe f32 [n + 1, 128] -> logits f32 [2]
+ *   op 2 attractor (H, W, Hp, Wp, nc, route, na, seed): t.hid f16 [H W, nc 128], t.w2 f32 [nc][na][128], t.b2
+ *        [nc][na], t.prev f32 [Hp Wp, seed ? nc 64 : 64] -> bins f32 [H W, 64]
+ *   op 3 log-binomial (H, W, He, We, nc, route, cat, hid): t.act f16 [H W, 32], t.emb f16 [He We, 128], t.bins f32
+ *        [He We, 64], t.lb f32 [nc][...], t.temp f32 {min, max}, t.w3 / t.b3 when cat -> depth f32 [H W] */
+int vd3d_zoe_kernel(vd3d_depth* e, int op, const int32_t* dims);
 
 #ifdef __cplusplus
 }

@@ -102,9 +102,9 @@ SYMBOLS = [
     "vd3d_profile", "vd3d_profile_collect", "vd3d_check_config", "vd3d_color_grade", "vd3d_resize_cubic", "vd3d_add_weighted",
     "vd3d_sr_create", "vd3d_sr_forward", "vd3d_sr_upscale", "vd3d_sr_set_rrdb",
     # depth forward (bound in depth_engine.py)
-    "vd3d_depth_create", "vd3d_depth_create_ex", "vd3d_depth_set_fit", "vd3d_depth_destroy", "vd3d_depth_last_error", "vd3d_depth_launch_count",
+    "vd3d_depth_create", "vd3d_depth_create_ex", "vd3d_depth_set_fit", "vd3d_depth_set_zoe", "vd3d_depth_destroy", "vd3d_depth_last_error", "vd3d_depth_launch_count",
     "vd3d_depth_set_tensor", "vd3d_depth_forward", "vd3d_depth_get_buffer", "vd3d_gemm_f16", "vd3d_conv_f16",
-    "vd3d_bit_kernel",
+    "vd3d_bit_kernel", "vd3d_zoe_kernel",
     "vd3d_depth_infer_batch", "vd3d_depth_infer_batch_device",
     "vd3d_set_depth_batch", "vd3d_get_depth_batch", "vd3d_render_clip_depth", "vd3d_depth_add_launches", "vd3d_depth_clone", "vd3d_release_depth",
     "vd3d_depth_profile", "vd3d_depth_profile_collect", "vd3d_depth_profile_spans",

@@ -57,6 +57,10 @@ struct vd3d_depth {
   PreprocParams pre = kImagenetBicubic;
   // BEiT's keep-aspect processor (vd3d_depth_set_fit): target and multiple; fit_multiple 0: a fixed size
   int fit_h = 0, fit_w = 0, fit_multiple = 0;
+  // ZoeDepth's metric head (vd3d_depth_set_zoe): bin configurations (0: not set), attractors per layer, temperature
+  // range, whether the relative depth is the log-binomial's 33rd input
+  int zoe_nc = 0, zoe_na[4] = {}, zoe_cat = 0;
+  float zoe_tmin = 0.f, zoe_tmax = 0.f;
   // the head's last activation (VD3D_HEAD_RELATIVE / _METRIC) and the metric head's scale; every EPI_HEAD reads them
   int head = VD3D_HEAD_RELATIVE;
   float max_depth = 1.f;
@@ -236,6 +240,10 @@ int conv(vd3d_depth* e, const __half* in, int H, int W, int cin, const __half* w
 
 int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
+// ZoeDepthImageProcessor's reflect padding of an h-row (or w-column) image: int(sqrt(h / 2) * 3), the same value
+// post_process_depth_estimation crops off
+int zoe_pad(int n) { return (int)(sqrt(n / 2.0) * 3.0); }
+
 }  // namespace
 
 extern "C" {
@@ -245,7 +253,9 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
   *out = nullptr;
   if (!load_encode()) return VD3D_ERR_CUDA;
   const vd3d_depth_config* cfg = &x->base;
-  const bool hybrid = x->family == VD3D_DEPTH_DPT_HYBRID, beit = x->family == VD3D_DEPTH_DPT_BEIT;
+  const bool hybrid = x->family == VD3D_DEPTH_DPT_HYBRID;
+  // ZoeDepth's trunk, neck and fusion are dpt-beit-large-512's
+  const bool beit = x->family == VD3D_DEPTH_DPT_BEIT || x->family == VD3D_DEPTH_ZOEDEPTH;
   const bool dpt = x->family == VD3D_DEPTH_DPT || hybrid || beit;
   if ((x->family != VD3D_DEPTH_DA_V2 && !dpt) || (x->patch != 14 && x->patch != 16) ||
       (x->resample != 2 && x->resample != 3) || !(x->ln_eps > 0.f) || cfg->heads < 1)
@@ -292,11 +302,29 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
 }
 
 int vd3d_depth_set_fit(vd3d_depth* e, int fit_h, int fit_w, int multiple) {
-  if (!e || e->family != VD3D_DEPTH_DPT_BEIT || (multiple != 0 && multiple != 32) || (multiple && (fit_h < 32 || fit_w < 32)))
+  if (!e || (e->family != VD3D_DEPTH_DPT_BEIT && e->family != VD3D_DEPTH_ZOEDEPTH) || (multiple != 0 && multiple != 32) || (multiple && (fit_h < 32 || fit_w < 32)))
     return VD3D_ERR_ARG;
   e->fit_h = multiple ? fit_h : 0;
   e->fit_w = multiple ? fit_w : 0;
   e->fit_multiple = multiple;
+  return VD3D_OK;
+}
+
+int vd3d_depth_set_zoe(vd3d_depth* e, int n_conf, int n_bins, const float* min_depth, const float* max_depth,
+                       float min_temp, float max_temp, const int32_t* attractors, int cat_relative) {
+  if (!e || e->family != VD3D_DEPTH_ZOEDEPTH || (n_conf != 1 && n_conf != 2) || n_bins != kZoeBins || !min_depth ||
+      !max_depth || !attractors || !(min_temp > 0.f) || !(max_temp > min_temp) || !isfinite(max_temp) ||
+      (cat_relative != 0 && cat_relative != 1))
+    return VD3D_ERR_ARG;
+  for (int i = 0; i < n_conf; ++i)
+    if (!(min_depth[i] >= 0.f) || !(max_depth[i] > min_depth[i]) || !isfinite(max_depth[i])) return VD3D_ERR_ARG;
+  for (int j = 0; j < 4; ++j)
+    if (attractors[j] < 1 || attractors[j] > kZoeMaxAttr) return VD3D_ERR_ARG;
+  e->zoe_nc = n_conf;
+  e->zoe_cat = cat_relative;
+  e->zoe_tmin = min_temp;
+  e->zoe_tmax = max_temp;
+  for (int j = 0; j < 4; ++j) e->zoe_na[j] = attractors[j];
   return VD3D_OK;
 }
 
@@ -389,6 +417,11 @@ int vd3d_depth_clone(vd3d_depth* src, void* stream, vd3d_depth** out) {
   e->fit_h = src->fit_h;
   e->fit_w = src->fit_w;
   e->fit_multiple = src->fit_multiple;
+  e->zoe_nc = src->zoe_nc;
+  e->zoe_cat = src->zoe_cat;
+  e->zoe_tmin = src->zoe_tmin;
+  e->zoe_tmax = src->zoe_tmax;
+  for (int j = 0; j < 4; ++j) e->zoe_na[j] = src->zoe_na[j];
   e->stream = (cudaStream_t)stream;
   e->w = src->w;
   e->owns_weights = false;
@@ -550,6 +583,66 @@ int vd3d_bit_kernel(vd3d_depth* e, int op, const int32_t* d) {
       launch_maxpool_same(in, H, Wd, C, (__half*)out, s);
     else
       launch_im2col_same(in, H, Wd, C, k, pb, (__half*)out, s);
+  }
+  DCK(cudaGetLastError());
+  DCK(cudaStreamSynchronize(s));
+  return VD3D_OK;
+}
+
+// unit-test hook: one ZoeDepth kernel on uploaded "t.*" tensors (vd3d.h vd3d_zoe_kernel), output in "t.out"
+int vd3d_zoe_kernel(vd3d_depth* e, int op, const int32_t* d) {
+  if (!e || !d || op < 0 || op > 3) return VD3D_ERR_ARG;
+  cudaStream_t s = e->stream;
+  int r;
+  void *out, *route;
+  if ((r = get_buf(e, "t.route", 16, &route))) return r;
+  if (op == 0) {
+    const int h = d[0], w = d[1], OH = d[2], OW = d[3];
+    const uint8_t* img;
+    if (h < 2 || w < 2 || OH < 1 || OW < 1) return VD3D_ERR_ARG;
+    if ((r = W(e, "t.img", &img, (size_t)h * w * 3)) || (r = get_buf(e, "t.out", (size_t)3 * OH * OW * 4, &out))) return r;
+    launch_zoe_preprocess(img, h, w, d[4] != 0, zoe_pad(h), zoe_pad(w), (float*)out, OH, OW, e->pre, s);
+  } else if (op == 1) {
+    const int n = d[0], F = d[1];
+    const float *x, *wt, *pe;
+    if (n < 1 || F < 64 || F % 64) return VD3D_ERR_ARG;
+    if ((r = W(e, "t.x", &x, (size_t)n * F)) || (r = W(e, "t.w", &wt, zoe_router_floats(F))) ||
+        (r = W(e, "t.pe", &pe, (size_t)(n + 1) * kZoeE)))
+      return r;
+    void* scratch;
+    if ((r = get_buf(e, "t.scratch", zoe_router_scratch(n) * 4, &scratch)) || (r = get_buf(e, "t.out", 8, &out))) return r;
+    launch_zoe_router(x, n, F, wt, pe, (float*)scratch, (float*)out, (int*)route, s);
+  } else {
+    const int H = d[0], Wd = d[1], Hp = d[2], Wp = d[3], nc = d[4], rt = d[5];
+    if (H < 1 || Wd < 1 || Hp < 1 || Wp < 1 || (nc != 1 && nc != 2) || rt < 0 || rt >= nc) return VD3D_ERR_ARG;
+    DCK(cudaMemcpyAsync(route, &rt, 4, cudaMemcpyHostToDevice, s));
+    if (op == 2) {  // d[6] attractors, d[7] 1: prev is the seed regressor's raw conv2 of every configuration
+      const int na = d[6], seed = d[7] != 0, ldp = seed ? nc * kZoeBins : kZoeBins;
+      const __half* hid;
+      const float *w2, *b2, *prev;
+      if (na < 1 || na > kZoeMaxAttr) return VD3D_ERR_ARG;
+      if ((r = W(e, "t.hid", &hid, (size_t)H * Wd * nc * kZoeE)) || (r = W(e, "t.w2", &w2, (size_t)nc * na * kZoeE)) ||
+          (r = W(e, "t.b2", &b2, (size_t)nc * na)) || (r = W(e, "t.prev", &prev, (size_t)Hp * Wp * ldp)) ||
+          (r = get_buf(e, "t.out", (size_t)H * Wd * kZoeBins * 4, &out)))
+        return r;
+      launch_zoe_attractor(hid, nc * kZoeE, kZoeE, w2, b2, na, prev, ldp, seed ? kZoeBins : 0, seed, Hp, Wp, (float*)out,
+                           H, Wd, (const int*)route, s);
+    } else {  // d[6] 1: the relative depth is the 33rd input; d[7] hidden units; t.temp f32 {min_temp, max_temp}
+      const int cat = d[6] != 0, hid = d[7], cin = 32 + cat + kZoeE;
+      const __half *act, *emb;
+      const float *w3 = nullptr, *b3 = nullptr, *bins, *lb, *temp;
+      if (hid != 40 && hid != 80) return VD3D_ERR_ARG;
+      if ((r = W(e, "t.act", &act, (size_t)H * Wd * 32)) || (r = W(e, "t.emb", &emb, (size_t)Hp * Wp * kZoeE)) ||
+          (r = W(e, "t.bins", &bins, (size_t)Hp * Wp * kZoeBins)) ||
+          (r = W(e, "t.lb", &lb, (size_t)nc * zoe_logbinom_floats(cin, hid))) || (r = W(e, "t.temp", &temp, 2)) ||
+          (cat && ((r = W(e, "t.w3", &w3, 32)) || (r = W(e, "t.b3", &b3, 1)))) ||
+          (r = get_buf(e, "t.out", (size_t)H * Wd * 4, &out)))
+        return r;
+      float tt[2];
+      DCK(cudaMemcpy(tt, temp, 8, cudaMemcpyDeviceToHost));
+      DCK(launch_zoe_logbinom(act, w3, b3, emb, bins, Hp, Wp, kZoeE, lb, cin, hid, tt[0], tt[1], (float*)out, H, Wd,
+                              (const int*)route, s));
+    }
   }
   DCK(cudaGetLastError());
   DCK(cudaStreamSynchronize(s));
@@ -725,6 +818,149 @@ int bit_backbone(vd3d_depth* e, int b, const float* px, const __half** stage3) {
   return VD3D_OK;
 }
 
+// ---- ZoeDepth's metric head (transformers 5.5 ZoeDepthMultipleMetricDepthEstimationHeads / ...MetricDepthEstimationHead)
+// on one image, on the stream of its tail.  bott: neck.convs[3]'s output f16 [bh bw, F]; fused[j]: the fusion outputs
+// (coarse to fine); act: the relative head's conv2 + ReLU f16 [IH IW, 32]; depth f32 [IH, IW].  The route is a device int
+// (the router's argmax, or 0 for a single configuration) that the configuration-specific kernels read: no host
+// synchronisation.  The config-independent 1x1 layers run on k_umma_gemm; the seed regressor's and the attractors' conv1,
+// whose inputs do not depend on the route, run every configuration in one GEMM (weights concatenated along N; the seed
+// conv2 block-diagonal) and the consumer reads the route's columns.
+// Weights ("z.*", depth_weights.prepare_zoedepth): z.bt (bottleneck conv2), z.s1 / z.s2 (seed regressor), z.sp1 / z.sp2
+// (seed projector), z.p{j}.1 / .2 (projectors), z.a{j}.1 (attractor conv1, f16) and z.a{j}.2.w / .b (attractor conv2,
+// f32 [nc][na][E] / [nc][na]), z.lb (log-binomial MLPs, f32 [nc][zoe_logbinom_floats]), z.router and z.r.pe (router).
+size_t wlen(vd3d_depth* e, const char* name) {
+  auto it = e->w.find(name);
+  return it == e->w.end() ? 0 : it->second.bytes / 4;
+}
+int zoe_head(vd3d_depth* e, const std::string& sfx, const __half* bott, int bh, int bw, const __half* const* fused,
+             const int* fh, const int* fw, const __half* act, float* depth) {
+  cudaStream_t s = e->cur ? e->cur : e->stream;
+  const int F = e->cfg.fusion, NC = e->zoe_nc, E = kZoeE, NB = kZoeBins, IH = e->cfg.image_h, IW = e->cfg.image_w;
+  const int nb3 = bh * bw;
+  const int ms = (int)(wlen(e, "z.s1.b") / NC), mp = (int)wlen(e, "z.sp1.b");
+  const int cin = 32 + e->zoe_cat + E;
+  const int hid = (int)((wlen(e, "z.lb") / NC - 4) / (cin + 5));
+  if (ms % 64 || mp % 64 || !ms || !mp || (hid != 40 && hid != 80) ||
+      wlen(e, "z.lb") != (size_t)NC * zoe_logbinom_floats(cin, hid))
+    return dfail(e, VD3D_ERR_STATE, "ZoeDepth: metric head tensors missing or of unserved sizes");
+  int r;
+  char nm[64];
+  auto buf = [&](const char* base, size_t bytes, void** p) { return get_buf(e, std::string(base) + sfx, bytes, p); };
+  auto wt = [&](const char* base, const __half** w16, const float** b32, size_t wn, size_t bn) {
+    snprintf(nm, sizeof nm, "%s.w", base);
+    int rr = W(e, nm, w16, wn);
+    if (rr) return rr;
+    snprintf(nm, sizeof nm, "%s.b", base);
+    return W(e, nm, b32, bn);
+  };
+  // 1x1 layer on k_umma_gemm: out = act(A W^T + b) [+ res], f16 (or f32 when out32)
+  auto lin = [&](const __half* A, int M, int K, const __half* w, const float* bias, int N, int relu, void* out,
+                 bool out32, const __half* res) {
+    GemmArgs g = base_args(M, N, K, out32 ? EPI_F32 : EPI_F16);
+    if (out32)
+      g.out_f32 = (float*)out;
+    else
+      g.out_f16 = (__half*)out;
+    g.bias = bias;
+    g.act = relu ? 2 : 0;
+    g.res_f16 = res;
+    return gemm(e, A, K, w, K, g);
+  };
+  const size_t R3 = round_up(nb3, 128);
+  void *zb16, *zb32, *route, *logits, *sh, *seed, *t1, *emb[2], *bins[2], *up, *x, *hb;
+  const size_t Mmax = (size_t)round_up(fh[3] * fw[3], 128);
+  if ((r = buf("z.zb16", R3 * F * 2, &zb16)) || (r = buf("z.zb32", R3 * F * 4, &zb32)) ||
+      (r = buf("z.route", 16, &route)) || (r = buf("z.logits", 16, &logits)) ||
+      (r = buf("z.sh", R3 * NC * ms * 2, &sh)) || (r = buf("z.seed", R3 * NC * NB * 4, &seed)) ||
+      (r = buf("z.t1", Mmax * std::max(mp, ms) * 2, &t1)) || (r = buf("z.emb0", Mmax * E * 2, &emb[0])) ||
+      (r = buf("z.emb1", Mmax * E * 2, &emb[1])) || (r = buf("z.bins0", Mmax * NB * 4, &bins[0])) ||
+      (r = buf("z.bins1", Mmax * NB * 4, &bins[1])) || (r = buf("z.up", Mmax * E * 2, &up)) ||
+      (r = buf("z.x", Mmax * E * 2, &x)) || (r = buf("z.hid", Mmax * NC * E * 2, &hb)))
+    return r;
+  const __half* w16;
+  const float* b32;
+  // ---- bottleneck conv2 (f16 for the GEMMs, f32 for the router), router, seed regressor, seed projector ----
+  int sp = e->span_begin("zoe.bottleneck", s);
+  if ((r = wt("z.bt", &w16, &b32, (size_t)F * F, F)) || (r = lin(bott, nb3, F, w16, b32, F, 0, zb16, false, nullptr)) ||
+      (r = lin(bott, nb3, F, w16, b32, F, 0, zb32, true, nullptr)))
+    return r;
+  e->span_end(sp, s);
+  sp = e->span_begin("zoe.router", s);
+  if (NC == 2) {
+    const float *rw, *pe;
+    if ((r = W(e, "z.router", &rw, zoe_router_floats(F))) || (r = W(e, "z.r.pe", &pe, (size_t)(nb3 + 1) * E))) return r;
+    void* scratch;
+    if ((r = buf("z.rscratch", zoe_router_scratch(nb3) * 4, &scratch))) return r;
+    launch_zoe_router((const float*)zb32, nb3, F, rw, pe, (float*)scratch, (float*)logits, (int*)route, s);
+    e->launches++;
+  } else {
+    DCK(cudaMemsetAsync(route, 0, 16, s));
+  }
+  e->span_end(sp, s);
+  sp = e->span_begin("zoe.seed", s);
+  if ((r = wt("z.s1", &w16, &b32, (size_t)NC * ms * F, NC * ms)) ||
+      (r = lin((const __half*)zb16, nb3, F, w16, b32, NC * ms, 1, sh, false, nullptr)) ||
+      (r = wt("z.s2", &w16, &b32, (size_t)NC * NB * NC * ms, NC * NB)) ||
+      (r = lin((const __half*)sh, nb3, NC * ms, w16, b32, NC * NB, 0, seed, true, nullptr)) ||
+      (r = wt("z.sp1", &w16, &b32, (size_t)mp * F, mp)) ||
+      (r = lin((const __half*)zb16, nb3, F, w16, b32, mp, 1, t1, false, nullptr)) ||
+      (r = wt("z.sp2", &w16, &b32, (size_t)E * mp, E)) ||
+      (r = lin((const __half*)t1, nb3, mp, w16, b32, E, 0, emb[1], false, nullptr)))
+    return r;
+  e->span_end(sp, s);
+  // ---- four attractor layers, coarse to fine ----
+  int ph_ = bh, pw_ = bw;
+  for (int j = 0; j < 4; ++j) {
+    const int H = fh[j], Wd = fw[j], M = H * Wd;
+    void *cur = emb[j & 1], *prev = emb[(j + 1) & 1];
+    char base[16];
+    sp = e->span_begin("zoe.proj", s);
+    snprintf(base, sizeof base, "z.p%d.1", j);
+    if ((r = wt(base, &w16, &b32, (size_t)mp * F, mp)) || (r = lin(fused[j], M, F, w16, b32, mp, 1, t1, false, nullptr)))
+      return r;
+    launch_upsample_ac((const __half*)prev, ph_, pw_, E, (__half*)up, H, Wd, s);
+    e->launches++;
+    snprintf(base, sizeof base, "z.p%d.2", j);
+    if ((r = wt(base, &w16, &b32, (size_t)E * mp, E)) ||
+        (r = lin((const __half*)t1, M, mp, w16, b32, E, 0, x, false, (const __half*)up)) ||
+        (r = lin((const __half*)t1, M, mp, w16, b32, E, 0, cur, false, nullptr)))
+      return r;
+    e->span_end(sp, s);
+    sp = e->span_begin("zoe.attractor", s);
+    snprintf(base, sizeof base, "z.a%d.1", j);
+    if ((r = wt(base, &w16, &b32, (size_t)NC * E * E, NC * E)) ||
+        (r = lin((const __half*)x, M, E, w16, b32, NC * E, 1, hb, false, nullptr)))
+      return r;
+    const float *w2, *b2;
+    const int na = e->zoe_na[j];
+    snprintf(nm, sizeof nm, "z.a%d.2.w", j);
+    if ((r = W(e, nm, &w2, (size_t)NC * na * E))) return r;
+    snprintf(nm, sizeof nm, "z.a%d.2.b", j);
+    if ((r = W(e, nm, &b2, (size_t)NC * na))) return r;
+    if (j == 0)
+      launch_zoe_attractor((const __half*)hb, NC * E, E, w2, b2, na, (const float*)seed, NC * NB, NB, 1, bh, bw,
+                           (float*)bins[0], H, Wd, (const int*)route, s);
+    else
+      launch_zoe_attractor((const __half*)hb, NC * E, E, w2, b2, na, (const float*)bins[(j + 1) & 1], NB, 0, 0, ph_, pw_,
+                           (float*)bins[j & 1], H, Wd, (const int*)route, s);
+    e->launches++;
+    e->span_end(sp, s);
+    ph_ = H;
+    pw_ = Wd;
+  }
+  // ---- conditional log-binomial + expectation at the processed size ----
+  const float *lb, *w3 = nullptr, *b3 = nullptr;
+  if ((r = W(e, "z.lb", &lb)) || (e->zoe_cat && ((r = W(e, "h.c3.w", &w3, 32)) || (r = W(e, "h.c3.b", &b3, 1)))))
+    return r;
+  sp = e->span_begin("zoe.logbinom", s);
+  cudaError_t ce = launch_zoe_logbinom(act, w3, b3, (const __half*)emb[1], (const float*)bins[1], ph_, pw_, E, lb, cin,
+                                       hid, e->zoe_tmin, e->zoe_tmax, depth, IH, IW, (const int*)route, s);
+  if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("zoe log-binomial launch: ") + cudaGetErrorString(ce));
+  e->launches++;
+  e->span_end(sp, s);
+  return VD3D_OK;
+}
+
 // B images through the network in one pass.  The token-wise stages (LayerNorm, QKV / proj / fc1 / fc2 GEMMs) see one
 // matrix of (B-1)*NP + NT rows -- image b owns rows [b*NP, b*NP + NT), NP = NT rounded up to the 128-row tile -- so the
 // GEMMs run at 3-4x the rows of one frame (the reference batches too: core/render_depth.py:1113-1119); attention runs
@@ -740,7 +976,9 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
   const int IH = c.image_h, IW = c.image_w;
   const int P = e->patch;
   const int KPE = round_up(3 * P * P, 16);  // 592 for patch 14 (588 + zero columns), 768 for 16
-  const bool hybrid = e->family == VD3D_DEPTH_DPT_HYBRID, beit = e->family == VD3D_DEPTH_DPT_BEIT;
+  const bool hybrid = e->family == VD3D_DEPTH_DPT_HYBRID, zoe = e->family == VD3D_DEPTH_ZOEDEPTH;
+  const bool beit = e->family == VD3D_DEPTH_DPT_BEIT || zoe;
+  if (zoe && !e->zoe_nc) return dfail(e, VD3D_ERR_STATE, "ZoeDepth: the metric head's settings are not set (vd3d_depth_set_zoe)");
   // raw taps and the project readout (DPT-Large and the hybrid without LayerScale: ls1 / ls2 of ones)
   const bool dpt = e->family == VD3D_DEPTH_DPT || hybrid || beit;
   int r;
@@ -1050,6 +1288,8 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
   // ---- fusion stage (coarsest first) ----
   void* fused = nullptr;
   int ch = 0, cw_ = 0;
+  const __half* fused_j[4];  // every fusion output and its size: ZoeDepth's feature blocks
+  int fused_h[4], fused_w[4];
   for (int j = 0; j < 4; ++j) {
     const int fi = 3 - j;
     const int Hc = fh[fi], Wc = fw[fi];
@@ -1134,6 +1374,9 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     fused = prj;
     ch = OH;
     cw_ = OW;
+    fused_j[j] = (const __half*)prj;
+    fused_h[j] = OH;
+    fused_w[j] = OW;
   }
 
   // ---- head ----
@@ -1155,13 +1398,27 @@ int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const*
     if ((r = conv(e, (const __half*)fused, ch, cw_, F, w1, true, g1))) return r;
     launch_upsample_ac((const __half*)h1, ch, cw_, F2, (__half*)h1u, IH, IW, s);
     e->launches++;
-    GemmArgs g2 = base_args(0, 32, 0, EPI_HEAD);
-    g2.out_f32 = (float*)depth_d;
-    g2.bias = b2h;
-    g2.w3 = w3;
-    g2.b3p = b3;
-    g2.head_max = e->head == VD3D_HEAD_METRIC ? e->max_depth : 0.f;
-    if ((r = conv(e, (const __half*)h1u, IH, IW, F2, w2, true, g2, 32))) return r;
+    if (zoe) {  // ZoeDepth: the conv2 + ReLU activation feeds the metric head
+      void* act;
+      if ((r = get_buf(e, bname("z.act"), (size_t)IH * IW * 32 * 2, &act))) return r;
+      GemmArgs g2 = base_args(0, 32, 0, EPI_F16);
+      g2.out_f16 = (__half*)act;
+      g2.bias = b2h;
+      g2.act = 2;
+      g2.ldc = 32;
+      if ((r = conv(e, (const __half*)h1u, IH, IW, F2, w2, true, g2, 32))) return r;
+      if ((r = zoe_head(e, fork ? "#" + std::to_string(b) : std::string(), (const __half*)feat[3], fh[3], fw[3],
+                        fused_j, fused_h, fused_w, (const __half*)act, (float*)depth_d)))
+        return r;
+    } else {
+      GemmArgs g2 = base_args(0, 32, 0, EPI_HEAD);
+      g2.out_f32 = (float*)depth_d;
+      g2.bias = b2h;
+      g2.w3 = w3;
+      g2.b3p = b3;
+      g2.head_max = e->head == VD3D_HEAD_METRIC ? e->max_depth : 0.f;
+      if ((r = conv(e, (const __half*)h1u, IH, IW, F2, w2, true, g2, 32))) return r;
+    }
   }
   if (fork) DCK(cudaEventRecord(e->ev_join[b], s));
   }  // images
@@ -1321,8 +1578,15 @@ int vd3d_depth_infer_batch_device(vd3d_depth* e, int B, const uint8_t* const* fr
     if ((r = get_buf(e, nm, (size_t)3 * IH * IW * 4, &px))) return r;
     snprintf(nm, sizeof nm, b ? "depth.%d" : "depth", b);
     if ((r = get_buf(e, nm, (size_t)IH * IW * 4, &dd))) return r;
-    launch_preprocess(frames_bgr_dev[b], h, w, (uint8_t*)tmp, (uint8_t*)rgb, (float*)px, IH, IW, s, 1, e->pre);
-    e->launches += 3;
+    if (e->family == VD3D_DEPTH_ZOEDEPTH) {
+      const int sp = e->span_begin("zoe.preprocess", s);
+      launch_zoe_preprocess(frames_bgr_dev[b], h, w, 1, zoe_pad(h), zoe_pad(w), (float*)px, IH, IW, e->pre, s);
+      e->span_end(sp, s);
+      e->launches++;
+    } else {
+      launch_preprocess(frames_bgr_dev[b], h, w, (uint8_t*)tmp, (uint8_t*)rgb, (float*)px, IH, IW, s, 1, e->pre);
+      e->launches += 3;
+    }
     pxs[b] = (const float*)px;
     dds[b] = (float*)dd;
   }
@@ -1330,7 +1594,10 @@ int vd3d_depth_infer_batch_device(vd3d_depth* e, int B, const uint8_t* const* fr
   for (int b = 0; b < B; ++b) {
     float* upt = (depth_f32_dev && depth_f32_dev[b]) ? depth_f32_dev[b] : (float*)up;
     uint8_t* u8 = depth_u8_dev ? depth_u8_dev[b] : nullptr;
-    launch_depth_post(dds[b], IH, IW, upt, h, w, (unsigned*)mm, u8, invert, s);
+    if (e->family == VD3D_DEPTH_ZOEDEPTH)
+      launch_depth_post_crop(dds[b], IH, IW, upt, h, w, zoe_pad(h), zoe_pad(w), (unsigned*)mm, u8, invert, s);
+    else
+      launch_depth_post(dds[b], IH, IW, upt, h, w, (unsigned*)mm, u8, invert, s);
     e->launches += u8 ? 3 : 2;
   }
   DCK(cudaGetLastError());
@@ -1418,10 +1685,13 @@ int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_r
     const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
     if (!images_rgb[b] || !depth_u8[b] || sh < 1 || sw < 1 || ih < 16 || iw < 16) return VD3D_ERR_ARG;
     int ph = IH, pw = IW;  // DPT's processor resizes every input to its fixed size
+    // ZoeDepth's processor sizes the reflect-padded image
+    const bool zoe = e->family == VD3D_DEPTH_ZOEDEPTH;
+    const int fh = zoe ? ih + 2 * zoe_pad(ih) : ih, fw = zoe ? iw + 2 * zoe_pad(iw) : iw;
     if (e->family == VD3D_DEPTH_DA_V2)
       processed_size(ih, iw, 518, 518, 14, &ph, &pw);
     else if (e->fit_multiple)
-      processed_size(ih, iw, e->fit_h, e->fit_w, e->fit_multiple, &ph, &pw);
+      processed_size(fh, fw, e->fit_h, e->fit_w, e->fit_multiple, &ph, &pw);
     if (ph != IH || pw != IW) {
       char m[160];
       snprintf(m, sizeof m, "image %d: a %dx%d input maps to processed size %dx%d, the engine serves %dx%d", b, iw, ih,
@@ -1487,15 +1757,22 @@ int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_r
       if ((r = pil_resize(e, img, sh, sw, (uint8_t*)ptmp, (uint8_t*)rs, ih, iw))) return r;
       img = (const uint8_t*)rs;
     }
-    launch_preprocess(img, ih, iw, (uint8_t*)tmp, (uint8_t*)rgb, (float*)pxs[b], IH, IW, s, 0, e->pre);
-    e->launches += 3;
+    if (e->family == VD3D_DEPTH_ZOEDEPTH) {
+      launch_zoe_preprocess(img, ih, iw, 0, zoe_pad(ih), zoe_pad(iw), (float*)pxs[b], IH, IW, e->pre, s);
+      e->launches++;
+    } else {
+      launch_preprocess(img, ih, iw, (uint8_t*)tmp, (uint8_t*)rgb, (float*)pxs[b], IH, IW, s, 0, e->pre);
+      e->launches += 3;
+    }
   }
   if ((r = forward_core(e, B, pxs, dds))) return r;
   for (int b = 0; b < B; ++b) {
     const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
     const bool back = ih != sh || iw != sw;
-    launch_depth_post(dds[b], IH, IW, o32[b] ? o32[b] : (float*)up, ih, iw, (unsigned*)mm,
-                      back ? (uint8_t*)u8in : o8[b], invert, s);
+    const int pad_h = e->family == VD3D_DEPTH_ZOEDEPTH ? zoe_pad(ih) : 0;
+    const int pad_w = e->family == VD3D_DEPTH_ZOEDEPTH ? zoe_pad(iw) : 0;
+    launch_depth_post_crop(dds[b], IH, IW, o32[b] ? o32[b] : (float*)up, ih, iw, pad_h, pad_w, (unsigned*)mm,
+                           back ? (uint8_t*)u8in : o8[b], invert, s);
     e->launches += 3;
     if (back) {
       launch_resize_cubic_u8((const uint8_t*)u8in, ih, iw, 1, o8[b], sh, sw, s);

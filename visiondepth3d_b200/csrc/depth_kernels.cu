@@ -302,19 +302,21 @@ __device__ __forceinline__ unsigned f2ord(float f) {  // order-preserving float 
 __device__ __forceinline__ float ord2f(unsigned u) {
   return __uint_as_float((u & 0x80000000u) ? (u & 0x7FFFFFFFu) : ~u);
 }
+// The output is the window [oy0, oy0 + OH) x [ox0, ox0 + OW) of a VH x VW resize (ZoeDepth: the padded size, cropped);
+// VH = OH, VW = OW and zero offsets for every other model.
 __global__ void __launch_bounds__(256) k_depth_upsample_minmax(const float* __restrict__ d, int IH, int IW,
-                                                               float* __restrict__ out, int OH, int OW,
-                                                               unsigned* __restrict__ mm) {
+                                                               float* __restrict__ out, int OH, int OW, int VH, int VW,
+                                                               int oy0, int ox0, unsigned* __restrict__ mm) {
   int ox = blockIdx.x * 32 + (threadIdx.x & 31);
   int oy = blockIdx.y * 8 + (threadIdx.x >> 5);
   float v = 0.f;
   bool ok = ox < OW && oy < OH;
   if (ok) {
-    if (IH == OH && IW == OW) {
-      v = d[(size_t)oy * IW + ox];
+    if (IH == VH && IW == VW) {
+      v = d[(size_t)(oy + oy0) * IW + ox + ox0];
     } else {
-      float sy = (float)IH / (float)OH, sx = (float)IW / (float)OW;
-      float fy = sy * ((float)oy + 0.5f) - 0.5f, fx = sx * ((float)ox + 0.5f) - 0.5f;
+      float sy = (float)IH / (float)VH, sx = (float)IW / (float)VW;
+      float fy = sy * ((float)(oy + oy0) + 0.5f) - 0.5f, fx = sx * ((float)(ox + ox0) + 0.5f) - 0.5f;
       int iy = (int)floorf(fy), ix = (int)floorf(fx);
       float cy[4], cx[4];
       cubic_coeffs(fy - (float)iy, cy);
@@ -644,8 +646,401 @@ __global__ void __launch_bounds__(256) k_im2col_same(const __half* __restrict__ 
 }
 
 // ---------------------------------------------------------------------------
+// ZoeDepth (transformers 5.5 models/zoedepth): image processor, domain router, attractor update and the conditional
+// log-binomial head.  Every f32 step writes its products and sums with explicit _rn intrinsics where the order matters,
+// so that the compiler does not contract them into FMAs the CPU reference does not use.
+// ---------------------------------------------------------------------------
+
+// torch upsample_bilinear2d(align_corners=True) index and weight of one axis, in f32 as ATen's CPU kernel computes them
+__device__ __forceinline__ void ac_axis(int o, int in, int out, int& i0, int& i1, float& l0, float& l1) {
+  const float scale = out > 1 ? (float)(in - 1) / (float)(out - 1) : 0.f;
+  const float real = scale * (float)o;
+  i0 = min((int)floorf(real), in - 1);
+  l1 = fminf(fmaxf(real - (float)i0, 0.f), 1.f);
+  l0 = 1.f - l1;
+  i1 = i0 + (i0 < in - 1 ? 1 : 0);
+}
+// ((x00 w0 + x01 w1) h0) + ((x10 w0 + x11 w1) h1): ATen's Interpolate<2> order
+__device__ __forceinline__ float bilerp(float x00, float x01, float x10, float x11, float h0, float h1, float w0,
+                                        float w1) {
+  const float t0 = __fadd_rn(__fmul_rn(x00, w0), __fmul_rn(x01, w1));
+  const float t1 = __fadd_rn(__fmul_rn(x10, w0), __fmul_rn(x11, w1));
+  return __fadd_rn(__fmul_rn(t0, h0), __fmul_rn(t1, h1));
+}
+__device__ __forceinline__ float softplus_t(float x) { return x > 20.f ? x : log1pf(expf(x)); }  // torch beta 1, 20
+
+// ZoeDepthImageProcessor: rescale (x * (1/255) in f32), reflect-pad pad_h rows / pad_w columns, bilinear
+// align_corners=True to OH x OW, (v - mean) / std.  The padding is folded into the sampler: padded index p maps to
+// source row |p - pad| reflected at the far edge.  u8 [h, w, 3] (BGR when swap_rb) -> f32 [3, OH, OW].
+__device__ __forceinline__ int reflect_idx(int p, int pad, int n) {
+  int r = p - pad;
+  if (r < 0) r = -r;
+  if (r >= n) r = 2 * (n - 1) - r;
+  return r;
+}
+__global__ void __launch_bounds__(256) k_zoe_preprocess(const uint8_t* __restrict__ img, int h, int w, int swap_rb,
+                                                        int pad_h, int pad_w, float* __restrict__ px, int OH, int OW,
+                                                        PreprocParams pp) {
+  const int ox = blockIdx.x * 32 + (threadIdx.x & 31), oy = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (ox >= OW || oy >= OH) return;
+  int y0, y1, x0, x1;
+  float h0, h1, w0, w1;
+  ac_axis(oy, h + 2 * pad_h, OH, y0, y1, h0, h1);
+  ac_axis(ox, w + 2 * pad_w, OW, x0, x1, w0, w1);
+  y0 = reflect_idx(y0, pad_h, h);
+  y1 = reflect_idx(y1, pad_h, h);
+  x0 = reflect_idx(x0, pad_w, w);
+  x1 = reflect_idx(x1, pad_w, w);
+  const float rs = 1.0f / 255.0f;
+  const uint8_t *p00 = img + ((size_t)y0 * w + x0) * 3, *p01 = img + ((size_t)y0 * w + x1) * 3,
+                *p10 = img + ((size_t)y1 * w + x0) * 3, *p11 = img + ((size_t)y1 * w + x1) * 3;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int sc = swap_rb ? 2 - c : c;
+    const float v = bilerp(__fmul_rn((float)p00[sc], rs), __fmul_rn((float)p01[sc], rs), __fmul_rn((float)p10[sc], rs),
+                           __fmul_rn((float)p11[sc], rs), h0, h1, w0, w1);
+    px[((size_t)c * OH + oy) * OW + ox] = __fdiv_rn(__fsub_rn(v, pp.mean[c]), pp.std[c]);
+  }
+}
+
+// ---- router: ZoeDepthPatchTransformerEncoder + ZoeDepthMLPClassifier on one image, one CTA, f32 throughout ----
+// Y[r, n] (= or +=) act(sum_k X[r, k] W[n, k] (/ div) + b[n]) for r < R, n < N; W element (n, k) at W[n wsn + k wsk].
+// 32 x 32 output tiles, K staged 32 at a time in shared memory; each of the 256 threads owns 4 rows of one column.
+// mode 0: store, 1: ReLU then store, 2: add to Y (the post-norm residual).  Ends with a barrier.
+__device__ __forceinline__ void zr_linear(const float* __restrict__ X, int ldx, int R, int K, const float* __restrict__ Wt, int wsn,
+                          int wsk, const float* __restrict__ b, int N, float* Y, int ldy, int mode, float div) {
+  __shared__ float xs[32][33], ws[32][33];
+  const int tid = threadIdx.x, col = tid & 31, rg = tid >> 5;
+  for (int r0 = 0; r0 < R; r0 += 32)
+    for (int n0 = 0; n0 < N; n0 += 32) {
+      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int k0 = 0; k0 < K; k0 += 32) {
+        for (int i = tid; i < 32 * 32; i += 256) {
+          const int rr = i >> 5, kk = i & 31;
+          xs[rr][kk] = (r0 + rr < R && k0 + kk < K) ? X[(size_t)(r0 + rr) * ldx + k0 + kk] : 0.f;
+          ws[rr][kk] = (n0 + rr < N && k0 + kk < K) ? Wt[(size_t)(n0 + rr) * wsn + (size_t)(k0 + kk) * wsk] : 0.f;
+        }
+        __syncthreads();
+#pragma unroll 8
+        for (int kk = 0; kk < 32; ++kk) {
+          const float wv = ws[col][kk];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) acc[i] = fmaf(xs[rg * 4 + i][kk], wv, acc[i]);
+        }
+        __syncthreads();
+      }
+      const int n = n0 + col;
+      if (n < N)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int r = r0 + rg * 4 + i;
+          float v = div != 1.f ? acc[i] / div : acc[i];
+          if (b) v += b[n];
+          if (mode == 1) v = fmaxf(v, 0.f);
+          if (r < R) {
+            float* y = Y + (size_t)r * ldy + n;
+            *y = mode == 2 ? *y + v : v;
+          }
+        }
+    }
+  __syncthreads();
+}
+// LayerNorm(eps 1e-5) of rows [0, R) of X [., 128] in place, one warp per row
+__device__ __forceinline__ void zr_layernorm(float* X, int R, const float* __restrict__ g, const float* __restrict__ b) {
+  const int lane = threadIdx.x & 31;
+  for (int r = threadIdx.x >> 5; r < R; r += blockDim.x >> 5) {
+    float* x = X + (size_t)r * kZoeE;
+    float v[4], s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) s += v[i] = x[lane + 32 * i];
+    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    const float mean = s / (float)kZoeE;
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) q += (v[i] - mean) * (v[i] - mean);
+    for (int o = 16; o; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+    const float rstd = 1.f / sqrtf(q / (float)kZoeE + 1e-5f);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) x[lane + 32 * i] = (v[i] - mean) * rstd * g[lane + 32 * i] + b[lane + 32 * i];
+  }
+  __syncthreads();
+}
+// softmax of rows [0, R) of P [., S] in place, one warp per row
+__device__ __forceinline__ void zr_softmax(float* P, int R, int S) {
+  const int lane = threadIdx.x & 31;
+  for (int r = threadIdx.x >> 5; r < R; r += blockDim.x >> 5) {
+    float* p = P + (size_t)r * S;
+    float m = -INFINITY;
+    for (int j = lane; j < S; j += 32) m = fmaxf(m, p[j]);
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    float s = 0.f;
+    for (int j = lane; j < S; j += 32) s += p[j] = expf(p[j] - m);
+    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    for (int j = lane; j < S; j += 32) p[j] = p[j] / s;
+  }
+  __syncthreads();
+}
+// x: the bottleneck conv2 output f32 [n, F]; wts: the packed router (zoe_router_floats); pe f32 [n + 1, 128];
+// scratch: zoe_router_scratch(n) floats.  Writes logits[2] and route (1 when logits[1] > logits[0], torch.argmax's
+// first index on a tie).  The last encoder layer computes the CLS row only: nothing else of it is read.
+__global__ void __launch_bounds__(256, 1) k_zoe_router(const float* __restrict__ x, int n, int F,
+                                                    const float* __restrict__ wts, const float* __restrict__ pe,
+                                                    float* __restrict__ scratch, float* __restrict__ logits,
+                                                    int* __restrict__ route) {
+  constexpr int E = kZoeE, FF = kZoeFF, HD = E / kZoeHeads;
+  const int S = n + 1;
+  float *X = scratch, *QKV = X + (size_t)S * E, *A = QKV + (size_t)S * 3 * E, *Hb = A + (size_t)S * E,
+        *P = Hb + (size_t)S * FF;
+  const float* w = wts;
+  const float *ew = w, *eb = ew + E * F;
+  w = eb + E;
+  for (int i = threadIdx.x; i < E; i += blockDim.x) X[i] = 0.f;  // the zero CLS token
+  zr_linear(x, F, n, F, ew, F, 1, eb, E, X + E, E, 0, 1.f);
+  for (int i = threadIdx.x; i < S * E; i += blockDim.x) X[i] = X[i] + pe[i];
+  __syncthreads();
+  for (int l = 0; l < kZoeLayers; ++l) {
+    const int Rq = l == kZoeLayers - 1 ? 1 : S;
+    const float *qw = w, *qb = qw + 3 * E * E, *ow = qb + 3 * E, *ob = ow + E * E, *n1g = ob + E, *n1b = n1g + E,
+                *l1w = n1b + E, *l1b = l1w + FF * E, *l2w = l1b + FF, *l2b = l2w + E * FF, *n2g = l2b + E,
+                *n2b = n2g + E;
+    w = n2b + E;
+    zr_linear(X, E, S, E, qw, E, 1, qb, 3 * E, QKV, 3 * E, 0, 1.f);
+    for (int h = 0; h < kZoeHeads; ++h) {
+      zr_linear(QKV + h * HD, 3 * E, Rq, HD, QKV + E + h * HD, 3 * E, 1, nullptr, S, P, S, 0, sqrtf((float)HD));
+      zr_softmax(P, Rq, S);
+      zr_linear(P, S, Rq, S, QKV + 2 * E + h * HD, 1, 3 * E, nullptr, HD, A + h * HD, E, 0, 1.f);
+    }
+    zr_linear(A, E, Rq, E, ow, E, 1, ob, E, X, E, 2, 1.f);
+    zr_layernorm(X, Rq, n1g, n1b);
+    zr_linear(X, E, Rq, E, l1w, E, 1, l1b, FF, Hb, FF, 1, 1.f);
+    zr_linear(Hb, FF, Rq, FF, l2w, FF, 1, l2b, E, X, E, 2, 1.f);
+    zr_layernorm(X, Rq, n2g, n2b);
+  }
+  const float *c1w = w, *c1b = c1w + E * E, *c2w = c1b + E, *c2b = c2w + 2 * E;
+  zr_linear(X, E, 1, E, c1w, E, 1, c1b, E, Hb, E, 1, 1.f);
+  zr_linear(Hb, E, 1, E, c2w, E, 1, c2b, 2, A, 2, 0, 1.f);
+  if (threadIdx.x == 0) {
+    logits[0] = A[0];
+    logits[1] = A[1];
+    *route = A[1] > A[0] ? 1 : 0;
+  }
+}
+
+// ZoeDepthAttractorLayerUnnormed on an H x W map, one thread per pixel: attractors a = Softplus(conv2(hid)) with the
+// route's conv2 (staged in shared memory; hid f16 [H W, ldh] holds ReLU(conv1) of every configuration, the route's at
+// column route * E), bins c = bilinear_ac(prev) (prev f32 [Hp Wp, ldp] at column route * prev_cfg_stride, Softplus
+// applied first when prev_softplus: the seed regressor's raw conv2), then c += (sum_i dx / (1 + 300 dx^2)) / na with
+// dx = a_i - c, summed attractor by attractor -> out f32 [H W, kZoeBins].
+__global__ void __launch_bounds__(128) k_zoe_attractor(const __half* __restrict__ hid, int ldh, int E,
+                                                       const float* __restrict__ w2, const float* __restrict__ b2,
+                                                       int na, const float* __restrict__ prev, int ldp,
+                                                       int prev_cfg_stride, int prev_softplus, int Hp, int Wp,
+                                                       float* __restrict__ out, int H, int W,
+                                                       const int* __restrict__ route) {
+  __shared__ float sw[kZoeMaxAttr * kZoeE + kZoeMaxAttr];
+  const int rt = *route;
+  for (int i = threadIdx.x; i < na * E; i += blockDim.x) sw[i] = w2[(size_t)rt * na * E + i];
+  for (int i = threadIdx.x; i < na; i += blockDim.x) sw[na * E + i] = b2[rt * na + i];
+  __syncthreads();
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= H * W) return;
+  const int oy = pix / W, ox = pix % W;
+  float a[kZoeMaxAttr];
+#pragma unroll
+  for (int i = 0; i < kZoeMaxAttr; ++i) a[i] = 0.f;
+  const __half* hp = hid + (size_t)pix * ldh + (size_t)rt * E;
+  for (int e0 = 0; e0 < E; e0 += 8) {
+    const uint4 u = *(const uint4*)(hp + e0);
+    const __half2* h2 = (const __half2*)&u;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = __half22float2(h2[j]);
+#pragma unroll
+      for (int i = 0; i < kZoeMaxAttr; ++i)
+        if (i < na) a[i] = fmaf(sw[i * E + e0 + 2 * j + 1], f.y, fmaf(sw[i * E + e0 + 2 * j], f.x, a[i]));
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < kZoeMaxAttr; ++i)
+    if (i < na) a[i] = softplus_t(a[i] + sw[na * E + i]);
+  int y0, y1, x0, x1;
+  float h0, h1, w0, w1;
+  ac_axis(oy, Hp, H, y0, y1, h0, h1);
+  ac_axis(ox, Wp, W, x0, x1, w0, w1);
+  const float *q00 = prev + ((size_t)y0 * Wp + x0) * ldp + (size_t)rt * prev_cfg_stride,
+              *q01 = prev + ((size_t)y0 * Wp + x1) * ldp + (size_t)rt * prev_cfg_stride,
+              *q10 = prev + ((size_t)y1 * Wp + x0) * ldp + (size_t)rt * prev_cfg_stride,
+              *q11 = prev + ((size_t)y1 * Wp + x1) * ldp + (size_t)rt * prev_cfg_stride;
+  const float nf = (float)na;
+  float* o = out + (size_t)pix * kZoeBins;
+  for (int j0 = 0; j0 < kZoeBins; j0 += 16) {
+    float c[16], dc[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      float v00 = q00[j0 + j], v01 = q01[j0 + j], v10 = q10[j0 + j], v11 = q11[j0 + j];
+      if (prev_softplus) {
+        v00 = softplus_t(v00);
+        v01 = softplus_t(v01);
+        v10 = softplus_t(v10);
+        v11 = softplus_t(v11);
+      }
+      c[j] = bilerp(v00, v01, v10, v11, h0, h1, w0, w1);
+      dc[j] = 0.f;
+    }
+#pragma unroll
+    for (int i = 0; i < kZoeMaxAttr; ++i)
+      if (i < na)
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float dx = __fsub_rn(a[i], c[j]);
+          dc[j] = __fadd_rn(dc[j], __fdiv_rn(dx, __fadd_rn(1.f, __fmul_rn(300.f, __fmul_rn(dx, dx)))));
+        }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) o[j0 + j] = __fadd_rn(c[j], __fdiv_rn(dc[j], nf));
+  }
+}
+
+// ZoeDepthConditionalLogBinomialSoftmax and the expectation, one thread per pixel of the H x W processed size:
+// the input is cat(act (32 channels f16 [H W, 32]) [, relu(w3 . act + b3) when w3], bilinear_ac(emb) (f16 [He We, E]));
+// MLP conv -> GELU -> conv(4) -> Softplus with the route's weights (staged in shared memory: w1 [cin][HID], b1 [HID],
+// w2 [4][HID], b2 [4]); p and t from the normalised pairs (+1e-4); y_k = log_binom(K - 1, k) + k log p + (K - 1 - k)
+// log(1 - p) with p clamped to [1e-4, 1]; depth = sum_k softmax(y / t)_k * bilinear_ac(bins)_k (bins f32 [He We, K]).
+template <int HID>
+__global__ void __launch_bounds__(128) k_zoe_logbinom(const __half* __restrict__ act, const float* __restrict__ w3,
+                                                      const float* __restrict__ b3, const __half* __restrict__ emb,
+                                                      const float* __restrict__ bins, int He, int We, int E,
+                                                      const float* __restrict__ mlp, int cin, float min_t, float max_t,
+                                                      float* __restrict__ depth, int H, int W,
+                                                      const int* __restrict__ route) {
+  extern __shared__ float sm[];
+  const int per = cin * HID + HID + 4 * HID + 4;
+  const float* src = mlp + (size_t)(*route) * per;
+  for (int i = threadIdx.x; i < per; i += blockDim.x) sm[i] = src[i];
+  __syncthreads();
+  const float *w1 = sm, *b1 = w1 + cin * HID, *w2 = b1 + HID, *b2 = w2 + 4 * HID;
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= H * W) return;
+  const int oy = pix / W, ox = pix % W;
+  float hacc[HID];
+#pragma unroll
+  for (int j = 0; j < HID; ++j) hacc[j] = b1[j];
+  int k = 0;
+  auto feed = [&](float v) {
+#pragma unroll
+    for (int j = 0; j < HID; ++j) hacc[j] = fmaf(w1[k * HID + j], v, hacc[j]);
+    ++k;
+  };
+  const __half* ap = act + (size_t)pix * 32;
+  float rel = b3 ? b3[0] : 0.f;
+  for (int c0 = 0; c0 < 32; c0 += 8) {
+    const uint4 u = *(const uint4*)(ap + c0);
+    const __half2* h2 = (const __half2*)&u;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = __half22float2(h2[j]);
+      feed(f.x);
+      feed(f.y);
+      if (b3) rel = fmaf(w3[c0 + 2 * j + 1], f.y, fmaf(w3[c0 + 2 * j], f.x, rel));
+    }
+  }
+  if (b3) feed(fmaxf(rel, 0.f));
+  int y0, y1, x0, x1;
+  float h0, h1, wx0, wx1;
+  ac_axis(oy, He, H, y0, y1, h0, h1);
+  ac_axis(ox, We, W, x0, x1, wx0, wx1);
+  const size_t i00 = (size_t)y0 * We + x0, i01 = (size_t)y0 * We + x1, i10 = (size_t)y1 * We + x0,
+               i11 = (size_t)y1 * We + x1;
+  for (int e = 0; e < E; ++e)
+    feed(bilerp(__half2float(emb[i00 * E + e]), __half2float(emb[i01 * E + e]), __half2float(emb[i10 * E + e]),
+                __half2float(emb[i11 * E + e]), h0, h1, wx0, wx1));
+  float o4[4];
+#pragma unroll
+  for (int m = 0; m < 4; ++m) o4[m] = b2[m];
+#pragma unroll
+  for (int j = 0; j < HID; ++j) {
+    const float g = 0.5f * hacc[j] * (1.f + erff(hacc[j] * 0.70710678118654752f));
+#pragma unroll
+    for (int m = 0; m < 4; ++m) o4[m] = fmaf(w2[m * HID + j], g, o4[m]);
+  }
+#pragma unroll
+  for (int m = 0; m < 4; ++m) o4[m] = softplus_t(o4[m]);
+  const float pe = 1e-4f;
+  const float pa = __fadd_rn(o4[0], pe), pb = __fadd_rn(o4[1], pe);
+  float p = __fdiv_rn(pa, __fadd_rn(pa, pb));
+  const float ta = __fadd_rn(o4[2], pe), tb = __fadd_rn(o4[3], pe);
+  const float t = __fadd_rn(__fmul_rn(max_t - min_t, __fdiv_rn(ta, __fadd_rn(ta, tb))), min_t);
+  const float q = fminf(fmaxf(__fsub_rn(1.f, p), pe), 1.f);
+  p = fminf(fmaxf(p, pe), 1.f);
+  const float lp = logf(p), lq = logf(q);
+  constexpr int K = kZoeBins;
+  const float n = __fadd_rn((float)(K - 1), 1e-7f), nl = __fmul_rn(n, logf(n));
+  auto logit = [&](int kk) {
+    const float kf = __fadd_rn((float)kk, 1e-7f), nk = __fsub_rn(n, kf);
+    const float lb = __fsub_rn(__fsub_rn(nl, __fmul_rn(kf, logf(kf))), __fmul_rn(nk, logf(__fadd_rn(nk, 1e-7f))));
+    const float y = __fadd_rn(__fadd_rn(lb, __fmul_rn((float)kk, lp)), __fmul_rn((float)(K - 1 - kk), lq));
+    return __fdiv_rn(y, t);
+  };
+  float mx = -INFINITY;
+  for (int kk = 0; kk < K; ++kk) mx = fmaxf(mx, logit(kk));
+  float s = 0.f;
+  for (int kk = 0; kk < K; ++kk) s = __fadd_rn(s, expf(__fsub_rn(logit(kk), mx)));
+  float d = 0.f;
+  for (int kk = 0; kk < K; ++kk) {
+    const float c = bilerp(bins[i00 * K + kk], bins[i01 * K + kk], bins[i10 * K + kk], bins[i11 * K + kk], h0, h1, wx0,
+                           wx1);
+    d = __fadd_rn(d, __fmul_rn(__fdiv_rn(expf(__fsub_rn(logit(kk), mx)), s), c));
+  }
+  depth[pix] = d;
+}
+
+// ---------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------
+size_t zoe_router_floats(int F) {
+  constexpr size_t E = kZoeE, FF = kZoeFF;
+  const size_t layer = 3 * E * E + 3 * E + E * E + E + 2 * E + FF * E + FF + E * FF + E + 2 * E;
+  return E * F + E + kZoeLayers * layer + E * E + E + 2 * E + 2;
+}
+size_t zoe_router_scratch(int n) {
+  const size_t S = n + 1;
+  return S * kZoeE * 5 + S * kZoeFF + S * S;
+}
+void launch_zoe_preprocess(const uint8_t* img, int h, int w, int swap_rb, int pad_h, int pad_w, float* px, int OH,
+                           int OW, const PreprocParams& pp, cudaStream_t s) {
+  dim3 g((OW + 31) / 32, (OH + 7) / 8);
+  k_zoe_preprocess<<<g, 256, 0, s>>>(img, h, w, swap_rb, pad_h, pad_w, px, OH, OW, pp);
+}
+void launch_zoe_router(const float* x, int n, int F, const float* wts, const float* pe, float* scratch, float* logits,
+                       int* route, cudaStream_t s) {
+  k_zoe_router<<<1, 256, 0, s>>>(x, n, F, wts, pe, scratch, logits, route);
+}
+void launch_zoe_attractor(const __half* hid, int ldh, int E, const float* w2, const float* b2, int na, const float* prev,
+                          int ldp, int prev_cfg_stride, int prev_softplus, int Hp, int Wp, float* out, int H, int W,
+                          const int* route, cudaStream_t s) {
+  k_zoe_attractor<<<(H * W + 127) / 128, 128, 0, s>>>(hid, ldh, E, w2, b2, na, prev, ldp, prev_cfg_stride,
+                                                      prev_softplus, Hp, Wp, out, H, W, route);
+}
+size_t zoe_logbinom_floats(int cin, int hid) { return (size_t)cin * hid + hid + 4 * hid + 4; }
+template <int HID>
+static cudaError_t launch_logbinom_t(const __half* act, const float* w3, const float* b3, const __half* emb,
+                                     const float* bins, int He, int We, int E, const float* mlp, int cin, float min_t,
+                                     float max_t, float* depth, int H, int W, const int* route, cudaStream_t s) {
+  const size_t smem = zoe_logbinom_floats(cin, HID) * sizeof(float);
+  cudaError_t e = cudaFuncSetAttribute(k_zoe_logbinom<HID>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  k_zoe_logbinom<HID><<<(H * W + 127) / 128, 128, smem, s>>>(act, w3, b3, emb, bins, He, We, E, mlp, cin, min_t, max_t,
+                                                            depth, H, W, route);
+  return cudaGetLastError();
+}
+cudaError_t launch_zoe_logbinom(const __half* act, const float* w3, const float* b3, const __half* emb,
+                                const float* bins, int He, int We, int E, const float* mlp, int cin, int hid,
+                                float min_t, float max_t, float* depth, int H, int W, const int* route, cudaStream_t s) {
+  if (hid == 40)
+    return launch_logbinom_t<40>(act, w3, b3, emb, bins, He, We, E, mlp, cin, min_t, max_t, depth, H, W, route, s);
+  if (hid == 80)
+    return launch_logbinom_t<80>(act, w3, b3, emb, bins, He, We, E, mlp, cin, min_t, max_t, depth, H, W, route, s);
+  return cudaErrorInvalidValue;
+}
 void launch_preprocess(const uint8_t* frame_bgr, int H, int W, uint8_t* tmp_u8, uint8_t* rgb_u8, float* px, int OH,
                        int OW, cudaStream_t s, int swap_rb, const PreprocParams& pp) {
   dim3 g1((OW + 31) / 32, (H + 7) / 8), g2((OW + 31) / 32, (OH + 7) / 8);
@@ -660,9 +1055,13 @@ void launch_resize_pil_u8(const uint8_t* src, int IH, int IW, uint8_t* dst, int 
 }
 void launch_depth_post(const float* depth, int IH, int IW, float* up, int OH, int OW, unsigned* mm, uint8_t* out_u8,
                        int invert, cudaStream_t s) {
+  launch_depth_post_crop(depth, IH, IW, up, OH, OW, 0, 0, mm, out_u8, invert, s);
+}
+void launch_depth_post_crop(const float* depth, int IH, int IW, float* up, int OH, int OW, int pad_h, int pad_w,
+                            unsigned* mm, uint8_t* out_u8, int invert, cudaStream_t s) {
   k_minmax_reset<<<1, 1, 0, s>>>(mm);
   dim3 g((OW + 31) / 32, (OH + 7) / 8);
-  k_depth_upsample_minmax<<<g, 256, 0, s>>>(depth, IH, IW, up, OH, OW, mm);
+  k_depth_upsample_minmax<<<g, 256, 0, s>>>(depth, IH, IW, up, OH, OW, OH + 2 * pad_h, OW + 2 * pad_w, pad_h, pad_w, mm);
   if (out_u8) k_depth_to_u8<<<(OH * OW + 255) / 256, 256, 0, s>>>(up, OH * OW, mm, out_u8, invert);
 }
 void launch_add_relu_f16(const __half* a, const __half* b, __half* sum, __half* sum_relu, size_t n, cudaStream_t s) {

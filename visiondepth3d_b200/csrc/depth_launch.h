@@ -35,6 +35,30 @@ void launch_resize_pil_u8(const uint8_t* src, int IH, int IW, uint8_t* dst, int 
 // bicubic to (OH,OW) + min/max (+ u8 quantisation when out_u8 != null) (2-3 launches)
 void launch_depth_post(const float* depth, int IH, int IW, float* up, int OH, int OW, unsigned* mm, uint8_t* out_u8,
                        int invert, cudaStream_t s);
+// ZoeDepth's post-process: the same, evaluating only the (OH, OW) window at (pad_h, pad_w) of the bicubic resize to
+// (OH + 2 pad_h, OW + 2 pad_w), i.e. the resize to the padded size, then the crop
+void launch_depth_post_crop(const float* depth, int IH, int IW, float* up, int OH, int OW, int pad_h, int pad_w,
+                            unsigned* mm, uint8_t* out_u8, int invert, cudaStream_t s);
+// ---- ZoeDepth metric head (see depth_kernels.cu) ----
+// the patch transformer of the router: width 128, 4 heads, FFN 1024, 4 post-norm layers; 64 bins; at most 16 attractors
+constexpr int kZoeE = 128, kZoeHeads = 4, kZoeFF = 1024, kZoeLayers = 4, kZoeBins = 64, kZoeMaxAttr = 16;
+// u8 [h, w, 3] (BGR when swap_rb) -> reflect pad -> bilinear align_corners to OH x OW -> f32 [3, OH, OW] normalised
+void launch_zoe_preprocess(const uint8_t* img, int h, int w, int swap_rb, int pad_h, int pad_w, float* px, int OH,
+                           int OW, const PreprocParams& pp, cudaStream_t s);
+// floats of the packed router weights for a bottleneck of F channels, and of the scratch of a router over n tokens
+size_t zoe_router_floats(int F);
+size_t zoe_router_scratch(int n);
+// one image: x f32 [n, F] (the bottleneck conv2) -> logits f32 [2] and route (device int)
+void launch_zoe_router(const float* x, int n, int F, const float* wts, const float* pe, float* scratch, float* logits,
+                       int* route, cudaStream_t s);
+void launch_zoe_attractor(const __half* hid, int ldh, int E, const float* w2, const float* b2, int na, const float* prev,
+                          int ldp, int prev_cfg_stride, int prev_softplus, int Hp, int Wp, float* out, int H, int W,
+                          const int* route, cudaStream_t s);
+// floats of one configuration's packed log-binomial MLP (cin inputs, hid hidden units: 40 or 80)
+size_t zoe_logbinom_floats(int cin, int hid);
+cudaError_t launch_zoe_logbinom(const __half* act, const float* w3, const float* b3, const __half* emb,
+                                const float* bins, int He, int We, int E, const float* mlp, int cin, int hid,
+                                float min_t, float max_t, float* depth, int H, int W, const int* route, cudaStream_t s);
 void launch_add_relu_f16(const __half* a, const __half* b, __half* sum, __half* sum_relu, size_t n, cudaStream_t s);
 void launch_relu_f16(const __half* in, __half* out, size_t n, cudaStream_t s);
 // Real-ESRGAN stage: BGR u8 -> 64-channel f16 NHWC (RGB/255 in channels 0..2); pixel-shuffle + base + clip + u8 BGR

@@ -6,8 +6,9 @@ import numpy as np
 
 from . import _lib
 from .depth_weights import (DA_PROCESSOR, DPT_BEIT_CONFIGS, DPT_BEIT_PROCESSOR, DPT_CONFIGS, DPT_HYBRID_CONFIGS,
-                            DPT_PROCESSOR, da_spec, dpt_beit_processed_size, dpt_processed_size, is_plain_v2, prepare,
-                            prepare_dpt, prepare_dpt_beit, prepare_dpt_hybrid)
+                            DPT_PROCESSOR, ZOEDEPTH_CONFIGS, ZOEDEPTH_PROCESSOR, da_spec, dpt_beit_processed_size,
+                            dpt_processed_size, is_plain_v2, prepare, prepare_dpt, prepare_dpt_beit, prepare_dpt_hybrid,
+                            prepare_zoedepth, zoedepth_processed_size)
 
 
 def processed_size(width, height, target=518, multiple=14):
@@ -39,10 +40,13 @@ HEAD_KINDS = {"relative": 0, "metric": 1}  # VD3D_HEAD_RELATIVE / VD3D_HEAD_METR
 
 
 FAMILY_DA_V2, FAMILY_DPT, FAMILY_DPT_HYBRID, FAMILY_DPT_BEIT = "da-v2", "dpt", "dpt-hybrid", "dpt-beit"
-# VD3D_DEPTH_DA_V2 / _DPT / _DPT_HYBRID / _DPT_BEIT
-_FAMILY_CODES = {FAMILY_DA_V2: 0, FAMILY_DPT: 1, FAMILY_DPT_HYBRID: 2, FAMILY_DPT_BEIT: 3}
-_DPT_LIKE = (FAMILY_DPT, FAMILY_DPT_HYBRID, FAMILY_DPT_BEIT)  # DPTForDepthEstimation: DPT's processor settings
-_DPT_CONFIG_SETS = {FAMILY_DPT: DPT_CONFIGS, FAMILY_DPT_HYBRID: DPT_HYBRID_CONFIGS, FAMILY_DPT_BEIT: DPT_BEIT_CONFIGS}
+FAMILY_ZOEDEPTH = "zoedepth"
+# VD3D_DEPTH_DA_V2 / _DPT / _DPT_HYBRID / _DPT_BEIT / _ZOEDEPTH
+_FAMILY_CODES = {FAMILY_DA_V2: 0, FAMILY_DPT: 1, FAMILY_DPT_HYBRID: 2, FAMILY_DPT_BEIT: 3, FAMILY_ZOEDEPTH: 4}
+# the DPT neck on a ViT trunk, with the processor settings of depth_weights (ZoeDepth: DPT-BEiT's trunk and neck)
+_DPT_LIKE = (FAMILY_DPT, FAMILY_DPT_HYBRID, FAMILY_DPT_BEIT, FAMILY_ZOEDEPTH)
+_DPT_CONFIG_SETS = {FAMILY_DPT: DPT_CONFIGS, FAMILY_DPT_HYBRID: DPT_HYBRID_CONFIGS, FAMILY_DPT_BEIT: DPT_BEIT_CONFIGS,
+                    FAMILY_ZOEDEPTH: ZOEDEPTH_CONFIGS}
 
 
 def _bind(lib):
@@ -57,6 +61,11 @@ def _bind(lib):
         raise OSError(f"libvd3d ABI mismatch for DepthConfigEx: {lib.vd3d_struct_size(6)} != {C.sizeof(DepthConfigEx)}")
     lib.vd3d_depth_set_fit.argtypes = [vp, i, i, i]
     lib.vd3d_depth_set_fit.restype = i
+    fp = C.POINTER(C.c_float)
+    lib.vd3d_depth_set_zoe.argtypes = [vp, i, i, fp, fp, C.c_float, C.c_float, C.POINTER(C.c_int32), i]
+    lib.vd3d_depth_set_zoe.restype = i
+    lib.vd3d_zoe_kernel.argtypes = [vp, i, C.POINTER(C.c_int32)]
+    lib.vd3d_zoe_kernel.restype = i
     lib.vd3d_depth_destroy.argtypes = [vp]
     lib.vd3d_depth_destroy.restype = None
     lib.vd3d_depth_last_error.argtypes = [vp]
@@ -103,7 +112,9 @@ class DepthEngine:
     preprocessor_config.json); the processed size is the processor's, image_h / image_w default to it.  family
     "dpt-beit": MiDaS v3.1 BEiT-L 512, `cfg` a key of DPT_BEIT_CONFIGS or a dict, `processor` DPT_BEIT_PROCESSOR or
     dpt_beit_processor_from_json's; with a keep-aspect processor the engine serves the frames whose processed size is
-    (image_h, image_w) (default: the processor's target, a square frame's)."""
+    (image_h, image_w) (default: the processor's target, a square frame's).  family "zoedepth": ZoeDepth, `cfg` a key
+    of ZOEDEPTH_CONFIGS or zoedepth_config_from_json's dict, `processor` ZOEDEPTH_PROCESSOR or
+    zoedepth_processor_from_json's; forward returns metric depth."""
 
     def __init__(self, cfg="vits", image_h=None, image_w=None, ctx=None, device=0, family=FAMILY_DA_V2,
                  processor=None):
@@ -118,8 +129,8 @@ class DepthEngine:
         else:
             self.cfg = da_spec(cfg)  # taps, head and max_depth of the spec; V2's relative head by default
         c = self.cfg
-        if family == FAMILY_DPT_BEIT:
-            self.processor = dict(processor or DPT_BEIT_PROCESSOR)
+        if family in (FAMILY_DPT_BEIT, FAMILY_ZOEDEPTH):
+            self.processor = dict(processor or (ZOEDEPTH_PROCESSOR if family == FAMILY_ZOEDEPTH else DPT_BEIT_PROCESSOR))
             image_h, image_w = image_h or self.processor["size"][0], image_w or self.processor["size"][1]
         elif family in _DPT_LIKE:
             self.processor = dict(processor or DPT_PROCESSOR)
@@ -140,8 +151,15 @@ class DepthEngine:
             rc = self.lib.vd3d_depth_create_ex(C.byref(dx), stream, C.byref(h))
             if rc == 0 and p.get("keep_aspect"):
                 rc = self.lib.vd3d_depth_set_fit(h, p["size"][0], p["size"][1], p["multiple"])
-                if rc != 0:
-                    self.lib.vd3d_depth_destroy(h)
+            if rc == 0 and family == FAMILY_ZOEDEPTH:
+                bins = c["bins"]
+                # the two-configuration head has 16 attractors in every layer (transformers' constructor default)
+                na = [16] * 4 if len(bins) > 1 else list(c["attractors"])
+                rc = self.lib.vd3d_depth_set_zoe(h, len(bins), 64, (C.c_float * 2)(*[b["min_depth"] for b in bins]),
+                                                 (C.c_float * 2)(*[b["max_depth"] for b in bins]), c["min_temp"],
+                                                 c["max_temp"], (C.c_int32 * 4)(*na), int(len(bins) == 1))
+            if rc != 0 and h:
+                self.lib.vd3d_depth_destroy(h)
         elif not is_plain_v2(c):  # Depth Anything V1, Distill-Any-Depth, the V2 metric models
             p = DA_PROCESSOR
             dx = DepthConfigEx(dc, 0, 14, 1e-6, p["resample"], (C.c_float * 3)(*p["mean"]), (C.c_float * 3)(*p["std"]),
@@ -158,6 +176,8 @@ class DepthEngine:
         multiple-of-14 size, DPT's fixed size, DPT-BEiT's processor's (keep-aspect multiples of 32 or fixed)."""
         if self.family == FAMILY_DPT_BEIT:
             return dpt_beit_processed_size(width, height, self.processor)
+        if self.family == FAMILY_ZOEDEPTH:
+            return zoedepth_processed_size(width, height, self.processor)
         if self.family in _DPT_LIKE:
             return dpt_processed_size(self.processor)
         return processed_size(width, height)
@@ -168,7 +188,7 @@ class DepthEngine:
 
     def load_state_dict(self, sd):
         prep = {FAMILY_DPT: prepare_dpt, FAMILY_DPT_HYBRID: prepare_dpt_hybrid,
-                FAMILY_DPT_BEIT: prepare_dpt_beit}.get(self.family, prepare)
+                FAMILY_DPT_BEIT: prepare_dpt_beit, FAMILY_ZOEDEPTH: prepare_zoedepth}.get(self.family, prepare)
         for name, arr in prep(sd, self.cfg, self.image_h, self.image_w).items():
             arr = np.ascontiguousarray(arr)
             self.check(self.lib.vd3d_depth_set_tensor(self.h, name.encode(), arr.ctypes.data, arr.nbytes))

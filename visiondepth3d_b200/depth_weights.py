@@ -917,3 +917,297 @@ def prepare_dpt_beit(sd, cfg, image_h, image_w):
         out[f"l{i}.rpb"] = _f32(beit_bias_table(t, (W, W), (ph, pw)).t())
     out.update(_prepare_dpt_neck(sd, cfg, range(4)))
     return out
+
+
+# ---------------------------------------------------------------------------
+# ZoeDepth (Intel/zoedepth-nyu-kitti, -nyu, -kitti; transformers 5.5 ZoeDepthForDepthEstimation): dpt-beit-large-512's
+# trunk, neck and fusion on a BEiT-L/16 with a 24 x 24 pretraining window, DPT's relative head up to its conv2 + ReLU,
+# then the metric-bins head (softplus seed bins, four unnormed attractor layers, the conditional log-binomial).  The
+# two-configuration checkpoint routes each image through a patch transformer + MLP classifier.
+# ---------------------------------------------------------------------------
+ZOEDEPTH_CONFIGS = {
+    "zoedepth-nyu-kitti": dict(DPT_BEIT_CONFIGS["dpt-beit-large-512"], image_size=384,
+                               bins=[dict(name="nyu", n_bins=64, min_depth=1e-3, max_depth=10.0),
+                                     dict(name="kitti", n_bins=64, min_depth=1e-3, max_depth=80.0)],
+                               attractors=[16, 8, 4, 1], min_temp=0.0212, max_temp=50.0, bottleneck=256, embed=128),
+    "zoedepth-nyu": dict(DPT_BEIT_CONFIGS["dpt-beit-large-512"], image_size=384,
+                         bins=[dict(name="nyu", n_bins=64, min_depth=1e-3, max_depth=10.0)],
+                         attractors=[16, 8, 4, 1], min_temp=0.0212, max_temp=50.0, bottleneck=256, embed=128),
+}
+ZOEDEPTH_CONFIGS["zoedepth-kitti"] = dict(ZOEDEPTH_CONFIGS["zoedepth-nyu"],
+                                          bins=[dict(name="kitti", n_bins=64, min_depth=1e-3, max_depth=80.0)])
+
+# ZoeDepthImageProcessor as the checkpoints configure it: reflect padding, keep-aspect multiples of 32 near 384 x 512,
+# bilinear with align_corners, mean = std = 0.5.  The checkpoint's preprocessor_config.json is what the drivers read.
+ZOEDEPTH_PROCESSOR = dict(size=(384, 512), resample=2, mean=(0.5, 0.5, 0.5), std=(0.5, 0.5, 0.5), keep_aspect=True,
+                          multiple=32)
+
+
+def hf_zoedepth_config(name="zoedepth-nyu-kitti", **cfg):
+    """transformers ZoeDepthConfig equal to the checkpoint's as far as the engine reads it; `cfg` overrides entries of
+    ZOEDEPTH_CONFIGS[name] (a smaller BEiT for tests)."""
+    from transformers import BeitConfig, ZoeDepthConfig
+    c = dict(ZOEDEPTH_CONFIGS[name], **cfg)
+    bc = BeitConfig(image_size=c["image_size"], patch_size=c["patch"], num_channels=3, hidden_size=c["hidden"],
+                    num_hidden_layers=c["layers"], num_attention_heads=c["heads"], intermediate_size=4 * c["hidden"],
+                    hidden_act="gelu", layer_norm_eps=c["ln_eps"], use_mask_token=False,
+                    use_absolute_position_embeddings=False, use_relative_position_bias=True,
+                    use_shared_relative_position_bias=False, layer_scale_init_value=0.1 if c["layer_scale"] else 0.0,
+                    out_indices=list(c["taps"]), reshape_hidden_states=False, add_fpn=False)
+    multi = len(c["bins"]) > 1
+    return ZoeDepthConfig(backbone_config=bc, readout_type="project", reassemble_factors=[4, 2, 1, 0.5],
+                          neck_hidden_sizes=c["neck"], fusion_hidden_size=c["fusion"], head_in_index=-1,
+                          use_batch_norm_in_fusion_residual=False, use_bias_in_fusion_residual=None,
+                          num_relative_features=32, add_projection=False, bottleneck_features=c["bottleneck"],
+                          num_attractors=list(c["attractors"]), bin_embedding_dim=c["embed"], attractor_alpha=1000,
+                          attractor_gamma=2, attractor_kind="mean", min_temp=c["min_temp"], max_temp=c["max_temp"],
+                          bin_centers_type="softplus", bin_configurations=[dict(b) for b in c["bins"]],
+                          num_patch_transformer_layers=4 if multi else None,
+                          patch_transformer_hidden_size=128 if multi else None,
+                          patch_transformer_intermediate_size=1024 if multi else None,
+                          patch_transformer_num_attention_heads=4 if multi else None)
+
+
+def zoedepth_config_from_json(cj):
+    """The engine configuration of a ZoeDepth config.json (dict), or ValueError naming every field the engine does not
+    compute: a non-BEiT backbone (and the BEiT fields dpt_beit_config_from_json refuses), a "normed" bin type, an
+    attractor kind other than "mean", add_projection, batch norm in fusion, a bin_configurations list of other than 1
+    or 2 entries or with n_bins other than 64, a bin embedding other than 128 or a bottleneck other than the fusion
+    width, a relative feature count other than 32, and a patch transformer other than 4 layers of 128 / 4 heads / 1024.
+    transformers ignores attractor_alpha / attractor_gamma (inv_attractor runs with 300 / 2), and so does the engine."""
+    bad = []
+    if cj.get("model_type") != "zoedepth":
+        bad.append(("model_type", cj.get("model_type")))
+    try:
+        base = dpt_beit_config_from_json(dict(cj, model_type="dpt"))
+    except ValueError as ex:
+        bad.append(("backbone / neck", str(ex)))
+        base = None
+    for field, want in (("bin_centers_type", "softplus"), ("attractor_kind", "mean")):
+        if cj.get(field, want) != want:
+            bad.append((field, cj.get(field)))
+    if cj.get("num_relative_features", 32) != 32:
+        bad.append(("num_relative_features", cj.get("num_relative_features")))
+    if cj.get("bin_embedding_dim", 128) != 128:
+        bad.append(("bin_embedding_dim", cj.get("bin_embedding_dim")))
+    fusion = cj.get("fusion_hidden_size", 256)
+    if cj.get("bottleneck_features", 256) != fusion:
+        bad.append(("bottleneck_features", cj.get("bottleneck_features")))
+    bins = cj.get("bin_configurations") or [{"n_bins": 64, "min_depth": 0.001, "max_depth": 10.0}]
+    if not isinstance(bins, list) or len(bins) not in (1, 2):
+        bad.append(("bin_configurations", bins))
+        bins = []
+    for b in bins:
+        if (not isinstance(b, dict) or b.get("n_bins") != 64
+                or not 0 <= float(b.get("min_depth", -1)) < float(b.get("max_depth", -1))):
+            bad.append(("bin_configurations", b))
+    att = cj.get("num_attractors", [16, 8, 4, 1])
+    if not isinstance(att, list) or len(att) != 4 or any(type(a) is not int or not 1 <= a <= 16 for a in att):
+        bad.append(("num_attractors", att))
+    if len(bins) == 2:
+        for field, want in (("num_patch_transformer_layers", 4), ("patch_transformer_hidden_size", 128),
+                            ("patch_transformer_intermediate_size", 1024),
+                            ("patch_transformer_num_attention_heads", 4)):
+            if cj.get(field) != want:
+                bad.append((field, cj.get(field)))
+    tmin, tmax = cj.get("min_temp", 0.0212), cj.get("max_temp", 50.0)
+    if not (isinstance(tmin, (int, float)) and isinstance(tmax, (int, float)) and 0 < tmin < tmax):
+        bad.append(("min_temp / max_temp", (tmin, tmax)))
+    if bad:
+        raise ValueError("config.json: " + ", ".join(f"{f} = {v!r}" for f, v in bad) + " not served (ZoeDepth: BEiT "
+                         "trunk, softplus bins with unnormed mean attractors, one or two bin configurations)")
+    bj = cj["backbone_config"]
+    return dict(base, image_size=int(bj.get("image_size", 384)),
+                bins=[dict(name=b.get("name", f"c{i}"), n_bins=64, min_depth=float(b["min_depth"]),
+                           max_depth=float(b["max_depth"])) for i, b in enumerate(bins)],
+                attractors=list(att), min_temp=float(tmin), max_temp=float(tmax), bottleneck=fusion, embed=128)
+
+
+def zoedepth_processor_from_json(pj):
+    """ZOEDEPTH_PROCESSOR updated from a preprocessor_config.json (dict), or ValueError: padding on, keep_aspect_ratio
+    with ensure_multiple_of 32 (the class default 1/32 is not served), bilinear, 1/255."""
+    def bad(field, value):
+        raise ValueError(f"preprocessor_config.json: {field} = {value!r} is not served (ZoeDepth processor: reflect "
+                         "padding, keep_aspect_ratio with ensure_multiple_of 32, bilinear)")
+    for field in ("do_resize", "do_rescale", "do_normalize", "do_pad", "keep_aspect_ratio"):
+        if field not in pj:
+            bad(field, "missing")
+        if pj[field] is not True:
+            bad(field, pj[field])
+    if pj.get("ensure_multiple_of") != 32:
+        bad("ensure_multiple_of", pj.get("ensure_multiple_of"))
+    rf = pj.get("rescale_factor", 1 / 255)
+    if not isinstance(rf, (int, float)) or abs(rf - 1 / 255) > 1e-9:
+        bad("rescale_factor", rf)
+    if pj.get("resample", 2) != 2:
+        bad("resample", pj.get("resample"))
+    size = pj.get("size")
+    if not isinstance(size, dict) or type(size.get("height")) is not int or type(size.get("width")) is not int \
+            or size["height"] < 32 or size["width"] < 32:
+        bad("size", size)
+    p = dict(ZOEDEPTH_PROCESSOR, size=(size["height"], size["width"]))
+    for k, key in (("mean", "image_mean"), ("std", "image_std")):
+        if key in pj:
+            v = pj[key]
+            v = v if isinstance(v, (list, tuple)) else [v] * 3
+            if len(v) != 3 or any(not isinstance(x, (int, float)) for x in v):
+                bad(key, pj[key])
+            p[k] = tuple(float(x) for x in v)
+    return p
+
+
+def zoedepth_pad(n):
+    """ZoeDepthImageProcessor's reflect padding of a side of n pixels (post_process_depth_estimation crops the same)."""
+    return int(np.sqrt(n / 2) * 3)
+
+
+def zoedepth_processed_size(width, height, processor=None):
+    """(h, w) ZoeDepthImageProcessor resizes a (width, height) image to: DPT's keep-aspect rule on the padded size."""
+    return dpt_beit_processed_size(width + 2 * zoedepth_pad(width), height + 2 * zoedepth_pad(height),
+                                   processor or ZOEDEPTH_PROCESSOR)
+
+
+_ZM = "metric_head."
+
+
+def zoedepth_keys(cfg):
+    """Every state_dict key (and its shape) the ZoeDepth forward reads: the BEiT trunk and DPT neck of dpt_beit_keys
+    (the relative head named relative_head.conv1..3) and the metric head."""
+    F, E = cfg["fusion"], cfg["embed"]
+    k = {n: v for n, v in dpt_beit_keys(cfg).items() if not n.startswith("head.")}
+    F2 = F // 2
+    k["relative_head.conv1.weight"], k["relative_head.conv1.bias"] = (F2, F, 3, 3), (F2,)
+    k["relative_head.conv2.weight"], k["relative_head.conv2.bias"] = (32, F2, 3, 3), (32,)
+    k["relative_head.conv3.weight"], k["relative_head.conv3.bias"] = (1, 32, 1, 1), (1,)
+    multi = len(cfg["bins"]) > 1
+
+    def conv(name, o, i):
+        k[_ZM + name + ".weight"], k[_ZM + name + ".bias"] = (o, i, 1, 1), (o,)
+    conv("conv2", F, F)
+    mlp = E // 2 if multi else 128  # the projectors' hidden width (ZoeDepthProjector's default 128 on one configuration)
+    conv("seed_projector.conv1", mlp, F)
+    conv("seed_projector.conv2", E, mlp)
+    for j in range(4):
+        conv(f"projectors.{j}.conv1", mlp, F)
+        conv(f"projectors.{j}.conv2", E, mlp)
+    if multi:
+        for c in cfg["bins"]:
+            n = c["name"]
+            conv(f"seed_bin_regressors.{n}.conv1", E // 2, F)
+            conv(f"seed_bin_regressors.{n}.conv2", 64, E // 2)
+            for j in range(4):
+                conv(f"attractors.{n}.{j}.conv1", E, E)
+                conv(f"attractors.{n}.{j}.conv2", 16, E)  # the constructor's default n_attractors on every layer
+            conv(f"conditional_log_binomial.{n}.mlp.0", (32 + E) // 4, 32 + E)
+            conv(f"conditional_log_binomial.{n}.mlp.2", 4, (32 + E) // 4)
+        p = "patch_transformer."
+        conv(p + "embedding_convPxP", 128, F)
+        for i in range(4):
+            a = f"{_ZM}{p}transformer_encoder.{i}."
+            for n in ("query", "key", "value", "out_proj"):
+                k[a + f"self_attn.{n}.weight"], k[a + f"self_attn.{n}.bias"] = (128, 128), (128,)
+            k[a + "linear1.weight"], k[a + "linear1.bias"] = (1024, 128), (1024,)
+            k[a + "linear2.weight"], k[a + "linear2.bias"] = (128, 1024), (128,)
+            for n in ("norm1", "norm2"):
+                k[a + n + ".weight"] = k[a + n + ".bias"] = (128,)
+        for n, o in (("linear1", 128), ("linear2", 2)):
+            k[f"{_ZM}mlp_classifier.{n}.weight"], k[f"{_ZM}mlp_classifier.{n}.bias"] = (o, 128), (o,)
+    else:
+        conv("seed_bin_regressor.conv1", 256, F)
+        conv("seed_bin_regressor.conv2", 64, 256)
+        for j, na in enumerate(cfg["attractors"]):
+            conv(f"attractors.{j}.conv1", E, E)
+            conv(f"attractors.{j}.conv2", na, E)
+        conv("conditional_log_binomial.mlp.0", (33 + E) // 2, 33 + E)
+        conv("conditional_log_binomial.mlp.2", 4, (33 + E) // 2)
+    return k
+
+
+def check_zoedepth_state_dict(sd, cfg):
+    """ValueError naming the first missing or mis-shaped key the ZoeDepth forward reads."""
+    for name, shape in zoedepth_keys(cfg).items():
+        if name not in sd:
+            raise ValueError(f"ZoeDepth state dict: missing key {name}")
+        if tuple(sd[name].shape) != shape:
+            raise ValueError(f"ZoeDepth state dict: {name} has shape {tuple(sd[name].shape)}, expected {shape}")
+
+
+def zoedepth_attractors(sd, cfg):
+    """Attractors per layer as the weights define them: 16 on every layer of the two-configuration head (transformers
+    passes num_attractors to the unused n_bins), num_attractors on the single-configuration head."""
+    if len(cfg["bins"]) > 1:
+        n = cfg["bins"][0]["name"]
+        return [int(sd[f"{_ZM}attractors.{n}.{j}.conv2.weight"].shape[0]) for j in range(4)]
+    return [int(sd[f"{_ZM}attractors.{j}.conv2.weight"].shape[0]) for j in range(4)]
+
+
+def zoedepth_position_code(n, dim=128):
+    """ZoeDepthPatchTransformerEncoder.positional_encoding_1d for n tokens, with the same torch ops in f32."""
+    position = torch.arange(0, n, dtype=torch.float32).unsqueeze(1)
+    index = torch.arange(0, dim, 2, dtype=torch.float32).unsqueeze(0)
+    div_term = torch.exp(index * (-torch.log(torch.tensor(10000.0)) / dim))
+    pe = position * div_term
+    return torch.cat([torch.sin(pe), torch.cos(pe)], dim=1)
+
+
+def prepare_zoedepth(sd, cfg, image_h, image_w):
+    """ZoeDepth state_dict -> {name: np.ndarray} in the layouts depth_engine.cu expects: prepare_dpt_beit's trunk, neck
+    and relative head, and the metric head's "z.*" tensors (zoe_head in depth_engine.cu)."""
+    check_zoedepth_state_dict(sd, cfg)
+    sdb = {k: v for k, v in sd.items() if not k.startswith("relative_head.") and not k.startswith(_ZM)}
+    for j, n in ((0, "conv1"), (2, "conv2"), (4, "conv3")):
+        sdb[f"head.head.{j}.weight"] = sd[f"relative_head.{n}.weight"]
+        sdb[f"head.head.{j}.bias"] = sd[f"relative_head.{n}.bias"]
+    out = prepare_dpt_beit(sdb, cfg, image_h, image_w)
+    names = [c["name"] for c in cfg["bins"]]
+    multi = len(names) > 1
+
+    def w2(name):
+        return sd[_ZM + name + ".weight"].float().reshape(sd[_ZM + name + ".weight"].shape[0], -1)
+
+    def b(name):
+        return sd[_ZM + name + ".bias"].float()
+
+    def put(dst, name):
+        out[dst + ".w"], out[dst + ".b"] = _f16(w2(name)), _f32(b(name))
+    put("z.bt", "conv2")
+    put("z.sp1", "seed_projector.conv1")
+    put("z.sp2", "seed_projector.conv2")
+    for j in range(4):
+        put(f"z.p{j}.1", f"projectors.{j}.conv1")
+        put(f"z.p{j}.2", f"projectors.{j}.conv2")
+    seed = [f"seed_bin_regressors.{n}" for n in names] if multi else ["seed_bin_regressor"]
+    att = [f"attractors.{n}." for n in names] if multi else ["attractors."]
+    clb = [f"conditional_log_binomial.{n}" for n in names] if multi else ["conditional_log_binomial"]
+    out["z.s1.w"] = _f16(torch.cat([w2(s + ".conv1") for s in seed]))
+    out["z.s1.b"] = _f32(torch.cat([b(s + ".conv1") for s in seed]))
+    s2 = torch.block_diag(*[w2(s + ".conv2") for s in seed])  # each configuration's conv2 on its own seed columns
+    out["z.s2.w"], out["z.s2.b"] = _f16(s2), _f32(torch.cat([b(s + ".conv2") for s in seed]))
+    for j in range(4):
+        out[f"z.a{j}.1.w"] = _f16(torch.cat([w2(a + f"{j}.conv1") for a in att]))
+        out[f"z.a{j}.1.b"] = _f32(torch.cat([b(a + f"{j}.conv1") for a in att]))
+        out[f"z.a{j}.2.w"] = _f32(torch.stack([w2(a + f"{j}.conv2") for a in att]))
+        out[f"z.a{j}.2.b"] = _f32(torch.stack([b(a + f"{j}.conv2") for a in att]))
+    lb = []
+    for c in clb:  # per configuration: w1 [cin][hid], b1, w2 [4][hid], b2
+        lb += [w2(c + ".mlp.0").t().reshape(-1), b(c + ".mlp.0"), w2(c + ".mlp.2").reshape(-1), b(c + ".mlp.2")]
+    out["z.lb"] = _f32(torch.cat(lb))
+    if multi:
+        p = "patch_transformer."
+        blob = [w2(p + "embedding_convPxP").reshape(-1), b(p + "embedding_convPxP")]
+        for i in range(4):
+            a = f"{_ZM}{p}transformer_encoder.{i}."
+            g = lambda n: sd[a + n].float().reshape(-1)  # noqa: E731
+            blob += [g("self_attn.query.weight"), g("self_attn.key.weight"), g("self_attn.value.weight"),
+                     g("self_attn.query.bias"), g("self_attn.key.bias"), g("self_attn.value.bias"),
+                     g("self_attn.out_proj.weight"), g("self_attn.out_proj.bias"), g("norm1.weight"), g("norm1.bias"),
+                     g("linear1.weight"), g("linear1.bias"), g("linear2.weight"), g("linear2.bias"),
+                     g("norm2.weight"), g("norm2.bias")]
+        for n in ("linear1", "linear2"):
+            blob += [sd[f"{_ZM}mlp_classifier.{n}.weight"].float().reshape(-1),
+                     sd[f"{_ZM}mlp_classifier.{n}.bias"].float()]
+        out["z.router"] = _f32(torch.cat(blob))
+        P = cfg["patch"]
+        nb = ((image_h // P - 1) // 2 + 1) * ((image_w // P - 1) // 2 + 1)
+        out["z.r.pe"] = _f32(zoedepth_position_code(nb + 1))
+    return out

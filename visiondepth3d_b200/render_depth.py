@@ -17,13 +17,15 @@ from ctypes import c_void_p as C_void_p
 
 import numpy as np
 
-from .depth_engine import (FAMILY_DA_V2, FAMILY_DPT, FAMILY_DPT_BEIT, FAMILY_DPT_HYBRID, DepthEngine,
+from .depth_engine import (FAMILY_DA_V2, FAMILY_DPT, FAMILY_DPT_BEIT, FAMILY_DPT_HYBRID, FAMILY_ZOEDEPTH, DepthEngine,
                            processed_size as _processed_size)
 from .depth_weights import (CONFIGS, DPT_BEIT_CONFIGS, DPT_BEIT_PROCESSOR, DPT_CONFIGS, DPT_HYBRID_CONFIGS, DPT_PROCESSOR, da_arch,
                             da_config_from_json, da_processor_from_json, da_spec, dpt_beit_config_from_json,
                             dpt_beit_processed_size, dpt_beit_processor_from_json, dpt_config_from_json,
                             dpt_hybrid_config_from_json, dpt_processed_size, dpt_processor_from_json, hf_config,
                             hf_dpt_beit_config, hf_dpt_config, hf_dpt_hybrid_config, is_plain_v2)
+from .depth_weights import (ZOEDEPTH_CONFIGS, ZOEDEPTH_PROCESSOR, hf_zoedepth_config, zoedepth_config_from_json,
+                            zoedepth_processed_size, zoedepth_processor_from_json)
 from .render_3d import _dialog, _val
 
 try:
@@ -57,6 +59,7 @@ supported_models = {
     "Manojb - DPT-Large": ("Manojb/dpt-large", "dpt-large"),
     "MiDaS 3.0": ("Intel/dpt-hybrid-midas", "dpt-hybrid-midas"),
     "dpt-beit-large-512": ("Intel/dpt-beit-large-512", "dpt-beit-large-512"),
+    "ZoeDepth": ("Intel/zoedepth-nyu-kitti", "zoedepth-nyu-kitti"),
 }
 # the Depth-Anything checkpoints other than V2's: their taps and head are only in config.json (the tensors have V2's
 # shapes), so they load only with it, and with Depth-Anything's preprocessor_config.json when one is present
@@ -67,8 +70,10 @@ DPT_HYBRID_CONFIG_REQUIRED = frozenset(v[0] for v in supported_models.values() i
 # DPT-BEiT's out-indices, LayerScale and processed size live only in config.json and preprocessor_config.json: guessing
 # them would silently change the depth, so its checkpoints load only with both
 DPT_BEIT_FILES_REQUIRED = frozenset(v[0] for v in supported_models.values() if v[1] in DPT_BEIT_CONFIGS)
-_SERVED = ("Depth-Anything (V2, V1, Distill-Any-Depth, V2-Metric), DPT-Large, MiDaS 3.0 (DPT-Hybrid) or "
-           "dpt-beit-large-512 (MiDaS v3.1 BEiT-L)")
+# ZoeDepth's bin configurations and padded processor likewise live only in those two files
+ZOEDEPTH_FILES_REQUIRED = frozenset(v[0] for v in supported_models.values() if v[1] in ZOEDEPTH_CONFIGS)
+_SERVED = ("Depth-Anything (V2, V1, Distill-Any-Depth, V2-Metric), DPT-Large, MiDaS 3.0 (DPT-Hybrid), "
+           "dpt-beit-large-512 (MiDaS v3.1 BEiT-L) or ZoeDepth")
 
 
 def _family_of(arch):
@@ -76,17 +81,37 @@ def _family_of(arch):
         return FAMILY_DPT_HYBRID
     if arch in DPT_BEIT_CONFIGS:
         return FAMILY_DPT_BEIT
+    if arch in ZOEDEPTH_CONFIGS:
+        return FAMILY_ZOEDEPTH
     return FAMILY_DPT if arch in DPT_CONFIGS else FAMILY_DA_V2
 
 
 def _dpt_like(arch):
-    """DPT-Large, DPT-Hybrid and DPT-BEiT: DPT's processor settings, no tiled depth."""
-    return _family_of(arch) in (FAMILY_DPT, FAMILY_DPT_HYBRID, FAMILY_DPT_BEIT)
+    """DPT-Large, DPT-Hybrid, DPT-BEiT and ZoeDepth: their own processor settings, no tiled depth."""
+    return _family_of(arch) in (FAMILY_DPT, FAMILY_DPT_HYBRID, FAMILY_DPT_BEIT, FAMILY_ZOEDEPTH)
 
 
 def _dpt_configs(arch):
-    return {FAMILY_DPT_HYBRID: DPT_HYBRID_CONFIGS, FAMILY_DPT_BEIT: DPT_BEIT_CONFIGS}.get(_family_of(arch),
-                                                                                     DPT_CONFIGS)[arch]
+    return {FAMILY_DPT_HYBRID: DPT_HYBRID_CONFIGS, FAMILY_DPT_BEIT: DPT_BEIT_CONFIGS,
+            FAMILY_ZOEDEPTH: ZOEDEPTH_CONFIGS}.get(_family_of(arch), DPT_CONFIGS)[arch]
+
+
+def _load_zoedepth_checkpoint(sd, cfg_path):
+    """arch of a ZoeDepth state dict (metric_head.* keys): the ZOEDEPTH_CONFIGS key whose configuration config.json
+    (required) describes -- the bin configurations' names matter only where the two-configuration head's keys use them."""
+    import json
+    if not os.path.exists(cfg_path):
+        raise ValueError(f"a ZoeDepth checkpoint needs its config.json (not found: {cfg_path})")
+    with open(cfg_path) as f:
+        got = zoedepth_config_from_json(json.load(f))
+
+    def key(c):
+        bins = c["bins"] if len(c["bins"]) > 1 else [dict(c["bins"][0], name=None)]
+        return dict(c, bins=bins)
+    for name, c in ZOEDEPTH_CONFIGS.items():
+        if key(c) == key(got):
+            return name
+    raise ValueError(f"config.json {got} matches none of the ZoeDepth configurations served ({sorted(ZOEDEPTH_CONFIGS)})")
 
 
 def _load_dpt_beit_checkpoint(sd, cfg_path):
@@ -161,6 +186,8 @@ def load_checkpoint(path):
         return _load_dpt_hybrid_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
     if "dpt.embeddings.cls_token" in sd:
         return _load_dpt_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
+    if any(k.startswith("metric_head.") for k in sd):  # ZoeDepth's BEiT trunk has bias tables too: test it first
+        return _load_zoedepth_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
     if any(k.endswith("relative_position_bias_table") for k in sd):
         return _load_dpt_beit_checkpoint(sd, os.path.join(os.path.dirname(path), "config.json")), sd
     if "backbone.embeddings.cls_token" not in sd:
@@ -201,6 +228,8 @@ def model_processed_size(width, height):
     dpt-beit-large-512 keeps the aspect at multiples of 32 near 512 (or its processor's fixed size)."""
     if _family_of(_arch) == FAMILY_DPT_BEIT:
         return dpt_beit_processed_size(width, height, _processor)
+    if _family_of(_arch) == FAMILY_ZOEDEPTH:
+        return zoedepth_processed_size(width, height, _processor)
     if _dpt_like(_arch):
         return dpt_processed_size(_processor)
     return _processed_size(width, height)
@@ -208,8 +237,8 @@ def model_processed_size(width, height):
 
 def _check_tiled_supported():
     if USE_TILED_DEPTH and _dpt_like(_arch):
-        raise ValueError("USE_TILED_DEPTH is served for Depth-Anything-V2 models only, not for DPT-Large, MiDaS 3.0 or "
-                         "dpt-beit-large-512")
+        raise ValueError("USE_TILED_DEPTH is served for Depth-Anything-V2 models only, not for DPT-Large, MiDaS 3.0, "
+                         "dpt-beit-large-512 or ZoeDepth")
 
 
 def _engine_for(width, height):
@@ -255,12 +284,17 @@ def load_depth_model(arch="vits", state_dict=None, width=1920, height=1080, seed
     beit = _family_of(arch) == FAMILY_DPT_BEIT
     if beit:
         processor = dict(processor or DPT_BEIT_PROCESSOR)
+    elif _family_of(arch) == FAMILY_ZOEDEPTH:
+        processor = dict(processor or ZOEDEPTH_PROCESSOR)
     elif dpt:
         processor = dict(processor or DPT_PROCESSOR)
         dpt_processed_size(processor)  # refuse an unserved processor before anything is built
     if state_dict is None:
         torch.manual_seed(seed)
-        if dpt:
+        if _family_of(arch) == FAMILY_ZOEDEPTH:
+            from transformers import ZoeDepthForDepthEstimation
+            state_dict = ZoeDepthForDepthEstimation(hf_zoedepth_config(arch)).eval().state_dict()
+        elif dpt:
             from transformers import DPTForDepthEstimation
             hf = {FAMILY_DPT_HYBRID: hf_dpt_hybrid_config, FAMILY_DPT_BEIT: hf_dpt_beit_config}.get(
                 _family_of(arch), hf_dpt_config)(arch)
@@ -654,7 +688,7 @@ def ensure_model_downloaded(checkpoint):
     if checkpoint in DPT_HYBRID_CONFIG_REQUIRED and not os.path.exists(os.path.join(ckdir, "config.json")):
         print(f"❌ {checkpoint}: no config.json next to {path} (its BiT backbone is described only there)")
         return None, None
-    if checkpoint in DPT_BEIT_FILES_REQUIRED:
+    if checkpoint in DPT_BEIT_FILES_REQUIRED or checkpoint in ZOEDEPTH_FILES_REQUIRED:
         for name in ("config.json", "preprocessor_config.json"):
             if not os.path.exists(os.path.join(ckdir, name)):
                 print(f"❌ {checkpoint}: no {name} next to {path} (its out-indices, LayerScale and processed size are "
@@ -684,11 +718,12 @@ def ensure_model_downloaded(checkpoint):
             except ValueError as e:
                 print(f"❌ {pp}: {e}")
                 return None, None
-    if _family_of(arch) == FAMILY_DPT_BEIT:
+    if _family_of(arch) in (FAMILY_DPT_BEIT, FAMILY_ZOEDEPTH):
         pp = os.path.join(ckdir, "preprocessor_config.json")
+        parse = dpt_beit_processor_from_json if _family_of(arch) == FAMILY_DPT_BEIT else zoedepth_processor_from_json
         try:
             with open(pp) as f:
-                meta["processor"] = dpt_beit_processor_from_json(json.load(f))
+                meta["processor"] = parse(json.load(f))
         except (OSError, ValueError) as e:
             print(f"❌ {pp}: {e}")
             return None, None
