@@ -494,7 +494,11 @@ int vd3d_conv_f16(vd3d_depth* e, const void* in_nhwc_f16, int H, int W, int cin,
  *   op 0 stem conv (dims H, W): t.in f32 [3, H, W], t.w f32 [64, 147] -> f32 [H/2 * W/2, 64]
  *   op 1 GroupNorm (dims rows, C, flags: 1 ReLU, 2 + GN(t.in2; t.g2, t.b2), 4 + t.res f16): t.in f32 [rows, C] -> f16
  *   op 2 max-pool (dims H, W, C): t.in f16 [H, W, C] -> f16 [H/2, W/2, C]
- *   op 3 SAME im2col (dims H, W, C, k, pb): t.in f16 [H, W, C] -> f16 [H/2 * W/2, k * k * C] */
+ *   op 3 SAME im2col (dims H, W, C, k, pb): t.in f16 [H, W, C] -> f16 [H/2 * W/2, k * k * C]
+ *   op 4 backbone conv, the launches of the forward's (dims H, W, cin, cout, kind: 0 1x1, 1 3x3 stride 1 pad 1, 2 3x3
+ *        stride 2 SAME (0 before, 1 after), 3 1x1 stride 2; cin and cout multiples of 64, H and W even at stride 2):
+ *        t.in f16 [H, W, cin], t.w f16 [cout, cin] (1x1) or [cout, 9 cin] (3x3, tap-major) -> f32 [Ho * Wo, cout],
+ *        Ho = H / 2 at stride 2 (the im2col rows in "t.col") */
 int vd3d_bit_kernel(vd3d_depth* e, int op, const int32_t* dims);
 /* unit-test hook for the ZoeDepth kernels, in the style of vd3d_bit_kernel (output "t.out"; the route in "t.route").
  *   op 0 preprocess (h, w, OH, OW, swap_rb): t.img u8 [h, w, 3] -> f32 [3, OH, OW] with the engine's mean / std

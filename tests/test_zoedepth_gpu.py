@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import hybrid_zoe_kernel_refs as HZ
 from tests import zoedepth_oracle as ZO
 
 pytestmark = pytest.mark.gpu
@@ -163,37 +164,10 @@ def test_router_logits_against_float64(multi, hook):
     xm = torch.from_numpy(x).double().t().reshape(1, F_, 12, 21)
     with torch.no_grad():
         # the oracle's router in float64 (the sinusoid in f32 as transformers builds it, then widened)
-        ref = _router64(sd64, xm).numpy()
+        ref = HZ.router64(sd64, xm).numpy()
     err = float(np.abs(got - ref).max())
     print(f"router logits {got} vs float64 {ref}: max abs {err:.3e}")
     assert err <= ROUTER_BOUND
-
-
-def _router64(sd, x):
-    import torch.nn.functional as F
-    from visiondepth3d_b200.depth_weights import zoedepth_position_code
-    p = ZO.M + "patch_transformer."
-    e = F.conv2d(x, sd[p + "embedding_convPxP.weight"], sd[p + "embedding_convPxP.bias"]).flatten(2)
-    e = F.pad(e, (1, 0)).permute(0, 2, 1)
-    e = e + zoedepth_position_code(e.shape[1]).double()[None]
-    for i in range(4):
-        a = f"{p}transformer_encoder.{i}."
-        q, k, v = (F.linear(e, sd[a + f"self_attn.{n}.weight"], sd[a + f"self_attn.{n}.bias"]).view(1, -1, 4, 32)
-                   .transpose(1, 2) for n in ("query", "key", "value"))
-        s = torch.softmax(q @ k.transpose(-1, -2) / np.sqrt(32), dim=-1)
-        o = F.linear((s @ v).transpose(1, 2).reshape(1, -1, 128), sd[a + "self_attn.out_proj.weight"],
-                     sd[a + "self_attn.out_proj.bias"])
-        e = F.layer_norm(e + o, (128,), sd[a + "norm1.weight"], sd[a + "norm1.bias"], 1e-5)
-        h = F.linear(F.relu(F.linear(e, sd[a + "linear1.weight"], sd[a + "linear1.bias"])), sd[a + "linear2.weight"],
-                     sd[a + "linear2.bias"])
-        e = F.layer_norm(e + h, (128,), sd[a + "norm2.weight"], sd[a + "norm2.bias"], 1e-5)
-    c = F.relu(F.linear(e[:, 0], sd[ZO.M + "mlp_classifier.linear1.weight"], sd[ZO.M + "mlp_classifier.linear1.bias"]))
-    return F.linear(c, sd[ZO.M + "mlp_classifier.linear2.weight"], sd[ZO.M + "mlp_classifier.linear2.bias"])[0]
-
-
-def _up64(x, H, W):
-    return torch.nn.functional.interpolate(torch.from_numpy(x).double(), (H, W), mode="bilinear",
-                                           align_corners=True).numpy()
 
 
 @pytest.mark.parametrize("seed_stage,route", [(True, 1), (False, 0)])
@@ -224,11 +198,8 @@ def test_attractor_against_float64(hook, seed_stage, route):
     _put(hook, "t.prev", prev)
     _run(hook, 2, [H, W, Hp, Wp, nc, route, na, int(seed_stage)])
     got = hook.get_buffer("t.out", (H * W, K), np.float32)
-    a = hid[:, route * E:(route + 1) * E].astype(np.float64) @ w2[route].astype(np.float64).T + b2[route]
-    a = np.log1p(np.exp(a))
-    c = _up64(nat64.T.reshape(1, K, Hp, Wp), H, W).reshape(K, H * W).T
-    dx = a[:, :, None] - c[:, None, :]
-    ref = c + (dx / (1 + 300 * dx * dx)).mean(1)
+    ref, _, _ = HZ.attractor(hid[:, route * E:(route + 1) * E], w2[route], b2[route], prev[:, route * K:(route + 1) * K]
+                             if seed_stage else prev, Hp, Wp, H, W, prev_softplus=seed_stage)
     err = float(np.abs(got - ref).max() / (np.abs(ref).max()))
     print(f"attractor (seed {seed_stage}, route {route}): max abs / max {err:.3e}")
     assert err <= 2e-6
@@ -262,27 +233,8 @@ def test_log_binomial_against_float64(hook, cat, hid, route, p_end):
         _put(hook, n, v)
     _run(hook, 3, [H, W, He, We, nc, route, cat, hid])
     got = hook.get_buffer("t.out", (H * W,), np.float32)
-    w1, b1, w2, b2 = (x.astype(np.float64) for x in blocks[route])
-    a64 = act.astype(np.float64)
-    cols = [a64]
-    if cat:
-        cols.append(np.maximum(a64 @ w3.astype(np.float64) + float(b3[0]), 0)[:, None])
-    cols.append(_up64(emb.astype(np.float32).T.reshape(1, E, He, We), H, W).reshape(E, H * W).T)
-    x = np.concatenate(cols, 1)
-    z = x @ w1 + b1
-    from scipy.special import erf
-    z = 0.5 * z * (1 + erf(z / np.sqrt(2)))
-    o = np.log1p(np.exp(z @ w2.T + b2))
-    p = (o[:, 0] + 1e-4) / (o[:, 0] + o[:, 1] + 2e-4)
-    q, p = np.clip(1 - p, 1e-4, 1), np.clip(p, 1e-4, 1)
-    k = np.arange(K, dtype=np.float64)
-    n_, kk = K - 1 + 1e-7, k + 1e-7
-    lbk = n_ * np.log(n_) - kk * np.log(kk) - (n_ - kk) * np.log(n_ - kk + 1e-7)
-    y = (lbk[None] + k[None] * np.log(p)[:, None] + (K - 1 - k)[None] * np.log(q)[:, None]) / tmin
-    y = np.exp(y - y.max(1, keepdims=True))
-    y /= y.sum(1, keepdims=True)
-    c = _up64(bins.T.reshape(1, K, He, We), H, W).reshape(K, H * W).T
-    ref = (y * c).sum(1)
+    ref = HZ.log_binomial(act, emb, bins, He, We, H, W, HZ.logbinom_unpack(lb, nc, cin, hid, route), tmin, tmin,
+                          w3 if cat else None, b3 if cat else None)
     err = float(np.abs(got - ref).max() / 10.0)
     print(f"log-binomial (cat {cat}, hid {hid}, route {route}, p -> {p_end}): max abs / bin span {err:.3e}")
     assert err <= 1e-5

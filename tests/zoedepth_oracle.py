@@ -169,14 +169,14 @@ def forward(sd, cfg, pixel_values, route=None, return_parts=False):
 SMALL = dict(BO.SMALL, bottleneck=64)
 
 
-def random_model(multi=True, small=True, seed=0):
+def random_model(multi=True, small=True, seed=0, **cfg):
     """(state_dict, cfg) of a random-init transformers ZoeDepthForDepthEstimation (the SMALL BEiT or BEiT-L/16 384) with
     filled bias tables, LayerScale lambdas in [0.05, 0.3], and the bins' seed made positive and spread so that the
-    metric depth has a range worth measuring."""
+    metric depth has a range worth measuring.  cfg overrides entries of the configuration (e.g. the fusion width)."""
     from transformers import ZoeDepthForDepthEstimation
     from visiondepth3d_b200.depth_weights import ZOEDEPTH_CONFIGS, hf_zoedepth_config
     name = "zoedepth-nyu-kitti" if multi else "zoedepth-nyu"
-    over = SMALL if small else {}
+    over = dict(SMALL if small else {}, **cfg)
     cfg = dict(ZOEDEPTH_CONFIGS[name], **over)
     torch.manual_seed(seed)
     sd = ZoeDepthForDepthEstimation(hf_zoedepth_config(name, **over)).eval().state_dict()

@@ -240,6 +240,33 @@ int conv(vd3d_depth* e, const __half* in, int H, int W, int cin, const __half* w
 
 int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
+// One conv of the BiT backbone (bit_backbone; vd3d_bit_kernel op 4) on k_umma_gemm, no bias: f16 NHWC in [H, W, cin]
+// -> f32 out [Ho * Wo, cout].  BIT_1X1: a GEMM on the map's pixel rows, w [cout, cin].  BIT_3X3: stride 1, pad 1, on
+// the implicit-GEMM conv, w [cout, 9 cin] tap-major.  BIT_3X3_S2: stride 2 with TF-SAME pads (0 before, 1 after), a
+// GEMM on k_im2col_same's rows written to col.  BIT_1X1_S2: stride 2, a GEMM on the even pixels gathered into col.
+// Ho = H / 2 and Wo = W / 2 at stride 2; col holds round_up(Ho * Wo, 128) rows of the GEMM's K columns.
+enum { BIT_1X1 = 0, BIT_3X3 = 1, BIT_3X3_S2 = 2, BIT_1X1_S2 = 3 };
+int bit_conv(vd3d_depth* e, int kind, const __half* in, int H, int Wd, int cin, const __half* w, int cout, float* out,
+             __half* col) {
+  cudaStream_t s = e->stream;
+  const bool s2 = kind == BIT_3X3_S2 || kind == BIT_1X1_S2;
+  const int k = (kind == BIT_3X3 || kind == BIT_3X3_S2) ? 3 : 1, K = k * k * cin;
+  GemmArgs g = base_args(s2 ? (H / 2) * (Wd / 2) : H * Wd, cout, K, EPI_F32);
+  g.out_f32 = out;
+  const __half* a = in;
+  if (s2) {
+    const int sp = e->span_begin("bit.im2col", s);
+    launch_im2col_same(in, H, Wd, cin, k, 0, col, s);
+    e->span_end(sp, s);
+    e->launches++;
+    a = col;
+  }
+  const int sp = e->span_begin("bit.conv", s);
+  const int r = kind == BIT_3X3 ? conv(e, in, H, Wd, cin, w, true, g) : gemm(e, a, K, w, K, g);
+  e->span_end(sp, s);
+  return r;
+}
+
 // ZoeDepthImageProcessor's reflect padding of an h-row (or w-column) image: int(sqrt(h / 2) * 3), the same value
 // post_process_depth_estimation crops off
 int zoe_pad(int n) { return (int)(sqrt(n / 2.0) * 3.0); }
@@ -540,11 +567,26 @@ int vd3d_conv_f16(vd3d_depth* e, const void* in_nhwc, int H, int W, int cin, con
 }
 
 int vd3d_bit_kernel(vd3d_depth* e, int op, const int32_t* d) {
-  if (!e || !d || op < 0 || op > 3) return VD3D_ERR_ARG;
+  if (!e || !d || op < 0 || op > 4) return VD3D_ERR_ARG;
   cudaStream_t s = e->stream;
   int r;
   void* out;
-  if (op == 0) {
+  if (op == 4) {
+    const int H = d[0], Wd = d[1], cin = d[2], cout = d[3], kind = d[4];
+    const bool s2 = kind == BIT_3X3_S2 || kind == BIT_1X1_S2;
+    const int taps = (kind == BIT_3X3 || kind == BIT_3X3_S2) ? 9 : 1;
+    if (kind < BIT_1X1 || kind > BIT_1X1_S2 || H < 2 || Wd < 2 || (s2 && (H | Wd) & 1) || cin < 64 || cin % 64 ||
+        cout < 64 || cout % 64)
+      return VD3D_ERR_ARG;
+    const int rows = s2 ? (H / 2) * (Wd / 2) : H * Wd;
+    const __half *in, *w;
+    void* col = nullptr;
+    if ((r = W(e, "t.in", &in, (size_t)H * Wd * cin)) || (r = W(e, "t.w", &w, (size_t)cout * taps * cin)) ||
+        (r = get_buf(e, "t.out", (size_t)rows * cout * 4, &out)) ||
+        (s2 && (r = get_buf(e, "t.col", (size_t)round_up(rows, 128) * taps * cin * 2, &col))))
+      return r;
+    if ((r = bit_conv(e, kind, in, H, Wd, cin, w, cout, (float*)out, (__half*)col))) return r;
+  } else if (op == 0) {
     const int H = d[0], Wd = d[1];
     if (H < 2 || Wd < 2 || (H | Wd) & 1) return VD3D_ERR_ARG;
     const float *in, *w;
@@ -720,17 +762,13 @@ int bit_backbone(vd3d_depth* e, int b, const float* px, const __half** stage3) {
     e->launches += nb ? 3 : 2;
     return VD3D_OK;
   };
-  // 1x1 conv as a GEMM: A [rows, cin] f16 -> f32 [rows, cout]
-  auto conv1 = [&](const char* wname, const __half* in, int rows, int cin, int cout, float* out) -> int {
+  // one conv (bit_conv) of an Hin x Hin map with the weight tensor wname
+  auto bconv = [&](const std::string& wname, int kind, const __half* in, int Hin, int cin, int cout, float* out) -> int {
     const __half* w;
     int rr;
-    if ((rr = W(e, wname, &w, (size_t)cout * cin))) return rr;
-    GemmArgs g = base_args(rows, cout, cin, EPI_F32);
-    g.out_f32 = out;
-    const int sp = e->span_begin("bit.conv", s);
-    rr = gemm(e, in, cin, w, cin, g);
-    e->span_end(sp, s);
-    return rr;
+    const size_t taps = (kind == BIT_3X3 || kind == BIT_3X3_S2) ? 9 : 1;
+    if ((rr = W(e, wname, &w, (size_t)cout * taps * cin))) return rr;
+    return bit_conv(e, kind, in, Hin, Hin, cin, w, cout, out, (__half*)col);
   };
 
   // ---- stem ----
@@ -762,47 +800,19 @@ int bit_backbone(vd3d_depth* e, int b, const float* px, const __half** stage3) {
         return std::string(nm);
       };
       // conv1 (1x1) + GN1 + ReLU at the input resolution
-      if ((r = conv1(wn("c1.w").c_str(), x, rows_in, cin, mid, (float*)y))) return r;
+      if ((r = bconv(wn("c1.w"), BIT_1X1, x, H, cin, mid, (float*)y))) return r;
       if ((r = groupnorm(wn("n1").c_str(), (const float*)y, nullptr, nullptr, nullptr, 1, rows_in, mid, (__half*)t1)))
         return r;
       // conv2 (3x3, stride 1 or 2) + GN2 + ReLU
-      {
-        const __half* w;
-        if ((r = W(e, wn("c2.w"), &w, (size_t)mid * 9 * mid))) return r;
-        GemmArgs g = base_args(rows, mid, 9 * mid, EPI_F32);
-        g.out_f32 = (float*)y;
-        g.ldc = mid;
-        if (s2) {
-          int sp = e->span_begin("bit.im2col", s);
-          launch_im2col_same((const __half*)t1, H, H, mid, 3, 0, (__half*)col, s);
-          e->span_end(sp, s);
-          e->launches++;
-          sp = e->span_begin("bit.conv", s);
-          r = gemm(e, (const __half*)col, 9 * mid, w, 9 * mid, g);
-          e->span_end(sp, s);
-        } else {
-          const int sp = e->span_begin("bit.conv", s);
-          r = conv(e, (const __half*)t1, H, H, mid, w, true, g);
-          e->span_end(sp, s);
-        }
-        if (r) return r;
-      }
+      if ((r = bconv(wn("c2.w"), s2 ? BIT_3X3_S2 : BIT_3X3, (const __half*)t1, H, mid, mid, (float*)y))) return r;
       if ((r = groupnorm(wn("n2").c_str(), (const float*)y, nullptr, nullptr, nullptr, 1, rows, mid, (__half*)t2)))
         return r;
       // conv3 (1x1) -> y; the first block's shortcut conv -> y2
-      if ((r = conv1(wn("c3.w").c_str(), (const __half*)t2, rows, mid, out_c, (float*)y))) return r;
+      if ((r = bconv(wn("c3.w"), BIT_1X1, (const __half*)t2, Ho, mid, out_c, (float*)y))) return r;
       __half* out = (k == kBitDepths[st] - 1 && st < 2) ? (__half*)(st == 0 ? st1 : st2)
                                                         : (__half*)(x == (const __half*)xa ? xb : xa);
       if (first) {
-        const __half* xs = x;
-        if (s2) {  // stride-2 1x1: the even pixels
-          const int sp = e->span_begin("bit.im2col", s);
-          launch_im2col_same(x, H, H, cin, 1, 0, (__half*)col, s);
-          e->span_end(sp, s);
-          e->launches++;
-          xs = (const __half*)col;
-        }
-        if ((r = conv1(wn("ds.w").c_str(), xs, rows, cin, out_c, (float*)y2))) return r;
+        if ((r = bconv(wn("ds.w"), s2 ? BIT_1X1_S2 : BIT_1X1, x, H, cin, out_c, (float*)y2))) return r;
         if ((r = groupnorm(wn("n3").c_str(), (const float*)y, wn("ds").c_str(), (const float*)y2, nullptr, 1, rows,
                            out_c, out)))
           return r;
