@@ -31,6 +31,17 @@ PIXEL_SHIFT = {"fast": 5, "exact": 23}
 # vd3d_render_clip_depth over CLIP_DEPTH_FRAMES frames: (context launches, depth engine launches) by depth batch
 CLIP_DEPTH_FRAMES = 8
 CLIP_DEPTH = {1: (40, 1128), 4: (40, 624)}
+# one eager infer_batch of the small random-init model of each depth family (the family tests' models): depth engine
+# launches by batch size, pre- and post-process included
+FAMILY_BATCH = {
+    "da-v2": {1: 141, 4: 312},
+    "da-metric": {1: 141, 4: 312},
+    "dpt": {1: 93, 4: 252},
+    "dpt-hybrid": {1: 240, 4: 858},
+    "dpt-beit": {1: 93, 4: 252},
+    "zoedepth-2": {1: 123, 4: 372},
+    "zoedepth-1": {1: 122, 4: 368},
+}
 
 
 @pytest.fixture
@@ -172,3 +183,49 @@ def test_render_clip_depth_launches(ctx, batch):
         assert clip_depth_launches(ctx, eng, batch, 1) == CLIP_DEPTH[batch]
     finally:
         eng.close()
+
+
+def family_engine(name):
+    """The small random-init model of a depth family on an engine of the size its family tests use."""
+    from tests import da_family_oracle as DO
+    from tests import dpt_beit_oracle as OB
+    from tests import dpt_hybrid_oracle as OH
+    from tests import dpt_oracle as OD
+    from tests import zoedepth_oracle as ZO
+    from visiondepth3d_b200.depth_engine import DepthEngine
+    from visiondepth3d_b200.depth_weights import da_spec
+    proc128 = dict(size=(128, 128), resample=3, mean=(0.5,) * 3, std=(0.5,) * 3)
+    if name == "da-v2":
+        return depth_engine(None)
+    if name == "da-metric":
+        sd, spec = DO.random_model(da_spec("vits", head="metric", max_depth=20.0), seed=5)
+        e = DepthEngine(spec, 70, 98)
+    elif name == "dpt":
+        sd, cfg = OD.random_model(small=True)
+        e = DepthEngine(cfg, family="dpt", processor=proc128)
+    elif name == "dpt-hybrid":
+        sd, cfg = OH.random_model(small=True)
+        e = DepthEngine(cfg, family="dpt-hybrid", processor=proc128)
+    elif name == "dpt-beit":
+        sd, cfg = OB.random_model(small=True, seed=3)
+        e = DepthEngine(cfg, 64, 96, family="dpt-beit")
+    else:
+        sd, cfg = ZO.random_model(multi=name == "zoedepth-2", seed=3 if name == "zoedepth-2" else 4)
+        e = DepthEngine(cfg, 64, 96, family="zoedepth")
+    e.load_state_dict(sd)
+    return e
+
+
+@pytest.mark.parametrize("family", list(FAMILY_BATCH))
+def test_depth_family_batch_launches(family):
+    """Launches of one eager vd3d_depth_infer_batch per family and batch size, after a warm-up call."""
+    e = family_engine(family)
+    try:
+        for batch, want in FAMILY_BATCH[family].items():
+            frames = [synth_frame(i, W, H, "natural")[0] for i in range(batch)]
+            e.infer_batch(frames, check_size=False)
+            l0 = e.launches
+            e.infer_batch(frames, check_size=False)
+            assert e.launches - l0 == want, (family, batch)
+    finally:
+        e.close()

@@ -47,15 +47,40 @@ struct DTensor {
   size_t bytes = 0;
 };
 
-}  // namespace
+// What a model family changes in the forward and in the drivers (family_traits).
+struct FamilyTraits {
+  bool bit_front_end;    // DPT-Hybrid: a BiT backbone replaces the patch embedding; its stages 1 and 2 feed neck
+                         // inputs 0 and 1
+  bool readout;          // DPT: raw taps through the project readout (else Depth-Anything's final-LayerNorm taps)
+  bool rel_pos_bias;     // BEiT: a relative position bias table per layer in the attention
+  bool zoe_head;         // ZoeDepth: the metric-bins head, the reflect-pad pre-process and the cropped post-process
+  bool square_grid;      // the tokens are reshaped as a square grid (DPT-Large, DPT-Hybrid)
+  bool keep_aspect_fit;  // the processor may keep the aspect ratio (vd3d_depth_set_fit)
+};
 
-struct vd3d_depth {
+// the traits of a VD3D_DEPTH_* code; false for an unknown code
+bool family_traits(int family, FamilyTraits* t) {
+  switch (family) {
+    case VD3D_DEPTH_DA_V2: *t = {false, false, false, false, false, false}; return true;
+    case VD3D_DEPTH_DPT: *t = {false, true, false, false, true, false}; return true;
+    case VD3D_DEPTH_DPT_HYBRID: *t = {true, true, false, false, true, false}; return true;
+    case VD3D_DEPTH_DPT_BEIT: *t = {false, true, true, false, false, true}; return true;
+    // ZoeDepth's trunk, neck and fusion are dpt-beit-large-512's
+    case VD3D_DEPTH_ZOEDEPTH: *t = {false, true, true, true, false, true}; return true;
+  }
+  return false;
+}
+
+// The model an engine serves: everything vd3d_depth_clone hands to a clone besides the weights.
+struct DepthSettings {
   vd3d_depth_config cfg;
   // model family, patch, LayerNorm epsilon and image processor (vd3d_depth_create_ex; DA-V2 defaults otherwise)
   int family = VD3D_DEPTH_DA_V2, patch = 14;
+  FamilyTraits traits = {};
   float ln_eps = 1e-6f;
   PreprocParams pre = kImagenetBicubic;
-  // BEiT's keep-aspect processor (vd3d_depth_set_fit): target and multiple; fit_multiple 0: a fixed size
+  // the keep-aspect processor of vd3d_depth_infer_images: target and multiple; fit_multiple 0: a fixed size.
+  // Depth-Anything's is 518 x 518 and 14; BEiT's is set by vd3d_depth_set_fit
   int fit_h = 0, fit_w = 0, fit_multiple = 0;
   // ZoeDepth's metric head (vd3d_depth_set_zoe): bin configurations (0: not set), attractors per layer, temperature
   // range, whether the relative depth is the log-binomial's 33rd input
@@ -64,15 +89,19 @@ struct vd3d_depth {
   // the head's last activation (VD3D_HEAD_RELATIVE / _METRIC) and the metric head's scale; every EPI_HEAD reads them
   int head = VD3D_HEAD_RELATIVE;
   float max_depth = 1.f;
+  int ph = 0, pw = 0, ntok = 0, npad = 0;  // token grid, tokens with CLS, tokens rounded up to the 128-row tile
+};
+
+}  // namespace
+
+struct vd3d_depth : DepthSettings {
   cudaStream_t stream = nullptr;
   std::string err;
   std::map<std::string, DTensor> w;    // weights by name
   std::map<std::string, DTensor> buf;  // activations by name
   uint64_t launches = 0;
-  int ph = 0, pw = 0, ntok = 0, npad = 0;
-  bool planned = false;
   // the per-image neck / head tails of a batch run on side streams (forked after the transformer, joined at the end)
-  cudaStream_t cur = nullptr;          // stream the helpers launch on (null: `stream`)
+  cudaStream_t cur = nullptr;          // stream the helpers launch on (null: `stream`; set by StreamScope only)
   cudaStream_t aux[8] = {};
   cudaEvent_t ev_fork = nullptr, ev_join[8] = {};
   bool owns_weights = true;  // clones share the weight tensors of their parent
@@ -122,7 +151,19 @@ int dfail(vd3d_depth* e, int code, const std::string& msg) {
   return code;
 }
 
-int get_buf(vd3d_depth* e, const std::string& name, size_t bytes, void** out, bool zero = false) {
+// the stream gemm, conv and get_buf's zeroing enqueue on
+cudaStream_t launch_stream(const vd3d_depth* e) { return e->cur ? e->cur : e->stream; }
+
+// Makes the helpers launch on `s` until it goes out of scope, on every return path (a per-image tail of forward_core)
+struct StreamScope {
+  vd3d_depth* e;
+  cudaStream_t prev;
+  StreamScope(vd3d_depth* e_, cudaStream_t s) : e(e_), prev(e_->cur) { e->cur = s; }
+  ~StreamScope() { e->cur = prev; }
+};
+
+template <typename T>
+int get_buf(vd3d_depth* e, const std::string& name, size_t bytes, T** out, bool zero = false) {
   DTensor& t = e->buf[name];
   if (t.bytes < bytes) {
     if (t.p) DCK(cudaFree(t.p));
@@ -130,8 +171,8 @@ int get_buf(vd3d_depth* e, const std::string& name, size_t bytes, void** out, bo
     t.bytes = bytes;
     zero = true;
   }
-  if (zero) DCK(cudaMemsetAsync(t.p, 0, t.bytes, e->cur ? e->cur : e->stream));
-  *out = t.p;
+  if (zero) DCK(cudaMemsetAsync(t.p, 0, t.bytes, launch_stream(e)));
+  *out = (T*)t.p;
   return VD3D_OK;
 }
 
@@ -143,6 +184,19 @@ int W(vd3d_depth* e, const std::string& name, const T** out, size_t min_count = 
     return dfail(e, VD3D_ERR_STATE, "weight tensor too small: " + name);
   *out = (const T*)it->second.p;
   return VD3D_OK;
+}
+
+// the f16 weight "<base>.w" (at least nw elements) and f32 bias "<base>.b" (nb) of a layer
+int layer(vd3d_depth* e, const std::string& base, const __half** w, size_t nw, const float** b, size_t nb) {
+  const int r = W(e, base + ".w", w, nw);
+  return r ? r : W(e, base + ".b", b, nb);
+}
+
+// a tensor or buffer name from a printf format with integer arguments, e.g. fmt("r%d.proj", i)
+std::string fmt(const char* f, int a, int b = 0) {
+  char nm[64];
+  snprintf(nm, sizeof nm, f, a, b);
+  return nm;
 }
 
 // f16 3-D tensor map: dims (d0 inner, d1, d2), strides in ELEMENTS for d1 and d2, box (64, b1, b2)
@@ -190,7 +244,7 @@ int gemm(vd3d_depth* e, const __half* A, int lda, const __half* B, int ldb, Gemm
   int r;
   if ((r = make_map(e, &ma, A, g.K, g.M, 1, lda, (uint64_t)lda * g.M, 128, 1))) return r;
   if ((r = make_map(e, &mb, B, g.K, g.N, 1, ldb, (uint64_t)ldb * g.N, bn, 1))) return r;
-  cudaError_t ce = launch_gemm(bn, ma, mb, g, (g.M + 127) / 128, 1, e->cur ? e->cur : e->stream);
+  cudaError_t ce = launch_gemm(bn, ma, mb, g, (g.M + 127) / 128, 1, launch_stream(e));
   if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("gemm launch: ") + cudaGetErrorString(ce));
   e->launches++;
   return VD3D_OK;
@@ -231,7 +285,7 @@ int conv(vd3d_depth* e, const __half* in, int H, int W, int cin, const __half* w
   if ((r = make_map(e, &ma, in, cin, W, H, pitch, (uint64_t)pitch * W, tw, th))) return r;
   if ((r = make_map(e, &mb, wt, g.K, g.N, 1, g.K, (uint64_t)g.K * g.N, bn, 1))) return r;
   int m_tiles = ((W + tw - 1) / tw) * ((H + th - 1) / th);
-  cudaStream_t s = e->cur ? e->cur : e->stream;
+  cudaStream_t s = launch_stream(e);
   cudaError_t ce = sr ? launch_gemm_sr(bn, ma, mb, g, m_tiles, s) : launch_gemm(bn, ma, mb, g, m_tiles, 1, s);
   if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("conv launch: ") + cudaGetErrorString(ce));
   e->launches++;
@@ -280,32 +334,32 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
   *out = nullptr;
   if (!load_encode()) return VD3D_ERR_CUDA;
   const vd3d_depth_config* cfg = &x->base;
-  const bool hybrid = x->family == VD3D_DEPTH_DPT_HYBRID;
-  // ZoeDepth's trunk, neck and fusion are dpt-beit-large-512's
-  const bool beit = x->family == VD3D_DEPTH_DPT_BEIT || x->family == VD3D_DEPTH_ZOEDEPTH;
-  const bool dpt = x->family == VD3D_DEPTH_DPT || hybrid || beit;
-  if ((x->family != VD3D_DEPTH_DA_V2 && !dpt) || (x->patch != 14 && x->patch != 16) ||
-      (x->resample != 2 && x->resample != 3) || !(x->ln_eps > 0.f) || cfg->heads < 1)
+  FamilyTraits t;
+  if (!family_traits(x->family, &t) || (x->patch != 14 && x->patch != 16) || (x->resample != 2 && x->resample != 3) ||
+      !(x->ln_eps > 0.f) || cfg->heads < 1)
     return VD3D_ERR_ARG;
   if ((x->head != VD3D_HEAD_RELATIVE && x->head != VD3D_HEAD_METRIC) || !(x->max_depth > 0.f) ||
-      !isfinite(x->max_depth) || (dpt && x->head == VD3D_HEAD_METRIC))
+      !isfinite(x->max_depth) || (t.readout && x->head == VD3D_HEAD_METRIC))
     return VD3D_ERR_ARG;
   if (cfg->hidden % 128 || cfg->hidden > 1024 || cfg->hidden / cfg->heads != 64 || cfg->fusion % 64 ||
       cfg->image_h % x->patch || cfg->image_w % x->patch)
     return VD3D_ERR_ARG;
   // every fusion x2 must land on the next map: sides that are multiples of 32.  DPT-Large and the hybrid reshape the
   // tokens as a square grid; BEiT takes the grid of the input (patch_height x patch_width), rectangular included
-  if (dpt && (cfg->image_h % 32 || cfg->image_w % 32 || (!beit && cfg->image_h != cfg->image_w))) return VD3D_ERR_ARG;
+  if (t.readout && (cfg->image_h % 32 || cfg->image_w % 32)) return VD3D_ERR_ARG;
+  if (t.square_grid && cfg->image_h != cfg->image_w) return VD3D_ERR_ARG;
   // the hybrid's fixed BiT front end: patch 16 (stage 3 is the S/16 token grid), stage maps of 256 / 512 channels
-  if (hybrid && (x->patch != 16 || cfg->neck[0] != 256 || cfg->neck[1] != 512)) return VD3D_ERR_ARG;
+  if (t.bit_front_end && (x->patch != 16 || cfg->neck[0] != 256 || cfg->neck[1] != 512)) return VD3D_ERR_ARG;
   // BEiT: the relative position bias table of the grid is staged in the attention's shared memory
-  if (beit && (x->patch != 16 || attention_bias_smem(cfg->image_h / 16, cfg->image_w / 16) > (size_t)kAttnSmemMax))
+  if (t.rel_pos_bias &&
+      (x->patch != 16 || attention_bias_smem(cfg->image_h / 16, cfg->image_w / 16) > (size_t)kAttnSmemMax))
     return VD3D_ERR_ARG;
   for (int c = 0; c < 3; ++c)
     if (!(x->std[c] != 0.f)) return VD3D_ERR_ARG;
   vd3d_depth* e = new vd3d_depth();
   e->cfg = *cfg;
   e->family = x->family;
+  e->traits = t;
   e->patch = x->patch;
   e->ln_eps = x->ln_eps;
   e->head = x->head;
@@ -314,6 +368,10 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
   for (int c = 0; c < 3; ++c) {
     e->pre.mean[c] = x->mean[c];
     e->pre.std[c] = x->std[c];
+  }
+  if (!t.readout) {  // Depth-Anything's processor (depth_engine.py processed_size); DPT's resizes to a fixed size
+    e->fit_h = e->fit_w = 518;
+    e->fit_multiple = 14;
   }
   e->stream = (cudaStream_t)stream;
   e->ph = cfg->image_h / x->patch;
@@ -329,7 +387,7 @@ int vd3d_depth_create_ex(const vd3d_depth_config_ex* x, void* stream, vd3d_depth
 }
 
 int vd3d_depth_set_fit(vd3d_depth* e, int fit_h, int fit_w, int multiple) {
-  if (!e || (e->family != VD3D_DEPTH_DPT_BEIT && e->family != VD3D_DEPTH_ZOEDEPTH) || (multiple != 0 && multiple != 32) || (multiple && (fit_h < 32 || fit_w < 32)))
+  if (!e || !e->traits.keep_aspect_fit || (multiple != 0 && multiple != 32) || (multiple && (fit_h < 32 || fit_w < 32)))
     return VD3D_ERR_ARG;
   e->fit_h = multiple ? fit_h : 0;
   e->fit_w = multiple ? fit_w : 0;
@@ -339,7 +397,7 @@ int vd3d_depth_set_fit(vd3d_depth* e, int fit_h, int fit_w, int multiple) {
 
 int vd3d_depth_set_zoe(vd3d_depth* e, int n_conf, int n_bins, const float* min_depth, const float* max_depth,
                        float min_temp, float max_temp, const int32_t* attractors, int cat_relative) {
-  if (!e || e->family != VD3D_DEPTH_ZOEDEPTH || (n_conf != 1 && n_conf != 2) || n_bins != kZoeBins || !min_depth ||
+  if (!e || !e->traits.zoe_head || (n_conf != 1 && n_conf != 2) || n_bins != kZoeBins || !min_depth ||
       !max_depth || !attractors || !(min_temp > 0.f) || !(max_temp > min_temp) || !isfinite(max_temp) ||
       (cat_relative != 0 && cat_relative != 1))
     return VD3D_ERR_ARG;
@@ -434,28 +492,10 @@ int vd3d_depth_profile_collect(vd3d_depth* e, double* total_ms, int* count, doub
 int vd3d_depth_clone(vd3d_depth* src, void* stream, vd3d_depth** out) {
   if (!src || !out) return VD3D_ERR_ARG;
   vd3d_depth* e = new vd3d_depth();
-  e->cfg = src->cfg;
-  e->family = src->family;
-  e->patch = src->patch;
-  e->ln_eps = src->ln_eps;
-  e->head = src->head;
-  e->max_depth = src->max_depth;
-  e->pre = src->pre;
-  e->fit_h = src->fit_h;
-  e->fit_w = src->fit_w;
-  e->fit_multiple = src->fit_multiple;
-  e->zoe_nc = src->zoe_nc;
-  e->zoe_cat = src->zoe_cat;
-  e->zoe_tmin = src->zoe_tmin;
-  e->zoe_tmax = src->zoe_tmax;
-  for (int j = 0; j < 4; ++j) e->zoe_na[j] = src->zoe_na[j];
+  static_cast<DepthSettings&>(*e) = *src;
   e->stream = (cudaStream_t)stream;
   e->w = src->w;
   e->owns_weights = false;
-  e->ph = src->ph;
-  e->pw = src->pw;
-  e->ntok = src->ntok;
-  e->npad = src->npad;
   *out = e;
   return VD3D_OK;
 }
@@ -709,18 +749,18 @@ constexpr int kMaxBatch = 8;
 // 1 after) and stride-2 1x1 shortcut on k_im2col_same's rows.  Block outputs are f16 NHWC.
 // Weights: "bit.stem.w" f32 [64, 147], "bit.s{st}.b{k}.c{1,2,3}.w" f16 ([mid, cin], [mid, 9 mid] tap-major, [out, mid]),
 // ".n{1,2,3}.g/.b" f32, first blocks ".ds.w" f16 [out, cin] and ".ds.g/.b"; "bit.stem.g/.b".
-// Outputs: stage1 f16 [(S/4)^2, 256] and stage2 f16 [(S/8)^2, 512] in the per-image buffers "bit.stage1.{b}" /
-// "bit.stage2.{b}" (neck inputs 0 and 1), stage3 f16 [(S/16)^2, 1024] in *stage3.  The image's launches run in order on
-// the engine stream with shared scratch buffers: "bit.y" / "bit.y2" (f32 conv outputs), "bit.t1" / "bit.t2" (f16 mids),
-// "bit.xa" / "bit.xb" (f16 block outputs), "bit.col" (im2col), "bit.gn0" / "bit.gn1" (GroupNorm partials).
+// Outputs: maps[0] = stage1 f16 [(S/4)^2, 256] and maps[1] = stage2 f16 [(S/8)^2, 512] in the per-image buffers
+// "bit.stage1.{b}" / "bit.stage2.{b}" (neck inputs 0 and 1), maps[2] = stage3 f16 [(S/16)^2, 1024] in a scratch
+// buffer (the patch projection's input).  The image's launches run in order on the engine stream with shared scratch
+// buffers: "bit.y" / "bit.y2" (f32 conv outputs), "bit.t1" / "bit.t2" (f16 mids), "bit.xa" / "bit.xb" (f16 block
+// outputs), "bit.col" (im2col), "bit.gn0" / "bit.gn1" (GroupNorm partials).
 constexpr int kBitDepths[3] = {3, 4, 9}, kBitWidths[3] = {256, 512, 1024};
 
-int bit_backbone(vd3d_depth* e, int b, const float* px, const __half** stage3) {
+int bit_backbone(vd3d_depth* e, int b, const float* px, const __half** maps) {
   cudaStream_t s = e->stream;
   const int S = e->cfg.image_h, S2 = S / 2, S4 = S / 4;
   const size_t big = (size_t)S2 * S2 * 64;  // the largest map: stem output = stage-1 output = stage-2 block 0's conv1
   int r;
-  char nm[64];
   void *y, *y2, *t1, *t2, *xa, *xb, *col, *p0, *p1, *st1, *st2;
   // im2col rows of the stride-2 3x3 convs (stages 2 and 3), rounded up to the GEMM's 128-row tiles
   const size_t col_el = std::max((size_t)round_up((S / 8) * (S / 8), 128) * 9 * 128,
@@ -732,16 +772,13 @@ int bit_backbone(vd3d_depth* e, int b, const float* px, const __half** stage3) {
       (r = get_buf(e, "bit.gn0", (size_t)kGnMaxChunks * 32 * sizeof(float2), &p0)) ||
       (r = get_buf(e, "bit.gn1", (size_t)kGnMaxChunks * 32 * sizeof(float2), &p1)))
     return r;
-  snprintf(nm, sizeof nm, "bit.stage1.%d", b);
-  if ((r = get_buf(e, nm, (size_t)S4 * S4 * 256 * 2, &st1))) return r;
-  snprintf(nm, sizeof nm, "bit.stage2.%d", b);
-  if ((r = get_buf(e, nm, (size_t)(S / 8) * (S / 8) * 512 * 2, &st2))) return r;
+  if ((r = get_buf(e, fmt("bit.stage1.%d", b), (size_t)S4 * S4 * 256 * 2, &st1)) ||
+      (r = get_buf(e, fmt("bit.stage2.%d", b), (size_t)(S / 8) * (S / 8) * 512 * 2, &st2)))
+    return r;
   auto gn_in = [&](const char* base, const float* map, const void* part, GnInput* out) -> int {
     int rr;
-    snprintf(nm, sizeof nm, "%s.g", base);
-    if ((rr = W(e, nm, &out->gamma))) return rr;
-    snprintf(nm, sizeof nm, "%s.b", base);
-    if ((rr = W(e, nm, &out->beta))) return rr;
+    if ((rr = W(e, std::string(base) + ".g", &out->gamma)) || (rr = W(e, std::string(base) + ".b", &out->beta)))
+      return rr;
     out->y = map;
     out->part = (const float2*)part;
     return VD3D_OK;
@@ -793,12 +830,8 @@ int bit_backbone(vd3d_depth* e, int b, const float* px, const __half** stage3) {
     for (int k = 0; k < kBitDepths[st]; ++k) {
       const bool first = k == 0, s2 = first && st > 0;
       const int Ho = s2 ? H / 2 : H, rows_in = H * H, rows = Ho * Ho;
-      char pfx[32];
-      snprintf(pfx, sizeof pfx, "bit.s%d.b%d", st, k);
-      auto wn = [&](const char* suffix) {
-        snprintf(nm, sizeof nm, "%s.%s", pfx, suffix);
-        return std::string(nm);
-      };
+      const std::string pfx = fmt("bit.s%d.b%d.", st, k);
+      auto wn = [&](const char* suffix) { return pfx + suffix; };
       // conv1 (1x1) + GN1 + ReLU at the input resolution
       if ((r = bconv(wn("c1.w"), BIT_1X1, x, H, cin, mid, (float*)y))) return r;
       if ((r = groupnorm(wn("n1").c_str(), (const float*)y, nullptr, nullptr, nullptr, 1, rows_in, mid, (__half*)t1)))
@@ -824,9 +857,25 @@ int bit_backbone(vd3d_depth* e, int b, const float* px, const __half** stage3) {
       cin = out_c;
     }
   }
-  *stage3 = x;
+  maps[0] = (const __half*)st1;
+  maps[1] = (const __half*)st2;
+  maps[2] = x;
   return VD3D_OK;
 }
+
+// an activation map of one image: NHWC f16 [h, w, C]
+struct Map {
+  const __half* p;
+  int h, w;
+};
+
+// the per-image tail of a batch (neck, fusion, head): the stream of its launches and the suffix of its activation
+// buffers ("#b" for image b when the tails of a batch run concurrently, else none)
+struct Tail {
+  cudaStream_t s;
+  std::string sfx;
+  std::string name(const std::string& base) const { return base + sfx; }
+};
 
 // ---- ZoeDepth's metric head (transformers 5.5 ZoeDepthMultipleMetricDepthEstimationHeads / ...MetricDepthEstimationHead)
 // on one image, on the stream of its tail.  bott: neck.convs[3]'s output f16 [bh bw, F]; fused[j]: the fusion outputs
@@ -842,11 +891,10 @@ size_t wlen(vd3d_depth* e, const char* name) {
   auto it = e->w.find(name);
   return it == e->w.end() ? 0 : it->second.bytes / 4;
 }
-int zoe_head(vd3d_depth* e, const std::string& sfx, const __half* bott, int bh, int bw, const __half* const* fused,
-             const int* fh, const int* fw, const __half* act, float* depth) {
-  cudaStream_t s = e->cur ? e->cur : e->stream;
+int zoe_head(vd3d_depth* e, const Tail& t, Map bott, const Map* fused, const __half* act, float* depth) {
+  cudaStream_t s = t.s;
   const int F = e->cfg.fusion, NC = e->zoe_nc, E = kZoeE, NB = kZoeBins, IH = e->cfg.image_h, IW = e->cfg.image_w;
-  const int nb3 = bh * bw;
+  const int bh = bott.h, bw = bott.w, nb3 = bh * bw;
   const int ms = (int)(wlen(e, "z.s1.b") / NC), mp = (int)wlen(e, "z.sp1.b");
   const int cin = 32 + e->zoe_cat + E;
   const int hid = (int)((wlen(e, "z.lb") / NC - 4) / (cin + 5));
@@ -854,15 +902,7 @@ int zoe_head(vd3d_depth* e, const std::string& sfx, const __half* bott, int bh, 
       wlen(e, "z.lb") != (size_t)NC * zoe_logbinom_floats(cin, hid))
     return dfail(e, VD3D_ERR_STATE, "ZoeDepth: metric head tensors missing or of unserved sizes");
   int r;
-  char nm[64];
-  auto buf = [&](const char* base, size_t bytes, void** p) { return get_buf(e, std::string(base) + sfx, bytes, p); };
-  auto wt = [&](const char* base, const __half** w16, const float** b32, size_t wn, size_t bn) {
-    snprintf(nm, sizeof nm, "%s.w", base);
-    int rr = W(e, nm, w16, wn);
-    if (rr) return rr;
-    snprintf(nm, sizeof nm, "%s.b", base);
-    return W(e, nm, b32, bn);
-  };
+  auto buf = [&](const char* base, size_t bytes, void** p) { return get_buf(e, t.name(base), bytes, p); };
   // 1x1 layer on k_umma_gemm: out = act(A W^T + b) [+ res], f16 (or f32 when out32)
   auto lin = [&](const __half* A, int M, int K, const __half* w, const float* bias, int N, int relu, void* out,
                  bool out32, const __half* res) {
@@ -878,7 +918,7 @@ int zoe_head(vd3d_depth* e, const std::string& sfx, const __half* bott, int bh, 
   };
   const size_t R3 = round_up(nb3, 128);
   void *zb16, *zb32, *route, *logits, *sh, *seed, *t1, *emb[2], *bins[2], *up, *x, *hb;
-  const size_t Mmax = (size_t)round_up(fh[3] * fw[3], 128);
+  const size_t Mmax = (size_t)round_up(fused[3].h * fused[3].w, 128);
   if ((r = buf("z.zb16", R3 * F * 2, &zb16)) || (r = buf("z.zb32", R3 * F * 4, &zb32)) ||
       (r = buf("z.route", 16, &route)) || (r = buf("z.logits", 16, &logits)) ||
       (r = buf("z.sh", R3 * NC * ms * 2, &sh)) || (r = buf("z.seed", R3 * NC * NB * 4, &seed)) ||
@@ -891,8 +931,9 @@ int zoe_head(vd3d_depth* e, const std::string& sfx, const __half* bott, int bh, 
   const float* b32;
   // ---- bottleneck conv2 (f16 for the GEMMs, f32 for the router), router, seed regressor, seed projector ----
   int sp = e->span_begin("zoe.bottleneck", s);
-  if ((r = wt("z.bt", &w16, &b32, (size_t)F * F, F)) || (r = lin(bott, nb3, F, w16, b32, F, 0, zb16, false, nullptr)) ||
-      (r = lin(bott, nb3, F, w16, b32, F, 0, zb32, true, nullptr)))
+  if ((r = layer(e, "z.bt", &w16, (size_t)F * F, &b32, F)) ||
+      (r = lin(bott.p, nb3, F, w16, b32, F, 0, zb16, false, nullptr)) ||
+      (r = lin(bott.p, nb3, F, w16, b32, F, 0, zb32, true, nullptr)))
     return r;
   e->span_end(sp, s);
   sp = e->span_begin("zoe.router", s);
@@ -908,45 +949,41 @@ int zoe_head(vd3d_depth* e, const std::string& sfx, const __half* bott, int bh, 
   }
   e->span_end(sp, s);
   sp = e->span_begin("zoe.seed", s);
-  if ((r = wt("z.s1", &w16, &b32, (size_t)NC * ms * F, NC * ms)) ||
+  if ((r = layer(e, "z.s1", &w16, (size_t)NC * ms * F, &b32, NC * ms)) ||
       (r = lin((const __half*)zb16, nb3, F, w16, b32, NC * ms, 1, sh, false, nullptr)) ||
-      (r = wt("z.s2", &w16, &b32, (size_t)NC * NB * NC * ms, NC * NB)) ||
+      (r = layer(e, "z.s2", &w16, (size_t)NC * NB * NC * ms, &b32, NC * NB)) ||
       (r = lin((const __half*)sh, nb3, NC * ms, w16, b32, NC * NB, 0, seed, true, nullptr)) ||
-      (r = wt("z.sp1", &w16, &b32, (size_t)mp * F, mp)) ||
+      (r = layer(e, "z.sp1", &w16, (size_t)mp * F, &b32, mp)) ||
       (r = lin((const __half*)zb16, nb3, F, w16, b32, mp, 1, t1, false, nullptr)) ||
-      (r = wt("z.sp2", &w16, &b32, (size_t)E * mp, E)) ||
+      (r = layer(e, "z.sp2", &w16, (size_t)E * mp, &b32, E)) ||
       (r = lin((const __half*)t1, nb3, mp, w16, b32, E, 0, emb[1], false, nullptr)))
     return r;
   e->span_end(sp, s);
   // ---- four attractor layers, coarse to fine ----
   int ph_ = bh, pw_ = bw;
   for (int j = 0; j < 4; ++j) {
-    const int H = fh[j], Wd = fw[j], M = H * Wd;
+    const int H = fused[j].h, Wd = fused[j].w, M = H * Wd;
     void *cur = emb[j & 1], *prev = emb[(j + 1) & 1];
-    char base[16];
     sp = e->span_begin("zoe.proj", s);
-    snprintf(base, sizeof base, "z.p%d.1", j);
-    if ((r = wt(base, &w16, &b32, (size_t)mp * F, mp)) || (r = lin(fused[j], M, F, w16, b32, mp, 1, t1, false, nullptr)))
+    if ((r = layer(e, fmt("z.p%d.1", j), &w16, (size_t)mp * F, &b32, mp)) ||
+        (r = lin(fused[j].p, M, F, w16, b32, mp, 1, t1, false, nullptr)))
       return r;
     launch_upsample_ac((const __half*)prev, ph_, pw_, E, (__half*)up, H, Wd, s);
     e->launches++;
-    snprintf(base, sizeof base, "z.p%d.2", j);
-    if ((r = wt(base, &w16, &b32, (size_t)E * mp, E)) ||
+    if ((r = layer(e, fmt("z.p%d.2", j), &w16, (size_t)E * mp, &b32, E)) ||
         (r = lin((const __half*)t1, M, mp, w16, b32, E, 0, x, false, (const __half*)up)) ||
         (r = lin((const __half*)t1, M, mp, w16, b32, E, 0, cur, false, nullptr)))
       return r;
     e->span_end(sp, s);
     sp = e->span_begin("zoe.attractor", s);
-    snprintf(base, sizeof base, "z.a%d.1", j);
-    if ((r = wt(base, &w16, &b32, (size_t)NC * E * E, NC * E)) ||
+    if ((r = layer(e, fmt("z.a%d.1", j), &w16, (size_t)NC * E * E, &b32, NC * E)) ||
         (r = lin((const __half*)x, M, E, w16, b32, NC * E, 1, hb, false, nullptr)))
       return r;
     const float *w2, *b2;
     const int na = e->zoe_na[j];
-    snprintf(nm, sizeof nm, "z.a%d.2.w", j);
-    if ((r = W(e, nm, &w2, (size_t)NC * na * E))) return r;
-    snprintf(nm, sizeof nm, "z.a%d.2.b", j);
-    if ((r = W(e, nm, &b2, (size_t)NC * na))) return r;
+    if ((r = W(e, fmt("z.a%d.2.w", j), &w2, (size_t)NC * na * E)) ||
+        (r = W(e, fmt("z.a%d.2.b", j), &b2, (size_t)NC * na)))
+      return r;
     if (j == 0)
       launch_zoe_attractor((const __half*)hb, NC * E, E, w2, b2, na, (const float*)seed, NC * NB, NB, 1, bh, bw,
                            (float*)bins[0], H, Wd, (const int*)route, s);
@@ -971,471 +1008,456 @@ int zoe_head(vd3d_depth* e, const std::string& sfx, const __half* bott, int bh, 
   return VD3D_OK;
 }
 
-// B images through the network in one pass.  The token-wise stages (LayerNorm, QKV / proj / fc1 / fc2 GEMMs) see one
-// matrix of (B-1)*NP + NT rows -- image b owns rows [b*NP, b*NP + NT), NP = NT rounded up to the 128-row tile -- so the
-// GEMMs run at 3-4x the rows of one frame (the reference batches too: core/render_depth.py:1113-1119); attention runs
-// with grid.y = B * heads; patch embedding, taps, neck and head stay per image (their maps are per-image 2-D tensors).
-// px_dev / depth_dev: DEVICE pointers, f32 [3, image_h, image_w] in, f32 [image_h, image_w] out.
-int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const* depth_dev) {
-  if (B < 1 || B > kMaxBatch) return dfail(e, VD3D_ERR_ARG, "batch must be in [1, 8]");
-  e->cur = nullptr;  // (an earlier call may have failed inside its forked section)
-  const vd3d_depth_config& c = e->cfg;
-  cudaStream_t s = e->stream;
-  const int D = c.hidden, L = c.layers, Hh = c.heads, F = c.fusion;
-  const int ph = e->ph, pw = e->pw, NT = e->ntok, NP = e->npad, NPATCH = ph * pw;
-  const int IH = c.image_h, IW = c.image_w;
-  const int P = e->patch;
-  const int KPE = round_up(3 * P * P, 16);  // 592 for patch 14 (588 + zero columns), 768 for 16
-  const bool hybrid = e->family == VD3D_DEPTH_DPT_HYBRID, zoe = e->family == VD3D_DEPTH_ZOEDEPTH;
-  const bool beit = e->family == VD3D_DEPTH_DPT_BEIT || zoe;
-  if (zoe && !e->zoe_nc) return dfail(e, VD3D_ERR_STATE, "ZoeDepth: the metric head's settings are not set (vd3d_depth_set_zoe)");
-  // raw taps and the project readout (DPT-Large and the hybrid without LayerScale: ls1 / ls2 of ones)
-  const bool dpt = e->family == VD3D_DEPTH_DPT || hybrid || beit;
-  int r;
-  char nm[96];
-  // ---- buffers ----
-  void *x, *xn, *q, *k, *vt, *attn, *hb, *ape;
-  const int MT = (B - 1) * NP + NT;  // rows of the stacked token matrix
-  if ((r = get_buf(e, "x", (size_t)B * NP * D * 4, &x))) return r;
-  if ((r = get_buf(e, "xn", (size_t)B * NP * D * 2, &xn))) return r;
-  if ((r = get_buf(e, "q", (size_t)B * Hh * NP * 64 * 2, &q))) return r;
-  if ((r = get_buf(e, "k", (size_t)B * Hh * NP * 64 * 2, &k))) return r;
-  if ((r = get_buf(e, "vt", (size_t)B * Hh * 64 * NP * 2, &vt))) return r;
-  if ((r = get_buf(e, "attn", (size_t)B * NP * D * 2, &attn))) return r;
-  if ((r = get_buf(e, "h", (size_t)B * NP * 4 * D * 2, &hb))) return r;
-  if (!hybrid && (r = get_buf(e, "ape", (size_t)NPATCH * KPE * 2, &ape))) return r;
+// One forward of B images (forward_core).  The token-wise stages (LayerNorm, QKV / proj / fc1 / fc2 GEMMs) see one
+// matrix of MT = (B-1)*NP + NT rows -- image b owns rows [b*NP, b*NP + NT), NP = NT rounded up to the 128-row tile --
+// so the GEMMs run at 3-4x the rows of one frame (the reference batches too: core/render_depth.py:1113-1119);
+// attention runs with grid.y = B * heads; patch embedding, taps, neck and head stay per image (their maps are
+// per-image 2-D tensors).
+struct Fwd {
+  int B, MT;
+  float* x;                            // residual stream f32 [B*NP, D]
+  __half *xn, *q, *k, *vt, *attn, *h;  // LayerNorm output, per-head q / k / v^T, attention output, fc1 output
+};
 
-  // ---- patch embedding + CLS + position embeddings ----
-  const int sp_embed = hybrid ? -1 : e->span_begin("embed", s);  // the hybrid's backbone has spans of its own
-  // DPT-Hybrid: the BiT stage-3 map [NPATCH, 1024] takes the place of the patch matrix (a 1x1 projection with bias)
-  const int KE = hybrid ? 1024 : KPE;
+// Patch embedding + CLS + position embeddings of every image into its rows of x.  DPT-Hybrid: the BiT stage-3 map
+// [NPATCH, 1024] takes the place of the patch matrix (a 1x1 projection with bias), and the stage-1 / stage-2 maps are
+// the image's neck inputs 0 and 1 (in[b][0..1]).
+int embed(vd3d_depth* e, const Fwd& f, const float* const* px_dev, const __half* (*in)[4]) {
+  cudaStream_t s = e->stream;
+  const bool bit = e->traits.bit_front_end;
+  const int D = e->cfg.hidden, P = e->patch, NT = e->ntok, NP = e->npad, NPATCH = e->ph * e->pw;
+  const int KPE = round_up(3 * P * P, 16);  // 592 for patch 14 (588 + zero columns), 768 for 16
+  const int KE = bit ? 1024 : KPE;
+  __half* ape = nullptr;
+  int r;
+  if (!bit && (r = get_buf(e, "ape", (size_t)NPATCH * KPE * 2, &ape))) return r;
+  const int sp_embed = bit ? -1 : e->span_begin("embed", s);  // the hybrid's backbone has spans of its own
   const __half* pe_w;
   const float *pe_b, *cls, *pos;
-  if ((r = W(e, "pe.w", &pe_w, (size_t)D * KE)) || (r = W(e, "pe.b", &pe_b, D)) || (r = W(e, "cls", &cls, D)) ||
+  if ((r = layer(e, "pe", &pe_w, (size_t)D * KE, &pe_b, D)) || (r = W(e, "cls", &cls, D)) ||
       (r = W(e, "pos", &pos, (size_t)NT * D)))
     return r;
-  for (int b = 0; b < B; ++b) {
-    float* xb = (float*)x + (size_t)b * NP * D;
-    const __half* a_emb = (const __half*)ape;
-    if (hybrid) {
-      if ((r = bit_backbone(e, b, px_dev[b], &a_emb))) return r;
+  for (int b = 0; b < f.B; ++b) {
+    float* xb = f.x + (size_t)b * NP * D;
+    const __half* a = ape;
+    if (bit) {
+      const __half* maps[3];
+      if ((r = bit_backbone(e, b, px_dev[b], maps))) return r;
+      in[b][0] = maps[0];
+      in[b][1] = maps[1];
+      a = maps[2];
     } else {
-      launch_patch_im2col(px_dev[b], IH, IW, ph, pw, (__half*)ape, KPE, P, s);
+      launch_patch_im2col(px_dev[b], e->cfg.image_h, e->cfg.image_w, e->ph, e->pw, ape, KPE, P, s);
       e->launches++;
     }
-    const int sp_proj = hybrid ? e->span_begin("bit.proj", s) : -1;
+    const int sp_proj = bit ? e->span_begin("bit.proj", s) : -1;
     GemmArgs g = base_args(NPATCH, D, KE, EPI_PATCH);
     g.out_f32 = xb;
     g.bias = pe_b;
     g.pos = pos;
     g.ldc = D;
-    if ((r = gemm(e, a_emb, KE, pe_w, KE, g))) return r;
+    if ((r = gemm(e, a, KE, pe_w, KE, g))) return r;
     launch_set_cls(xb, cls, pos, D, s);
     e->launches++;
     e->span_end(sp_proj, s);
     // rows [NT, NP) of every image but the last take part in the stacked GEMMs: keep them at zero so that they stay
     // finite from frame to frame (they are never read as keys / values: the attention tensor maps end at NT)
-    if (b + 1 < B) DCK(cudaMemsetAsync(xb + (size_t)NT * D, 0, (size_t)(NP - NT) * D * 4, s));
+    if (b + 1 < f.B) DCK(cudaMemsetAsync(xb + (size_t)NT * D, 0, (size_t)(NP - NT) * D * 4, s));
   }
-
   e->span_end(sp_embed, s);
-  // ---- transformer blocks ----
-  int tap_idx = hybrid ? 2 : 0;  // the hybrid's neck inputs 0 and 1 are BiT stages, not ViT taps
-  for (int l = 0; l < L; ++l) {
-    const float *g1, *b1, *g2, *b2, *bqkv, *bo, *ls1, *bf1, *bf2, *ls2;
-    const __half *wqkv, *wo, *wf1, *wf2;
-    auto nmf = [&](const char* suffix) {
-      snprintf(nm, sizeof nm, "l%d.%s", l, suffix);
-      return std::string(nm);
-    };
-    if ((r = W(e, nmf("ln1.g"), &g1, D)) || (r = W(e, nmf("ln1.b"), &b1, D)) || (r = W(e, nmf("ln2.g"), &g2, D)) ||
-        (r = W(e, nmf("ln2.b"), &b2, D)) || (r = W(e, nmf("qkv.w"), &wqkv, (size_t)3 * D * D)) ||
-        (r = W(e, nmf("qkv.b"), &bqkv, 3 * D)) || (r = W(e, nmf("proj.w"), &wo, (size_t)D * D)) ||
-        (r = W(e, nmf("proj.b"), &bo, D)) || (r = W(e, nmf("ls1"), &ls1, D)) ||
-        (r = W(e, nmf("fc1.w"), &wf1, (size_t)4 * D * D)) || (r = W(e, nmf("fc1.b"), &bf1, 4 * D)) ||
-        (r = W(e, nmf("fc2.w"), &wf2, (size_t)4 * D * D)) || (r = W(e, nmf("fc2.b"), &bf2, D)) ||
-        (r = W(e, nmf("ls2"), &ls2, D)))
+  return VD3D_OK;
+}
+
+// Encoder layer l on the stacked token matrix: x += ls1 * proj(attn(LN1(x))); x += ls2 * fc2(GELU(fc1(LN2(x)))).
+// BEiT adds the layer's relative position bias to the attention scores.
+int encoder_layer(vd3d_depth* e, const Fwd& f, int l) {
+  cudaStream_t s = e->stream;
+  const int D = e->cfg.hidden, Hh = e->cfg.heads, MT = f.MT, NT = e->ntok, NP = e->npad;
+  const float *g1, *b1, *g2, *b2, *bqkv, *bo, *ls1, *bf1, *bf2, *ls2;
+  const __half *wqkv, *wo, *wf1, *wf2;
+  auto nmf = [&](const char* suffix) { return fmt("l%d.", l) + suffix; };
+  int r;
+  if ((r = W(e, nmf("ln1.g"), &g1, D)) || (r = W(e, nmf("ln1.b"), &b1, D)) || (r = W(e, nmf("ln2.g"), &g2, D)) ||
+      (r = W(e, nmf("ln2.b"), &b2, D)) || (r = layer(e, nmf("qkv"), &wqkv, (size_t)3 * D * D, &bqkv, 3 * D)) ||
+      (r = layer(e, nmf("proj"), &wo, (size_t)D * D, &bo, D)) || (r = W(e, nmf("ls1"), &ls1, D)) ||
+      (r = layer(e, nmf("fc1"), &wf1, (size_t)4 * D * D, &bf1, 4 * D)) ||
+      (r = layer(e, nmf("fc2"), &wf2, (size_t)4 * D * D, &bf2, D)) || (r = W(e, nmf("ls2"), &ls2, D)))
+    return r;
+  // BEiT: the layer's relative position bias, one table per head for this grid
+  const float* rpb = nullptr;
+  if (e->traits.rel_pos_bias &&
+      (r = W(e, nmf("rpb"), &rpb, (size_t)Hh * ((2 * e->ph - 1) * (2 * e->pw - 1) + 3))))
+    return r;
+  int sp = e->span_begin("ln", s);
+  launch_layernorm(f.x, MT, D, g1, b1, f.xn, 0, e->ln_eps, s);
+  e->launches++;
+  e->span_end(sp, s);
+  sp = e->span_begin("qkv", s);
+  GemmArgs g = base_args(MT, 3 * D, D, EPI_QKV);
+  g.bias = bqkv;
+  g.q = f.q;
+  g.k = f.k;
+  g.vt = f.vt;
+  g.heads = Hh;
+  g.npad = NP;
+  g.dmodel = D;
+  g.qscale = 0.125f;  // 1/sqrt(64), exact in f16
+  if ((r = gemm(e, f.xn, D, wqkv, D, g))) return r;
+  e->span_end(sp, s);
+  // fused wgmma attention: scores and probabilities stay in registers
+  sp = e->span_begin("attn", s);
+  CUtensorMap mq, mk, mv;
+  if ((r = make_map(e, &mq, f.q, 64, NT, f.B * Hh, 64, (uint64_t)NP * 64, kAttnRows, 1)) ||
+      (r = make_map(e, &mk, f.k, 64, NT, f.B * Hh, 64, (uint64_t)NP * 64, 128, 1)) ||
+      (r = make_map(e, &mv, f.vt, NT, 64, f.B * Hh, NP, (uint64_t)64 * NP, 64, 1)))
+    return r;
+  cudaError_t ce = launch_attention(mq, mk, mv, NT, D, f.attn, Hh, f.B, NP, s, rpb, e->pw);
+  if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("attention launch: ") + cudaGetErrorString(ce));
+  e->launches++;
+  e->span_end(sp, s);
+  sp = e->span_begin("proj", s);
+  g = base_args(MT, D, D, EPI_RESID_LS);
+  g.out_f32 = f.x;
+  g.bias = bo;
+  g.ls = ls1;
+  g.ldc = D;
+  if ((r = gemm(e, f.attn, D, wo, D, g))) return r;
+  e->span_end(sp, s);
+  sp = e->span_begin("ln", s);
+  launch_layernorm(f.x, MT, D, g2, b2, f.xn, 0, e->ln_eps, s);
+  e->launches++;
+  e->span_end(sp, s);
+  sp = e->span_begin("fc1", s);
+  g = base_args(MT, 4 * D, D, EPI_F16);
+  g.out_f16 = f.h;
+  g.bias = bf1;
+  g.act = 1;
+  g.ldc = 4 * D;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (e->prof) {
+    cudaEventCreate(&e0);
+    cudaEventCreate(&e1);
+    cudaEventRecord(e0, s);
+    e->prof_rows += MT;
+  }
+  if ((r = gemm(e, f.xn, D, wf1, D, g))) return r;
+  if (e->prof) {
+    cudaEventRecord(e1, s);
+    e->prof_ev.push_back(e0);
+    e->prof_ev.push_back(e1);
+  }
+  e->span_end(sp, s);
+  sp = e->span_begin("fc2", s);
+  g = base_args(MT, D, 4 * D, EPI_RESID_LS);
+  g.out_f32 = f.x;
+  g.bias = bf2;
+  g.ls = ls2;
+  g.ldc = D;
+  if ((r = gemm(e, f.h, 4 * D, wf2, 4 * D, g))) return r;
+  e->span_end(sp, s);
+  return VD3D_OK;
+}
+
+// Neck input i of every image (in[b][i]), taken after its encoder layer.  DPT (readout): the raw residual stream
+// (hidden_states[l + 1]), then the project readout over the patch rows of all images in one GEMM,
+// GELU(W_t tok + (W_c cls_b + bias)), the CLS term computed once per image; image b's rows start at b * NPATCH.
+// Depth-Anything: the backbone output, final LayerNorm applied (apply_layernorm=True) per image, CLS dropped.
+int take_tap(vd3d_depth* e, const Fwd& f, int i, const __half* (*in)[4]) {
+  cudaStream_t s = e->stream;
+  const int D = e->cfg.hidden, NP = e->npad, NPATCH = e->ph * e->pw;
+  int r;
+  if (e->traits.readout) {
+    __half *tp, *ro;
+    float* cb;
+    const __half *wt, *wc;
+    const float* rb;
+    const int MR = f.B * NPATCH;
+    if ((r = W(e, fmt("ro%d.wt", i), &wt, (size_t)D * D)) || (r = W(e, fmt("ro%d.wc", i), &wc, (size_t)D * D)) ||
+        (r = W(e, fmt("ro%d.b", i), &rb, D)) ||
+        (r = get_buf(e, fmt("tap%d", i), (size_t)round_up(MR, 128) * D * 2, &tp)) ||
+        (r = get_buf(e, fmt("ro%d.c", i), (size_t)f.B * D * 4, &cb)) ||
+        (r = get_buf(e, fmt("ro%d", i), (size_t)round_up(MR, 128) * D * 2, &ro)))
       return r;
-    // BEiT: the layer's relative position bias, one table per head for this grid
-    const float* rpb = nullptr;
-    if (beit && (r = W(e, nmf("rpb"), &rpb, (size_t)Hh * ((2 * ph - 1) * (2 * pw - 1) + 3)))) return r;
-    int sp_ = e->span_begin("ln", s);
-    launch_layernorm((const float*)x, MT, D, g1, b1, (__half*)xn, 0, e->ln_eps, s);
-    e->span_end(sp_, s);
-    sp_ = e->span_begin("qkv", s);
-    {
-      GemmArgs g = base_args(MT, 3 * D, D, EPI_QKV);
-      g.bias = bqkv;
-      g.q = (__half*)q;
-      g.k = (__half*)k;
-      g.vt = (__half*)vt;
-      g.heads = Hh;
-      g.npad = NP;
-      g.dmodel = D;
-      g.qscale = 0.125f;  // 1/sqrt(64), exact in f16
-      if ((r = gemm(e, (const __half*)xn, D, wqkv, D, g))) return r;
-    }
-    e->span_end(sp_, s);
-    sp_ = e->span_begin("attn", s);
-    {  // fused wgmma attention: scores and probabilities stay in registers
-      CUtensorMap mq, mk, mv;
-      if ((r = make_map(e, &mq, q, 64, NT, B * Hh, 64, (uint64_t)NP * 64, kAttnRows, 1))) return r;
-      if ((r = make_map(e, &mk, k, 64, NT, B * Hh, 64, (uint64_t)NP * 64, 128, 1))) return r;
-      if ((r = make_map(e, &mv, vt, NT, 64, B * Hh, NP, (uint64_t)64 * NP, 64, 1))) return r;
-      cudaError_t ce = launch_attention(mq, mk, mv, NT, D, (__half*)attn, Hh, B, NP, s, rpb, pw);
-      if (ce != cudaSuccess) return dfail(e, VD3D_ERR_CUDA, std::string("attention launch: ") + cudaGetErrorString(ce));
+    launch_tap_f16(f.x, NP, NPATCH, D, f.B, tp, s);
+    e->launches++;
+    launch_readout_cls(f.x, NP, D, f.B, wc, rb, D, cb, s);
+    e->launches++;
+    GemmArgs g = base_args(MR, D, D, EPI_READOUT);
+    g.out_f16 = ro;
+    g.img_bias = cb;
+    g.npad = NPATCH;
+    g.ldc = D;
+    if ((r = gemm(e, tp, D, wt, D, g))) return r;
+    for (int b = 0; b < f.B; ++b) in[b][i] = ro + (size_t)b * NPATCH * D;
+    return VD3D_OK;
+  }
+  const float *ng, *nb;
+  if ((r = W(e, "norm.g", &ng, D)) || (r = W(e, "norm.b", &nb, D))) return r;
+  for (int b = 0; b < f.B; ++b) {
+    __half* tp;
+    if ((r = get_buf(e, fmt("tap%d.%d", i, b), (size_t)round_up(NPATCH, 128) * D * 2, &tp))) return r;
+    launch_layernorm(f.x + (size_t)b * NP * D, NPATCH, D, ng, nb, tp, 1, e->ln_eps, s);
+    e->launches++;
+    in[b][i] = tp;
+  }
+  return VD3D_OK;
+}
+
+// Reassemble stage i of one image: the 1x1 projection of its token rows tok [NPATCH, D] to CP channels, then the
+// resample to the stage's scale: ConvTranspose2d (kernel = stride = 4 / 2), none, or Conv2d (3x3, stride 2, pad 1)
+int reassemble(vd3d_depth* e, const Tail& t, int i, const __half* tok, Map* out) {
+  const int D = e->cfg.hidden, ph = e->ph, pw = e->pw, NPATCH = ph * pw, CP = round_up(e->cfg.neck[i], 64);
+  const __half* wp;
+  const float* bp;
+  __half *rp, *rs;
+  int r;
+  if ((r = layer(e, fmt("r%d.proj", i), &wp, (size_t)CP * D, &bp, CP)) ||
+      (r = get_buf(e, t.name(fmt("r%d.p", i)), (size_t)round_up(NPATCH, 128) * CP * 2, &rp)))
+    return r;
+  GemmArgs g = base_args(NPATCH, CP, D, EPI_F16);
+  g.out_f16 = rp;
+  g.bias = bp;
+  g.ldc = CP;
+  if ((r = gemm(e, tok, D, wp, D, g))) return r;
+  if (i == 2) {
+    *out = {rp, ph, pw};
+    return VD3D_OK;
+  }
+  if (i < 2) {
+    const int kk = (i == 0) ? 4 : 2;
+    const __half* uw;
+    const float* ub;
+    if ((r = layer(e, fmt("r%d.up", i), &uw, (size_t)kk * kk * CP * CP, &ub, (size_t)kk * kk * CP)) ||
+        (r = get_buf(e, t.name(fmt("r%d.s", i)), (size_t)ph * kk * pw * kk * CP * 2, &rs)))
+      return r;
+    g = base_args(NPATCH, kk * kk * CP, CP, EPI_CONVT);
+    g.out_f16 = rs;
+    g.bias = ub;
+    g.ct_k = kk;
+    g.ct_cout = CP;
+    g.ct_w = pw;
+    if ((r = gemm(e, rp, CP, uw, CP, g))) return r;
+    *out = {rs, ph * kk, pw * kk};
+    return VD3D_OK;
+  }
+  const __half* dw;
+  const float* db;
+  const int oh = (ph - 1) / 2 + 1, ow = (pw - 1) / 2 + 1;
+  __half* col;
+  if ((r = layer(e, "r3.down", &dw, (size_t)CP * 9 * CP, &db, CP)) ||
+      (r = get_buf(e, t.name("r3.col"), (size_t)round_up(oh * ow, 128) * 9 * CP * 2, &col)))
+    return r;
+  launch_im2col_s2(rp, ph, pw, CP, CP, col, oh, ow, t.s);
+  e->launches++;
+  if ((r = get_buf(e, t.name("r3.s"), (size_t)round_up(oh * ow, 128) * CP * 2, &rs))) return r;
+  g = base_args(oh * ow, CP, 9 * CP, EPI_F16);
+  g.out_f16 = rs;
+  g.bias = db;
+  g.ldc = CP;
+  if ((r = gemm(e, col, 9 * CP, dw, 9 * CP, g))) return r;
+  *out = {rs, oh, ow};
+  return VD3D_OK;
+}
+
+// The neck of one image: each input reassembled to its scale (DPT-Hybrid's BiT stage maps, inputs 0 and 1, are at
+// theirs already), then the 3x3 conv to the fusion width -> feat[i] ("f{i}")
+int neck(vd3d_depth* e, const Tail& t, const __half* const* in, Map* feat) {
+  const int F = e->cfg.fusion;
+  int r;
+  for (int i = 0; i < 4; ++i) {
+    const int CP = round_up(e->cfg.neck[i], 64);
+    Map m;
+    if (e->traits.bit_front_end && i < 2)
+      m = {in[i], e->ph * (4 >> i), e->pw * (4 >> i)};
+    else if ((r = reassemble(e, t, i, in[i], &m)))
+      return r;
+    const __half* cw;
+    __half* out;
+    if ((r = W(e, fmt("n%d.conv.w", i), &cw, (size_t)F * 9 * CP)) ||
+        (r = get_buf(e, t.name(fmt("f%d", i)), (size_t)m.h * m.w * F * 2, &out)))
+      return r;
+    GemmArgs g = base_args(0, F, 0, EPI_F16);
+    g.out_f16 = out;
+    g.ldc = F;
+    if ((r = conv(e, m.p, m.h, m.w, CP, cw, true, g))) return r;
+    feat[i] = {out, m.h, m.w};
+  }
+  return VD3D_OK;
+}
+
+// One ResidualConvUnit ("rl1" / "rl2") of fusion block j on an H x Wd map: out = conv2(relu(conv1(x_relu))) + res,
+// x_relu = relu(x) computed by the caller; mid receives conv1's output
+int residual_unit(vd3d_depth* e, int j, const char* unit, const __half* x_relu, const __half* res, int H, int Wd,
+                  __half* mid, __half* out) {
+  const int F = e->cfg.fusion;
+  const __half *w1, *w2;
+  const float *b1, *b2;
+  const std::string base = fmt("f%d.", j) + unit;
+  int r;
+  if ((r = layer(e, base + ".c1", &w1, (size_t)F * 9 * F, &b1, F)) ||
+      (r = layer(e, base + ".c2", &w2, (size_t)F * 9 * F, &b2, F)))
+    return r;
+  GemmArgs g1 = base_args(0, F, 0, EPI_F16);
+  g1.out_f16 = mid;
+  g1.bias = b1;
+  g1.act = 2;
+  g1.ldc = F;
+  if ((r = conv(e, x_relu, H, Wd, F, w1, true, g1))) return r;
+  GemmArgs g2 = base_args(0, F, 0, EPI_F16);
+  g2.out_f16 = out;
+  g2.bias = b2;
+  g2.res_f16 = res;
+  g2.ldc = F;
+  return conv(e, mid, H, Wd, F, w2, true, g2);
+}
+
+// The fusion stage of one image, coarsest first: block j takes feat[3 - j] (plus, after the first block, the previous
+// block's output), upsamples to the next map's size (x2 after the last block) and projects (1x1) -> fused[j]
+int fusion(vd3d_depth* e, const Tail& t, const Map* feat, Map* fused) {
+  cudaStream_t s = t.s;
+  const int F = e->cfg.fusion;
+  int r;
+  for (int j = 0; j < 4; ++j) {
+    const Map& in = feat[3 - j];
+    const int Hc = in.h, Wc = in.w;
+    const size_t n = (size_t)Hc * Wc * F;
+    __half *t_relu, *t_mid, *hraw, *hrelu, *yraw, *up, *prj;
+    if ((r = get_buf(e, t.name("fu.relu"), n * 2, &t_relu)) || (r = get_buf(e, t.name("fu.mid"), n * 2, &t_mid)) ||
+        (r = get_buf(e, t.name("fu.h"), n * 2, &hraw)) || (r = get_buf(e, t.name("fu.hrelu"), n * 2, &hrelu)) ||
+        (r = get_buf(e, t.name("fu.y"), n * 2, &yraw)))
+      return r;
+    const __half* h = in.p;  // residual_layer2's input; hrelu: its ReLU
+    if (j == 0) {
+      launch_relu_f16(in.p, hrelu, n, s);
       e->launches++;
+    } else {  // h = fused + residual_layer1(feat)
+      launch_relu_f16(in.p, t_relu, n, s);
+      e->launches++;
+      if ((r = residual_unit(e, j, "rl1", t_relu, in.p, Hc, Wc, t_mid, yraw))) return r;
+      launch_add_relu_f16(fused[j - 1].p, yraw, hraw, hrelu, n, s);
+      e->launches++;
+      h = hraw;
     }
-    e->span_end(sp_, s);
-    sp_ = e->span_begin("proj", s);
-    {
-      GemmArgs g = base_args(MT, D, D, EPI_RESID_LS);
-      g.out_f32 = (float*)x;
-      g.bias = bo;
-      g.ls = ls1;
-      g.ldc = D;
-      if ((r = gemm(e, (const __half*)attn, D, wo, D, g))) return r;
-    }
-    e->span_end(sp_, s);
-    sp_ = e->span_begin("ln", s);
-    launch_layernorm((const float*)x, MT, D, g2, b2, (__half*)xn, 0, e->ln_eps, s);
-    e->span_end(sp_, s);
-    sp_ = e->span_begin("fc1", s);
-    {
-      GemmArgs g = base_args(MT, 4 * D, D, EPI_F16);
-      g.out_f16 = (__half*)hb;
-      g.bias = bf1;
-      g.act = 1;
-      g.ldc = 4 * D;
-      cudaEvent_t e0 = nullptr, e1 = nullptr;
-      if (e->prof) {
-        cudaEventCreate(&e0);
-        cudaEventCreate(&e1);
-        cudaEventRecord(e0, s);
-        e->prof_rows += MT;
-      }
-      if ((r = gemm(e, (const __half*)xn, D, wf1, D, g))) return r;
-      if (e->prof) {
-        cudaEventRecord(e1, s);
-        e->prof_ev.push_back(e0);
-        e->prof_ev.push_back(e1);
-      }
-    }
-    e->span_end(sp_, s);
-    sp_ = e->span_begin("fc2", s);
-    {
-      GemmArgs g = base_args(MT, D, 4 * D, EPI_RESID_LS);
-      g.out_f32 = (float*)x;
-      g.bias = bf2;
-      g.ls = ls2;
-      g.ldc = D;
-      if ((r = gemm(e, (const __half*)hb, 4 * D, wf2, 4 * D, g))) return r;
-    }
-    e->span_end(sp_, s);
-    e->launches += 2;
-    if (tap_idx < 4 && c.taps[tap_idx] == l + 1 && dpt) {
-      // DPT: the raw residual stream (hidden_states[l + 1]), then the project readout over the patch rows of all
-      // images in one GEMM: GELU(W_t tok + (W_c cls_b + bias)), the CLS term computed once per image
-      void *tp, *cb, *ro;
-      const __half *wt, *wc;
-      const float* rb;
-      const int MR = B * NPATCH;
-      snprintf(nm, sizeof nm, "ro%d.wt", tap_idx);
-      if ((r = W(e, nm, &wt, (size_t)D * D))) return r;
-      snprintf(nm, sizeof nm, "ro%d.wc", tap_idx);
-      if ((r = W(e, nm, &wc, (size_t)D * D))) return r;
-      snprintf(nm, sizeof nm, "ro%d.b", tap_idx);
-      if ((r = W(e, nm, &rb, D))) return r;
-      snprintf(nm, sizeof nm, "tap%d", tap_idx);
-      if ((r = get_buf(e, nm, (size_t)round_up(MR, 128) * D * 2, &tp))) return r;
-      snprintf(nm, sizeof nm, "ro%d.c", tap_idx);
-      if ((r = get_buf(e, nm, (size_t)B * D * 4, &cb))) return r;
-      snprintf(nm, sizeof nm, "ro%d", tap_idx);
-      if ((r = get_buf(e, nm, (size_t)round_up(MR, 128) * D * 2, &ro))) return r;
-      launch_tap_f16((const float*)x, NP, NPATCH, D, B, (__half*)tp, s);
-      launch_readout_cls((const float*)x, NP, D, B, wc, rb, D, (float*)cb, s);
-      e->launches += 2;
-      GemmArgs g = base_args(MR, D, D, EPI_READOUT);
-      g.out_f16 = (__half*)ro;
-      g.img_bias = (const float*)cb;
-      g.npad = NPATCH;
-      g.ldc = D;
-      if ((r = gemm(e, (const __half*)tp, D, wt, D, g))) return r;
-      ++tap_idx;
-    } else if (tap_idx < 4 && c.taps[tap_idx] == l + 1) {
-      // backbone output: final LayerNorm applied (apply_layernorm=True), CLS dropped by the neck
-      const float *ng, *nb;
-      if ((r = W(e, "norm.g", &ng, D)) || (r = W(e, "norm.b", &nb, D))) return r;
-      for (int b = 0; b < B; ++b) {
-        void* tp;
-        snprintf(nm, sizeof nm, "tap%d.%d", tap_idx, b);
-        if ((r = get_buf(e, nm, (size_t)round_up(NPATCH, 128) * D * 2, &tp))) return r;
-        launch_layernorm((const float*)x + (size_t)b * NP * D, NPATCH, D, ng, nb, (__half*)tp, 1, e->ln_eps, s);
-        e->launches++;
-      }
-      ++tap_idx;
+    if ((r = residual_unit(e, j, "rl2", hrelu, h, Hc, Wc, t_mid, yraw))) return r;
+    const int OH = (j < 3) ? feat[2 - j].h : Hc * 2, OW = (j < 3) ? feat[2 - j].w : Wc * 2;
+    if ((r = get_buf(e, t.name(fmt("fu.up%d", j)), (size_t)OH * OW * F * 2, &up))) return r;
+    launch_upsample_ac(yraw, Hc, Wc, F, up, OH, OW, s);
+    e->launches++;
+    const __half* pwt;
+    const float* pbs;
+    if ((r = layer(e, fmt("f%d.proj", j), &pwt, (size_t)F * F, &pbs, F)) ||
+        (r = get_buf(e, t.name(fmt("fused%d", j)), (size_t)round_up(OH * OW, 128) * F * 2, &prj)))
+      return r;
+    GemmArgs g = base_args(OH * OW, F, F, EPI_F16);
+    g.out_f16 = prj;
+    g.bias = pbs;
+    g.ldc = F;
+    if ((r = gemm(e, up, F, pwt, F, g))) return r;
+    fused[j] = {prj, OH, OW};
+  }
+  return VD3D_OK;
+}
+
+// The head of one image on the last fusion output: conv1 (3x3), bilinear (align corners) to the processed size, then
+// conv2 (3x3) + ReLU with conv3 (1x1) and the last activation in the EPI_HEAD epilogue -> depth f32 [IH, IW].
+// ZoeDepth: conv2 + ReLU ("z.act") feeds the metric head, with the bottleneck feat[3] and every fusion output.
+int head(vd3d_depth* e, const Tail& t, const Map* feat, const Map* fused, float* depth) {
+  const int F = e->cfg.fusion, F2 = round_up(F / 2, 64), IH = e->cfg.image_h, IW = e->cfg.image_w;
+  const int ch = fused[3].h, cw = fused[3].w;
+  const __half *w1, *w2;
+  const float *b1, *b2, *w3, *b3;
+  __half *h1, *h1u;
+  int r;
+  if ((r = layer(e, "h.c1", &w1, (size_t)F2 * 9 * F, &b1, F2)) ||
+      (r = layer(e, "h.c2", &w2, (size_t)32 * 9 * F2, &b2, 32)) || (r = W(e, "h.c3.w", &w3, 32)) ||
+      (r = W(e, "h.c3.b", &b3, 1)) ||
+      (r = get_buf(e, t.name("h1"), (size_t)ch * cw * F2 * 2, &h1)) ||
+      (r = get_buf(e, t.name("h1u"), (size_t)IH * IW * F2 * 2, &h1u)))
+    return r;
+  GemmArgs g1 = base_args(0, F2, 0, EPI_F16);
+  g1.out_f16 = h1;
+  g1.bias = b1;
+  g1.ldc = F2;
+  if ((r = conv(e, fused[3].p, ch, cw, F, w1, true, g1))) return r;
+  launch_upsample_ac(h1, ch, cw, F2, h1u, IH, IW, t.s);
+  e->launches++;
+  if (e->traits.zoe_head) {
+    __half* act;
+    if ((r = get_buf(e, t.name("z.act"), (size_t)IH * IW * 32 * 2, &act))) return r;
+    GemmArgs g2 = base_args(0, 32, 0, EPI_F16);
+    g2.out_f16 = act;
+    g2.bias = b2;
+    g2.act = 2;
+    g2.ldc = 32;
+    if ((r = conv(e, h1u, IH, IW, F2, w2, true, g2, 32))) return r;
+    return zoe_head(e, t, feat[3], fused, act, depth);
+  }
+  GemmArgs g2 = base_args(0, 32, 0, EPI_HEAD);
+  g2.out_f32 = depth;
+  g2.bias = b2;
+  g2.w3 = w3;
+  g2.b3p = b3;
+  g2.head_max = e->head == VD3D_HEAD_METRIC ? e->max_depth : 0.f;
+  return conv(e, h1u, IH, IW, F2, w2, true, g2, 32);
+}
+
+// neck, fusion and head of one image, every launch on t.s; in: its four neck inputs
+int tail(vd3d_depth* e, const Tail& t, const __half* const* in, float* depth) {
+  StreamScope on(e, t.s);
+  Map feat[4], fused[4];
+  int r;
+  if ((r = neck(e, t, in, feat)) || (r = fusion(e, t, feat, fused))) return r;
+  return head(e, t, feat, fused, depth);
+}
+
+// B images through the network in one pass.  px_dev / depth_dev: DEVICE pointers, f32 [3, image_h, image_w] in, f32
+// [image_h, image_w] out.
+int forward_core(vd3d_depth* e, int B, const float* const* px_dev, float* const* depth_dev) {
+  if (B < 1 || B > kMaxBatch) return dfail(e, VD3D_ERR_ARG, "batch must be in [1, 8]");
+  if (e->traits.zoe_head && !e->zoe_nc)
+    return dfail(e, VD3D_ERR_STATE, "ZoeDepth: the metric head's settings are not set (vd3d_depth_set_zoe)");
+  Fwd f{B, (B - 1) * e->npad + e->ntok};
+  const size_t D = e->cfg.hidden, Hh = e->cfg.heads, NP = e->npad;
+  const __half* in[kMaxBatch][4];  // the neck inputs of every image
+  int r;
+  if ((r = get_buf(e, "x", B * NP * D * 4, &f.x)) || (r = get_buf(e, "xn", B * NP * D * 2, &f.xn)) ||
+      (r = get_buf(e, "q", B * Hh * NP * 64 * 2, &f.q)) || (r = get_buf(e, "k", B * Hh * NP * 64 * 2, &f.k)) ||
+      (r = get_buf(e, "vt", B * Hh * 64 * NP * 2, &f.vt)) || (r = get_buf(e, "attn", B * NP * D * 2, &f.attn)) ||
+      (r = get_buf(e, "h", B * NP * 4 * D * 2, &f.h)) || (r = embed(e, f, px_dev, in)))
+    return r;
+  int tap = e->traits.bit_front_end ? 2 : 0;  // the hybrid's neck inputs 0 and 1 are BiT stages, not taps
+  for (int l = 0; l < e->cfg.layers; ++l) {
+    if ((r = encoder_layer(e, f, l))) return r;
+    if (tap < 4 && e->cfg.taps[tap] == l + 1) {
+      if ((r = take_tap(e, f, tap, in))) return r;
+      ++tap;
     }
   }
-  if (tap_idx != 4) return dfail(e, VD3D_ERR_ARG, "taps must be increasing layer indices <= layers");
+  if (tap != 4) return dfail(e, VD3D_ERR_ARG, "taps must be increasing layer indices <= layers");
 
   // neck + head: independent per image.  With more than one image each tail runs on its own side stream (forked here,
   // joined below) with its own activation buffers, so that the many small launches of the tails (grids of 5..77 CTAs on
   // the coarse maps) overlap each other instead of leaving most SMs idle; captured into the same CUDA graph.
   const bool fork = B > 1;
-  cudaStream_t s_main = s;
-  const int sp_tail = e->span_begin("tail(all images, forked)", s_main);
+  const int sp_tail = e->span_begin("tail(all images, forked)", e->stream);
   if (fork) {
     if (!e->ev_fork) DCK(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
-    DCK(cudaEventRecord(e->ev_fork, s_main));
+    DCK(cudaEventRecord(e->ev_fork, e->stream));
   }
   for (int b = 0; b < B; ++b) {
-  if (fork) {
-    if (!e->aux[b]) DCK(cudaStreamCreateWithFlags(&e->aux[b], cudaStreamNonBlocking));
-    if (!e->ev_join[b]) DCK(cudaEventCreateWithFlags(&e->ev_join[b], cudaEventDisableTiming));
-    s = e->aux[b];
-    e->cur = s;
-    DCK(cudaStreamWaitEvent(s, e->ev_fork, 0));
+    Tail t{e->stream, ""};
+    if (fork) {
+      if (!e->aux[b]) DCK(cudaStreamCreateWithFlags(&e->aux[b], cudaStreamNonBlocking));
+      if (!e->ev_join[b]) DCK(cudaEventCreateWithFlags(&e->ev_join[b], cudaEventDisableTiming));
+      t = Tail{e->aux[b], "#" + std::to_string(b)};
+      DCK(cudaStreamWaitEvent(t.s, e->ev_fork, 0));
+    }
+    if ((r = tail(e, t, in[b], depth_dev[b]))) return r;
+    if (fork) DCK(cudaEventRecord(e->ev_join[b], t.s));
   }
-  auto bname = [&](const char* base) {  // per-image activation buffers when the tails run concurrently
-    std::string n(base);
-    if (fork) n += "#" + std::to_string(b);
-    return n;
-  };
-  void* depth_d = depth_dev[b];
-  // ---- neck: reassemble + 3x3 conv to the fusion width ----
-  int fh[4], fw[4];
-  void* feat[4];
-  for (int i = 0; i < 4; ++i) {
-    const int C = c.neck[i], CP = round_up(C, 64);
-    const __half *pw_, *cw;
-    const float* pb;
-    if (hybrid && i < 2) {  // the BiT stage-1 / stage-2 map (NHWC f16, C channels) is the neck input as it is
-      fh[i] = ph * (4 >> i);
-      fw[i] = pw * (4 >> i);
-      snprintf(nm, sizeof nm, "n%d.conv.w", i);
-      if ((r = W(e, nm, &cw, (size_t)F * 9 * CP))) return r;
-      snprintf(nm, sizeof nm, "bit.stage%d.%d", i + 1, b);
-      const void* stage = e->buf[nm].p;
-      snprintf(nm, sizeof nm, "f%d", i);
-      if ((r = get_buf(e, bname(nm), (size_t)fh[i] * fw[i] * F * 2, &feat[i]))) return r;
-      GemmArgs g = base_args(0, F, 0, EPI_F16);
-      g.out_f16 = (__half*)feat[i];
-      g.ldc = F;
-      if ((r = conv(e, (const __half*)stage, fh[i], fw[i], CP, cw, true, g))) return r;
-      continue;
-    }
-    snprintf(nm, sizeof nm, "r%d.proj.w", i);
-    if ((r = W(e, nm, &pw_, (size_t)CP * D))) return r;
-    snprintf(nm, sizeof nm, "r%d.proj.b", i);
-    if ((r = W(e, nm, &pb, CP))) return r;
-    void *tp, *rp, *rs = nullptr;
-    if (dpt) {  // image b's rows of the readout output
-      snprintf(nm, sizeof nm, "ro%d", i);
-      tp = (__half*)e->buf[nm].p + (size_t)b * NPATCH * D;
-    } else {
-      snprintf(nm, sizeof nm, "tap%d.%d", i, b);
-      tp = e->buf[nm].p;
-    }
-    snprintf(nm, sizeof nm, "r%d.p", i);
-    if ((r = get_buf(e, bname(nm), (size_t)round_up(NPATCH, 128) * CP * 2, &rp))) return r;
-    {
-      GemmArgs g = base_args(NPATCH, CP, D, EPI_F16);
-      g.out_f16 = (__half*)rp;
-      g.bias = pb;
-      g.ldc = CP;
-      if ((r = gemm(e, (const __half*)tp, D, pw_, D, g))) return r;
-    }
-    if (i < 2) {  // ConvTranspose2d(kernel=stride=4 / 2)
-      const int kk = (i == 0) ? 4 : 2;
-      const __half* uw;
-      const float* ub;
-      snprintf(nm, sizeof nm, "r%d.up.w", i);
-      if ((r = W(e, nm, &uw, (size_t)kk * kk * CP * CP))) return r;
-      snprintf(nm, sizeof nm, "r%d.up.b", i);
-      if ((r = W(e, nm, &ub, (size_t)kk * kk * CP))) return r;
-      fh[i] = ph * kk;
-      fw[i] = pw * kk;
-      snprintf(nm, sizeof nm, "r%d.s", i);
-      if ((r = get_buf(e, bname(nm), (size_t)fh[i] * fw[i] * CP * 2, &rs))) return r;
-      GemmArgs g = base_args(NPATCH, kk * kk * CP, CP, EPI_CONVT);
-      g.out_f16 = (__half*)rs;
-      g.bias = ub;
-      g.ct_k = kk;
-      g.ct_cout = CP;
-      g.ct_w = pw;
-      if ((r = gemm(e, (const __half*)rp, CP, uw, CP, g))) return r;
-    } else if (i == 2) {
-      fh[i] = ph;
-      fw[i] = pw;
-      rs = rp;
-    } else {  // Conv2d(3x3, stride 2, pad 1)
-      const __half* dw;
-      const float* db;
-      if ((r = W(e, "r3.down.w", &dw, (size_t)CP * 9 * CP)) || (r = W(e, "r3.down.b", &db, CP))) return r;
-      fh[i] = (ph - 1) / 2 + 1;
-      fw[i] = (pw - 1) / 2 + 1;
-      void* col;
-      if ((r = get_buf(e, bname("r3.col"), (size_t)round_up(fh[i] * fw[i], 128) * 9 * CP * 2, &col))) return r;
-      launch_im2col_s2((const __half*)rp, ph, pw, CP, CP, (__half*)col, fh[i], fw[i], s);
-      e->launches++;
-      if ((r = get_buf(e, bname("r3.s"), (size_t)round_up(fh[i] * fw[i], 128) * CP * 2, &rs))) return r;
-      GemmArgs g = base_args(fh[i] * fw[i], CP, 9 * CP, EPI_F16);
-      g.out_f16 = (__half*)rs;
-      g.bias = db;
-      g.ldc = CP;
-      if ((r = gemm(e, (const __half*)col, 9 * CP, dw, 9 * CP, g))) return r;
-    }
-    snprintf(nm, sizeof nm, "n%d.conv.w", i);
-    if ((r = W(e, nm, &cw, (size_t)F * 9 * CP))) return r;
-    snprintf(nm, sizeof nm, "f%d", i);
-    if ((r = get_buf(e, bname(nm), (size_t)fh[i] * fw[i] * F * 2, &feat[i]))) return r;
-    GemmArgs g = base_args(0, F, 0, EPI_F16);
-    g.out_f16 = (__half*)feat[i];
-    g.ldc = F;
-    if ((r = conv(e, (const __half*)rs, fh[i], fw[i], CP, cw, true, g))) return r;
-  }
-
-  // ---- fusion stage (coarsest first) ----
-  void* fused = nullptr;
-  int ch = 0, cw_ = 0;
-  const __half* fused_j[4];  // every fusion output and its size: ZoeDepth's feature blocks
-  int fused_h[4], fused_w[4];
-  for (int j = 0; j < 4; ++j) {
-    const int fi = 3 - j;
-    const int Hc = fh[fi], Wc = fw[fi];
-    const size_t n = (size_t)Hc * Wc * F;
-    void *t_relu, *t_mid, *hraw, *hrelu, *yraw, *up, *prj;
-    if ((r = get_buf(e, bname("fu.relu"), n * 2, &t_relu)) || (r = get_buf(e, bname("fu.mid"), n * 2, &t_mid)) ||
-        (r = get_buf(e, bname("fu.h"), n * 2, &hraw)) || (r = get_buf(e, bname("fu.hrelu"), n * 2, &hrelu)) ||
-        (r = get_buf(e, bname("fu.y"), n * 2, &yraw)))
-      return r;
-    auto cv = [&](const char* unit, const char* which, const __half** wv, const float** bv) -> int {
-      snprintf(nm, sizeof nm, "f%d.%s.%s.w", j, unit, which);
-      int rr = W(e, nm, wv, (size_t)F * 9 * F);
-      if (rr) return rr;
-      snprintf(nm, sizeof nm, "f%d.%s.%s.b", j, unit, which);
-      return W(e, nm, bv, F);
-    };
-    const __half *w1, *w2;
-    const float *bb1, *bb2;
-    const __half* hin_raw;
-    if (j == 0) {
-      hin_raw = (const __half*)feat[fi];
-      launch_relu_f16(hin_raw, (__half*)hrelu, n, s);
-      e->launches++;
-    } else {
-      // h = fused + residual_layer1(feat)
-      if ((r = cv("rl1", "c1", &w1, &bb1)) || (r = cv("rl1", "c2", &w2, &bb2))) return r;
-      launch_relu_f16((const __half*)feat[fi], (__half*)t_relu, n, s);
-      e->launches++;
-      GemmArgs g1 = base_args(0, F, 0, EPI_F16);
-      g1.out_f16 = (__half*)t_mid;
-      g1.bias = bb1;
-      g1.act = 2;
-      g1.ldc = F;
-      if ((r = conv(e, (const __half*)t_relu, Hc, Wc, F, w1, true, g1))) return r;
-      // y = conv2(mid) + b2 + feat ; h = y + fused  (two residual adds: second via res on a 1x1-free pass)
-      GemmArgs g2 = base_args(0, F, 0, EPI_F16);
-      g2.out_f16 = (__half*)yraw;
-      g2.bias = bb2;
-      g2.res_f16 = (const __half*)feat[fi];
-      g2.ldc = F;
-      if ((r = conv(e, (const __half*)t_mid, Hc, Wc, F, w2, true, g2))) return r;
-      // h = fused + y ; relu(h) feeds residual_layer2's first conv
-      launch_add_relu_f16((const __half*)fused, (const __half*)yraw, (__half*)hraw, (__half*)hrelu, n, s);
-      e->launches++;
-      hin_raw = (const __half*)hraw;
-    }
-    // residual_layer2
-    if ((r = cv("rl2", "c1", &w1, &bb1)) || (r = cv("rl2", "c2", &w2, &bb2))) return r;
-    {
-      GemmArgs g1 = base_args(0, F, 0, EPI_F16);
-      g1.out_f16 = (__half*)t_mid;
-      g1.bias = bb1;
-      g1.act = 2;
-      g1.ldc = F;
-      if ((r = conv(e, (const __half*)hrelu, Hc, Wc, F, w1, true, g1))) return r;
-      GemmArgs g2 = base_args(0, F, 0, EPI_F16);
-      g2.out_f16 = (__half*)yraw;
-      g2.bias = bb2;
-      g2.res_f16 = hin_raw;
-      g2.ldc = F;
-      if ((r = conv(e, (const __half*)t_mid, Hc, Wc, F, w2, true, g2))) return r;
-    }
-    // upsample (to the next feature's size, or x2 at the end), then 1x1 projection
-    int OH = (j < 3) ? fh[fi - 1] : Hc * 2, OW = (j < 3) ? fw[fi - 1] : Wc * 2;
-    snprintf(nm, sizeof nm, "fu.up%d", j);
-    if ((r = get_buf(e, bname(nm), (size_t)OH * OW * F * 2, &up))) return r;
-    launch_upsample_ac((const __half*)yraw, Hc, Wc, F, (__half*)up, OH, OW, s);
-    e->launches++;
-    const __half* pwt;
-    const float* pbs;
-    snprintf(nm, sizeof nm, "f%d.proj.w", j);
-    if ((r = W(e, nm, &pwt, (size_t)F * F))) return r;
-    snprintf(nm, sizeof nm, "f%d.proj.b", j);
-    if ((r = W(e, nm, &pbs, F))) return r;
-    snprintf(nm, sizeof nm, "fused%d", j);
-    if ((r = get_buf(e, bname(nm), (size_t)round_up(OH * OW, 128) * F * 2, &prj))) return r;
-    GemmArgs g = base_args(OH * OW, F, F, EPI_F16);
-    g.out_f16 = (__half*)prj;
-    g.bias = pbs;
-    g.ldc = F;
-    if ((r = gemm(e, (const __half*)up, F, pwt, F, g))) return r;
-    fused = prj;
-    ch = OH;
-    cw_ = OW;
-    fused_j[j] = (const __half*)prj;
-    fused_h[j] = OH;
-    fused_w[j] = OW;
-  }
-
-  // ---- head ----
-  {
-    const int F2 = round_up(F / 2, 64);
-    const __half *w1, *w2;
-    const float *b1h, *b2h, *w3, *b3;
-    if ((r = W(e, "h.c1.w", &w1, (size_t)F2 * 9 * F)) || (r = W(e, "h.c1.b", &b1h, F2)) ||
-        (r = W(e, "h.c2.w", &w2, (size_t)32 * 9 * F2)) || (r = W(e, "h.c2.b", &b2h, 32)) ||
-        (r = W(e, "h.c3.w", &w3, 32)) || (r = W(e, "h.c3.b", &b3, 1)))
-      return r;
-    void *h1, *h1u;
-    if ((r = get_buf(e, bname("h1"), (size_t)ch * cw_ * F2 * 2, &h1)) || (r = get_buf(e, bname("h1u"), (size_t)IH * IW * F2 * 2, &h1u)))
-      return r;
-    GemmArgs g1 = base_args(0, F2, 0, EPI_F16);
-    g1.out_f16 = (__half*)h1;
-    g1.bias = b1h;
-    g1.ldc = F2;
-    if ((r = conv(e, (const __half*)fused, ch, cw_, F, w1, true, g1))) return r;
-    launch_upsample_ac((const __half*)h1, ch, cw_, F2, (__half*)h1u, IH, IW, s);
-    e->launches++;
-    if (zoe) {  // ZoeDepth: the conv2 + ReLU activation feeds the metric head
-      void* act;
-      if ((r = get_buf(e, bname("z.act"), (size_t)IH * IW * 32 * 2, &act))) return r;
-      GemmArgs g2 = base_args(0, 32, 0, EPI_F16);
-      g2.out_f16 = (__half*)act;
-      g2.bias = b2h;
-      g2.act = 2;
-      g2.ldc = 32;
-      if ((r = conv(e, (const __half*)h1u, IH, IW, F2, w2, true, g2, 32))) return r;
-      if ((r = zoe_head(e, fork ? "#" + std::to_string(b) : std::string(), (const __half*)feat[3], fh[3], fw[3],
-                        fused_j, fused_h, fused_w, (const __half*)act, (float*)depth_d)))
-        return r;
-    } else {
-      GemmArgs g2 = base_args(0, 32, 0, EPI_HEAD);
-      g2.out_f32 = (float*)depth_d;
-      g2.bias = b2h;
-      g2.w3 = w3;
-      g2.b3p = b3;
-      g2.head_max = e->head == VD3D_HEAD_METRIC ? e->max_depth : 0.f;
-      if ((r = conv(e, (const __half*)h1u, IH, IW, F2, w2, true, g2, 32))) return r;
-    }
-  }
-  if (fork) DCK(cudaEventRecord(e->ev_join[b], s));
-  }  // images
-  e->cur = nullptr;
   if (fork)
-    for (int b = 0; b < B; ++b) DCK(cudaStreamWaitEvent(s_main, e->ev_join[b], 0));
-  e->span_end(sp_tail, s_main);
+    for (int b = 0; b < B; ++b) DCK(cudaStreamWaitEvent(e->stream, e->ev_join[b], 0));
+  e->span_end(sp_tail, e->stream);
   DCK(cudaGetLastError());
   return VD3D_OK;
 }
@@ -1482,8 +1504,7 @@ int pil_bicubic_table(int in_size, int out_size, std::vector<int>& tab) {
 
 // the device table of one (in, out) axis, built and uploaded on first use, then cached by the engine
 int pil_table(vd3d_depth* e, int in_size, int out_size, const int** out, int* ksize) {
-  char nm[48];
-  snprintf(nm, sizeof nm, "pil.%d.%d", in_size, out_size);
+  const std::string nm = fmt("pil.%d.%d", in_size, out_size);
   const double scale = (double)in_size / out_size;
   *ksize = (int)ceil(2.0 * (scale < 1.0 ? 1.0 : scale)) * 2 + 1;
   const size_t bytes = (size_t)out_size * (2 + *ksize) * sizeof(int);
@@ -1541,6 +1562,39 @@ void processed_size(int h, int w, int th, int tw, int mult, int* ph, int* pw) {
   *pw = rnd(sw * w);
 }
 
+// the f32 pixel and depth slots of image b of a forward: "px" / "depth" for the first, "px.{b}" / "depth.{b}" after
+int batch_slots(vd3d_depth* e, int b, float** px, float** depth) {
+  const size_t n = (size_t)e->cfg.image_h * e->cfg.image_w;
+  const int r = get_buf(e, fmt(b ? "px.%d" : "px", b), 3 * n * 4, px);
+  return r ? r : get_buf(e, fmt(b ? "depth.%d" : "depth", b), n * 4, depth);
+}
+
+// The model's image processor on one u8 image [h, w, 3] (BGR when swap_rb) into its pixel slot px: ZoeDepth's reflect
+// padding and resize, or the resize (width pass into tmp, height pass into rgb) and normalisation.  timed: the
+// ZoeDepth kernel is a "zoe.preprocess" span
+void preprocess(vd3d_depth* e, const uint8_t* img, int h, int w, int swap_rb, void* tmp, void* rgb, float* px,
+                bool timed) {
+  cudaStream_t s = e->stream;
+  const int IH = e->cfg.image_h, IW = e->cfg.image_w;
+  if (e->traits.zoe_head) {
+    const int sp = timed ? e->span_begin("zoe.preprocess", s) : -1;
+    launch_zoe_preprocess(img, h, w, swap_rb, zoe_pad(h), zoe_pad(w), px, IH, IW, e->pre, s);
+    e->span_end(sp, s);
+    e->launches++;
+  } else {
+    launch_preprocess(img, h, w, (uint8_t*)tmp, (uint8_t*)rgb, px, IH, IW, s, swap_rb, e->pre);
+    e->launches += 3;
+  }
+}
+
+// The processed-size depth of one image back to its (h, w) input size: the bicubic resize into up f32 [h, w]
+// (ZoeDepth: of the reflect-padded size, cropped) with its min / max in mm, and the min-max u8 [h, w] when u8 is set
+void postprocess(vd3d_depth* e, const float* depth, int h, int w, float* up, unsigned* mm, uint8_t* u8, int invert) {
+  const int pad_h = e->traits.zoe_head ? zoe_pad(h) : 0, pad_w = e->traits.zoe_head ? zoe_pad(w) : 0;
+  launch_depth_post_crop(depth, e->cfg.image_h, e->cfg.image_w, up, h, w, pad_h, pad_w, mm, u8, invert, e->stream);
+  e->launches += u8 ? 3 : 2;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1551,15 +1605,12 @@ int vd3d_depth_forward(vd3d_depth* e, const float* pixel_values, float* depth_ou
   const int IH = e->cfg.image_h, IW = e->cfg.image_w;
   cudaStream_t s = e->stream;
   int r;
-  void *px_d = (void*)pixel_values, *depth_d = depth_out;
+  float *px_d = (float*)pixel_values, *depth_d = depth_out;
   if (mem == VD3D_MEM_HOST) {
-    if ((r = get_buf(e, "px", (size_t)3 * IH * IW * 4, &px_d))) return r;
-    if ((r = get_buf(e, "depth", (size_t)IH * IW * 4, &depth_d))) return r;
+    if ((r = batch_slots(e, 0, &px_d, &depth_d))) return r;
     DCK(cudaMemcpyAsync(px_d, pixel_values, (size_t)3 * IH * IW * 4, cudaMemcpyHostToDevice, s));
   }
-  const float* pxs[1] = {(const float*)px_d};
-  float* ds[1] = {(float*)depth_d};
-  if ((r = forward_core(e, 1, pxs, ds))) return r;
+  if ((r = forward_core(e, 1, &px_d, &depth_d))) return r;
   if (mem == VD3D_MEM_HOST) {
     DCK(cudaMemcpyAsync(depth_out, depth_d, (size_t)IH * IW * 4, cudaMemcpyDeviceToHost, s));
     DCK(cudaStreamSynchronize(s));
@@ -1573,42 +1624,20 @@ int vd3d_depth_infer_batch_device(vd3d_depth* e, int B, const uint8_t* const* fr
                                   uint8_t* const* depth_u8_dev, float* const* depth_f32_dev, int invert) {
   if (!e || !frames_bgr_dev || B < 1 || B > kMaxBatch || h < 16 || w < 16) return VD3D_ERR_ARG;
   const int IH = e->cfg.image_h, IW = e->cfg.image_w;
-  cudaStream_t s = e->stream;
   void *tmp, *rgb, *mm, *up;
   int r;
-  char nm[32];
-  const float* pxs[kMaxBatch];
-  float* dds[kMaxBatch];
+  float *pxs[kMaxBatch], *dds[kMaxBatch];
   if ((r = get_buf(e, "pp.tmp", (size_t)h * IW * 3, &tmp)) || (r = get_buf(e, "pp.rgb", (size_t)IH * IW * 3, &rgb)) ||
       (r = get_buf(e, "post.up", (size_t)h * w * 4, &up)) || (r = get_buf(e, "post.mm", 64, &mm)))
     return r;
   for (int b = 0; b < B; ++b) {
-    void *px, *dd;
-    snprintf(nm, sizeof nm, b ? "px.%d" : "px", b);
-    if ((r = get_buf(e, nm, (size_t)3 * IH * IW * 4, &px))) return r;
-    snprintf(nm, sizeof nm, b ? "depth.%d" : "depth", b);
-    if ((r = get_buf(e, nm, (size_t)IH * IW * 4, &dd))) return r;
-    if (e->family == VD3D_DEPTH_ZOEDEPTH) {
-      const int sp = e->span_begin("zoe.preprocess", s);
-      launch_zoe_preprocess(frames_bgr_dev[b], h, w, 1, zoe_pad(h), zoe_pad(w), (float*)px, IH, IW, e->pre, s);
-      e->span_end(sp, s);
-      e->launches++;
-    } else {
-      launch_preprocess(frames_bgr_dev[b], h, w, (uint8_t*)tmp, (uint8_t*)rgb, (float*)px, IH, IW, s, 1, e->pre);
-      e->launches += 3;
-    }
-    pxs[b] = (const float*)px;
-    dds[b] = (float*)dd;
+    if ((r = batch_slots(e, b, &pxs[b], &dds[b]))) return r;
+    preprocess(e, frames_bgr_dev[b], h, w, 1, tmp, rgb, pxs[b], true);
   }
   if ((r = forward_core(e, B, pxs, dds))) return r;
   for (int b = 0; b < B; ++b) {
     float* upt = (depth_f32_dev && depth_f32_dev[b]) ? depth_f32_dev[b] : (float*)up;
-    uint8_t* u8 = depth_u8_dev ? depth_u8_dev[b] : nullptr;
-    if (e->family == VD3D_DEPTH_ZOEDEPTH)
-      launch_depth_post_crop(dds[b], IH, IW, upt, h, w, zoe_pad(h), zoe_pad(w), (unsigned*)mm, u8, invert, s);
-    else
-      launch_depth_post(dds[b], IH, IW, upt, h, w, (unsigned*)mm, u8, invert, s);
-    e->launches += u8 ? 3 : 2;
+    postprocess(e, dds[b], h, w, upt, (unsigned*)mm, depth_u8_dev ? depth_u8_dev[b] : nullptr, invert);
   }
   DCK(cudaGetLastError());
   return VD3D_OK;
@@ -1619,22 +1648,14 @@ int vd3d_depth_infer_batch(vd3d_depth* e, int B, const uint8_t* const* frames_bg
                            uint8_t* const* depth_u8, int invert) {
   if (!e || !frames_bgr || B < 1 || B > kMaxBatch) return VD3D_ERR_ARG;
   int r;
-  char nm[32];
-  const uint8_t* fd[kMaxBatch];
-  uint8_t* u8d[kMaxBatch];
+  uint8_t *fd[kMaxBatch], *u8d[kMaxBatch];
   float* f32d[kMaxBatch];
   for (int b = 0; b < B; ++b) {
-    void *a, *c, *d;
-    snprintf(nm, sizeof nm, "io.frame.%d", b);
-    if ((r = get_buf(e, nm, (size_t)h * w * 3, &a))) return r;
-    snprintf(nm, sizeof nm, "io.u8.%d", b);
-    if ((r = get_buf(e, nm, (size_t)h * w, &c))) return r;
-    snprintf(nm, sizeof nm, "io.f32.%d", b);
-    if ((r = get_buf(e, nm, (size_t)h * w * 4, &d))) return r;
-    DCK(cudaMemcpyAsync(a, frames_bgr[b], (size_t)h * w * 3, cudaMemcpyHostToDevice, e->stream));
-    fd[b] = (const uint8_t*)a;
-    u8d[b] = (uint8_t*)c;
-    f32d[b] = (float*)d;
+    if ((r = get_buf(e, fmt("io.frame.%d", b), (size_t)h * w * 3, &fd[b])) ||
+        (r = get_buf(e, fmt("io.u8.%d", b), (size_t)h * w, &u8d[b])) ||
+        (r = get_buf(e, fmt("io.f32.%d", b), (size_t)h * w * 4, &f32d[b])))
+      return r;
+    DCK(cudaMemcpyAsync(fd[b], frames_bgr[b], (size_t)h * w * 3, cudaMemcpyHostToDevice, e->stream));
   }
   if ((r = vd3d_depth_infer_batch_device(e, B, fd, h, w, u8d, f32d, invert))) return r;
   for (int b = 0; b < B; ++b) {
@@ -1694,14 +1715,11 @@ int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_r
   for (int b = 0; b < B; ++b) {
     const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
     if (!images_rgb[b] || !depth_u8[b] || sh < 1 || sw < 1 || ih < 16 || iw < 16) return VD3D_ERR_ARG;
-    int ph = IH, pw = IW;  // DPT's processor resizes every input to its fixed size
+    int ph = IH, pw = IW;  // a processor without keep-aspect fit resizes every input to its fixed size
     // ZoeDepth's processor sizes the reflect-padded image
-    const bool zoe = e->family == VD3D_DEPTH_ZOEDEPTH;
+    const bool zoe = e->traits.zoe_head;
     const int fh = zoe ? ih + 2 * zoe_pad(ih) : ih, fw = zoe ? iw + 2 * zoe_pad(iw) : iw;
-    if (e->family == VD3D_DEPTH_DA_V2)
-      processed_size(ih, iw, 518, 518, 14, &ph, &pw);
-    else if (e->fit_multiple)
-      processed_size(fh, fw, e->fit_h, e->fit_w, e->fit_multiple, &ph, &pw);
+    if (e->fit_multiple) processed_size(fh, fw, e->fit_h, e->fit_w, e->fit_multiple, &ph, &pw);
     if (ph != IH || pw != IW) {
       char m[160];
       snprintf(m, sizeof m, "image %d: a %dx%d input maps to processed size %dx%d, the engine serves %dx%d", b, iw, ih,
@@ -1719,38 +1737,21 @@ int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_r
   // every buffer first, so that no reallocation lands between enqueued launches
   void *src_d = nullptr, *rs = nullptr, *ptmp = nullptr, *tmp, *rgb, *mm, *up, *u8in;
   int r;
-  char nm[32];
   if ((host && (r = get_buf(e, "im.src", src_max, &src_d))) || (rs_max && (r = get_buf(e, "im.rs", rs_max, &rs))) ||
       (tmp_max && (r = get_buf(e, "pil.tmp", tmp_max, &ptmp))) || (r = get_buf(e, "pp.tmp", pp_max, &tmp)) ||
       (r = get_buf(e, "pp.rgb", (size_t)IH * IW * 3, &rgb)) || (r = get_buf(e, "post.mm", 64, &mm)) ||
       (r = get_buf(e, "im.up", in_max * 4, &up)) || (r = get_buf(e, "im.u8in", in_max, &u8in)))
     return r;
-  const float* pxs[kMaxBatch];
-  float* dds[kMaxBatch];
+  float *pxs[kMaxBatch], *dds[kMaxBatch], *o32[kMaxBatch];
   uint8_t* o8[kMaxBatch];
-  float* o32[kMaxBatch];
   for (int b = 0; b < B; ++b) {
     const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
-    void *px, *dd;
-    snprintf(nm, sizeof nm, b ? "px.%d" : "px", b);
-    if ((r = get_buf(e, nm, (size_t)3 * IH * IW * 4, &px))) return r;
-    snprintf(nm, sizeof nm, b ? "depth.%d" : "depth", b);
-    if ((r = get_buf(e, nm, (size_t)IH * IW * 4, &dd))) return r;
-    pxs[b] = (const float*)px;
-    dds[b] = (float*)dd;
     o8[b] = depth_u8[b];
     o32[b] = depth_f32 ? depth_f32[b] : nullptr;
-    if (host) {
-      void* p;
-      snprintf(nm, sizeof nm, "im.u8.%d", b);
-      if ((r = get_buf(e, nm, (size_t)sh * sw, &p))) return r;
-      o8[b] = (uint8_t*)p;
-      if (o32[b]) {
-        snprintf(nm, sizeof nm, "im.f32.%d", b);
-        if ((r = get_buf(e, nm, (size_t)ih * iw * 4, &p))) return r;
-        o32[b] = (float*)p;
-      }
-    }
+    if ((r = batch_slots(e, b, &pxs[b], &dds[b])) ||
+        (host && (r = get_buf(e, fmt("im.u8.%d", b), (size_t)sh * sw, &o8[b]))) ||
+        (host && o32[b] && (r = get_buf(e, fmt("im.f32.%d", b), (size_t)ih * iw * 4, &o32[b]))))
+      return r;
     // the Pillow tables of this image, so that a first use uploads before anything of this call is enqueued
     const int* t;
     int k;
@@ -1767,23 +1768,13 @@ int vd3d_depth_infer_images(vd3d_depth* e, int B, const uint8_t* const* images_r
       if ((r = pil_resize(e, img, sh, sw, (uint8_t*)ptmp, (uint8_t*)rs, ih, iw))) return r;
       img = (const uint8_t*)rs;
     }
-    if (e->family == VD3D_DEPTH_ZOEDEPTH) {
-      launch_zoe_preprocess(img, ih, iw, 0, zoe_pad(ih), zoe_pad(iw), (float*)pxs[b], IH, IW, e->pre, s);
-      e->launches++;
-    } else {
-      launch_preprocess(img, ih, iw, (uint8_t*)tmp, (uint8_t*)rgb, (float*)pxs[b], IH, IW, s, 0, e->pre);
-      e->launches += 3;
-    }
+    preprocess(e, img, ih, iw, 0, tmp, rgb, pxs[b], false);
   }
   if ((r = forward_core(e, B, pxs, dds))) return r;
   for (int b = 0; b < B; ++b) {
     const int sh = sizes[4 * b], sw = sizes[4 * b + 1], ih = sizes[4 * b + 2], iw = sizes[4 * b + 3];
     const bool back = ih != sh || iw != sw;
-    const int pad_h = e->family == VD3D_DEPTH_ZOEDEPTH ? zoe_pad(ih) : 0;
-    const int pad_w = e->family == VD3D_DEPTH_ZOEDEPTH ? zoe_pad(iw) : 0;
-    launch_depth_post_crop(dds[b], IH, IW, o32[b] ? o32[b] : (float*)up, ih, iw, pad_h, pad_w, (unsigned*)mm,
-                           back ? (uint8_t*)u8in : o8[b], invert, s);
-    e->launches += 3;
+    postprocess(e, dds[b], ih, iw, o32[b] ? o32[b] : (float*)up, (unsigned*)mm, back ? (uint8_t*)u8in : o8[b], invert);
     if (back) {
       launch_resize_cubic_u8((const uint8_t*)u8in, ih, iw, 1, o8[b], sh, sw, s);
       e->launches++;

@@ -1053,10 +1053,6 @@ void launch_resize_pil_u8(const uint8_t* src, int IH, int IW, uint8_t* dst, int 
   dim3 g((OW + 31) / 32, (OH + 7) / 8);
   k_resize_pil_u8<<<g, 256, 0, s>>>(src, IH, IW, dst, OH, OW, tab, ksize, axis_y);
 }
-void launch_depth_post(const float* depth, int IH, int IW, float* up, int OH, int OW, unsigned* mm, uint8_t* out_u8,
-                       int invert, cudaStream_t s) {
-  launch_depth_post_crop(depth, IH, IW, up, OH, OW, 0, 0, mm, out_u8, invert, s);
-}
 void launch_depth_post_crop(const float* depth, int IH, int IW, float* up, int OH, int OW, int pad_h, int pad_w,
                             unsigned* mm, uint8_t* out_u8, int invert, cudaStream_t s) {
   k_minmax_reset<<<1, 1, 0, s>>>(mm);

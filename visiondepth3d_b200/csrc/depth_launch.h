@@ -32,11 +32,9 @@ void launch_preprocess(const uint8_t* frame_bgr, int H, int W, uint8_t* tmp_u8, 
 // one pass of Pillow's 8-bit bicubic resize on u8 [IH,IW,3] (axis_y = 0: width, 1: height) with a host-built table
 void launch_resize_pil_u8(const uint8_t* src, int IH, int IW, uint8_t* dst, int OH, int OW, const int* tab, int ksize,
                           int axis_y, cudaStream_t s);
-// bicubic to (OH,OW) + min/max (+ u8 quantisation when out_u8 != null) (2-3 launches)
-void launch_depth_post(const float* depth, int IH, int IW, float* up, int OH, int OW, unsigned* mm, uint8_t* out_u8,
-                       int invert, cudaStream_t s);
-// ZoeDepth's post-process: the same, evaluating only the (OH, OW) window at (pad_h, pad_w) of the bicubic resize to
-// (OH + 2 pad_h, OW + 2 pad_w), i.e. the resize to the padded size, then the crop
+// bicubic to (OH,OW) + min/max (+ u8 quantisation when out_u8 != null) (2-3 launches).  pad_h / pad_w > 0 (ZoeDepth's
+// post-process): only the (OH, OW) window at (pad_h, pad_w) of the bicubic resize to (OH + 2 pad_h, OW + 2 pad_w) is
+// evaluated, i.e. the resize to the padded size, then the crop
 void launch_depth_post_crop(const float* depth, int IH, int IW, float* up, int OH, int OW, int pad_h, int pad_w,
                             unsigned* mm, uint8_t* out_u8, int invert, cudaStream_t s);
 // ---- ZoeDepth metric head (see depth_kernels.cu) ----
